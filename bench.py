@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- the driver's benchmark contract for the fuzzysearch hot path on B200.
+"""bench.py -- the benchmark of the fuzzysearch hot path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload ...]
+                    [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic input: ONE bounded-Levenshtein
 search (``find_near_matches(pattern, haystack, max_l_dist=2)``, |pattern| = 20) of a 4 GiB
@@ -13,11 +14,14 @@ N x 4 GiB, sharded with a halo of |pattern|+k = configs[3], weak scaling).
 * ``e2e``    = same metric through the C-ABI one-shot call with HOST (pinned) buffers: H2D copy of
   the haystack and D2H of the matches inside the timed region.
 * ``roofline`` = the dominant kernel (k_filter_sampled): algorithmic bytes (1 per haystack byte) /
-  its CUDA-event duration, against the measured HBM peak of MEASURED_PEAKS.json.
-* ``cpu_baseline`` / ``--impl reference`` = the reference itself (oracle/_ref, compiled from
-  /root/reference by oracle/build_ref.py) on the box's host cores, on a bounded sample.
+  its CUDA-event duration, against the measured HBM peak of MEASURED_PEAKS.json if present, else
+  the H100 SXM data-sheet figure.
+* ``cpu_baseline`` / ``--impl reference`` = the reference itself (oracle/_ref, compiled from the
+  reference's sources by oracle/build_ref.py) on the box's host cores, on a bounded sample.
+* ``--dump-outputs DIR`` writes the final match list of the last timed step as DIR/<name>.npy
+  (float64), so that two builds can be compared output for output on identical, seeded inputs.
 
-Inputs are far larger than L2 (4 GiB vs 126 MB), so no explicit L2 flush is needed between steps.
+Inputs are far larger than L2 (4 GiB vs 50 MB), so no explicit L2 flush is needed between steps.
 """
 import argparse
 import json
@@ -128,15 +132,24 @@ def hbm_peak():
         v = json.load(open(p))
         return float(v["hbm_gbs"]), "measured (MEASURED_PEAKS.json, copy read+write)"
     except (OSError, KeyError, ValueError):
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
-def ncu_traffic():
-    """DRAM bytes per launch of the dominant kernel from the committed ncu capture, or None."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "filter_traffic.json")))
-    except (OSError, ValueError):
-        return None
+DUMP_LIMIT = 64 << 20  # bytes of .npy payload --dump-outputs may write
+
+
+def dump_outputs(out_dir, cols, seed):
+    """Writes each column of `cols` (name -> 1-D array, all the same length) as out_dir/<name>.npy in
+    float64.  Above DUMP_LIMIT a fixed, seeded sample of rows is kept, in order, and its row numbers
+    are written as `row.npy`."""
+    os.makedirs(out_dir, exist_ok=True)
+    n = len(next(iter(cols.values())))
+    max_rows = DUMP_LIMIT // (8 * (len(cols) + 1))
+    if n > max_rows:
+        rows = np.sort(np.random.default_rng(seed).choice(n, max_rows, replace=False))
+        cols = dict({k: np.asarray(v)[rows] for k, v in cols.items()}, row=rows)
+    for name, v in cols.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(v, dtype=np.float64))
 
 
 # -------------------------------------------------------------------------------------------------
@@ -453,7 +466,11 @@ def main():
                     help="multi-GPU reduction: inside the library over NVLink peer memory (default; 'nccl' is an "
                          "alias), or through torch.distributed (tools/torch_reduce.py, comparison only)")
     ap.add_argument("--ref-cores", type=int, default=0, help="reference arm: processes to use (0 = all cores)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the final matches of the last timed step as DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
 
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -482,12 +499,10 @@ def main():
             return 0
         hay = synth_sample_host(alphabet, seed, pat, sample, m, k, kind)
         times, nm = [], 0
-        for i in range(args.warmup + max(args.steps, 5)):  # >= 5 timed steps: the arm is noisy (fork pool)
+        for i in range(args.warmup + args.steps):
             dt, nm = run_reference_sample(hay, pat, kind, k, cores)
             if i >= args.warmup:
                 times.append(dt)
-            if sum(times) > 240:
-                break
         sec = float(np.median(times))
         val = sample / sec / 1e9
         # the reference as it actually ships is single-threaded: one plain find_near_matches call
@@ -524,7 +539,7 @@ def main():
         from torch_reduce import gather_and_merge_groups
 
     # the single-pattern workloads shard the haystack (weak scaling: N x 4 GiB, configs[3]); the batch (configs[4]:
-    # "1024 patterns over ONE 4 GiB haystack, 8 x B200") keeps the whole haystack on every GPU and splits the PATTERNS
+    # "1024 patterns over ONE 4 GiB haystack, 8 x H100") keeps the whole haystack on every GPU and splits the PATTERNS
     # (strong scaling: nothing to merge, every pattern's list is complete on the rank that searched it)
     global_len = per_gpu * world if kind != "batch" else per_gpu
     halo = m + k
@@ -578,24 +593,55 @@ def main():
             return h.search_levenshtein(pat, k, gflag)
         return h.search_hamming(pat, k, gflag)
 
-    def step(h=None):
+    def step(h=None, keep=None):
         # one search of this rank's shard (local consolidation on the device); multi-GPU: the per-shard
         # groups are all-gathered by NCCL inside the library, on the search's stream, and merged
-        # (--reduce torch: the same reduction through torch.distributed, for comparison)
+        # (--reduce torch: the same reduction through torch.distributed, for comparison).
+        # keep (a list): the step's final matches are appended to it instead of being discarded; they are
+        # read back after the timer stops (see final_columns)
         if kind == "batch":
             results, st = (h or hs).search_levenshtein_batch(batch_pats, batch_ks)
             nfinal = sum(r.count(F.FINAL) for r in results)
             for r in results:
-                r.close()
+                if keep is not None:
+                    keep.append(r)
+                else:
+                    r.close()
             return st, nfinal
         res = one_search(h or hs)
         st = res.stats()
         if world > 1 and not in_library:
-            nfinal = len(gather_and_merge_groups(result=res, as_arrays=True)[0])
+            merged = gather_and_merge_groups(result=res, as_arrays=True)
+            nfinal = len(merged[0])
+            if keep is not None:
+                keep.append(merged)
         else:
             nfinal = res.count(F.FINAL)
+            if keep is not None:
+                keep.append(res)
+                return st, nfinal
         res.close()
         return st, nfinal
+
+    def final_columns(kept):
+        """The matches a caller of the timed path receives, as columns: (start, end, dist) of the final
+        list; for the batch also the pattern's index in the 1024-pattern list, in pattern order."""
+        if kind == "batch":
+            cols = {"pattern": [], "start": [], "end": [], "dist": []}
+            for i, r in enumerate(kept):
+                s, e, d = r.arrays(F.FINAL)
+                r.close()
+                cols["pattern"].append(np.full(len(s), rank + i * world, dtype=np.int64))
+                for name, v in zip(("start", "end", "dist"), (s, e, d)):
+                    cols[name].append(np.asarray(v))
+            return {name: np.concatenate(v) for name, v in cols.items()}
+        (got,) = kept
+        if isinstance(got, tuple):
+            s, e, d = got
+        else:
+            s, e, d = got.arrays(F.FINAL)
+            got.close()
+        return {"start": s, "end": e, "dist": d}
 
     def sync_all():
         if dist is not None:
@@ -610,15 +656,19 @@ def main():
     time.sleep(0.3)
     sync_all()
     filt_ms, launches, nfinal = [], 0, 0
+    kept = [] if args.dump_outputs else None
     hs.timer_start()
     t0 = time.perf_counter()
-    for _ in range(args.steps):
-        st, nfinal = step()
+    for i in range(args.steps):
+        st, nfinal = step(keep=kept if i == args.steps - 1 else None)
         filt_ms.append(st["filter_ms"])
         launches += st["n_launches"]
     dev_ms = hs.timer_stop()
     wall_ms = (time.perf_counter() - t0) * 1e3
     sync_all()
+    if kept is not None:
+        out_dir = args.dump_outputs if world == 1 else os.path.join(args.dump_outputs, "rank%d" % rank)
+        dump_outputs(out_dir, final_columns(kept), seed)
     # the timed region of a default run lasts ~20 ms, shorter than one nvidia-smi sampling period: keep
     # the SAME searches running (untimed, same count on every rank) so the clock monitor sees the load
     soak = 0 if kind == "batch" else max(0, 400 - args.steps)
@@ -729,7 +779,6 @@ def main():
         secondary = run_secondary(F, hs, alphabet, seed, peak)  # (plants more patterns into hs: keep it last)
     filt = float(np.mean(filt_ms))
     achieved = (bhi - blo) / (filt * 1e-3) / 1e9 if filt > 0 else 0.0
-    traffic = ncu_traffic()
     line = {"metric": metric, "value": value, "unit": unit, "n_gpus": world, "steps": args.steps,
             "warmup": max(args.warmup, 3), "ms_per_step": ms_per_step, "higher_is_better": True,
             "scaling": "weak" if kind != "batch" else "strong", "vs_baseline": None, "dtype": "u8",
@@ -739,10 +788,7 @@ def main():
                                      "ham": "k_hamming_count"}.get(kind, "all scans of the batch")),
                          "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "peak_source": peak_src, "kernel_ms": filt,
-                         "algorithmic_bytes_per_launch": bhi - blo,
-                         "traffic": (traffic or {}).get("dram_bytes_per_launch") if (kind == "lev" and len(alphabet) > 16) else None,
-                         "traffic_source": "profiles/filter_traffic.json (ncu --set full capture of this kernel; a constant, not "
-                                           "measured in this run)"},
+                         "algorithmic_bytes_per_launch": bhi - blo},
             "clocks": clocks}
     if secondary is not None:
         line["secondary"] = secondary

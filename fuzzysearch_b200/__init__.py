@@ -1,4 +1,4 @@
-"""fuzzysearch_b200 -- B200-native (sm_100a CUDA) drop-in for fuzzysearch's near-match search.
+"""fuzzysearch_b200 -- H100-native (sm_90a CUDA) drop-in for fuzzysearch's near-match search.
 
 Same public API as the reference (fuzzysearch/__init__.py:35-83):
 

@@ -1,6 +1,6 @@
 // api.cu -- host side of libfuzzb200.so: the C-ABI declared in include/fuzzb200.h.
 //
-// No CPU search path exists in this file: every search launches the sm_100a kernels of kernels.cuh
+// No CPU search path exists in this file: every search launches the sm_90a kernels of kernels.cuh
 // and fails with FZB_E_CUDA when no device is usable.  The only host-side algorithm is the
 // O(N log N) consolidation of the (small) match list, which the reference also performs after its
 // search (common.py:185-189).
@@ -167,7 +167,7 @@ struct fzb_haystack {
     int64_t *h_send = nullptr, *h_recv = nullptr;  // pinned
     uint32_t gather_alloc = 0;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    int sm_count = 148;
+    int sm_count = 132;
     uint64_t *d_hits = nullptr;     // dense route: list of confirmed n-gram hits
     uint32_t hits_cap = 0;
     uint32_t *d_glist = nullptr;    // compacted list of marked granules
@@ -523,7 +523,7 @@ extern "C" uint64_t fzb_haystack_len(const fzb_haystack *h) {
 
 // ------------------------------------------------------------------------------------------------
 // Upload of PAGEABLE host memory (what a Python bytes object is).  cudaMemcpy from pageable memory stages through
-// the driver's own bounce buffer at 7-10 GB/s on these hosts; page-locking the caller's buffer in place
+// the driver's own bounce buffer, well below PCIe speed; page-locking the caller's buffer in place
 // (cudaHostRegister) costs more than the copy.  Instead: a ring of three 64 MiB pinned buffers; a small pool of
 // host threads copies slice i+1 of the caller's buffer into one of them while the DMA engine moves slice i
 // to the device -- the pipeline runs at min(host memcpy bandwidth of the pool, PCIe).
@@ -2549,7 +2549,7 @@ static int ham_counter_layout(int threshold) {  // (read per search: a probe can
     const char *e = getenv("FZB_HAM_COUNTERS");
     if (e && !strcmp(e, "nibble")) return 0;
     if (e && !strcmp(e, "sliced3")) return 1;
-    // measured on 4 GiB of DNA, m = 32, k = 3: 0.881 ms (three slices) vs 0.948 ms (nibble fields)
+    // fewer instructions per word: two slices where the threshold allows, else three (nibble fields: A/B only)
     return threshold <= 4 ? 2 : 1;
 }
 

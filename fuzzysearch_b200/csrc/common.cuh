@@ -1,4 +1,4 @@
-// common.cuh -- shared declarations for the libfuzzb200 kernels (sm_100a).
+// common.cuh -- shared declarations for the libfuzzb200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

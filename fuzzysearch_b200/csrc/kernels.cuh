@@ -1,4 +1,4 @@
-// kernels.cuh -- sm_100a kernels of libfuzzb200 (Levenshtein n-gram route, exact search, Hamming).
+// kernels.cuh -- sm_90a kernels of libfuzzb200 (Levenshtein n-gram route, exact search, Hamming).
 //
 // Pipeline of one n-gram search (DESIGN.md section 3):
 //   k_filter_sampled / k_filter_dense : ONE pass over the haystack (the HBM-bound kernel); marks

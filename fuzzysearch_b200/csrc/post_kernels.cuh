@@ -7,9 +7,9 @@
 //   every CTA  (one per SM) loads the packed canonical keys (start, end-start, dist; written by emit() next to each record) of ALL
 //              records into shared memory and ranks its slice of them against all of them (rank = number of
 //              smaller keys; a warp ranks two records per pass over the list), scatters its keys to their
-//              sorted positions in global memory and takes a ticket.  Measured alternatives for 7 K records:
-//              a single-SM bitonic network 60 us, a single-SM sample sort 38 us, this all-pairs ranking
-//              spread over 148 SMs 20 us -- one SM issues 4 warp-instructions per clock whatever the algorithm.
+//              sorted positions in global memory and takes a ticket.  The all-pairs ranking is spread over every
+//              SM rather than run as a single-SM bitonic network or sample sort: one SM issues 4
+//              warp-instructions per clock whatever the algorithm.
 //   the last   CTA to finish (ticket == grid-1) runs consolidate_overlapping_matches (common.py:145-189) on
 //              the sorted keys, one element per thread per round (bank-conflict free): running maximum of
 //              `end` as the hull, a record opens a new group iff start >= hull (connected components of

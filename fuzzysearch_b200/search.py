@@ -3,7 +3,7 @@
 ``fuzzysearch.choose_search_class`` (__init__.py:60-83) picks one of ExactSearch /
 SubstitutionsOnlySearch / LevenshteinSearch / GenericSearch, each a ``FuzzySearchBase`` with
 ``search(subsequence, sequence, search_params)`` and ``consolidate_matches(matches)``
-(common.py:192-209).  Here each ``search`` is ONE call into libfuzzb200.so (sm_100a kernels);
+(common.py:192-209).  Here each ``search`` is ONE call into libfuzzb200.so (sm_90a kernels);
 there is no CPU implementation behind them.
 """
 import threading

@@ -1,5 +1,5 @@
 /*
- * fuzzb200.h -- C-ABI of libfuzzb200.so: the B200-native (sm_100a) replacement for the
+ * fuzzb200.h -- C-ABI of libfuzzb200.so: the H100-native (sm_90a) replacement for the
  * fuzzysearch hot path (bounded-Levenshtein / Hamming / generic near-match search of a short
  * byte pattern in a long byte haystack).
  *

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on a machine with an H100)")
 
 
 def load_emulated_library():
@@ -32,7 +32,7 @@ def load_emulated_library():
 
 def pytest_sessionstart(session):
     # FZB_TEST_BACKEND=emu python -m pytest tests -m gpu : replay the GPU parity tests on the CPU emulator
-    # (developer tool for boxes without a GPU; sizes that need a real B200 are skipped by the tests themselves)
+    # (developer tool for boxes without a GPU; sizes that need a real GPU are skipped by the tests themselves)
     if os.environ.get("FZB_TEST_BACKEND") == "emu":
         from fuzzysearch_b200 import _native
         _native._lib = load_emulated_library()
@@ -50,7 +50,7 @@ def needs_real_gpu(what):
     """For the handful of gpu tests the CPU emulator cannot stand in for (FZB_TEST_BACKEND=emu replays): NCCL,
     CUDA IPC between processes, 4 GiB inputs."""
     if os.environ.get("FZB_TEST_BACKEND") == "emu":
-        pytest.skip("needs a real B200: " + what)
+        pytest.skip("needs a real GPU: " + what)
 
 
 @pytest.fixture(scope="session")

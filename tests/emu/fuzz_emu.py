@@ -2,7 +2,7 @@
 
     python tests/emu/fuzz_emu.py --seed 1 --trials 400 [--routes world,lev,ham,generic,exact,shard,batch,has]
 
-Far more geometry than the `-m gpu` suite can afford on a B200 budget: tiny and empty sequences, every pattern
+Far more geometry than the `-m gpu` suite can afford on a GPU budget: tiny and empty sequences, every pattern
 length, forced filters, capped work lists (overflow paths), shards with arbitrary seams, grid sizes (FZB_EMU_SMS),
 all three Hamming counter layouts.  Every mismatch prints a reproducer line and the run exits non-zero.
 """

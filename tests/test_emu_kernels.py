@@ -6,7 +6,7 @@ tests/emu/_build/libfuzzb200_emu.so with the same C-ABI.  The tests below bind i
 the bodies of the `-m gpu` parity tests (same functions, same oracle, same fixtures) at the sizes a CPU can do in
 seconds.  It proves kernel LOGIC and host logic -- filters lose no match, work lists and overflow paths, bit-parallel
 expansions, consolidation, batches, wide symbols, file loops, locking, the peer-memory reduction of in-process
-multi-shard worlds -- not timing, memory-model behaviour, CUDA IPC or NCCL (those need the B200:
+multi-shard worlds -- not timing, memory-model behaviour, CUDA IPC or NCCL (those need a real GPU:
 tests/test_gpu_global.py, bench.py).  The emulated library is test
 infrastructure: nothing in the product can load it.
 

@@ -1,6 +1,6 @@
-"""One invocation of every hot kernel on the 4 GiB workloads, for ncu (see profiles/README.md):
+"""One invocation of every hot kernel on the 4 GiB workloads, for ncu:
    ncu --set full --clock-control none --import-source on -k regex:'k_(filter|verify|post|hamming|lp_|merge|push)' \
-       -o gpurun_out/r02_all python tools/profile_all.py"""
+       -o profiles/all_kernels python tools/profile_all.py"""
 import os
 import sys
 

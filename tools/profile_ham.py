@@ -1,6 +1,6 @@
 """One Hamming search of 4 GiB of DNA (configs[2]) for ncu:
    ncu --set full --clock-control none --import-source on -k regex:k_hamming_count -c 1 \
-       -o gpurun_out/r02_ham_sliced python tools/profile_ham.py"""
+       -o profiles/ham_sliced python tools/profile_ham.py"""
 import os
 import sys
 

@@ -1,5 +1,5 @@
-"""Per-kernel SASS opcode histogram of the shipped library (-> profiles/r02_sass_opcodes.txt):
-   python tools/sass_histogram.py > profiles/r02_sass_opcodes.txt"""
+"""Per-kernel SASS opcode histogram of the shipped library:
+   mkdir -p profiles && python tools/sass_histogram.py > profiles/sass_opcodes.txt"""
 import collections
 import os
 import re
@@ -20,7 +20,7 @@ for line in out.splitlines():
     m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)", line)
     if m and cur is not None:
         cur[m.group(1)] += 1
-print("SASS opcode histogram of fuzzysearch_b200/libfuzzb200.so (cuobjdump -sass, sm_100a), per kernel.")
+print("SASS opcode histogram of fuzzysearch_b200/libfuzzb200.so (cuobjdump -sass, sm_90a), per kernel.")
 print("UTMALDG / SYNCS.ARRIVE.TRANS64 = TMA (cp.async.bulk.tensor) + mbarrier; LDG.E.128 = coalesced uint4 streaming loads.")
 print()
 for name, ops in kernels.items():
