@@ -199,6 +199,7 @@ struct fzb_result {
     fzb_haystack *owner = nullptr;  // non-null while raw records / global rows still sit in the owner's mapped buffers
     bool raw_in_stage = false;
     void fetch_raw();
+    void discard_attempt();
     std::vector<RawRec> fin;
     std::vector<int64_t> hulls;  // (hull_start, hull_end) of the group behind each final match
     bool unconsolidated = false;  // exact / Hamming routes: FINAL is the whole raw list in (start, end, dist) order
@@ -217,6 +218,16 @@ struct fzb_result {
 };
 
 static uint64_t round_up(uint64_t x, uint64_t a) { return (x + a - 1) / a * a; }
+
+static RawRec make_rec(int64_t start, int64_t end, int64_t dist) {  // a match without an anchor
+    RawRec r;
+    r.start = start;
+    r.end = end;
+    r.dist = (int32_t)dist;
+    r.idx = -1;
+    r.ngram = -1;
+    return r;
+}
 
 // Every entry point that touches a handle's device state (buffer, counters, output area, stream order) holds the
 // handle's mutex for the whole call: two threads sharing one resident sequence take turns, like callers of the
@@ -261,16 +272,19 @@ void fzb_result::fetch_raw() {
         gfin.resize(gcount);
         for (uint32_t i = 0; i < gcount; i++) {
             const int64_t s0 = owner->h_grows[2 * (size_t)i], v = owner->h_grows[2 * (size_t)i + 1];
-            gfin[i].start = s0;
-            gfin[i].end = s0 + (v >> 32);
-            gfin[i].dist = (int32_t)(v & 0xFFFFFFFF);
-            gfin[i].idx = -1;
-            gfin[i].ngram = -1;
+            gfin[i] = make_rec(s0, s0 + (v >> 32), v & 0xFFFFFFFF);
         }
         global_on_device = false;
     }
     owner->pending = nullptr;
     owner = nullptr;
+}
+
+void fzb_result::discard_attempt() {  // a search attempt that has to be redone: unlink and drop its matches
+    fetch_raw();
+    raw.clear();
+    raw_n = 0;
+    fin.clear();
 }
 
 static void detach_pending(fzb_haystack *h) {  // before h->d_out / h->h_grows are overwritten or freed
@@ -319,7 +333,6 @@ static int check_shard(uint64_t buf_len, uint64_t buf_lo, uint64_t global_len, u
 }
 
 static int alloc_buffer(fzb_haystack *h) {
-    h->padded_len = round_up(h->buf_len, 128) + 128;
     CK(cudaSetDevice(h->device));
     CK(cudaMalloc(&h->d, h->padded_len));
     h->capacity = h->padded_len;
@@ -372,12 +385,15 @@ extern "C" void fzb_haystack_destroy(fzb_haystack *h) {
     delete h;
 }
 
-extern "C" int fzb_haystack_create_shard(const uint8_t *host, uint64_t buf_len, uint64_t buf_lo,
-                                         uint64_t global_len, uint64_t own_lo, uint64_t own_hi,
-                                         int device, fzb_haystack **out) {
+// The constructors' common part.  `arg_error`: the caller's own argument check failed (reported after the `out`
+// check).  `dev_ptr` non-null adopts that caller-owned buffer, otherwise the handle allocates its own and uploads
+// `host` into it, if given.
+static int haystack_new(const char *arg_error, const uint8_t *host, const void *dev_ptr, uint64_t buf_len,
+                        uint64_t buf_lo, uint64_t global_len, uint64_t own_lo, uint64_t own_hi, int device,
+                        fzb_haystack **out) {
     if (!out) return fail(FZB_E_INVALID, "out is NULL");
     *out = nullptr;
-    if (!host && buf_len) return fail(FZB_E_INVALID, "host buffer is NULL");
+    if (arg_error) return fail(FZB_E_INVALID, "%s", arg_error);
     int rc = check_shard(buf_len, buf_lo, global_len, own_lo, own_hi);
     if (rc) return rc;
     if (fzb_device_count() <= device || device < 0)
@@ -385,20 +401,30 @@ extern "C" int fzb_haystack_create_shard(const uint8_t *host, uint64_t buf_len, 
     fzb_haystack *h = new (std::nothrow) fzb_haystack();
     if (!h) return fail(FZB_E_CUDA, "out of host memory");
     h->device = device;
+    h->owned = !dev_ptr;
+    h->d = (uint8_t *)dev_ptr;
     h->buf_len = buf_len;
     h->buf_lo = buf_lo;
     h->global_len = global_len;
     h->own_lo = own_lo;
     h->own_hi = own_hi;
-    rc = alloc_buffer(h);
+    h->padded_len = round_up(buf_len, 128) + 128;
+    rc = h->owned ? alloc_buffer(h) : FZB_OK;
     if (rc == FZB_OK) rc = haystack_common_init(h);
-    if (rc == FZB_OK && buf_len) rc = upload_bytes(h, 0, host, buf_len);
+    if (rc == FZB_OK && host) rc = upload_bytes(h, 0, host, buf_len);
     if (rc) {
         fzb_haystack_destroy(h);
         return rc;
     }
     *out = h;
     return FZB_OK;
+}
+
+extern "C" int fzb_haystack_create_shard(const uint8_t *host, uint64_t buf_len, uint64_t buf_lo,
+                                         uint64_t global_len, uint64_t own_lo, uint64_t own_hi,
+                                         int device, fzb_haystack **out) {
+    return haystack_new(!host && buf_len ? "host buffer is NULL" : nullptr, host, nullptr, buf_len, buf_lo,
+                        global_len, own_lo, own_hi, device, out);
 }
 
 extern "C" int fzb_haystack_create(const uint8_t *host, uint64_t n, int device, fzb_haystack **out) {
@@ -408,56 +434,15 @@ extern "C" int fzb_haystack_create(const uint8_t *host, uint64_t n, int device, 
 extern "C" int fzb_haystack_adopt_device(const void *dev_ptr, uint64_t buf_len, uint64_t buf_lo,
                                          uint64_t global_len, uint64_t own_lo, uint64_t own_hi,
                                          int device, fzb_haystack **out) {
-    if (!out) return fail(FZB_E_INVALID, "out is NULL");
-    *out = nullptr;
-    if (!dev_ptr || ((uintptr_t)dev_ptr & 15)) return fail(FZB_E_INVALID, "dev_ptr must be 16-byte aligned");
-    int rc = check_shard(buf_len, buf_lo, global_len, own_lo, own_hi);
-    if (rc) return rc;
-    if (fzb_device_count() <= device || device < 0) return fail(FZB_E_CUDA, "CUDA device %d not available", device);
-    fzb_haystack *h = new (std::nothrow) fzb_haystack();
-    if (!h) return fail(FZB_E_CUDA, "out of host memory");
-    h->device = device;
-    h->owned = false;
-    h->d = (uint8_t *)dev_ptr;
-    h->buf_len = buf_len;
-    h->buf_lo = buf_lo;
-    h->global_len = global_len;
-    h->own_lo = own_lo;
-    h->own_hi = own_hi;
-    h->padded_len = round_up(buf_len, 128) + 128;
-    rc = haystack_common_init(h);
-    if (rc) {
-        fzb_haystack_destroy(h);
-        return rc;
-    }
-    *out = h;
-    return FZB_OK;
+    return haystack_new(!dev_ptr || ((uintptr_t)dev_ptr & 15) ? "dev_ptr must be 16-byte aligned" : nullptr, nullptr,
+                        dev_ptr, buf_len, buf_lo, global_len, own_lo, own_hi, device, out);
 }
 
 extern "C" int fzb_haystack_alloc(uint64_t buf_len, uint64_t buf_lo, uint64_t global_len, uint64_t own_lo,
                                   uint64_t own_hi, int device, fzb_haystack **out, void **dev_ptr) {
-    if (!out) return fail(FZB_E_INVALID, "out is NULL");
-    *out = nullptr;
-    int rc = check_shard(buf_len, buf_lo, global_len, own_lo, own_hi);
-    if (rc) return rc;
-    if (fzb_device_count() <= device || device < 0) return fail(FZB_E_CUDA, "CUDA device %d not available", device);
-    fzb_haystack *h = new (std::nothrow) fzb_haystack();
-    if (!h) return fail(FZB_E_CUDA, "out of host memory");
-    h->device = device;
-    h->buf_len = buf_len;
-    h->buf_lo = buf_lo;
-    h->global_len = global_len;
-    h->own_lo = own_lo;
-    h->own_hi = own_hi;
-    rc = alloc_buffer(h);
-    if (rc == FZB_OK) rc = haystack_common_init(h);
-    if (rc) {
-        fzb_haystack_destroy(h);
-        return rc;
-    }
-    if (dev_ptr) *dev_ptr = h->d;
-    *out = h;
-    return FZB_OK;
+    const int rc = haystack_new(nullptr, nullptr, nullptr, buf_len, buf_lo, global_len, own_lo, own_hi, device, out);
+    if (rc == FZB_OK && dev_ptr) *dev_ptr = (*out)->d;
+    return rc;
 }
 
 extern "C" void fzb_synth_host(uint8_t *dst, uint64_t global_offset, uint64_t n, const uint8_t *alphabet,
@@ -645,14 +630,18 @@ static int upload_bytes(fzb_haystack *h, uint64_t dst_off, const uint8_t *host, 
     return rc;
 }
 
+// The handle holds a whole sequence, not a shard of a longer one.
+static bool is_whole_sequence(const fzb_haystack *h) {
+    return h->buf_lo == 0 && h->global_len == h->buf_len && h->own_lo == 0 && h->own_hi == h->buf_len;
+}
+
 extern "C" int fzb_haystack_upload(fzb_haystack *h, const uint8_t *host, uint64_t n) {
     HandleLock handle_lock(h);
     if (!h || (!host && n)) return fail(FZB_E_INVALID, "bad arguments");
     if (!h->owned) return fail(FZB_E_INVALID, "upload needs an owned handle");
     if (round_up(n, 128) + 128 > h->capacity) return fail(FZB_E_INVALID, "upload larger than the handle's capacity");
     CK(cudaSetDevice(h->device));
-    const bool shard = h->buf_lo != 0 || h->global_len != h->buf_len || h->own_lo != 0 || h->own_hi != h->buf_len;
-    if (shard) {  // a shard keeps its geometry: the new bytes replace the same window of the global sequence
+    if (!is_whole_sequence(h)) {  // a shard keeps its geometry: the new bytes replace the same window of the global sequence
         if (n != h->buf_len) return fail(FZB_E_INVALID, "a shard upload must supply exactly buf_len bytes");
     } else {
         h->buf_len = h->global_len = h->own_hi = n;
@@ -676,8 +665,7 @@ extern "C" int fzb_haystack_upload_symbols(fzb_haystack *h, const void *host, ui
         if (alphabet[i - 1] >= alphabet[i]) return fail(FZB_E_INVALID, "the alphabet must be strictly ascending");
     if (!h->owned) return fail(FZB_E_INVALID, "upload needs an owned handle");
     if (round_up(n, 128) + 128 > h->capacity) return fail(FZB_E_INVALID, "upload larger than the handle's capacity");
-    if (h->buf_lo != 0 || h->global_len != h->buf_len || h->own_lo != 0 || h->own_hi != h->buf_len)
-        return fail(FZB_E_INVALID, "symbol uploads replace a whole (unsharded) sequence");
+    if (!is_whole_sequence(h)) return fail(FZB_E_INVALID, "symbol uploads replace a whole (unsharded) sequence");
     CK(cudaSetDevice(h->device));
     h->buf_len = h->global_len = h->own_hi = n;
     h->padded_len = round_up(n, 128) + 128;
@@ -810,12 +798,16 @@ static int p2p_alloc(fzb_haystack *h) {
     return FZB_OK;
 }
 
-static void p2p_free(fzb_haystack *h) {
+static void close_peers(fzb_haystack *h) {
     for (int r = 0; r < kMaxWorld; r++) {
         if (h->peer_opened[r] && h->peer_base[r]) cudaIpcCloseMemHandle(h->peer_base[r]);
         h->peer_opened[r] = false;
         h->peer_base[r] = nullptr;
     }
+}
+
+static void p2p_free(fzb_haystack *h) {
+    close_peers(h);
     if (h->d_p2p) cudaFree(h->d_p2p);
     if (h->d_ms) cudaFree(h->d_ms);
     if (h->d_mscore) cudaFree(h->d_mscore);
@@ -831,22 +823,27 @@ static void p2p_free(fzb_haystack *h) {
     h->p2p = false;
 }
 
+// Leaves the handle's current world (communicator, peer memory) and makes it rank `rank` of a new one.
+static void reset_world(fzb_haystack *h, int rank, int world_size, bool local_world) {
+    if (h->comm) nccl_comm_destroy(h->comm);
+    h->comm = nullptr;
+    p2p_free(h);
+    h->rank = rank;
+    h->world = world_size;
+    h->epoch = 0;
+    h->local_world = local_world;
+}
+
 extern "C" int fzb_haystack_comm_init(fzb_haystack *h, const uint8_t id[FZB_NCCL_ID_BYTES], int rank,
                                       int world_size) {
     if (!h || !id || world_size < 1 || rank < 0 || rank >= world_size) return fail(FZB_E_INVALID, "bad arguments");
     int rc = nccl_load();
     if (rc) return rc;
     CK(cudaSetDevice(h->device));
-    if (h->comm) nccl_comm_destroy(h->comm);
-    h->comm = nullptr;
-    p2p_free(h);
-    h->local_world = false;
+    reset_world(h, rank, world_size, false);
     NcclId nid;
     memcpy(nid.b, id, FZB_NCCL_ID_BYTES);
     NCCLCK(g_nccl.CommInitRank(&h->comm, world_size, nid, rank));
-    h->rank = rank;
-    h->world = world_size;
-    h->epoch = 0;
     rc = ensure_gather_buffers(h, h->gather_cap);
     if (rc) return rc;
     // Peer-memory world: every rank exports its receive area through CUDA IPC; the handles travel over the
@@ -903,13 +900,7 @@ extern "C" int fzb_haystack_comm_init(fzb_haystack *h, const uint8_t id[FZB_NCCL
     if (rc) return rc;
     for (int r = 0; r < world_size; r++) ok = ok && reinterpret_cast<Hello *>(all.data() + rec * r)->ok;
     h->p2p = ok;
-    if (!ok) {
-        for (int r = 0; r < kMaxWorld; r++) {
-            if (h->peer_opened[r] && h->peer_base[r]) cudaIpcCloseMemHandle(h->peer_base[r]);
-            h->peer_opened[r] = false;
-            h->peer_base[r] = nullptr;
-        }
-    }
+    if (!ok) close_peers(h);
     return FZB_OK;
 }
 
@@ -919,13 +910,7 @@ extern "C" int fzb_comm_init_local(fzb_haystack **handles, int world_size) {
         if (!handles[r]) return fail(FZB_E_INVALID, "NULL handle");
     for (int r = 0; r < world_size; r++) {
         fzb_haystack *h = handles[r];
-        if (h->comm) nccl_comm_destroy(h->comm);
-        h->comm = nullptr;
-        p2p_free(h);
-        h->rank = r;
-        h->world = world_size;
-        h->epoch = 0;
-        h->local_world = true;
+        reset_world(h, r, world_size, true);
         int rc = p2p_alloc(h);
         if (rc) return rc;
     }
@@ -958,13 +943,7 @@ extern "C" int fzb_p2p_export(fzb_haystack *h, int rank, int world_size, uint8_t
         return fail(FZB_E_INVALID, "bad arguments");
     static_assert(sizeof(cudaIpcMemHandle_t) == FZB_IPC_HANDLE_BYTES, "IPC handle size");
     CK(cudaSetDevice(h->device));
-    if (h->comm) nccl_comm_destroy(h->comm);
-    h->comm = nullptr;
-    p2p_free(h);
-    h->rank = rank;
-    h->world = world_size;
-    h->epoch = 0;
-    h->local_world = false;
+    reset_world(h, rank, world_size, false);
     int rc = p2p_alloc(h);
     if (rc) return rc;
     cudaIpcMemHandle_t mine;
@@ -987,11 +966,7 @@ extern "C" int fzb_p2p_connect(fzb_haystack *h, const uint8_t *handles) {
         const cudaError_t e = cudaIpcOpenMemHandle(&ptr, peer, cudaIpcMemLazyEnablePeerAccess);
         if (e != cudaSuccess) {
             cudaGetLastError();
-            for (int q = 0; q < kMaxWorld; q++) {
-                if (h->peer_opened[q] && h->peer_base[q]) cudaIpcCloseMemHandle(h->peer_base[q]);
-                h->peer_opened[q] = false;
-                h->peer_base[q] = nullptr;
-            }
+            close_peers(h);
             return fail(FZB_E_CUDA, "cudaIpcOpenMemHandle(rank %d) failed: %s", r, cudaGetErrorString(e));
         }
         h->peer_base[r] = (uint8_t *)ptr;
@@ -1014,61 +989,108 @@ extern "C" int fzb_haystack_p2p_enabled(const fzb_haystack *h) { return h && h->
 // group iff start < hull_end (this also reproduces the reference for empty matches, which never
 // overlap anything they merely touch).  Winner = min (dist, -(end-start)), ties -> smallest
 // (start,end).  Output sorted by (start,end,dist).
+//
+// The sweep runs over GROUPS: a winner (start, end, dist) and the hull [hull_start, hull_end) of its members.  A raw
+// match is a group of its own, whose hull is the match.  Groups of different shards that overlap belong to one
+// global group (a group's hull is covered by its members, so hulls overlap iff members do), and the winner of a
+// union is the better of the two winners -- so the global consolidate_overlapping_matches (common.py:185-189) is
+// the same sweep run over the per-shard groups instead of the raw matches.
 // ------------------------------------------------------------------------------------------------
-static void consolidate_recs(std::vector<RawRec> v, std::vector<RawRec> &out, std::vector<int64_t> *hulls = nullptr) {
+struct GroupRow {
+    int64_t s, e, d, hs, he;
+};
+
+static bool group_less(const GroupRow &a, const GroupRow &b) {
+    if (a.hs != b.hs) return a.hs < b.hs;
+    if (a.he != b.he) return a.he < b.he;
+    if (a.s != b.s) return a.s < b.s;
+    if (a.e != b.e) return a.e < b.e;
+    return a.d < b.d;
+}
+
+// `g` sorted by group_less.  Winners come out in group order, which is already (start, end, dist) order: groups
+// are disjoint and ordered, and an empty group at x sorts before a group starting at x.
+static void sweep_groups(const std::vector<GroupRow> &g, std::vector<RawRec> &out, std::vector<int64_t> *hulls = nullptr) {
+    auto better = [](const GroupRow &a, const GroupRow &b) {  // a strictly better than b
+        if (a.d != b.d) return a.d < b.d;
+        int64_t la = a.e - a.s, lb = b.e - b.s;
+        if (la != lb) return la > lb;
+        if (a.s != b.s) return a.s < b.s;
+        return a.e < b.e;
+    };
     out.clear();
     if (hulls) hulls->clear();
-    if (v.empty()) return;
-    auto canonical = [](const RawRec &a, const RawRec &b) {
-        if (a.start != b.start) return a.start < b.start;
-        if (a.end != b.end) return a.end < b.end;
-        return a.dist < b.dist;
-    };
-    std::sort(v.begin(), v.end(), canonical);
-    RawRec best = v[0];
-    int64_t hull_start = v[0].start, hull_end = v[0].end;
-    auto better = [](const RawRec &a, const RawRec &b) {  // a strictly better than b
-        if (a.dist != b.dist) return a.dist < b.dist;
-        int64_t la = a.end - a.start, lb = b.end - b.start;
-        if (la != lb) return la > lb;
-        if (a.start != b.start) return a.start < b.start;
-        return a.end < b.end;
-    };
-    auto close_group = [&]() {
-        out.push_back(best);
+    for (size_t i = 0, j; i < g.size(); i = j) {
+        GroupRow best = g[i];
+        int64_t hull_end = g[i].he;
+        for (j = i + 1; j < g.size() && g[j].hs < hull_end; j++) {
+            if (better(g[j], best)) best = g[j];
+            hull_end = std::max(hull_end, g[j].he);
+        }
+        out.push_back(make_rec(best.s, best.e, best.d));
         if (hulls) {
-            hulls->push_back(hull_start);
+            hulls->push_back(g[i].hs);
             hulls->push_back(hull_end);
         }
-    };
-    for (size_t i = 1; i < v.size(); i++) {
-        if (v[i].start < hull_end) {
-            if (better(v[i], best)) best = v[i];
-            hull_end = std::max(hull_end, v[i].end);
-        } else {
-            close_group();
-            best = v[i];
-            hull_start = v[i].start;
-            hull_end = v[i].end;
+    }
+}
+
+static GroupRow match_row(int64_t start, int64_t end, int64_t dist) { return GroupRow{start, end, dist, start, end}; }
+
+static void consolidate_recs(const std::vector<RawRec> &v, std::vector<RawRec> &out,
+                             std::vector<int64_t> *hulls = nullptr) {
+    std::vector<GroupRow> g;
+    g.reserve(v.size());
+    for (const RawRec &r : v) g.push_back(match_row(r.start, r.end, r.dist));
+    std::sort(g.begin(), g.end(), group_less);
+    sweep_groups(g, out, hulls);
+}
+
+static std::vector<GroupRow> match_rows(const int64_t *start, const int64_t *end, const int32_t *dist, uint64_t n) {
+    std::vector<GroupRow> g(n);
+    for (uint64_t i = 0; i < n; i++) g[i] = match_row(start[i], end[i], dist[i]);
+    std::sort(g.begin(), g.end(), group_less);
+    return g;
+}
+
+// Group rows (kFinCols columns) that arrive as one run of counts[r] rows per shard, in shard order, sorted for the
+// sweep.  Every run is sorted by hull start and runs only interleave within a halo of their seams, so instead of
+// sorting, each seam is fixed with an inplace_merge of the few out-of-order rows around it.
+static std::vector<GroupRow> read_group_runs(const int64_t *rows, const std::vector<uint64_t> &counts) {
+    uint64_t n = 0;
+    for (uint64_t c : counts) n += c;
+    std::vector<GroupRow> g;
+    g.reserve(n);
+    for (uint64_t c : counts) {
+        const size_t seam = g.size();
+        for (uint64_t i = 0; i < c; i++, rows += kFinCols) g.push_back(GroupRow{rows[0], rows[1], rows[2], rows[3], rows[4]});
+        if (!std::is_sorted(g.begin() + seam, g.end(), group_less)) std::sort(g.begin() + seam, g.end(), group_less);  // defensive
+        if (seam > 0 && seam < g.size() && group_less(g[seam], g[seam - 1])) {
+            auto lo = std::upper_bound(g.begin(), g.begin() + seam, g[seam], group_less);
+            auto hi = std::lower_bound(g.begin() + seam, g.end(), g[seam - 1], group_less);
+            std::inplace_merge(lo, g.begin() + seam, hi, group_less);
         }
     }
-    close_group();
-    // winners come out in group order, which is already (start, end, dist) order: groups are
-    // disjoint and ordered, and an empty group at x sorts before a group starting at x
+    if (!std::is_sorted(g.begin(), g.end(), group_less)) std::sort(g.begin(), g.end(), group_less);  // shards smaller than a halo
+    return g;
+}
+
+// The first n final matches and their hulls as group rows (start, end, dist, hull_start, hull_end).
+static void write_group_rows(const std::vector<RawRec> &fin, const std::vector<int64_t> &hulls, size_t n, int64_t *rows) {
+    for (size_t i = 0; i < n; i++, rows += kFinCols) {
+        rows[0] = fin[i].start;
+        rows[1] = fin[i].end;
+        rows[2] = fin[i].dist;
+        rows[3] = hulls[2 * i];
+        rows[4] = hulls[2 * i + 1];
+    }
 }
 
 extern "C" int64_t fzb_consolidate(const int64_t *start, const int64_t *end, const int32_t *dist, uint64_t n,
                                    int64_t *out_start, int64_t *out_end, int32_t *out_dist) {
     if (n && (!start || !end || !dist)) return fail(FZB_E_INVALID, "NULL input");
-    std::vector<RawRec> v(n), o;
-    for (uint64_t i = 0; i < n; i++) {
-        v[i].start = start[i];
-        v[i].end = end[i];
-        v[i].dist = dist[i];
-        v[i].idx = -1;
-        v[i].ngram = -1;
-    }
-    consolidate_recs(std::move(v), o);
+    std::vector<RawRec> o;
+    sweep_groups(match_rows(start, end, dist, n), o);
     for (size_t i = 0; i < o.size(); i++) {
         if (out_start) out_start[i] = o[i].start;
         if (out_end) out_end[i] = o[i].end;
@@ -1080,40 +1102,19 @@ extern "C" int64_t fzb_consolidate(const int64_t *start, const int64_t *end, con
 extern "C" int64_t fzb_consolidate_groups(const int64_t *start, const int64_t *end, const int32_t *dist, uint64_t n,
                                           int64_t *out_rows) {
     if (n && (!start || !end || !dist || !out_rows)) return fail(FZB_E_INVALID, "NULL input");
-    std::vector<RawRec> v(n), o;
+    std::vector<RawRec> o;
     std::vector<int64_t> hulls;
-    for (uint64_t i = 0; i < n; i++) {
-        v[i].start = start[i];
-        v[i].end = end[i];
-        v[i].dist = dist[i];
-        v[i].idx = -1;
-        v[i].ngram = -1;
-    }
-    consolidate_recs(std::move(v), o, &hulls);
-    for (size_t i = 0; i < o.size(); i++) {
-        out_rows[5 * i + 0] = o[i].start;
-        out_rows[5 * i + 1] = o[i].end;
-        out_rows[5 * i + 2] = o[i].dist;
-        out_rows[5 * i + 3] = hulls[2 * i];
-        out_rows[5 * i + 4] = hulls[2 * i + 1];
-    }
+    sweep_groups(match_rows(start, end, dist, n), o, &hulls);
+    write_group_rows(o, hulls, o.size(), out_rows);
     return (int64_t)o.size();
 }
 
 extern "C" int64_t fzb_result_group_rows(const fzb_result *r, int64_t *rows, uint64_t max_rows) {
     if (!r || (!rows && max_rows)) return fail(FZB_E_INVALID, "NULL argument");
-    const std::vector<RawRec> &v = r->fin;
-    if (!r->have_fin || r->hulls.size() != v.size() * 2)
+    if (!r->have_fin || r->hulls.size() != r->fin.size() * 2)
         return fail(FZB_E_INVALID, "result was produced with FZB_F_NO_FINAL");
-    const size_t n = std::min<size_t>(v.size(), max_rows);
-    for (size_t i = 0; i < n; i++) {
-        rows[5 * i + 0] = v[i].start;
-        rows[5 * i + 1] = v[i].end;
-        rows[5 * i + 2] = v[i].dist;
-        rows[5 * i + 3] = r->hulls[2 * i];
-        rows[5 * i + 4] = r->hulls[2 * i + 1];
-    }
-    return (int64_t)v.size();
+    write_group_rows(r->fin, r->hulls, std::min<size_t>(r->fin.size(), max_rows), rows);
+    return (int64_t)r->fin.size();
 }
 
 extern "C" int fzb_result_hulls(const fzb_result *r, int64_t *hull_start, int64_t *hull_end) {
@@ -1128,85 +1129,13 @@ extern "C" int fzb_result_hulls(const fzb_result *r, int64_t *hull_start, int64_
     return FZB_OK;
 }
 
-// Merge per-shard consolidated lists.  Each input row is one GROUP of overlapping matches found by a
-// shard: its winner (start, end, dist) and the group's hull [hull_start, hull_end).  Groups of
-// different shards that overlap belong to one global group (a group's hull is covered by its
-// members, so hulls overlap iff members do), and the winner of a union is the better of the two
-// winners -- so the global consolidate_overlapping_matches (common.py:185-189) is the same sweep run
-// over the groups instead of the raw matches.
-// Global consolidation over per-shard groups.  `runs` = (pointer, count) of each shard's rows, in shard
-// order; every run is sorted by hull start and runs only interleave within a halo of their seams, so
-// instead of sorting, each seam is fixed with an inplace_merge of the few out-of-order rows around it.
-struct GroupRow {
-    int64_t s, e, d, hs, he;
-};
-
-static void merge_group_runs(const std::vector<std::pair<const int64_t *, uint64_t>> &runs, std::vector<RawRec> &out) {
-    uint64_t n = 0;
-    for (auto &r : runs) n += r.second;
-    std::vector<GroupRow> g;
-    g.reserve(n);
-    auto less = [](const GroupRow &a, const GroupRow &b) {
-        if (a.hs != b.hs) return a.hs < b.hs;
-        if (a.he != b.he) return a.he < b.he;
-        if (a.s != b.s) return a.s < b.s;
-        if (a.e != b.e) return a.e < b.e;
-        return a.d < b.d;
-    };
-    for (auto &r : runs) {
-        const size_t seam = g.size();
-        for (uint64_t i = 0; i < r.second; i++) {
-            const int64_t *q = r.first + 5 * i;
-            g.push_back(GroupRow{q[0], q[1], q[2], q[3], q[4]});
-        }
-        if (!std::is_sorted(g.begin() + seam, g.end(), less)) std::sort(g.begin() + seam, g.end(), less);  // defensive
-        if (seam > 0 && seam < g.size() && less(g[seam], g[seam - 1])) {
-            auto lo = std::upper_bound(g.begin(), g.begin() + seam, g[seam], less);
-            auto hi = std::lower_bound(g.begin() + seam, g.end(), g[seam - 1], less);
-            std::inplace_merge(lo, g.begin() + seam, hi, less);
-        }
-    }
-    if (!std::is_sorted(g.begin(), g.end(), less)) std::sort(g.begin(), g.end(), less);  // shards smaller than a halo
-    auto better = [](const GroupRow &a, const GroupRow &b) {
-        if (a.d != b.d) return a.d < b.d;
-        int64_t la = a.e - a.s, lb = b.e - b.s;
-        if (la != lb) return la > lb;
-        if (a.s != b.s) return a.s < b.s;
-        return a.e < b.e;
-    };
-    out.clear();
-    out.reserve(n);
-    for (uint64_t i = 0; i < n;) {
-        GroupRow best = g[i];
-        int64_t hull_end = g[i].he;
-        uint64_t j = i + 1;
-        while (j < n && g[j].hs < hull_end) {
-            if (better(g[j], best)) best = g[j];
-            hull_end = std::max(hull_end, g[j].he);
-            j++;
-        }
-        RawRec r;
-        r.start = best.s;
-        r.end = best.e;
-        r.dist = (int32_t)best.d;
-        r.idx = -1;
-        r.ngram = -1;
-        out.push_back(r);
-        i = j;
-    }
-}
-
-static void merge_group_rows(const int64_t *rows, uint64_t n, std::vector<RawRec> &out) {
-    // one run per maximal sorted stretch is not known here: treat the input as a single run (sorted if needed)
-    std::vector<std::pair<const int64_t *, uint64_t>> runs{{rows, n}};
-    merge_group_runs(runs, out);
-}
-
+// Merge per-shard consolidated lists (group rows).  Where the shards' runs begin is not known here: the input is
+// treated as a single run, sorted if needed.
 extern "C" int64_t fzb_merge_groups(const int64_t *rows, uint64_t n, int64_t *out_start, int64_t *out_end,
                                     int32_t *out_dist) {
     if (n && !rows) return fail(FZB_E_INVALID, "NULL input");
     std::vector<RawRec> o;
-    merge_group_rows(rows, n, o);
+    sweep_groups(read_group_runs(rows, {n}), o);
     for (size_t i = 0; i < o.size(); i++) {
         if (out_start) out_start[i] = o[i].start;
         if (out_end) out_end[i] = o[i].end;
@@ -1416,11 +1345,7 @@ static int run_emitting(fzb_haystack *h, fzb_result *res, F enqueue, PostPlan po
                 res->fin.resize(nf);
                 res->hulls.resize((size_t)nf * 2);
                 for (uint32_t i = 0; i < nf; i++) {
-                    res->fin[i].start = h->h_fin[kFinCols * i];
-                    res->fin[i].end = h->h_fin[kFinCols * i + 1];
-                    res->fin[i].dist = (int32_t)h->h_fin[kFinCols * i + 2];
-                    res->fin[i].idx = -1;
-                    res->fin[i].ngram = -1;
+                    res->fin[i] = make_rec(h->h_fin[kFinCols * i], h->h_fin[kFinCols * i + 1], h->h_fin[kFinCols * i + 2]);
                     res->hulls[2 * i] = h->h_fin[kFinCols * i + 3];
                     res->hulls[2 * i + 1] = h->h_fin[kFinCols * i + 4];
                 }
@@ -1452,8 +1377,13 @@ static void sort_generation_order(std::vector<RawRec> &v) {
     });
 }
 
-static void sort_generation_order(std::vector<RawRec> &v);
-static void sort_canonical(std::vector<RawRec> &v);
+static void sort_canonical(std::vector<RawRec> &v) {
+    std::sort(v.begin(), v.end(), [](const RawRec &a, const RawRec &b) {
+        if (a.start != b.start) return a.start < b.start;
+        if (a.end != b.end) return a.end < b.end;
+        return a.dist < b.dist;
+    });
+}
 
 void fzb_result::order_raw() {
     fetch_raw();
@@ -1471,14 +1401,6 @@ void fzb_result::order_raw() {
             return a.dist < b.dist;
         });
     raw_ordered = true;
-}
-
-static void sort_canonical(std::vector<RawRec> &v) {
-    std::sort(v.begin(), v.end(), [](const RawRec &a, const RawRec &b) {
-        if (a.start != b.start) return a.start < b.start;
-        if (a.end != b.end) return a.end < b.end;
-        return a.dist < b.dist;
-    });
 }
 
 // Host twin of k_post for lists it does not take (more than kPostMax records).
@@ -1633,10 +1555,7 @@ static int search_lev_ngrams(fzb_haystack *h, const uint8_t *pattern, uint32_t m
     bool fuse_gather = post_mode != 0 && (flags & FZB_F_GLOBAL) != 0;
     bool bitmap_mode = false;
     if (flags & FZB_F_TINY_LIST) p.glist_cap = std::min(h->glist_cap, 8u);
-retry_without_hits:
-    p.hits = use_hits ? h->d_hits : nullptr;
-    p.hits_cap = use_hits ? ((flags & FZB_F_TINY_LIST) ? std::min(h->hits_cap, 8u) : h->hits_cap) : 0;
-    rc = run_emitting(h, res, [&]() -> int {
+    auto enqueue = [&]() -> int {
         int r2 = enqueue_filter(h, p, sampled, res);
         if (r2) return r2;
         if (use_hits) {
@@ -1664,30 +1583,28 @@ retry_without_hits:
         }
         res->stats.n_launches += 1;
         return FZB_OK;
-    }, PostPlan{post_mode, fuse_gather});  // the raw stream's order (n-gram, hit index) is restored lazily
-    if (rc) return rc;
-    if (!use_hits && !bitmap_mode && h->h_counters[CNT_GRAN] > p.glist_cap) {
-        // more marked granules than the work list holds: the verify kernel raised CNT_OVERFLOW and did nothing (so a fused
-        // reduction, if any, went out invalid); redo the search with the list switched off, sweeping the bitmap
-        bitmap_mode = true;
-        fuse_gather = false;
-        p.glist_cap = 0;
-        res->fetch_raw();
-        res->raw.clear();
-        res->raw_n = 0;
-        res->fin.clear();
-        goto retry_without_hits;
-    }
-    if (use_hits && h->h_counters[CNT_HITS] > p.hits_cap) {
-        // the fused all-gather (if any) went out with valid = 0 (k_verify_hits raised CNT_OVERFLOW), so every
-        // rank will take finish_global's staged round; the retry itself must not issue another collective
-        fuse_gather = false;
-        use_hits = false;
-        res->fetch_raw();  // unlink from the staging buffer
-        res->raw.clear();
-        res->raw_n = 0;
-        res->fin.clear();
-        goto retry_without_hits;
+    };
+    for (;;) {
+        p.hits = use_hits ? h->d_hits : nullptr;
+        p.hits_cap = use_hits ? ((flags & FZB_F_TINY_LIST) ? std::min(h->hits_cap, 8u) : h->hits_cap) : 0;
+        // (the raw stream's order (n-gram, hit index) is restored lazily)
+        rc = run_emitting(h, res, enqueue, PostPlan{post_mode, fuse_gather});
+        if (rc) return rc;
+        if (!use_hits && !bitmap_mode && h->h_counters[CNT_GRAN] > p.glist_cap) {
+            // more marked granules than the work list holds: the verify kernel raised CNT_OVERFLOW and did nothing (so a
+            // fused reduction, if any, went out invalid); redo the search with the list switched off, sweeping the bitmap
+            bitmap_mode = true;
+            fuse_gather = false;
+            p.glist_cap = 0;
+        } else if (use_hits && h->h_counters[CNT_HITS] > p.hits_cap) {
+            // the fused all-gather (if any) went out with valid = 0 (k_verify_hits raised CNT_OVERFLOW), so every
+            // rank will take finish_global's staged round; the retry itself must not issue another collective
+            fuse_gather = false;
+            use_hits = false;
+        } else {
+            break;
+        }
+        res->discard_attempt();
     }
     res->raw_order = 0;
     return FZB_OK;
@@ -1756,10 +1673,7 @@ static int search_lev_lp(fzb_haystack *h, const uint8_t *pattern, uint32_t m, ui
             res->raw_order = 1;
             return FZB_OK;
         }
-        res->fetch_raw();  // list overflow: nothing was verified (and the fused reduction saw an invalid shard)
-        res->raw.clear();
-        res->raw_n = 0;
-        res->fin.clear();
+        res->discard_attempt();  // list overflow: nothing was verified (and the fused reduction saw an invalid shard)
     }
     rc = run_lp(h, res, [&](int grid, int cap) -> int {
         k_lev_lp<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_scratch, cap, h->d_out, h->out_cap, h->d_counters);
@@ -1854,35 +1768,17 @@ static int finish_global(fzb_haystack *h, fzb_result *res) {
                     "matches); the staged fallback needs an NCCL communicator (fzb_haystack_comm_init)", h->p2p_cap, kPostMax);
     std::vector<int64_t> all;
     std::vector<uint64_t> counts;
-    const std::vector<RawRec> &v = res->fin;
-    std::vector<int64_t> rows(v.size() * kFinCols);
-    for (size_t i = 0; i < v.size(); i++) {
-        rows[kFinCols * i + 0] = v[i].start;
-        rows[kFinCols * i + 1] = v[i].end;
-        rows[kFinCols * i + 2] = v[i].dist;
-        rows[kFinCols * i + 3] = res->hulls[2 * i];
-        rows[kFinCols * i + 4] = res->hulls[2 * i + 1];
-    }
+    std::vector<int64_t> rows(res->fin.size() * kFinCols);
+    write_group_rows(res->fin, res->hulls, res->fin.size(), rows.data());
     int rc = allgather_groups_staged(h, rows, all, counts);
     if (rc) return rc;
     if (res->unconsolidated) {  // unconsolidated routes (exact, Hamming): the global list is the sorted union
         res->gfin.resize(all.size() / kFinCols);
-        for (size_t i = 0; i < res->gfin.size(); i++) {
-            res->gfin[i].start = all[kFinCols * i];
-            res->gfin[i].end = all[kFinCols * i + 1];
-            res->gfin[i].dist = (int32_t)all[kFinCols * i + 2];
-            res->gfin[i].idx = -1;
-            res->gfin[i].ngram = -1;
-        }
+        for (size_t i = 0; i < res->gfin.size(); i++)
+            res->gfin[i] = make_rec(all[kFinCols * i], all[kFinCols * i + 1], all[kFinCols * i + 2]);
         sort_canonical(res->gfin);
     } else {
-        std::vector<std::pair<const int64_t *, uint64_t>> runs;
-        uint64_t off = 0;
-        for (uint64_t c : counts) {
-            runs.push_back({all.data() + off * kFinCols, c});
-            off += c;
-        }
-        merge_group_runs(runs, res->gfin);
+        sweep_groups(read_group_runs(all.data(), counts), res->gfin);
     }
     res->gcount = (uint32_t)res->gfin.size();
     res->has_global = true;
@@ -1897,7 +1793,7 @@ static int make_result(fzb_result **out, fzb_result **res) {
     return FZB_OK;
 }
 
-static int check_pattern(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags = 0) {
+static int check_pattern(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags) {
     if (!h) return fail(FZB_E_INVALID, "haystack handle is NULL");
     if ((flags & FZB_F_GLOBAL) && !h->comm && !h->local_world)
         return fail(FZB_E_INVALID, "FZB_F_GLOBAL needs fzb_haystack_comm_init / fzb_comm_init_local on this handle");
@@ -1906,33 +1802,45 @@ static int check_pattern(const fzb_haystack *h, const uint8_t *pattern, uint32_t
     return FZB_OK;
 }
 
-extern "C" int fzb_search_levenshtein(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t k,
-                                      uint32_t flags, fzb_result **out) {
+// check_pattern in the words of the exact search (search_exact.py), which has only this one complaint
+static int check_exact_pattern(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags) {
+    const int rc = check_pattern(h, pattern, m, flags);
+    return rc == FZB_E_INVALID && h ? fail(FZB_E_INVALID, "subsequence must not be empty") : rc;
+}
+
+// The frame of the single-pattern entry points: handle lock, result, `check`, the route's `body(res)`, the
+// reduction to the global list if `global`, and the result destroyed on any error.
+template <class F>
+static int run_search(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags, bool global,
+                      fzb_result **out, F body, decltype(&check_pattern) check = check_pattern) {
     HandleLock handle_lock(h);
     fzb_result *res;
     int rc = make_result(out, &res);
     if (rc) return rc;
-    rc = check_pattern(h, pattern, m, flags);
-    if (rc == FZB_OK) {
-        // find_near_matches_levenshtein (levenshtein.py:9-38)
-        if (k >= m) k = m;  // every k >= len(pattern) takes the same branch (levenshtein.py:62-65): (i, i, m) for all i
-        bool ngrams = (k == 0) || (m / (k + 1) >= 3);
-        if (flags & FZB_F_FORCE_NGRAMS) ngrams = true;
-        if (flags & FZB_F_FORCE_LP) ngrams = false;
-        // LevenshteinSearch.consolidate_matches (levenshtein.py:158-160) also applies when k == 0
-        const bool want_final = !(flags & FZB_F_NO_FINAL);
-        if (ngrams)
-            rc = search_lev_ngrams(h, pattern, m, k, flags, res, want_final ? 1 : 0);
-        else
-            rc = search_lev_lp(h, pattern, m, k, flags, res, want_final ? 1 : 0);
-        if (rc == FZB_OK && want_final && (flags & FZB_F_GLOBAL)) rc = finish_global(h, res);
-    }
+    rc = check(h, pattern, m, flags);
+    if (rc == FZB_OK) rc = body(res);
+    if (rc == FZB_OK && global) rc = finish_global(h, res);
     if (rc) {
         fzb_result_destroy(res);
         return rc;
     }
     *out = res;
     return FZB_OK;
+}
+
+extern "C" int fzb_search_levenshtein(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t k,
+                                      uint32_t flags, fzb_result **out) {
+    // LevenshteinSearch.consolidate_matches (levenshtein.py:158-160) also applies when k == 0
+    const int post_mode = (flags & FZB_F_NO_FINAL) ? 0 : 1;
+    return run_search(h, pattern, m, flags, post_mode && (flags & FZB_F_GLOBAL), out, [&](fzb_result *res) {
+        // find_near_matches_levenshtein (levenshtein.py:9-38)
+        if (k >= m) k = m;  // every k >= len(pattern) takes the same branch (levenshtein.py:62-65): (i, i, m) for all i
+        bool ngrams = (k == 0) || (m / (k + 1) >= 3);
+        if (flags & FZB_F_FORCE_NGRAMS) ngrams = true;
+        if (flags & FZB_F_FORCE_LP) ngrams = false;
+        return ngrams ? search_lev_ngrams(h, pattern, m, k, flags, res, post_mode)
+                      : search_lev_lp(h, pattern, m, k, flags, res, post_mode);
+    });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1957,6 +1865,99 @@ static int ensure_batch_buffers(fzb_haystack *h) {
     CK(cudaMemset(h->d_mset, 0, (size_t)h->mset_slots * sizeof(unsigned long long)));
     CK(cudaMalloc(&h->d_mwork, (size_t)h->mwork_cap * sizeof(WorkItem)));
     CK(cudaFuncSetAttribute(k_filter_multi, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMultiSmem));
+    return FZB_OK;
+}
+
+static int read_counters(fzb_haystack *h, uint32_t cnts[CNT_COUNT]) {
+    CK(cudaMemcpyAsync(cnts, h->d_counters, CNT_COUNT * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return FZB_OK;
+}
+
+static void add_stats(fzb_stats *sum, const fzb_stats &s) {
+    sum->gpu_ms += s.gpu_ms;
+    sum->filter_ms += s.filter_ms;
+    sum->bytes_scanned += s.bytes_scanned;
+    sum->n_candidates += s.n_candidates;
+    sum->n_launches += s.n_launches;
+}
+
+// The attempt loop of a batch pass.  `enqueue()` puts the kernels of one attempt on h->stream (behind h->ev[0]) and
+// returns FZB_OK, an error, or +1 when a device structure of the pass overflowed.  Returns the same, +1 also when a
+// kernel raised CNT_OVERFLOW; an attempt whose raw records did not fit the output buffer is redone with a larger
+// one.  On FZB_OK `raw` holds the records, `cnts` the counters, and `pass` the time and the bytes scanned.
+template <class F>
+static int run_batch_pass(fzb_haystack *h, F enqueue, std::vector<RawRec> &raw, uint32_t cnts[CNT_COUNT],
+                          fzb_stats &pass) {
+    detach_pending(h);  // the kernels are about to overwrite the output buffer an earlier result may still point at
+    for (int attempt = 0; attempt < 8; attempt++) {
+        h->counters_clean = false;  // (a batch pass leaves its counters behind)
+        CK(cudaMemsetAsync(h->d_counters, 0, CNT_COUNT * sizeof(uint32_t), h->stream));
+        CK(cudaEventRecord(h->ev[0], h->stream));
+        int rc = enqueue();
+        if (rc) return rc;
+        CK(cudaEventRecord(h->ev[2], h->stream));
+        rc = read_counters(h, cnts);
+        if (rc) return rc;
+        if (cnts[CNT_OVERFLOW]) return 1;
+        const uint32_t n = cnts[CNT_OUT];
+        if (n > h->out_cap) {
+            rc = ensure_out_cap(h, n);
+            if (rc) return rc;
+            continue;
+        }
+        raw.resize(n);
+        if (n) {
+            CK(cudaMemcpyAsync(raw.data(), h->d_out, (size_t)n * sizeof(RawRec), cudaMemcpyDeviceToHost, h->stream));
+            CK(cudaStreamSynchronize(h->stream));
+        }
+        float ms = 0.f;
+        cudaEventElapsedTime(&ms, h->ev[0], h->ev[2]);
+        pass.gpu_ms = ms;
+        pass.bytes_scanned = h->buf_len;
+        return FZB_OK;
+    }
+    return fail(FZB_E_CUDA, "output buffer kept overflowing");
+}
+
+// Splits the raw records of a pass over the patterns ids[] (`ngram` = pattern ordinal << 8 | n-gram) into the results
+// out[ids[i]], consolidates each list, and adds the pass to `sum`.  Every result carries the pass's route, the first
+// one its other stats (the haystack is read once for the whole pass).
+static int split_batch(const std::vector<RawRec> &raw, const std::vector<uint32_t> &ids, const fzb_stats &pass,
+                       int raw_order, fzb_result **out, fzb_stats *sum) {
+    const uint32_t cnt = (uint32_t)ids.size();
+    std::vector<uint32_t> per(cnt, 0);
+    for (const RawRec &r : raw) per[(uint32_t)r.ngram >> 8]++;
+    for (uint32_t i = 0; i < cnt; i++) {
+        fzb_result *res = new (std::nothrow) fzb_result();
+        if (!res) return fail(FZB_E_CUDA, "out of host memory");
+        res->raw.reserve(per[i]);
+        if (i == 0) res->stats = pass;
+        res->stats.route = pass.route;
+        res->raw_order = raw_order;
+        out[ids[i]] = res;
+    }
+    for (const RawRec &r : raw) {
+        RawRec q = r;
+        q.ngram = r.ngram & 0xFF;
+        out[ids[(uint32_t)r.ngram >> 8]]->raw.push_back(q);
+    }
+    // consolidate the lists in parallel (LP patterns on text have tens of thousands of raw matches each)
+    const unsigned nthreads = std::min<unsigned>({8u, std::max(1u, std::thread::hardware_concurrency()), cnt});
+    std::atomic<uint32_t> next{0};
+    auto work = [&]() {
+        for (uint32_t i = next.fetch_add(1); i < cnt; i = next.fetch_add(1)) {
+            fzb_result *res = out[ids[i]];
+            res->raw_n = (uint32_t)res->raw.size();
+            consolidate_recs(res->raw, res->fin, &res->hulls);
+            res->have_fin = true;
+        }
+    };
+    std::vector<std::thread> pool;
+    for (unsigned t = 1; t < nthreads; t++) pool.emplace_back(work);
+    work();
+    for (auto &t : pool) t.join();
+    add_stats(sum, pass);
     return FZB_OK;
 }
 
@@ -2020,7 +2021,6 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
         CK(cudaMalloc(&h->d_mhits, (size_t)h->mhits_cap * sizeof(unsigned long long)));
         CK(cudaFuncSetAttribute(k_filter_mdense, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMdenseSmem));
     }
-    detach_pending(h);
     CK(cudaMemcpyAsync(h->d_mbits, bits.data(), bits.size() * 4, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_gtab, gtab.data(), gtab.size() * sizeof(uint2), cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_postings, postings.data(), postings.size() * 4, cudaMemcpyHostToDevice, h->stream));
@@ -2047,13 +2047,9 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
     const int64_t nvec = (int64_t)(round_up(h->buf_len, 16) / 16);
     const int64_t ntiles = (nvec + kMultiTileVecs - 1) / kMultiTileVecs;
     std::vector<RawRec> raw;
-    float gpu_ms = 0.f, filter_ms = 0.f;
-    uint32_t n_work = 0;
-    for (int attempt = 0;; attempt++) {
-        if (attempt == 8) return fail(FZB_E_CUDA, "output buffer kept overflowing");
-        h->counters_clean = false;  // (this pass leaves its counters behind)
-        CK(cudaMemsetAsync(h->d_counters, 0, CNT_COUNT * sizeof(uint32_t), h->stream));
-        CK(cudaEventRecord(h->ev[0], h->stream));
+    uint32_t cnts[CNT_COUNT];
+    fzb_stats pass{};
+    rc = run_batch_pass(h, [&]() -> int {
         MdenseParams dp{mp, h->d_bpats, h->d_mhits, h->mhits_cap};
         if (ntiles > 0) {
             const int grid = (int)std::min<int64_t>(ntiles, h->sm_count);
@@ -2068,64 +2064,20 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
         else
             k_verify_multi<<<h->sm_count * 8, kVmThreads, 0, h->stream>>>(mp, h->d_bpats, h->d_out, h->out_cap, h->d_counters);
         CK(cudaGetLastError());
-        CK(cudaEventRecord(h->ev[2], h->stream));
-        uint32_t cnts[CNT_COUNT];
-        CK(cudaMemcpyAsync(cnts, h->d_counters, sizeof cnts, cudaMemcpyDeviceToHost, h->stream));
+        return FZB_OK;
+    }, raw, cnts, pass);
+    if (rc > 0 && !dense) {  // work list / set too small for this batch: clean up, let the caller go one by one
+        CK(cudaMemsetAsync(h->d_mset, 0, (size_t)h->mset_slots * sizeof(unsigned long long), h->stream));
         CK(cudaStreamSynchronize(h->stream));
-        if (cnts[CNT_OVERFLOW]) {  // work list / set / hit list too small for this batch: clean up, let the caller go one by one
-            if (!dense) CK(cudaMemsetAsync(h->d_mset, 0, (size_t)h->mset_slots * sizeof(unsigned long long), h->stream));
-            CK(cudaStreamSynchronize(h->stream));
-            return 1;
-        }
-        const uint32_t n = cnts[CNT_OUT];
-        if (n > h->out_cap) {
-            rc = ensure_out_cap(h, n);
-            if (rc) return rc;
-            continue;
-        }
-        raw.resize(n);
-        if (n) {
-            CK(cudaMemcpyAsync(raw.data(), h->d_out, (size_t)n * sizeof(RawRec), cudaMemcpyDeviceToHost, h->stream));
-            CK(cudaStreamSynchronize(h->stream));
-        }
-        n_work = cnts[CNT_CAND];
-        cudaEventElapsedTime(&gpu_ms, h->ev[0], h->ev[2]);
-        cudaEventElapsedTime(&filter_ms, h->ev[0], h->ev[1]);
-        break;
     }
-    // split by pattern, consolidate each list on the host
-    std::vector<uint32_t> per(cnt, 0);
-    for (const RawRec &r : raw) per[(uint32_t)r.ngram >> 8]++;
-    for (uint32_t i = 0; i < cnt; i++) {
-        fzb_result *res = new (std::nothrow) fzb_result();
-        if (!res) return fail(FZB_E_CUDA, "out of host memory");
-        res->raw.reserve(per[i]);
-        res->stats.route = dense ? 2 : 1;
-        res->stats.bytes_scanned = i == 0 ? h->buf_len : 0;  // the haystack is read once for the whole pass
-        res->stats.gpu_ms = i == 0 ? gpu_ms : 0.0;
-        res->stats.filter_ms = i == 0 ? filter_ms : 0.0;
-        res->stats.n_candidates = i == 0 ? n_work : 0;
-        res->stats.n_launches = i == 0 ? 2 : 0;
-        out[ids[i]] = res;
-    }
-    for (const RawRec &r : raw) {
-        RawRec q = r;
-        q.ngram = r.ngram & 0xFF;
-        out[ids[(uint32_t)r.ngram >> 8]]->raw.push_back(q);
-    }
-    for (uint32_t i = 0; i < cnt; i++) {
-        fzb_result *res = out[ids[i]];
-        res->raw_n = (uint32_t)res->raw.size();
-        res->raw_order = 0;
-        consolidate_recs(res->raw, res->fin, &res->hulls);
-        res->have_fin = true;
-    }
-    sum->gpu_ms += gpu_ms;
-    sum->filter_ms += filter_ms;
-    sum->bytes_scanned += h->buf_len;
-    sum->n_candidates += n_work;
-    sum->n_launches += 2;
-    return FZB_OK;
+    if (rc) return rc;
+    float filter_ms = 0.f;
+    cudaEventElapsedTime(&filter_ms, h->ev[0], h->ev[1]);
+    pass.route = dense ? 2 : 1;
+    pass.filter_ms = filter_ms;
+    pass.n_candidates = cnts[CNT_CAND];
+    pass.n_launches = 2;
+    return split_batch(raw, ids, pass, 0, out, sum);
 }
 
 // One shared scan for up to 64 LP-route patterns (k_lp_scan_multi / k_lp_verify_multi).  Same return convention
@@ -2170,7 +2122,6 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
         CK(cudaMalloc(&h->d_lmhist, 256 * sizeof(uint32_t)));  // per-pattern counts [64] + kept total [1] | cursors [64]
         CK(cudaFuncSetAttribute(k_lp_scan_multi, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLmSmem));
     }
-    detach_pending(h);
     CK(cudaMemcpyAsync(h->d_lmlut, lut.data(), 256 * sizeof(ulonglong2), cudaMemcpyHostToDevice, h->stream));
     uint32_t *d_pm32 = reinterpret_cast<uint32_t *>(h->d_lmlut + 256);
     CK(cudaMemcpyAsync(d_pm32, pm32.data(), pm32.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
@@ -2194,16 +2145,14 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
     if (rc) return rc;
     const uint64_t chunk = 256ull << 20;  // starts per scan: bounds the survivor list
     std::vector<RawRec> raw;
-    float gpu_ms = 0.f, filter_ms = 0.f;
+    uint32_t cnts[CNT_COUNT];
+    fzb_stats pass{};
+    float scan_ms = 0.f;
     uint64_t n_work = 0;
-    for (int attempt = 0;; attempt++) {
-        if (attempt == 8) return fail(FZB_E_CUDA, "output buffer kept overflowing");
-        h->counters_clean = false;
-        CK(cudaMemsetAsync(h->d_counters, 0, CNT_COUNT * sizeof(uint32_t), h->stream));
-        CK(cudaEventRecord(h->ev[0], h->stream));
-        bool overflow = false;
-        float scan_ms = 0.f;
-        for (uint64_t lo = h->own_lo; lo < h->own_hi && !overflow; lo += chunk) {
+    rc = run_batch_pass(h, [&]() -> int {
+        scan_ms = 0.f;
+        n_work = 0;
+        for (uint64_t lo = h->own_lo; lo < h->own_hi; lo += chunk) {
             lp.own_lo = (int64_t)lo;
             lp.own_hi = (int64_t)std::min<uint64_t>(h->own_hi, lo + chunk);
             CK(cudaMemsetAsync(h->d_counters + CNT_LMLIST, 0, 2 * sizeof(uint32_t), h->stream));  // list length + flag
@@ -2223,74 +2172,22 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
                 k_lp_verify_multi<8><<<vgrid, kLpThreads, 0, h->stream>>>(lp, h->d_lmlist, h->d_lmhist, h->d_scratch, sim_cap,
                                                                           h->d_out, h->out_cap, h->d_counters);
             CK(cudaGetLastError());
-            uint32_t cnts[CNT_COUNT];
-            CK(cudaMemcpyAsync(cnts, h->d_counters, sizeof cnts, cudaMemcpyDeviceToHost, h->stream));
-            CK(cudaStreamSynchronize(h->stream));
+            const int r2 = read_counters(h, cnts);
+            if (r2) return r2;
             float ms = 0.f;
             cudaEventElapsedTime(&ms, h->ev[1], h->ev[2]);
             scan_ms += ms;
             n_work += cnts[CNT_LMLIST];
             sum->n_launches += 4;
-            if (cnts[CNT_LMWORK] || cnts[CNT_OVERFLOW]) overflow = true;  // survivor list / candidate lists too small
+            if (cnts[CNT_LMWORK] || cnts[CNT_OVERFLOW]) return 1;  // survivor list / candidate lists too small
         }
-        if (overflow) return 1;
-        CK(cudaEventRecord(h->ev[2], h->stream));
-        uint32_t cnts[CNT_COUNT];
-        CK(cudaMemcpyAsync(cnts, h->d_counters, sizeof cnts, cudaMemcpyDeviceToHost, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
-        const uint32_t n = cnts[CNT_OUT];
-        if (n > h->out_cap) {
-            rc = ensure_out_cap(h, n);
-            if (rc) return rc;
-            n_work = 0;
-            continue;
-        }
-        raw.resize(n);
-        if (n) {
-            CK(cudaMemcpyAsync(raw.data(), h->d_out, (size_t)n * sizeof(RawRec), cudaMemcpyDeviceToHost, h->stream));
-            CK(cudaStreamSynchronize(h->stream));
-        }
-        cudaEventElapsedTime(&gpu_ms, h->ev[0], h->ev[2]);
-        filter_ms = scan_ms;
-        break;
-    }
-    for (uint32_t i = 0; i < cnt; i++) {
-        fzb_result *res = new (std::nothrow) fzb_result();
-        if (!res) return fail(FZB_E_CUDA, "out of host memory");
-        res->stats.route = 3;
-        res->stats.bytes_scanned = i == 0 ? h->buf_len : 0;  // the haystack is read once for the whole pass
-        res->stats.gpu_ms = i == 0 ? gpu_ms : 0.0;
-        res->stats.filter_ms = i == 0 ? filter_ms : 0.0;
-        res->stats.n_candidates = i == 0 ? n_work : 0;
-        out[ids[i]] = res;
-    }
-    for (const RawRec &r : raw) {
-        RawRec q = r;
-        q.ngram = r.ngram & 0xFF;
-        out[ids[(uint32_t)r.ngram >> 8]]->raw.push_back(q);
-    }
-    {  // consolidate the lists in parallel (LP patterns on text have tens of thousands of raw matches each)
-        const unsigned nthreads = std::min<unsigned>(8, std::max(1u, std::thread::hardware_concurrency()));
-        std::atomic<uint32_t> next{0};
-        auto work = [&]() {
-            for (uint32_t i = next.fetch_add(1); i < cnt; i = next.fetch_add(1)) {
-                fzb_result *res = out[ids[i]];
-                res->raw_n = (uint32_t)res->raw.size();
-                res->raw_order = 1;
-                consolidate_recs(res->raw, res->fin, &res->hulls);
-                res->have_fin = true;
-            }
-        };
-        std::vector<std::thread> pool;
-        for (unsigned t = 1; t < nthreads; t++) pool.emplace_back(work);
-        work();
-        for (auto &t : pool) t.join();
-    }
-    sum->gpu_ms += gpu_ms;
-    sum->filter_ms += filter_ms;
-    sum->bytes_scanned += h->buf_len;
-    sum->n_candidates += n_work;
-    return FZB_OK;
+        return FZB_OK;
+    }, raw, cnts, pass);
+    if (rc) return rc;
+    pass.route = 3;
+    pass.filter_ms = scan_ms;
+    pass.n_candidates = n_work;
+    return split_batch(raw, ids, pass, 1, out, sum);
 }
 
 extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
@@ -2302,11 +2199,18 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
     for (uint32_t i = 0; i < count; i++)
         if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
     fzb_stats sum{};
-    auto cleanup = [&]() {
-        for (uint32_t j = 0; j < count; j++) {
-            if (out[j]) fzb_result_destroy(out[j]);
-            out[j] = nullptr;
-        }
+    auto drop = [&](uint32_t j) {
+        if (out[j]) fzb_result_destroy(out[j]);
+        out[j] = nullptr;
+    };
+    // the outcome of a shared pass: an error drops every result; an overflow leaves the pass's patterns to the
+    // one-by-one path below
+    auto settle = [&](int rc, const std::vector<uint32_t> &ids) -> int {
+        if (rc < 0)
+            for (uint32_t j = 0; j < count; j++) drop(j);
+        if (rc > 0)
+            for (uint32_t id : ids) drop(id);
+        return rc < 0 ? rc : FZB_OK;
     };
     // patterns the shared scan can take: n-gram route, q-sample lemma holds, 4-grams selective on this haystack,
     // short enough for the 64-bit match table; no special flags (forced routes, raw-only, multi-GPU reduction)
@@ -2336,18 +2240,8 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
             done -= ids.size();
             break;
         }
-        int rc = batch_pass(h, patterns, offsets, max_l_dist, ids, out, &sum, false);
-        if (rc < 0) {
-            cleanup();
-            return rc;
-        }
-        if (rc > 0) {  // overflow: these patterns fall through to the one-by-one path
-            for (uint32_t id : ids)
-                if (out[id]) {
-                    fzb_result_destroy(out[id]);
-                    out[id] = nullptr;
-                }
-        }
+        const int rc = settle(batch_pass(h, patterns, offsets, max_l_dist, ids, out, &sum, false), ids);
+        if (rc) return rc;
     }
     // the n-gram-route patterns the lemma does not cover share a scan of their own (n-gram prefixes at every position)
     std::vector<uint32_t> dense_ids;
@@ -2370,17 +2264,8 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
         }
     }
     if (dense_ids.size() >= 2) {
-        int rc = batch_pass(h, patterns, offsets, max_l_dist, dense_ids, out, &sum, true);
-        if (rc < 0) {
-            cleanup();
-            return rc;
-        }
-        if (rc > 0)
-            for (uint32_t id : dense_ids)
-                if (out[id]) {
-                    fzb_result_destroy(out[id]);
-                    out[id] = nullptr;
-                }
+        const int rc = settle(batch_pass(h, patterns, offsets, max_l_dist, dense_ids, out, &sum, true), dense_ids);
+        if (rc) return rc;
     }
     // LP-route patterns (m // (k+1) < 3) share scans of 64 patterns each (bit-sliced window counters)
     std::vector<uint32_t> lp_ids;
@@ -2397,31 +2282,15 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
     for (size_t first = 0; first + 2 <= lp_ids.size(); first += 64) {
         std::vector<uint32_t> ids(lp_ids.begin() + first, lp_ids.begin() + std::min(lp_ids.size(), first + 64));
         if (ids.size() < 2) break;
-        int rc = batch_pass_lp(h, patterns, offsets, max_l_dist, ids, out, &sum);
-        if (rc < 0) {
-            cleanup();
-            return rc;
-        }
-        if (rc > 0)
-            for (uint32_t id : ids)
-                if (out[id]) {
-                    fzb_result_destroy(out[id]);
-                    out[id] = nullptr;
-                }
+        const int rc = settle(batch_pass_lp(h, patterns, offsets, max_l_dist, ids, out, &sum), ids);
+        if (rc) return rc;
     }
     for (uint32_t i = 0; i < count; i++) {
         if (out[i]) continue;
-        int rc = fzb_search_levenshtein(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_l_dist[i], flags,
-                                        &out[i]);
-        if (rc) {
-            cleanup();
-            return rc;
-        }
-        sum.gpu_ms += out[i]->stats.gpu_ms;
-        sum.filter_ms += out[i]->stats.filter_ms;
-        sum.bytes_scanned += out[i]->stats.bytes_scanned;
-        sum.n_candidates += out[i]->stats.n_candidates;
-        sum.n_launches += out[i]->stats.n_launches;
+        const int rc = settle(fzb_search_levenshtein(h, patterns + offsets[i], offsets[i + 1] - offsets[i],
+                                                     max_l_dist[i], flags, &out[i]), {});
+        if (rc) return rc;
+        add_stats(&sum, out[i]->stats);
     }
     sum.route = 7;  // batch
     if (total) *total = sum;
@@ -2430,28 +2299,44 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
 
 extern "C" int fzb_search_exact(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
                                 fzb_result **out) {
-    HandleLock handle_lock(h);
-    fzb_result *res;
-    int rc = make_result(out, &res);
-    if (rc) return rc;
-    rc = check_pattern(h, pattern, m, flags);
-    if (rc == FZB_E_INVALID && h) rc = fail(FZB_E_INVALID, "subsequence must not be empty");
-    if (rc == FZB_OK) rc = search_lev_ngrams(h, pattern, m, 0, flags, res, 2);
-    if (rc) {
-        fzb_result_destroy(res);
-        return rc;
-    }
-    res->unconsolidated = true;  // ExactSearch.consolidate_matches is the base no-op (common.py:198-205)
-    if (flags & FZB_F_GLOBAL) {
-        rc = finish_global(h, res);
-        if (rc) {
-            fzb_result_destroy(res);
-            return rc;
-        }
-    }
-    *out = res;
-    return FZB_OK;
+    return run_search(h, pattern, m, flags, (flags & FZB_F_GLOBAL) != 0, out, [&](fzb_result *res) {
+        res->unconsolidated = true;  // ExactSearch.consolidate_matches is the base no-op (common.py:198-205)
+        return search_lev_ngrams(h, pattern, m, 0, flags, res, 2);
+    }, check_exact_pattern);
 }
+
+// Points a handle at a view of its buffer for its own lifetime; keeps the handle's geometry and restores all of it
+// (global_len and coll_prob included) on every exit.
+struct BufferView {
+    fzb_haystack *const h;
+    uint8_t *const d;
+    const uint64_t buf_len, buf_lo, own_lo, own_hi, padded_len, global_len;
+    const double coll_prob;
+    explicit BufferView(fzb_haystack *hs)
+        : h(hs), d(hs->d), buf_len(hs->buf_len), buf_lo(hs->buf_lo), own_lo(hs->own_lo), own_hi(hs->own_hi),
+          padded_len(hs->padded_len), global_len(hs->global_len), coll_prob(hs->coll_prob) {}
+    ~BufferView() {
+        h->d = d;
+        h->buf_len = buf_len;
+        h->buf_lo = buf_lo;
+        h->own_lo = own_lo;
+        h->own_hi = own_hi;
+        h->padded_len = padded_len;
+        h->global_len = global_len;
+        h->coll_prob = coll_prob;
+    }
+    BufferView(const BufferView &) = delete;
+    BufferView &operator=(const BufferView &) = delete;
+    // the bytes [vlo, vhi) of the sequence (vlo 128-byte aligned relative to the buffer start), owning [lo, hi)
+    void set(uint64_t vlo, uint64_t vhi, uint64_t lo, uint64_t hi) {
+        h->d = d + (vlo - buf_lo);
+        h->buf_lo = vlo;
+        h->buf_len = vhi - vlo;
+        h->padded_len = round_up(h->buf_len, 128) + 128;
+        h->own_lo = lo;
+        h->own_hi = hi;
+    }
+};
 
 // search_exact(subsequence, sequence, start_index, end_index) (search_exact.py:22-56): the occurrences lying wholly
 // inside [start, end).  The window is a VIEW of the resident buffer treated like a shard of a sequence that ends
@@ -2463,14 +2348,12 @@ extern "C" int fzb_search_exact_window(fzb_haystack *h, const uint8_t *pattern, 
     if (!h || !out) return fail(FZB_E_INVALID, "NULL argument");
     *out = nullptr;
     if (flags & FZB_F_GLOBAL) return fail(FZB_E_INVALID, "windowed exact search is per handle");
-    if (h->buf_lo != 0 || h->global_len != h->buf_len || h->own_lo != 0 || h->own_hi != h->buf_len)
-        return fail(FZB_E_INVALID, "windowed exact search needs a whole (unsharded) sequence");
+    if (!is_whole_sequence(h)) return fail(FZB_E_INVALID, "windowed exact search needs a whole (unsharded) sequence");
     // clamp (search_exact.py:29-30): start into [0, n], end into [start, n]
     start = std::min<uint64_t>(start, h->global_len);
     end = std::max<uint64_t>(start, std::min<uint64_t>(end, h->global_len));
     if (end - start < m) {  // no room for an occurrence (also: the empty window): nothing to launch
-        int rc0 = check_pattern(h, pattern, m, flags);
-        if (rc0 == FZB_E_INVALID) rc0 = fail(FZB_E_INVALID, "subsequence must not be empty");
+        int rc0 = check_exact_pattern(h, pattern, m, flags);
         if (rc0) return rc0;
         fzb_result *res;
         rc0 = make_result(out, &res);
@@ -2480,33 +2363,15 @@ extern "C" int fzb_search_exact_window(fzb_haystack *h, const uint8_t *pattern, 
         *out = res;
         return FZB_OK;
     }
-    struct Geometry {
-        uint8_t *d;
-        uint64_t buf_len, buf_lo, own_lo, own_hi, padded_len, global_len;
-        double coll_prob;
-    } const saved{h->d, h->buf_len, h->buf_lo, h->own_lo, h->own_hi, h->padded_len, h->global_len, h->coll_prob};
     // the view starts a halo before the window (the shard geometry check of the search wants one on both sides;
     // the right one ends at the view's global end), on a 128-byte boundary of the buffer
     const uint64_t halo = round_up((uint64_t)m, 128) + 128;
-    const uint64_t vlo = (start > halo ? start - halo : 0) / 128 * 128;
-    h->d = saved.d + vlo;
-    h->buf_lo = vlo;
-    h->buf_len = end - vlo;
-    h->padded_len = round_up(h->buf_len, 128) + 128;
+    BufferView view(h);
+    view.set((start > halo ? start - halo : 0) / 128 * 128, end, start, end);
     h->global_len = end;
-    h->own_lo = start;
-    h->own_hi = end;
-    h->coll_prob = -1.0;
+    h->coll_prob = -1.0;  // (the byte statistics of the window)
     const int rc = fzb_search_exact(h, pattern, m, flags, out);
     if (rc == FZB_OK && *out) (*out)->fetch_raw();  // the records leave the view's buffers before the geometry changes back
-    h->d = saved.d;
-    h->buf_len = saved.buf_len;
-    h->buf_lo = saved.buf_lo;
-    h->own_lo = saved.own_lo;
-    h->own_hi = saved.own_hi;
-    h->padded_len = saved.padded_len;
-    h->global_len = saved.global_len;
-    h->coll_prob = saved.coll_prob;
     return rc;
 }
 
@@ -2555,122 +2420,96 @@ static int ham_counter_layout(int threshold) {  // (read per search: a probe can
 
 extern "C" int fzb_search_hamming(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t k,
                                   uint32_t flags, fzb_result **out) {
-    HandleLock handle_lock(h);
-    fzb_result *res;
-    int rc = make_result(out, &res);
-    if (rc) return rc;
-    rc = check_pattern(h, pattern, m, flags);
-    if (rc == FZB_OK) rc = check_halo(h, m);
-    if (rc == FZB_OK) {
-        rc = [&]() -> int {
-            ScanParams p;
-            fill_params(h, pattern, m, p);
-            p.k = (int)std::min<uint32_t>(k, m);
-            CK(cudaSetDevice(h->device));
-            res->stats.route = 4;
-            res->stats.bytes_scanned = h->buf_len;
-            // counting q-sample filter needs W = floor((m-3)/4) >= k+1 aligned words and 4-bit fields (k <= 7)
-            const bool counting = !(flags & FZB_F_FORCE_DENSE) && (int)m >= 4 * p.k + 7 && p.k <= 7 && h->buf_len > 0;
-            HamCountParams hp{};
-            CUtensorMap map256, map8;
-            if (counting) {
-                hp.Wc = std::min<int>((int)(m - 3) / 4, 8);
-                hp.bias = 8 - (hp.Wc - p.k);
-                hp.nrows = (int64_t)(round_up(h->buf_len, kHcRowBytes) / kHcRowBytes);
-                int r3 = make_row_maps(h, &map256, &map8);
-                if (r3) return r3;
-                CK(cudaFuncSetAttribute(k_hamming_count<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
-                CK(cudaFuncSetAttribute(k_hamming_count<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
-                CK(cudaFuncSetAttribute(k_hamming_count<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
-            }
-            const int layout = counting ? ham_counter_layout(hp.Wc - p.k) : 0;
-            if (layout == 2) hp.bias = 4 - (hp.Wc - p.k);
-            bool bitmap_mode = false;
-            PostPlan plan{2, (flags & FZB_F_GLOBAL) != 0};  // FINAL == RAW in (start, end, dist) order, ordered by k_post
-        retry_bitmap:
-            int r2 = run_emitting(h, res, [&]() -> int {
-                if (counting) {
-                    const int64_t ntiles = (hp.nrows + kHcThreads - 1) / kHcThreads;
-                    const int grid = (int)std::min<int64_t>(ntiles, (int64_t)h->sm_count * 2);
-                    if (layout == 2)
-                        k_hamming_count<2><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
-                    else if (layout == 1)
-                        k_hamming_count<1><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
-                    else
-                        k_hamming_count<0><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
-                    CK(cudaEventRecord(h->ev[1], h->stream));
-                    h->ev1_recorded = true;
-                    // one verify launch: the granule work list -- or, after it overflowed, the whole bitmap
-                    k_verify_ham<<<h->sm_count * 4, kVerifyThreads, 0, h->stream>>>(
-                        p, h->bitmap_words, h->d_glist, p.glist_cap, bitmap_mode ? 1 : 0, h->d_out, h->out_cap,
-                        h->d_counters);
-                    res->stats.n_launches += 1;
-                } else {
-                    k_hamming_scan<<<h->sm_count * 8, kHamThreads, 0, h->stream>>>(p, h->d_out, h->out_cap,
-                                                                                   h->d_counters);
-                }
-                res->stats.n_launches++;
-                return FZB_OK;
-            }, plan);
-            if (r2) return r2;
-            if (counting && !bitmap_mode && h->h_counters[CNT_GRAN] > p.glist_cap) {  // work list overflowed (see search_lev_ngrams)
-                bitmap_mode = true;
-                plan.global = false;
-                p.glist_cap = 0;
-                res->fetch_raw();
-                res->raw.clear();
-                res->raw_n = 0;
-                res->fin.clear();
-                goto retry_bitmap;
-            }
-            res->raw_order = 1;
-            return FZB_OK;
-        }();
-    }
-    if (rc) {
-        fzb_result_destroy(res);
-        return rc;
-    }
-    res->unconsolidated = true;
-    if (flags & FZB_F_GLOBAL) {
-        rc = finish_global(h, res);
-        if (rc) {
-            fzb_result_destroy(res);
-            return rc;
+    return run_search(h, pattern, m, flags, (flags & FZB_F_GLOBAL) != 0, out, [&](fzb_result *res) -> int {
+        int rc = check_halo(h, m);
+        if (rc) return rc;
+        res->unconsolidated = true;
+        ScanParams p;
+        fill_params(h, pattern, m, p);
+        p.k = (int)std::min<uint32_t>(k, m);
+        CK(cudaSetDevice(h->device));
+        res->stats.route = 4;
+        res->stats.bytes_scanned = h->buf_len;
+        // counting q-sample filter needs W = floor((m-3)/4) >= k+1 aligned words and 4-bit fields (k <= 7)
+        const bool counting = !(flags & FZB_F_FORCE_DENSE) && (int)m >= 4 * p.k + 7 && p.k <= 7 && h->buf_len > 0;
+        HamCountParams hp{};
+        CUtensorMap map256, map8;
+        if (counting) {
+            hp.Wc = std::min<int>((int)(m - 3) / 4, 8);
+            hp.bias = 8 - (hp.Wc - p.k);
+            hp.nrows = (int64_t)(round_up(h->buf_len, kHcRowBytes) / kHcRowBytes);
+            rc = make_row_maps(h, &map256, &map8);
+            if (rc) return rc;
+            CK(cudaFuncSetAttribute(k_hamming_count<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
+            CK(cudaFuncSetAttribute(k_hamming_count<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
+            CK(cudaFuncSetAttribute(k_hamming_count<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
         }
-    }
-    *out = res;
-    return FZB_OK;
+        const int layout = counting ? ham_counter_layout(hp.Wc - p.k) : 0;
+        if (layout == 2) hp.bias = 4 - (hp.Wc - p.k);
+        bool bitmap_mode = false;
+        PostPlan plan{2, (flags & FZB_F_GLOBAL) != 0};  // FINAL == RAW in (start, end, dist) order, ordered by k_post
+        auto enqueue = [&]() -> int {
+            if (counting) {
+                const int64_t ntiles = (hp.nrows + kHcThreads - 1) / kHcThreads;
+                const int grid = (int)std::min<int64_t>(ntiles, (int64_t)h->sm_count * 2);
+                if (layout == 2)
+                    k_hamming_count<2><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
+                else if (layout == 1)
+                    k_hamming_count<1><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
+                else
+                    k_hamming_count<0><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
+                CK(cudaEventRecord(h->ev[1], h->stream));
+                h->ev1_recorded = true;
+                // one verify launch: the granule work list -- or, after it overflowed, the whole bitmap
+                k_verify_ham<<<h->sm_count * 4, kVerifyThreads, 0, h->stream>>>(
+                    p, h->bitmap_words, h->d_glist, p.glist_cap, bitmap_mode ? 1 : 0, h->d_out, h->out_cap,
+                    h->d_counters);
+                res->stats.n_launches += 1;
+            } else {
+                k_hamming_scan<<<h->sm_count * 8, kHamThreads, 0, h->stream>>>(p, h->d_out, h->out_cap,
+                                                                               h->d_counters);
+            }
+            res->stats.n_launches++;
+            return FZB_OK;
+        };
+        for (;;) {
+            rc = run_emitting(h, res, enqueue, plan);
+            if (rc) return rc;
+            if (!counting || bitmap_mode || h->h_counters[CNT_GRAN] <= p.glist_cap) break;
+            // the work list overflowed (see search_lev_ngrams)
+            bitmap_mode = true;
+            plan.global = false;
+            p.glist_cap = 0;
+            res->discard_attempt();
+        }
+        res->raw_order = 1;
+        return FZB_OK;
+    });
 }
 
 extern "C" int fzb_search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t max_subs,
                                   uint32_t max_ins, uint32_t max_dels, uint32_t max_l, uint32_t flags,
                                   fzb_result **out) {
-    HandleLock handle_lock(h);
-    fzb_result *res;
-    int rc = make_result(out, &res);
-    if (rc) return rc;
-    rc = check_pattern(h, pattern, m, flags);
-    if (rc == FZB_OK) {
+    const int post_mode = (flags & FZB_F_NO_FINAL) ? 0 : 1;
+    return run_search(h, pattern, m, flags, post_mode && (flags & FZB_F_GLOBAL), out, [&](fzb_result *res) {
         // find_near_matches_generic (generic_search.py:25-54)
-        const bool want_final = !(flags & FZB_F_NO_FINAL);
-        if (max_l == 0 && !(flags & (FZB_F_FORCE_LP | FZB_F_FORCE_NGRAMS))) {
-            rc = search_lev_ngrams(h, pattern, m, 0, flags, res, want_final ? 1 : 0);
-        } else {
-            bool ngrams = m / (max_l + 1) >= 3;
-            if (flags & FZB_F_FORCE_NGRAMS) ngrams = true;
-            if (flags & FZB_F_FORCE_LP) ngrams = false;
-            rc = search_generic(h, pattern, m, max_subs, max_ins, max_dels, max_l, ngrams, flags, res,
-                                want_final ? 1 : 0);
-        }
-        if (rc == FZB_OK && want_final && (flags & FZB_F_GLOBAL)) rc = finish_global(h, res);
-    }
-    if (rc) {
-        fzb_result_destroy(res);
-        return rc;
-    }
-    *out = res;
-    return FZB_OK;
+        if (max_l == 0 && !(flags & (FZB_F_FORCE_LP | FZB_F_FORCE_NGRAMS)))
+            return search_lev_ngrams(h, pattern, m, 0, flags, res, post_mode);
+        bool ngrams = m / (max_l + 1) >= 3;
+        if (flags & FZB_F_FORCE_NGRAMS) ngrams = true;
+        if (flags & FZB_F_FORCE_LP) ngrams = false;
+        return search_generic(h, pattern, m, max_subs, max_ins, max_dels, max_l, ngrams, flags, res, post_mode);
+    });
+}
+
+// choose_search_class (__init__.py:60-83) on normalised limits
+static int search_by_class(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t max_subs, uint32_t max_ins,
+                           uint32_t max_dels, uint32_t max_l, uint32_t flags, fzb_result **out) {
+    if (max_l == 0) return fzb_search_exact(h, pattern, m, flags, out);
+    if (max_ins == 0 && max_dels == 0) return fzb_search_hamming(h, pattern, m, std::min(max_l, max_subs), flags, out);
+    if (max_l <= std::min(max_subs, std::min(max_ins, max_dels)))
+        return fzb_search_levenshtein(h, pattern, m, max_l, flags, out);
+    return fzb_search_generic(h, pattern, m, max_subs, max_ins, max_dels, max_l, flags, out);
 }
 
 // One cached workspace per device for the one-shot call: the analogue of the reference's reusable
@@ -2705,16 +2544,7 @@ extern "C" int fzb_find_near_matches(const uint8_t *pattern, uint32_t m, const u
     }
     int rc = fzb_haystack_upload(h, haystack, n);
     if (rc) return rc;
-    // choose_search_class (__init__.py:60-83) on normalised limits
-    if (max_l == 0)
-        rc = fzb_search_exact(h, pattern, m, 0, out);
-    else if (max_ins == 0 && max_dels == 0)
-        rc = fzb_search_hamming(h, pattern, m, std::min(max_l, max_subs), 0, out);
-    else if (max_l <= std::min(max_subs, std::min(max_ins, max_dels)))
-        rc = fzb_search_levenshtein(h, pattern, m, max_l, 0, out);
-    else
-        rc = fzb_search_generic(h, pattern, m, max_subs, max_ins, max_dels, max_l, 0, out);
-    return rc;
+    return search_by_class(h, pattern, m, max_subs, max_ins, max_dels, max_l, 0, out);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2734,51 +2564,27 @@ extern "C" int fzb_has_near_match(fzb_haystack *h, const uint8_t *pattern, uint3
     *found = 0;
     int rc = check_pattern(h, pattern, m, 0);
     if (rc) return rc;
-    struct Geometry {
-        uint8_t *d;
-        uint64_t buf_len, buf_lo, own_lo, own_hi, padded_len;
-    } const saved{h->d, h->buf_len, h->buf_lo, h->own_lo, h->own_hi, h->padded_len};
     CK(cudaSetDevice(h->device));
     if (h->buf_len) sample_collision_prob(h);  // byte statistics of the WHOLE buffer (the views reuse them)
+    BufferView whole(h);  // (its fields: the geometry of the whole buffer)
     const uint64_t halo = round_up((uint64_t)m + std::min<uint64_t>(max_l, m), 128) + 128;
-    uint64_t chunk = 64ull << 20, lo = saved.own_lo;
+    uint64_t chunk = 64ull << 20, lo = whole.own_lo;
     if (const char *e = getenv("FZB_HAS_CHUNK_BYTES"))  // testing: chunk seams on small sequences
         chunk = std::max<uint64_t>(128, round_up(strtoull(e, nullptr, 10), 128));
-    rc = FZB_OK;
     do {  // (at least one pass: an empty sequence still has its k >= m matches)
-        uint64_t hi = std::min(saved.own_hi, round_up(lo + chunk, 128));
-        if (saved.own_hi - hi < chunk / 4) hi = saved.own_hi;  // no tiny last chunk
-        // view [vlo, vhi) of the buffer: the chunk plus its halo, 128-byte aligned relative to the buffer start
-        const uint64_t want_lo = lo > saved.buf_lo + halo ? lo - halo : saved.buf_lo;
-        const uint64_t vlo = saved.buf_lo + (want_lo - saved.buf_lo) / 128 * 128;
-        const uint64_t vhi = std::min(saved.buf_lo + saved.buf_len, hi + halo);
-        h->d = saved.d + (vlo - saved.buf_lo);
-        h->buf_lo = vlo;
-        h->buf_len = vhi - vlo;
-        h->padded_len = round_up(h->buf_len, 128) + 128;
-        h->own_lo = lo;
-        h->own_hi = hi;
+        uint64_t hi = std::min(whole.own_hi, round_up(lo + chunk, 128));
+        if (whole.own_hi - hi < chunk / 4) hi = whole.own_hi;  // no tiny last chunk
+        // the chunk plus its halo, 128-byte aligned relative to the buffer start
+        const uint64_t want_lo = lo > whole.buf_lo + halo ? lo - halo : whole.buf_lo;
+        whole.set(whole.buf_lo + (want_lo - whole.buf_lo) / 128 * 128, std::min(whole.buf_lo + whole.buf_len, hi + halo),
+                  lo, hi);
         fzb_result *res = nullptr;
-        // choose_search_class (__init__.py:60-83) on normalised limits; raw stream only
-        if (max_l == 0)
-            rc = fzb_search_exact(h, pattern, m, FZB_F_NO_FINAL, &res);
-        else if (max_ins == 0 && max_dels == 0)
-            rc = fzb_search_hamming(h, pattern, m, std::min(max_l, max_subs), FZB_F_NO_FINAL, &res);
-        else if (max_l <= std::min(max_subs, std::min(max_ins, max_dels)))
-            rc = fzb_search_levenshtein(h, pattern, m, max_l, FZB_F_NO_FINAL, &res);
-        else
-            rc = fzb_search_generic(h, pattern, m, max_subs, max_ins, max_dels, max_l, FZB_F_NO_FINAL, &res);
+        rc = search_by_class(h, pattern, m, max_subs, max_ins, max_dels, max_l, FZB_F_NO_FINAL, &res);  // raw stream only
         if (rc == FZB_OK && fzb_result_count(res, FZB_RAW) > 0) *found = 1;
         if (res) fzb_result_destroy(res);
         lo = hi;
         chunk *= 4;
-    } while (rc == FZB_OK && !*found && lo < saved.own_hi);
-    h->d = saved.d;
-    h->buf_len = saved.buf_len;
-    h->buf_lo = saved.buf_lo;
-    h->own_lo = saved.own_lo;
-    h->own_hi = saved.own_hi;
-    h->padded_len = saved.padded_len;
+    } while (rc == FZB_OK && !*found && lo < whole.own_hi);
     return rc;
 }
 
