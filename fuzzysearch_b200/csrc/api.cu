@@ -2408,16 +2408,6 @@ static int make_row_maps(fzb_haystack *h, CUtensorMap *map256, CUtensorMap *map8
     return FZB_OK;
 }
 
-// Counter layout of k_hamming_count (ham_recur.h).  FZB_HAM_COUNTERS=nibble|sliced overrides the default.
-// -> 0 nibble fields / 1 three slices / 2 two slices (thresholds <= 4 only)
-static int ham_counter_layout(int threshold) {  // (read per search: a probe can flip it between two searches)
-    const char *e = getenv("FZB_HAM_COUNTERS");
-    if (e && !strcmp(e, "nibble")) return 0;
-    if (e && !strcmp(e, "sliced3")) return 1;
-    // fewer instructions per word: two slices where the threshold allows, else three (nibble fields: A/B only)
-    return threshold <= 4 ? 2 : 1;
-}
-
 extern "C" int fzb_search_hamming(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t k,
                                   uint32_t flags, fzb_result **out) {
     return run_search(h, pattern, m, flags, (flags & FZB_F_GLOBAL) != 0, out, [&](fzb_result *res) -> int {
@@ -2434,30 +2424,28 @@ extern "C" int fzb_search_hamming(fzb_haystack *h, const uint8_t *pattern, uint3
         const bool counting = !(flags & FZB_F_FORCE_DENSE) && (int)m >= 4 * p.k + 7 && p.k <= 7 && h->buf_len > 0;
         HamCountParams hp{};
         CUtensorMap map256, map8;
+        int slices = 0;  // of the counters (ham_recur.h)
         if (counting) {
             hp.Wc = std::min<int>((int)(m - 3) / 4, 8);
-            hp.bias = 8 - (hp.Wc - p.k);
+            // fewer instructions per word: two slices (counting to 4) where the threshold allows, else three
+            slices = hp.Wc - p.k <= 4 ? 2 : 3;
+            hp.bias = (1 << slices) - (hp.Wc - p.k);
             hp.nrows = (int64_t)(round_up(h->buf_len, kHcRowBytes) / kHcRowBytes);
             rc = make_row_maps(h, &map256, &map8);
             if (rc) return rc;
-            CK(cudaFuncSetAttribute(k_hamming_count<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
-            CK(cudaFuncSetAttribute(k_hamming_count<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
             CK(cudaFuncSetAttribute(k_hamming_count<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
+            CK(cudaFuncSetAttribute(k_hamming_count<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
         }
-        const int layout = counting ? ham_counter_layout(hp.Wc - p.k) : 0;
-        if (layout == 2) hp.bias = 4 - (hp.Wc - p.k);
         bool bitmap_mode = false;
         PostPlan plan{2, (flags & FZB_F_GLOBAL) != 0};  // FINAL == RAW in (start, end, dist) order, ordered by k_post
         auto enqueue = [&]() -> int {
             if (counting) {
                 const int64_t ntiles = (hp.nrows + kHcThreads - 1) / kHcThreads;
                 const int grid = (int)std::min<int64_t>(ntiles, (int64_t)h->sm_count * 2);
-                if (layout == 2)
+                if (slices == 2)
                     k_hamming_count<2><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
-                else if (layout == 1)
-                    k_hamming_count<1><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
                 else
-                    k_hamming_count<0><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
+                    k_hamming_count<3><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
                 CK(cudaEventRecord(h->ev[1], h->stream));
                 h->ev1_recorded = true;
                 // one verify launch: the granule work list -- or, after it overflowed, the whole bitmap

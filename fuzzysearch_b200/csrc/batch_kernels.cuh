@@ -273,24 +273,14 @@ k_filter_mdense(const __grid_constant__ MdenseParams p, int64_t nvec, int64_t nt
         // flush decision reduced inside the barrier from what happened before it (see k_lp_scan): warps that are a
         // tile ahead may already be appending again when a slower warp would read the count
         if (__syncthreads_or(full)) {
-            const uint32_t n = min(*sN, (uint32_t)kMdBuf);
-            if (threadIdx.x == 0) sBase = atomicAdd(&p.mp.counters[CNT_MHITS], n);
-            __syncthreads();
-            for (uint32_t i = threadIdx.x; i < n; i += kMultiThreads)
-                if (sBase + i < p.hits_cap) p.hits[sBase + i] = sBuf[i];
-            __syncthreads();
-            if (threadIdx.x == 0) *sN = 0;
+            flush_cta_buffer(sBuf, sN, min(*sN, (uint32_t)kMdBuf), &sBase, p.hits, p.hits_cap,
+                             &p.mp.counters[CNT_MHITS], kMultiThreads);
             __syncthreads();
         }
     }
     __syncthreads();
     const uint32_t n = min(*sN, (uint32_t)kMdBuf);
-    if (n) {
-        if (threadIdx.x == 0) sBase = atomicAdd(&p.mp.counters[CNT_MHITS], n);
-        __syncthreads();
-        for (uint32_t i = threadIdx.x; i < n; i += kMultiThreads)
-            if (sBase + i < p.hits_cap) p.hits[sBase + i] = sBuf[i];
-    }
+    if (n) flush_cta_buffer(sBuf, sN, n, &sBase, p.hits, p.hits_cap, &p.mp.counters[CNT_MHITS], kMultiThreads);
 }
 
 constexpr int kMhThreads = 128;
@@ -340,14 +330,7 @@ k_verify_mhits(const __grid_constant__ MdenseParams p, RawRec *out, uint32_t cap
             c.n_ngrams = bp->n_ngrams;
             for (int w = 0; w < kBatchMaxM / 4; w++)
                 reinterpret_cast<uint32_t *>(myP)[w] = __ldg(reinterpret_cast<const uint32_t *>(bp->P) + w);
-            const int64_t p0 = idx - (int64_t)j * c.L;
-            const int64_t wlo = max(max(p0 - c.k, (int64_t)0), c.buf_lo);
-            const int64_t whi = min(min(p0 + c.m + c.k, c.N), c.buf_lo + c.buf_len);
-            alo = wlo & ~(int64_t)3;
-            const int nwords = (int)((whi - alo + 3) >> 2);
-            const uint32_t *src = reinterpret_cast<const uint32_t *>(c.H + (alo - c.buf_lo));
-            uint32_t *dst = reinterpret_cast<uint32_t *>(slot);
-            for (int w = 0; w < nwords; w++) dst[w] = __ldg(src + w);
+            alo = stage_lane_window(c, idx - (int64_t)j * c.L, slot);
         }
         verify_anchor_lev<3>(c, myP, nullptr, slot - alo, idx, valid, nullptr, out, cap, counters, j, j + 1, tag);
     }
@@ -472,23 +455,13 @@ k_lp_scan_multi(const __grid_constant__ LpMultiParams p) {
         }
         __syncthreads();
         const uint32_t n = min(*sN, (uint32_t)kLmBuf);
-        if (n >= (uint32_t)kLmFlush) {
-            if (threadIdx.x == 0) sBase = atomicAdd(&p.counters[CNT_LMLIST], n);
-            __syncthreads();
-            for (uint32_t i = threadIdx.x; i < n; i += kLmThreads)
-                if (sBase + i < p.list_cap) p.list[sBase + i] = sBuf[i];
-            __syncthreads();
-            if (threadIdx.x == 0) *sN = 0;
-        }
+        // (the barrier at the top of the next tile orders the reset before the next append)
+        if (n >= (uint32_t)kLmFlush)
+            flush_cta_buffer(sBuf, sN, n, &sBase, p.list, p.list_cap, &p.counters[CNT_LMLIST], kLmThreads);
     }
     __syncthreads();
     const uint32_t n = min(*sN, (uint32_t)kLmBuf);
-    if (n) {
-        if (threadIdx.x == 0) sBase = atomicAdd(&p.counters[CNT_LMLIST], n);
-        __syncthreads();
-        for (uint32_t i = threadIdx.x; i < n; i += kLmThreads)
-            if (sBase + i < p.list_cap) p.list[sBase + i] = sBuf[i];
-    }
+    if (n) flush_cta_buffer(sBuf, sN, n, &sBase, p.list, p.list_cap, &p.counters[CNT_LMLIST], kLmThreads);
 }
 
 // Between scan and verification: k_lm_refine applies each survivor's OWN window (the scan used the longest one of the

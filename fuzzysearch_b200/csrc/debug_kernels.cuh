@@ -40,36 +40,33 @@ k_debug_expand(const uint8_t *subs, const uint32_t *sub_off, const uint8_t *seqs
     bool ok;
     if (sublen <= 64) {
         if (sublen <= 32)
-            ok = expand_bp<uint32_t, 1>(sPM, 0, sublen, sSeq, seqlen, k, d, l, var);
+            ok = expand_bp<uint32_t, 1>(EqPM<1>{sPM, 0}, sublen, sSeq, seqlen, k, d, l, var);
         else
-            ok = expand_bp<unsigned long long, 1>(sPM, 0, sublen, sSeq, seqlen, k, d, l, var);
+            ok = expand_bp<unsigned long long, 1>(EqPM<1>{sPM, 0}, sublen, sSeq, seqlen, k, d, l, var);
         o[0] = ok ? d : -1;
         o[1] = ok ? l : -1;
         if (sublen <= 32)
-            ok = expand_bp<uint32_t, -1>(sPMR, sublen, sublen, sSeqR + seqlen - 1, seqlen, k, d, l, var);
+            ok = expand_bp<uint32_t, -1>(EqPM<-1>{sPMR, sublen}, sublen, sSeqR + seqlen - 1, seqlen, k, d, l, var);
         else
-            ok = expand_bp<unsigned long long, -1>(sPMR, sublen, sublen, sSeqR + seqlen - 1, seqlen, k, d, l, var);
+            ok = expand_bp<unsigned long long, -1>(EqPM<-1>{sPMR, sublen}, sublen, sSeqR + seqlen - 1, seqlen, k, d,
+                                                   l, var);
         o[2] = ok ? d : -1;
         o[3] = ok ? l : -1;
     } else {
         o[0] = o[1] = o[2] = o[3] = -2;
     }
     DpScratch S;
-    const bool is_long = var == 0 ? sublen > max(2 * k, 10) : var == 2;
+    const bool is_long = var == 2;  // (variant 0: expand_any picks it)
     if (var == 0)
         ok = expand_any<1>(sSub, sublen, sSeq, seqlen, k, S, d, l);
-    else if (is_long)
-        ok = expand_long<1>(sSub, sublen, sSeq, seqlen, k, S, d, l);
     else
-        ok = expand_short<1>(sSub, sublen, sSeq, seqlen, k, S, d, l);
+        ok = expand_dp<1>(sSub, sublen, sSeq, seqlen, k, is_long, S, d, l);
     o[4] = ok ? d : -1;
     o[5] = ok ? l : -1;
     if (var == 0)
         ok = expand_any<-1>(sSubR + sublen - 1, sublen, sSeqR + seqlen - 1, seqlen, k, S, d, l);
-    else if (is_long)
-        ok = expand_long<-1>(sSubR + sublen - 1, sublen, sSeqR + seqlen - 1, seqlen, k, S, d, l);
     else
-        ok = expand_short<-1>(sSubR + sublen - 1, sublen, sSeqR + seqlen - 1, seqlen, k, S, d, l);
+        ok = expand_dp<-1>(sSubR + sublen - 1, sublen, sSeqR + seqlen - 1, seqlen, k, is_long, S, d, l);
     o[6] = ok ? d : -1;
     o[7] = ok ? l : -1;
 }

@@ -7,13 +7,13 @@
 //   Wc = min(W, 8) aligned words inside it equal the pattern 4-gram at their own offset.  Unlike the
 //   Levenshtein filter a single q-gram hit is not selective on small alphabets (DNA: 29 grams among
 //   256 possible words), so the kernel COUNTS: per alignment class o0 = (first aligned word) - p in
-//   {0,1,2,3} it keeps a shift-add register S_o0 of Wc 4-bit fields; for every aligned text word w
-//        S_o0 = (S_o0 << 4) + T_o0[hash(w)]          (one IMAD per class)
-//   where T_o0[.] has a 1 in field i iff w == P[o0+4i : o0+4i+4)  (+ a bias of 8-(Wc-k) in field 0),
-//   so field Wc-1 reaches 8 (bit 3 set) exactly when >= Wc-k of the Wc words of the occurrence that
-//   ENDS its counted prefix at this word matched.  The table lives in shared memory, 16 B per bucket
-//   (the four classes: ONE LDS.128 per text word), replicated 8x so that the 8 lanes of a
-//   quarter-warp always hit distinct 16-byte bank groups (conflict-free).
+//   {0,1,2,3} it keeps Wc counters, one per occurrence whose counted words are still being read, and
+//   every aligned text word w adds 1 to the counters whose current pattern 4-gram equals w.  The 32
+//   counters of the four classes are bit-sliced (ham_recur.h): one register per bit of the counters, and
+//   the table entry of hash(w) is the 32 match bits, bit 8*o0 + i <-> w == P[o0+4i : o0+4i+4) -- one
+//   LDS.32 per text word, replicated per lane (bank = lane: conflict-free).  The carry out of the top
+//   slice flags the word at which an occurrence's (Wc-k)-th counted word matched.  Two slices count
+//   to 4 and serve thresholds Wc-k <= 4; three count to 8.
 //   The recurrence runs ALONG the text, so each thread owns one 128-byte row of a tile; tiles are
 //   staged global -> shared by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B so that the per-thread
 //   row reads are bank-conflict free, mbarrier complete_tx, 2-stage ring), one elected thread issuing.
@@ -29,6 +29,17 @@ namespace fzb {
 
 constexpr int kHamThreads = 256;
 
+// Mismatches between the text bytes text(0 .. m-1) and sP[0 .. m-1]; counting stops once they exceed k.
+template <class Text>
+__device__ __forceinline__ int ham_mismatches(Text text, const uint8_t *sP, int m, int k) {
+    int nd = 0;
+    for (int i = 0; i < m; i++) {
+        nd += (text(i) != sP[i]);
+        if (nd > k) break;
+    }
+    return nd;
+}
+
 __global__ void __launch_bounds__(kHamThreads)
 k_hamming_scan(const ScanParams p, RawRec *out, uint32_t cap, uint32_t *counters) {
     __shared__ uint8_t sP[256];
@@ -39,11 +50,7 @@ k_hamming_scan(const ScanParams p, RawRec *out, uint32_t cap, uint32_t *counters
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t pos = p.own_lo + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pos < last; pos += stride) {
         const uint8_t *h = p.H + (pos - p.buf_lo);
-        int nd = 0;
-        for (int i = 0; i < m; i++) {
-            nd += (__ldg(h + i) != sP[i]);
-            if (nd > k) break;
-        }
+        const int nd = ham_mismatches([&](int i) { return __ldg(h + i); }, sP, m, k);
         if (nd <= k) emit(out, cap, counters, pos, pos + m, pos, nd, 0);
     }
 }
@@ -94,12 +101,11 @@ constexpr int kHcHaloRows = 8;                // one swizzle atom; only its last
 constexpr int kHcTileRows = kHcHaloRows + kHcThreads;            // 264
 constexpr int kHcStageBytes = kHcTileRows * kHcRowBytes;         // 33792 (multiple of 1024)
 constexpr int kHcStages = 2;
-constexpr int kHcTableBytes = kHcBuckets * 8 * 16;               // 32 KiB (nibble fields: 8 replicas x 16 B;
-                                                                 //         bit-sliced: 32 replicas x 4 B)
+constexpr int kHcTableBytes = kHcBuckets * 32 * 4;               // 32 KiB: 32 replicas x 4 B per bucket
 constexpr size_t kHcSmem = (size_t)kHcStages * kHcStageBytes + kHcTableBytes + 64;
 struct HamCountParams {
     int Wc;        // counted words per occurrence (<= 8)
-    int bias;      // 8 - (Wc - k)
+    int bias;      // 2^slices - (Wc - k): the counters' start value, so that they carry out at Wc - k matches
     int64_t nrows; // rows of the buffer that hold data: ceil(buf_len / 128)
 };
 
@@ -129,27 +135,20 @@ __device__ __forceinline__ uint32_t lds32(uint32_t saddr) {
 #endif
 }
 
-// SLICED = 0: nibble fields, 16-byte table entries (4 wavefronts per lookup);  SLICED = 1: bit-sliced counters,
-// 4-byte table entries (1 wavefront per lookup, more ALU work per word);  SLICED = 2: the same with two slices
-// (thresholds Wc - k <= 4; hp.bias is then 4 - (Wc - k)) -- see ham_recur.h.
-template <int SLICED>
+// SLICES = 2 (thresholds Wc - k <= 4) or 3: the bit slices of the counters (ham_recur.h).
+template <int SLICES>
 __global__ void __launch_bounds__(kHcThreads, 2)
 k_hamming_count(const ScanParams p, const HamCountParams hp, const __grid_constant__ CUtensorMap map256,
                 const __grid_constant__ CUtensorMap map8) {
     extern __shared__ __align__(1024) uint8_t hc_smem[];  // SWIZZLE_128B tiles need 1024-byte alignment
     uint8_t *base = hc_smem;
-    uint4 *table = reinterpret_cast<uint4 *>(base + kHcStages * kHcStageBytes);
-    uint32_t *table32 = reinterpret_cast<uint32_t *>(table);
+    uint32_t *table = reinterpret_cast<uint32_t *>(base + kHcStages * kHcStageBytes);
     uint64_t *full = reinterpret_cast<uint64_t *>(base + kHcStages * kHcStageBytes + kHcTableBytes);
     const int tid = threadIdx.x, lane = tid & 31;
     const int Wc = hp.Wc;
 
-    if (SLICED) {  // bucket b, replica r (= lane): word b * 32 + r; bit 8 * o0 + i <-> w == P[o0+4i : o0+4i+4)
-        for (int i = tid; i < kHcBuckets * 32; i += kHcThreads) table32[i] = 0u;
-    } else {       // every bucket starts with the bias in field 0 of all four classes
-        for (int i = tid; i < kHcBuckets * 8; i += kHcThreads)
-            table[i] = make_uint4((uint32_t)hp.bias, (uint32_t)hp.bias, (uint32_t)hp.bias, (uint32_t)hp.bias);
-    }
+    // bucket b, replica r (= lane): word b * 32 + r; bit 8 * o0 + i <-> w == P[o0+4i : o0+4i+4)
+    for (int i = tid; i < kHcBuckets * 32; i += kHcThreads) table[i] = 0u;
     if (tid == 0) {
         for (int s = 0; s < kHcStages; s++) mbar_init(&full[s], 1);
 #ifndef FZB_EMU
@@ -157,22 +156,14 @@ k_hamming_count(const ScanParams p, const HamCountParams hp, const __grid_consta
 #endif
     }
     __syncthreads();
-    if (tid < (SLICED ? 32 : 8)) {  // replica `tid` of the table: add the pattern's 4-grams (serial per replica: no races)
+    if (tid < 32) {  // replica `tid` of the table: add the pattern's 4-grams (serial per replica: no races)
         for (int o0 = 0; o0 < 4; o0++)
-            for (int i = 0; i < Wc; i++) {  // each (class, field) pair exactly once
-                const uint32_t w = hc_gram(p.P, o0 + 4 * i);
-                if (SLICED) {
-                    table32[hc_bucket(w) * 32 + tid] |= 1u << (8 * o0 + i);
-                } else {
-                    uint32_t *e = reinterpret_cast<uint32_t *>(&table[hc_bucket(w) * 8 + tid]);
-                    e[o0] += 1u << (4 * i);
-                }
-            }
+            for (int i = 0; i < Wc; i++)  // each (class, field) pair exactly once
+                table[hc_bucket(hc_gram(p.P, o0 + 4 * i)) * 32 + tid] |= 1u << (8 * o0 + i);
     }
     __syncthreads();
 
     const int64_t ntiles = (hp.nrows + kHcThreads - 1) / kHcThreads;
-    const uint32_t flag_bit = 8u << (4 * (Wc - 1));
     const uint32_t B0 = (hp.bias & 1) ? 0x01010101u : 0u, B1 = (hp.bias & 2) ? 0x01010101u : 0u,
                    B2 = (hp.bias & 4) ? 0x01010101u : 0u;
     auto issue = [&](int64_t tile, int s) {  // one elected thread: 264 rows = 8 (halo atom) + 256
@@ -187,8 +178,7 @@ k_hamming_count(const ScanParams p, const HamCountParams hp, const __grid_consta
         if (tile < ntiles) issue(tile, 0);
         if (tile + gridDim.x < ntiles) issue(tile + gridDim.x, 1);
     }
-    // my replica of the table: bank group = lane % 8 (16-byte entries) / bank = lane (4-byte entries)
-    const uint32_t my_table = smem_u32(table) + (SLICED ? (lane << 2) : ((lane & 7) << 4));
+    const uint32_t my_table = smem_u32(table) + (lane << 2);  // my replica of the table: bank = lane
     const uint32_t stage0 = smem_u32(base);
     uint32_t phases = 0;  // bit s = parity to wait for on stage s
     for (int it = 0; tile < ntiles; tile += gridDim.x, it++) {
@@ -197,62 +187,34 @@ k_hamming_count(const ScanParams p, const HamCountParams hp, const __grid_consta
         phases ^= 1u << s;
         const uint32_t st = stage0 + s * kHcStageBytes;
         const int r = kHcHaloRows + tid;
-        bool flagged;
-        if (SLICED) {
-            HamSliced cnt{0u, 0u, 0u};
-            HamSliced2 cnt2{0u, 0u};
-            uint32_t acc = 0;
+        HamSliced cnt{0u, 0u, 0u};
+        HamSliced2 cnt2{0u, 0u};
+        uint32_t acc = 0;
 #define HS_STEP(WORD, track)                                                                 \
     {                                                                                        \
         const uint32_t M = lds32(my_table + (hc_bucket(WORD) << 7));                         \
-        const uint32_t c = SLICED == 2 ? ham_sliced2_step(cnt2, M, B0, B1)                   \
+        const uint32_t c = SLICES == 2 ? ham_sliced2_step(cnt2, M, B0, B1)                   \
                                        : ham_sliced_step(cnt, M, B0, B1, B2);                \
         if (track) acc |= c;                                                                 \
     }
-            {  // warm-up: the last 7 words of the previous row (their candidates belong to that row's thread)
-                const uint4 a = lds128(hc_chunk(st, r - 1, 6)), b = lds128(hc_chunk(st, r - 1, 7));
-                HS_STEP(a.y, false) HS_STEP(a.z, false) HS_STEP(a.w, false)
-                HS_STEP(b.x, false) HS_STEP(b.y, false) HS_STEP(b.z, false) HS_STEP(b.w, false)
-            }
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const uint4 d = lds128(hc_chunk(st, r, j));
-                HS_STEP(d.x, true) HS_STEP(d.y, true) HS_STEP(d.z, true) HS_STEP(d.w, true)
-            }
-#undef HS_STEP
-            flagged = acc != 0;
-        } else {
-            uint32_t S0 = 0, S1 = 0, S2 = 0, S3 = 0, acc = 0;
-#define HC_STEP(WORD, track)                                               \
-    {                                                                      \
-        const uint4 T = lds128(my_table + (hc_bucket(WORD) << 7));         \
-        S0 = S0 * 16u + T.x;                                               \
-        S1 = S1 * 16u + T.y;                                               \
-        S2 = S2 * 16u + T.z;                                               \
-        S3 = S3 * 16u + T.w;                                               \
-        if (track) acc |= S0 | S1 | S2 | S3;                               \
-    }
-            {  // warm-up: the last 7 words of the previous row (no flags: they belong to that row's thread)
-                const uint4 a = lds128(hc_chunk(st, r - 1, 6)), b = lds128(hc_chunk(st, r - 1, 7));
-                HC_STEP(a.y, false) HC_STEP(a.z, false) HC_STEP(a.w, false)
-                HC_STEP(b.x, false) HC_STEP(b.y, false) HC_STEP(b.z, false) HC_STEP(b.w, false)
-            }
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const uint4 d = lds128(hc_chunk(st, r, j));
-                HC_STEP(d.x, true) HC_STEP(d.y, true) HC_STEP(d.z, true) HC_STEP(d.w, true)
-            }
-#undef HC_STEP
-            flagged = (acc & flag_bit) != 0;
+        {  // warm-up: the last 7 words of the previous row (their candidates belong to that row's thread)
+            const uint4 a = lds128(hc_chunk(st, r - 1, 6)), b = lds128(hc_chunk(st, r - 1, 7));
+            HS_STEP(a.y, false) HS_STEP(a.z, false) HS_STEP(a.w, false)
+            HS_STEP(b.x, false) HS_STEP(b.y, false) HS_STEP(b.z, false) HS_STEP(b.w, false)
         }
-        if (flagged) {
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            const uint4 d = lds128(hc_chunk(st, r, j));
+            HS_STEP(d.x, true) HS_STEP(d.y, true) HS_STEP(d.z, true) HS_STEP(d.w, true)
+        }
+#undef HS_STEP
+        if (acc) {
             // some start passed the filter at a word of my row (rare: true near-matches): mark its granules;
-            // k_verify_ham re-checks them exactly.  Nibble fields fire at the occurrence's LAST counted word
-            // (first counted word = that word - Wc + 1); the sliced counters fire at the word of the
-            // (Wc-k)-th match, anywhere from the first to the last counted word.
+            // k_verify_ham re-checks them exactly.  The counters fire at the word of the (Wc-k)-th match,
+            // anywhere from the first to the last counted word of the occurrence.
             const int64_t grow = tile * kHcThreads + tid;  // buffer row index
             const int64_t pr_lo = 4 * (grow * 32 - Wc + 1) - 3;
-            const int64_t pr_hi = 4 * (grow * 32 + 31 - (SLICED ? 0 : Wc - 1));
+            const int64_t pr_hi = 4 * (grow * 32 + 31);
             mark_range_inline(p, p.buf_lo + max(pr_lo, (int64_t)0), p.buf_lo + pr_hi);
         }
         __syncthreads();  // everyone is done with stage s
@@ -272,11 +234,7 @@ __device__ __forceinline__ void verify_granule_ham(const ScanParams &p, const ui
     for (int half = 0; half < kGranule / 32; half++) {
         const int64_t pos = gbase + half * 32 + lane;
         if (pos < p.own_lo || pos >= p.own_hi || pos + m > p.N) continue;
-        int nd = 0;
-        for (int i = 0; i < m; i++) {
-            nd += (W[pos + i] != sP[i]);
-            if (nd > k) break;
-        }
+        const int nd = ham_mismatches([&](int i) { return W[pos + i]; }, sP, m, k);
         if (nd <= k) emit(out, cap, counters, pos, pos + m, pos, nd, 0);
     }
 }
@@ -286,48 +244,13 @@ k_verify_ham(const ScanParams p, uint64_t bitmap_words, const uint32_t *glist, u
              RawRec *out, uint32_t cap, uint32_t *counters) {
     __shared__ uint8_t sP[256];
     __shared__ uint32_t sWinAll[kVerifyThreads / 32][kWinWords];
-    const uint32_t ngran = counters[CNT_GRAN];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) sP[i] = p.P[i];
     __syncthreads();
     const int lane = threadIdx.x & 31;
     uint32_t *sWin = sWinAll[threadIdx.x >> 5];
-    if (!scan_mode) {
-        if (ngran > glist_cap) {  // work list overflowed: the host repeats the search in bitmap mode
-            if (blockIdx.x == 0 && threadIdx.x == 0) counters[CNT_OVERFLOW] = 1;
-            return;
-        }
-        const uint32_t nitems = ngran;
-        for (;;) {
-            uint32_t item = 0;
-            if (lane == 0) item = atomicAdd(&counters[CNT_WORK], 1u);
-            item = __shfl_sync(0xFFFFFFFFu, item, 0);
-            if (item >= nitems) break;
-            const uint32_t g = glist[item];
-            verify_granule_ham(p, sP, sWin, (int64_t)g, lane, out, cap, counters);
-            if (lane == 0) atomicAnd(&p.bitmap[g >> 5], ~(1u << (g & 31)));
-        }
-        if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&counters[CNT_CAND], nitems);
-        return;
-    }
-    const uint64_t gwarp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
-    for (uint64_t wbase = gwarp * 32; wbase < bitmap_words; wbase += nwarps * 32) {
-        const uint64_t wi = wbase + lane;
-        uint32_t bits = wi < bitmap_words ? p.bitmap[wi] : 0u;
-        if (bits) p.bitmap[wi] = 0u;
-        unsigned active = __ballot_sync(0xFFFFFFFFu, bits != 0);
-        while (active) {
-            const int src = __ffs(active) - 1;
-            active &= active - 1;
-            uint32_t b = __shfl_sync(0xFFFFFFFFu, bits, src);
-            if (lane == 0) atomicAdd(&counters[CNT_CAND], (uint32_t)__popc(b));
-            while (b) {
-                const int bit = __ffs(b) - 1;
-                b &= b - 1;
-                verify_granule_ham(p, sP, sWin, (int64_t)(wbase + src) * 32 + bit, lane, out, cap, counters);
-            }
-        }
-    }
+    for_each_marked_granule(p.bitmap, bitmap_words, glist, glist_cap, scan_mode, counters, [&](int64_t g) {
+        verify_granule_ham(p, sP, sWin, g, lane, out, cap, counters);
+    });
 }
 
 }  // namespace fzb

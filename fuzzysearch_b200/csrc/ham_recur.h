@@ -5,18 +5,14 @@
 // counters: counter i (a "field") belongs to the occurrence whose FIRST counted word was seen i words ago and
 // counts how many of its counted words so far equalled the pattern 4-gram at their own offset,
 // P[o0+4j : o0+4j+4) for word j of the occurrence.  Per word: every field moves up by one, field 0 restarts
-// at `bias` = 8 - (Wc - k), and field i gets +1 iff w == gram(o0, i).  A field reaching 8 means ">= Wc - k of
-// the occurrence's counted words match": a candidate.
+// at `bias`, and field i gets +1 iff w == gram(o0, i).
 //
-// Two layouts:
-//  * nibble fields: one 32-bit register per class, 4 bits per field; the table holds, per hash bucket, the
-//    four classes' increments (16 bytes: one LDS.128 = 4 shared-memory wavefronts per warp and word);
-//    S = 16*S + T[bucket].  The candidate test is bit 3 of field Wc-1.
-//  * bit-sliced: ONE 32-bit register per bit of the counters -- bit (8*o0 + i) of slice j is bit j of field i
-//    of class o0 -- and the table entry is just the 32 match bits (4 bytes: one LDS.32 = ONE wavefront per
-//    warp and word when replicated per lane); the increment is a 3-level ripple carry and the carry out of
-//    slice 2 IS the candidate signal, at the word where the (Wc-k)-th match happens.  (Two slices are enough
-//    when Wc - k <= 4.)
+// The counters are bit-sliced: ONE 32-bit register per bit of the counters -- bit (8*o0 + i) of slice j is bit j
+// of field i of class o0 -- so the table entry of a hash bucket is just the 32 match bits M (4 bytes: one LDS.32 =
+// ONE shared-memory wavefront per warp and word when replicated per lane) and the increment is a ripple carry
+// through the slices.  With three slices the fields count to 8 and bias = 8 - (Wc - k); the carry out of the top
+// slice means ">= Wc - k of the occurrence's counted words match" -- a candidate, signalled at the word of the
+// (Wc-k)-th match.  Thresholds Wc - k <= 4 need only two slices (fields count to 4, bias = 4 - (Wc - k)).
 #pragma once
 #include <stdint.h>
 

@@ -193,10 +193,12 @@ __device__ __forceinline__ uint32_t dense_key(uint32_t lo, uint32_t hi) {
     return (lo * kHashMul + hi * kHashMul2) >> (32 - kDenseBits);
 }
 
-// Flush the warp's buffered hits to the global hit list (one atomicAdd for all of them).
+// Flush the warp's buffered hits to the global hit list (one atomicAdd for all of them).  The count can exceed the
+// 32 buffered entries in k_filter_dense2, whose lanes append with an atomic and send the hits past a full buffer
+// straight to the list: only the first 32 are flushed.
 __device__ __forceinline__ void dense_flush_hits(const MarkCtx &mc, uint32_t *scratch, int lane) {
     __syncwarp();
-    const uint32_t n = scratch[8];
+    const uint32_t n = min(scratch[8], 32u);
     if (n == 0) return;
     uint32_t base = 0;
     if (lane == 0) base = atomicAdd(&mc.counters[CNT_HITS], n);
@@ -491,27 +493,11 @@ k_filter_dense2(const ScanParams p, int64_t nvec, int64_t ntiles) {
                 }
             }
             __syncwarp();
-            if (mc.hits_cap && scratch[8] >= 16u) {  // warp-uniform (shared memory)
-                const uint32_t n = min(scratch[8], 32u);
-                uint32_t b0 = 0;
-                if (lane == 0) b0 = atomicAdd(&mc.counters[CNT_HITS], n);
-                b0 = __shfl_sync(0xFFFFFFFFu, b0, 0);
-                if ((uint32_t)lane < n && b0 + lane < mc.hits_cap) mc.hits[b0 + lane] = hbuf[lane];
-                __syncwarp();
-                if (lane == 0) scratch[8] = 0;
-                __syncwarp();
-            }
+            if (mc.hits_cap && scratch[8] >= 16u) dense_flush_hits(mc, scratch, lane);  // warp-uniform (shared memory)
         }
         }
     }
-    __syncwarp();
-    if (mc.hits_cap && scratch[8]) {
-        const uint32_t n = min(scratch[8], 32u);
-        uint32_t b0 = 0;
-        if (lane == 0) b0 = atomicAdd(&mc.counters[CNT_HITS], n);
-        b0 = __shfl_sync(0xFFFFFFFFu, b0, 0);
-        if ((uint32_t)lane < n && b0 + lane < mc.hits_cap) mc.hits[b0 + lane] = hbuf[lane];
-    }
+    if (mc.hits_cap) dense_flush_hits(mc, scratch, lane);  // what is still buffered
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -519,26 +505,38 @@ k_filter_dense2(const ScanParams p, int64_t nvec, int64_t ntiles) {
 // the same statements independently).  `sub` lives in shared memory, `seq` in global memory; both
 // are walked with a stride of +1 (right expansion) or -1 (left expansion, reversed slices of
 // levenshtein_ngram.py:186-188).  Returns true and (dist,len), or false for (None, None).
+// is_long selects the variant: _py_expand_long (:77-143, Ukkonen band) or _py_expand_short (:22-74, full rows and
+// the early break); levenshtein_ngram.py:16 picks it, fzb_debug_expand may force either.
 // ------------------------------------------------------------------------------------------------
 struct DpScratch {
     uint16_t scores[kMaxPattern + 1];
 };
 
 template <int DIR>
-__device__ bool expand_short(const uint8_t *sub, int sublen, const uint8_t *seq, int seqlen, int max_l,
-                             DpScratch &S, int &dist, int &len) {
-    if (sublen == 0) {  // :42-43
+__device__ bool expand_dp(const uint8_t *sub, int sublen, const uint8_t *seq, int seqlen, int max_l, bool is_long,
+                          DpScratch &S, int &dist, int &len) {
+    if (sublen == 0) {  // :42-43, :86-88
         dist = 0;
         len = 0;
         return true;
     }
-    for (int j = 0; j < sublen; j++) S.scores[j] = (uint16_t)(j + 1);  // :47
-    int min_score = sublen, min_idx = -1;                             // :49-50
-    for (int si = 0; si < seqlen; si++) {                             // :52
+    for (int j = 0; j < sublen; j++) S.scores[j] = (uint16_t)(j + 1);  // :47, :92
+    int min_score = sublen, min_idx = -1;                             // :49-50, :94-95
+    int max_good = max_l;                                             // :96
+    int new_start = 0, new_end = sublen - 1;                          // :97-98
+    bool ns_none = false;
+    for (int si = 0; si < seqlen; si++) {  // :52, :100
         const uint8_t ch = seq[DIR * si];
-        int a = si, c = si + 1;  // :54-55
+        const int rstart = is_long ? new_start : 0;                   // :102
+        const int rend = is_long ? min(sublen, new_end + 1) : sublen;  // :103
+        int a = si, c = si + 1;                                       // :54-55, :105-106
+        if (is_long) {                                                // :108-113
+            new_start = 0;
+            ns_none = !(c <= max_good);
+            new_end = ns_none ? -1 : 0;
+        }
         int row_min = 1 << 30;
-        for (int j = 0; j < sublen; j++) {  // :56-63
+        for (int j = rstart; j < rend; j++) {  // :56-63, :115-122
             int b = S.scores[j];
             int v = a + (ch != sub[DIR * j]);
             v = min(v, min(b + 1, c + 1));
@@ -546,57 +544,7 @@ __device__ bool expand_short(const uint8_t *sub, int sublen, const uint8_t *seq,
             S.scores[j] = (uint16_t)v;
             row_min = min(row_min, v);
             a = b;
-        }
-        if (c <= min_score) {  // :66-68
-            min_score = c;
-            min_idx = si;
-        } else if (row_min >= min_score) {  // :71-72
-            break;
-        }
-    }
-    if (min_score <= max_l) {  // :74
-        dist = min_score;
-        len = min_idx + 1;
-        return true;
-    }
-    return false;
-}
-
-template <int DIR>
-__device__ bool expand_long(const uint8_t *sub, int sublen, const uint8_t *seq, int seqlen, int max_l,
-                            DpScratch &S, int &dist, int &len) {
-    if (sublen == 0) {  // :86-88
-        dist = 0;
-        len = 0;
-        return true;
-    }
-    for (int j = 0; j < sublen; j++) S.scores[j] = (uint16_t)(j + 1);  // :92
-    int min_score = sublen, min_idx = -1;                             // :94-95
-    int max_good = max_l;                                             // :96
-    int new_start = 0, new_end = sublen - 1;                          // :97-98
-    bool ns_none = false;
-    for (int si = 0; si < seqlen; si++) {  // :100
-        const uint8_t ch = seq[DIR * si];
-        const int rstart = new_start;                 // :102
-        const int rend = min(sublen, new_end + 1);    // :103
-        int a = si, c = si + 1;                       // :105-106
-        if (c <= max_good) {                          // :108-113
-            new_start = 0;
-            ns_none = false;
-            new_end = 0;
-        } else {
-            new_start = 0;
-            ns_none = true;
-            new_end = -1;
-        }
-        for (int j = rstart; j < rend; j++) {  // :115-122
-            int b = S.scores[j];
-            int v = a + (ch != sub[DIR * j]);
-            v = min(v, min(b + 1, c + 1));
-            c = v;
-            S.scores[j] = (uint16_t)v;
-            a = b;
-            if (c <= max_good) {  // :124-130
+            if (is_long && c <= max_good) {  // :124-130
                 if (ns_none) {
                     ns_none = false;
                     new_start = j;
@@ -604,14 +552,23 @@ __device__ bool expand_long(const uint8_t *sub, int sublen, const uint8_t *seq, 
                 new_end = max(new_end, j + 1 + (max_good - c));
             }
         }
-        if (ns_none) break;                     // :133-134
-        if (rend == sublen && c <= min_score) {  // :137-141
-            min_score = c;
-            min_idx = si;
-            if (min_score < max_good) max_good = min_score;
+        if (is_long) {
+            if (ns_none) break;                     // :133-134
+            if (rend == sublen && c <= min_score) {  // :137-141
+                min_score = c;
+                min_idx = si;
+                if (min_score < max_good) max_good = min_score;
+            }
+        } else {
+            if (c <= min_score) {  // :66-68
+                min_score = c;
+                min_idx = si;
+            } else if (row_min >= min_score) {  // :71-72
+                break;
+            }
         }
     }
-    if (min_score <= max_l) {  // :143
+    if (min_score <= max_l) {  // :74, :143
         dist = min_score;
         len = min_idx + 1;
         return true;
@@ -706,9 +663,11 @@ template <int DIR>
 __device__ __forceinline__ bool expand_any(const uint8_t *sub, int sublen, const uint8_t *seq,
                                            int seqlen, int max_l, DpScratch &S, int &dist, int &len) {
     if (sublen <= kRegSub) return expand_uni_reg<DIR>(sub, sublen, seq, seqlen, max_l, dist, len);
+    // a constant flag per call: each inlined copy carries only its own variant's state (one copy holding both
+    // raises the register count of k_verify_lev<2>)
     if (sublen > max(2 * max_l, 10))  // levenshtein_ngram.py:16
-        return expand_long<DIR>(sub, sublen, seq, seqlen, max_l, S, dist, len);
-    return expand_short<DIR>(sub, sublen, seq, seqlen, max_l, S, dist, len);
+        return expand_dp<DIR>(sub, sublen, seq, seqlen, max_l, true, S, dist, len);
+    return expand_dp<DIR>(sub, sublen, seq, seqlen, max_l, false, S, dist, len);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -736,10 +695,36 @@ __device__ __forceinline__ void build_pm(unsigned long long *sPM, const uint8_t 
     }
 }
 
-template <typename Wt, int DIR>
-__device__ __forceinline__ bool expand_bp(const unsigned long long *sPM, int s_off, int sublen, const uint8_t *seq,
-                                          int seqlen, int max_l, int &dist, int &len, int variant = 0) {
-    // DIR = +1: sub = P[s_off : s_off+sublen];  DIR = -1: sub = reversed P[:s_off] (sublen == s_off)
+// Sources of the Eq mask of a haystack character c.  EqPM reads the pattern's table:
+// DIR = +1: sub = P[s_off : s_off+sublen];  DIR = -1: sub = reversed P[:s_off] (sublen == s_off).
+template <int DIR>
+struct EqPM {
+    const unsigned long long *sPM;
+    int s_off;
+    __device__ __forceinline__ unsigned long long operator()(uint8_t c) const {
+        const unsigned long long pm = sPM[c];
+        return DIR > 0 ? pm >> s_off : __brevll(pm) >> (64 - s_off);
+    }
+};
+
+// EqOtf compares c with the sub-pattern's characters on the fly (no per-pattern table): used where every LANE
+// verifies a different pattern (k_verify_mhits, batch_kernels.cuh) and a 2 KiB table per lane is out of the question.
+// sub[DIR * i] is character i of the sub-pattern; sublen <= 32.
+template <int DIR>
+struct EqOtf {
+    const uint8_t *sub;
+    int sublen;
+    __device__ __forceinline__ uint32_t operator()(uint8_t c) const {
+        uint32_t Eq = 0;
+        for (int i = 0; i < sublen; i++) Eq |= (uint32_t)(sub[DIR * i] == c) << i;
+        return Eq;
+    }
+};
+
+// The sub-pattern has sublen characters and eq(c) gives their Eq mask (EqPM or EqOtf, walked in the same DIR).
+template <typename Wt, int DIR, class EqFn>
+__device__ __forceinline__ bool expand_bp(const EqFn &eq, int sublen, const uint8_t *seq, int seqlen, int max_l,
+                                          int &dist, int &len, int variant = 0) {
     if (sublen == 0) {  // :42-43, :86-88
         dist = 0;
         len = 0;
@@ -751,8 +736,7 @@ __device__ __forceinline__ bool expand_bp(const unsigned long long *sPM, int s_o
     const Wt top = (Wt)1 << (sublen - 1);
     int score = sublen, min_score = sublen, min_idx = -1;  // :49-50, :94-95
     for (int si = 0; si < seqlen; si++) {
-        const unsigned long long pm = sPM[seq[DIR * si]];
-        const Wt Eq = DIR > 0 ? (Wt)(pm >> s_off) : (Wt)(__brevll(pm) >> (64 - s_off));
+        const Wt Eq = (Wt)eq(seq[DIR * si]);
         const Wt Xv = Eq | VN;
         const Wt Xh = (((Eq & VP) + VP) ^ VP) | Eq;
         Wt HP = VN | ~(Xh | VP);
@@ -793,55 +777,6 @@ struct DpHolder<2> {
     DpScratch s;
     __device__ __forceinline__ DpScratch *get() { return &s; }
 };
-
-// Same recurrence with the Eq mask computed on the fly from the sub-pattern's characters (no per-pattern table):
-// used where every LANE verifies a different pattern (k_verify_mhits, batch_kernels.cuh) and a 2 KiB table per lane
-// is out of the question.  sub[DIR * i] is character i of the sub-pattern; sublen <= 32.
-template <int DIR>
-__device__ __forceinline__ bool expand_bp_otf(const uint8_t *sub, int sublen, const uint8_t *seq, int seqlen,
-                                              int max_l, int &dist, int &len) {
-    if (sublen == 0) {
-        dist = 0;
-        len = 0;
-        return true;
-    }
-    const bool is_long = sublen > max(2 * max_l, 10);  // levenshtein_ngram.py:16
-    uint32_t VP = ~0u, VN = 0;
-    const uint32_t top = 1u << (sublen - 1);
-    int score = sublen, min_score = sublen, min_idx = -1;
-    for (int si = 0; si < seqlen; si++) {
-        const uint8_t ch = seq[DIR * si];
-        uint32_t Eq = 0;
-        for (int i = 0; i < sublen; i++) Eq |= (uint32_t)(sub[DIR * i] == ch) << i;
-        const uint32_t Xv = Eq | VN;
-        const uint32_t Xh = (((Eq & VP) + VP) ^ VP) | Eq;
-        uint32_t HP = VN | ~(Xh | VP);
-        uint32_t HN = VP & Xh;
-        score += (HP & top) ? 1 : 0;
-        score -= (HN & top) ? 1 : 0;
-        HP = (HP << 1) | 1u;
-        HN <<= 1;
-        VP = HN | ~(Xv | HP);
-        VN = HP & Xv;
-        if (score <= min_score) {
-            min_score = score;
-            min_idx = si;
-        } else if (!is_long) {
-            int v = si + 1, row_min = 1 << 30;
-            for (int j = 0; j < sublen; j++) {
-                v += (int)((VP >> j) & 1) - (int)((VN >> j) & 1);
-                row_min = min(row_min, v);
-            }
-            if (row_min >= min_score) break;
-        }
-    }
-    if (min_score <= max_l) {
-        dist = min_score;
-        len = min_idx + 1;
-        return true;
-    }
-    return false;
-}
 
 // Verification mode of a pattern: 0 = bit-parallel, 32-bit words (m <= 64, m-L <= 32); 1 = bit-parallel, 64-bit
 // words (m <= 64); 2 = cell-by-cell DP with the row in registers / local memory (longer patterns).
@@ -903,6 +838,20 @@ __device__ __forceinline__ int64_t stage_window(const PT &p, int64_t gbase, int 
     return alo;
 }
 
+// One lane's window for a hit whose occurrence would start at p0: H[max(p0-k, 0) : min(p0+m+k, N)), clipped to the
+// buffer, copied into the lane's private slot.  Returns the global position of slot[0].
+template <class PT>
+__device__ __forceinline__ int64_t stage_lane_window(const PT &p, int64_t p0, uint8_t *slot) {
+    const int64_t wlo = max(max(p0 - p.k, (int64_t)0), p.buf_lo);
+    const int64_t whi = min(min(p0 + p.m + p.k, p.N), p.buf_lo + p.buf_len);
+    const int64_t alo = wlo & ~(int64_t)3;
+    const int nwords = (int)((whi - alo + 3) >> 2);
+    const uint32_t *src = reinterpret_cast<const uint32_t *>(p.H + (alo - p.buf_lo));
+    uint32_t *dst = reinterpret_cast<uint32_t *>(slot);
+    for (int w = 0; w < nwords; w++) dst[w] = __ldg(src + w);
+    return alo;
+}
+
 // All lanes of the warp call this together (lanes without an anchor pass valid = false).  Each lane
 // first finds the next n-gram that really occurs at its anchor (cheap), THEN the lanes that found one
 // run the two expansions side by side (converged), and the search for further n-grams resumes.
@@ -954,11 +903,11 @@ __device__ void verify_anchor_lev(const PT &p, const uint8_t *sP, const unsigned
             const int64_t rhi = min(N, p0 + m + k);
             const int rlen = (int)max((int64_t)0, rhi - (idx + L));
             if (VM == 3)  // per-lane patterns: Eq on the fly (m - L <= 32)
-                ok = expand_bp_otf<1>(sP + s + L, m - s - L, h + L, rlen, k, dr, rs);
+                ok = expand_bp<uint32_t, 1>(EqOtf<1>{sP + s + L, m - s - L}, m - s - L, h + L, rlen, k, dr, rs);
             else if (VM == 0)
-                ok = expand_bp<uint32_t, 1>(sPM, s + L, m - s - L, h + L, rlen, k, dr, rs);
+                ok = expand_bp<uint32_t, 1>(EqPM<1>{sPM, s + L}, m - s - L, h + L, rlen, k, dr, rs);
             else if (VM == 1)
-                ok = expand_bp<unsigned long long, 1>(sPM, s + L, m - s - L, h + L, rlen, k, dr, rs);
+                ok = expand_bp<unsigned long long, 1>(EqPM<1>{sPM, s + L}, m - s - L, h + L, rlen, k, dr, rs);
             else
                 ok = expand_any<1>(sP + s + L, m - s - L, h + L, rlen, k, *S, dr, rs);
         }
@@ -967,11 +916,11 @@ __device__ void verify_anchor_lev(const PT &p, const uint8_t *sP, const unsigned
             const int64_t llo = max((int64_t)0, p0 - (k - dr));
             const int llen = (int)max((int64_t)0, idx - llo);
             if (VM == 3)
-                ok = expand_bp_otf<-1>(sP + s - 1, s, h - 1, llen, k - dr, dl, ls);
+                ok = expand_bp<uint32_t, -1>(EqOtf<-1>{sP + s - 1, s}, s, h - 1, llen, k - dr, dl, ls);
             else if (VM == 0)
-                ok = expand_bp<uint32_t, -1>(sPM, s, s, h - 1, llen, k - dr, dl, ls);
+                ok = expand_bp<uint32_t, -1>(EqPM<-1>{sPM, s}, s, h - 1, llen, k - dr, dl, ls);
             else if (VM == 1)
-                ok = expand_bp<unsigned long long, -1>(sPM, s, s, h - 1, llen, k - dr, dl, ls);
+                ok = expand_bp<unsigned long long, -1>(EqPM<-1>{sPM, s}, s, h - 1, llen, k - dr, dl, ls);
             else
                 ok = expand_any<-1>(sP + s - 1, s, h - 1, llen, k - dr, *S, dl, ls);
         }
@@ -993,6 +942,53 @@ __device__ void verify_anchor_lev(const PT &p, const uint8_t *sP, const unsigned
 // whole GPU instead of serialising on the warp that owns their bitmap words.  Each processed granule
 // clears its own bit; if the list overflows (dense candidates, e.g. small alphabets) the bits left
 // set are swept by the bitmap-scanning fallback loop of the same kernel launched in "scan" mode.
+// All lanes of a warp call this together and run body(granule) together, once per granule.
+// scan_mode == 0: process glist[0 .. CNT_GRAN) one granule per warp (the normal case: ONE verify launch per search).
+// scan_mode == 1: no list -- sweep the whole bitmap (the host's second attempt after the list overflowed).
+template <class Body>
+__device__ __forceinline__ void for_each_marked_granule(uint32_t *bitmap, uint64_t bitmap_words, const uint32_t *glist,
+                                                        uint32_t glist_cap, int scan_mode, uint32_t *counters,
+                                                        Body body) {
+    const int lane = threadIdx.x & 31;
+    if (!scan_mode) {
+        const uint32_t nitems = counters[CNT_GRAN];
+        if (nitems > glist_cap) {  // the work list overflowed (pathologically dense marks): the host repeats the search in
+            if (blockIdx.x == 0 && threadIdx.x == 0) counters[CNT_OVERFLOW] = 1;  // bitmap mode (scan_mode = 1, no list)
+            return;
+        }
+        for (;;) {
+            uint32_t item = 0;
+            if (lane == 0) item = atomicAdd(&counters[CNT_WORK], 1u);
+            item = __shfl_sync(0xFFFFFFFFu, item, 0);
+            if (item >= nitems) break;
+            const uint32_t g = glist[item];
+            body((int64_t)g);
+            if (lane == 0) atomicAnd(&bitmap[g >> 5], ~(1u << (g & 31)));
+        }
+        if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&counters[CNT_CAND], nitems);
+        return;
+    }
+    const uint64_t gwarp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    for (uint64_t wbase = gwarp * 32; wbase < bitmap_words; wbase += nwarps * 32) {
+        const uint64_t wi = wbase + lane;
+        uint32_t bits = wi < bitmap_words ? bitmap[wi] : 0u;
+        if (bits) bitmap[wi] = 0u;  // consumed: the bitmap is all-zero again when the kernel ends
+        unsigned active = __ballot_sync(0xFFFFFFFFu, bits != 0);
+        while (active) {
+            const int src = __ffs(active) - 1;
+            active &= active - 1;
+            uint32_t b = __shfl_sync(0xFFFFFFFFu, bits, src);
+            if (lane == 0) atomicAdd(&counters[CNT_CAND], (uint32_t)__popc(b));
+            while (b) {
+                const int bit = __ffs(b) - 1;
+                b &= b - 1;
+                body((int64_t)(wbase + src) * 32 + bit);
+            }
+        }
+    }
+}
+
 template <int VM, class PT>
 __device__ __forceinline__ void verify_granule_lev(const PT &p, const uint8_t *sP,
                                                    const unsigned long long *sPM, uint32_t *sWin, int64_t granule,
@@ -1009,8 +1005,6 @@ __device__ __forceinline__ void verify_granule_lev(const PT &p, const uint8_t *s
     }
 }
 
-// scan_mode == 0: process glist[0 .. CNT_GRAN) one granule per warp (the normal case: ONE verify launch per search).
-// scan_mode == 1: no list -- sweep the whole bitmap (the host's second attempt after the list overflowed).
 template <int VM>
 __global__ void __launch_bounds__(kVerifyThreads)
 k_verify_lev(const ScanParams p, uint64_t bitmap_words, const uint32_t *glist, uint32_t glist_cap, int scan_mode,
@@ -1018,7 +1012,6 @@ k_verify_lev(const ScanParams p, uint64_t bitmap_words, const uint32_t *glist, u
     __shared__ uint8_t sP[256];
     __shared__ unsigned long long sPM[VM < 2 ? 256 : 1];
     __shared__ uint32_t sWinAll[kVerifyThreads / 32][kWinWords];
-    const uint32_t ngran = counters[CNT_GRAN];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) sP[i] = p.P[i];
     if (VM < 2) build_pm(sPM, p.P, p.m, threadIdx.x, blockDim.x);
     __syncthreads();
@@ -1026,44 +1019,9 @@ k_verify_lev(const ScanParams p, uint64_t bitmap_words, const uint32_t *glist, u
     DpScratch *S = dp_holder.get();
     const int lane = threadIdx.x & 31;
     uint32_t *sWin = sWinAll[threadIdx.x >> 5];
-    if (!scan_mode) {
-        if (ngran > glist_cap) {  // the work list overflowed (pathologically dense marks): the host repeats the search in
-            if (blockIdx.x == 0 && threadIdx.x == 0) counters[CNT_OVERFLOW] = 1;  // bitmap mode (scan_mode = 1, no list)
-            return;
-        }
-        const uint32_t nitems = ngran;
-        for (;;) {
-            uint32_t item = 0;
-            if (lane == 0) item = atomicAdd(&counters[CNT_WORK], 1u);
-            item = __shfl_sync(0xFFFFFFFFu, item, 0);
-            if (item >= nitems) break;
-            const uint32_t g = glist[item];
-            verify_granule_lev<VM>(p, sP, sPM, sWin, (int64_t)g, lane, S, out, cap, counters);
-            if (lane == 0) atomicAnd(&p.bitmap[g >> 5], ~(1u << (g & 31)));
-        }
-        if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&counters[CNT_CAND], nitems);
-        return;
-    }
-    const uint64_t gwarp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
-    for (uint64_t wbase = gwarp * 32; wbase < bitmap_words; wbase += nwarps * 32) {
-        const uint64_t wi = wbase + lane;
-        uint32_t bits = wi < bitmap_words ? p.bitmap[wi] : 0u;
-        if (bits) p.bitmap[wi] = 0u;  // consumed: the bitmap is all-zero again when the kernel ends
-        unsigned active = __ballot_sync(0xFFFFFFFFu, bits != 0);
-        while (active) {
-            const int src = __ffs(active) - 1;
-            active &= active - 1;
-            uint32_t b = __shfl_sync(0xFFFFFFFFu, bits, src);
-            if (lane == 0) atomicAdd(&counters[CNT_CAND], (uint32_t)__popc(b));
-            while (b) {
-                const int bit = __ffs(b) - 1;
-                b &= b - 1;
-                verify_granule_lev<VM>(p, sP, sPM, sWin, (int64_t)(wbase + src) * 32 + bit, lane, S, out, cap,
-                                       counters);
-            }
-        }
-    }
+    for_each_marked_granule(p.bitmap, bitmap_words, glist, glist_cap, scan_mode, counters, [&](int64_t g) {
+        verify_granule_lev<VM>(p, sP, sPM, sWin, g, lane, S, out, cap, counters);
+    });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1106,14 +1064,7 @@ k_verify_hits(const ScanParams p, RawRec *out, uint32_t cap, uint32_t *counters)
             const uint64_t hv = p.hits[item];
             idx = (int64_t)(hv >> 8);
             j = (int)(hv & 0xFFu);
-            const int64_t p0 = idx - (int64_t)j * p.L;
-            const int64_t wlo = max(max(p0 - p.k, (int64_t)0), p.buf_lo);
-            const int64_t whi = min(min(p0 + p.m + p.k, p.N), p.buf_lo + p.buf_len);
-            alo = wlo & ~(int64_t)3;
-            const int nwords = (int)((whi - alo + 3) >> 2);
-            const uint32_t *src = reinterpret_cast<const uint32_t *>(p.H + (alo - p.buf_lo));
-            uint32_t *dst = reinterpret_cast<uint32_t *>(slot);
-            for (int w = 0; w < nwords; w++) dst[w] = __ldg(src + w);
+            alo = stage_lane_window(p, idx - (int64_t)j * p.L, slot);
         }
         verify_anchor_lev<VM>(p, sP, sPM, slot - alo, idx, valid, S, out, cap, counters, j, j + 1);  // whole warp
     }

@@ -141,34 +141,22 @@ __device__ __forceinline__ void lp_prefix_counts(const uint8_t *text, int nchars
     __syncthreads();
 }
 
-__global__ void __launch_bounds__(kLpThreads)
-k_lev_lp(const ScanParams p, uint32_t *scratch, int cap, RawRec *out, uint32_t ocap, uint32_t *counters) {
-    __shared__ uint8_t sP[256];
-    __shared__ int16_t sFirst[256];
+// The tile loop of k_lev_lp and k_generic_lp.  A start survives phase 1 when opens(c) holds for its character c
+// (condition (a), or always) and the count test (b) with a window of m + k characters passes; phase 2 calls
+// sim(W, start) for every survivor, W[g] being the byte at global position g.  All threads of the CTA call this;
+// what the callers set up in shared memory before it is ordered by its first barrier.
+template <class Opens, class Sim>
+__device__ __forceinline__ void lp_tiles(const ScanParams &p, Opens opens, Sim sim) {
     __shared__ uint8_t sClass[256];
     __shared__ __align__(16) uint8_t sH[kLpTile + kLpHalo];
     __shared__ uint16_t sCnt[kLpTile + kLpHalo + 2];
     __shared__ uint16_t sQueue[kLpTile];
     __shared__ uint32_t sQn;
     __shared__ uint32_t sWarpTot[kLpThreads / 32];
-    for (int i = threadIdx.x; i < 256; i += blockDim.x) {
-        sP[i] = p.P[i];
-        sFirst[i] = -1;
-        sClass[i] = 0;
-    }
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) sClass[i] = 0;
     __syncthreads();
-    if (threadIdx.x == 0) {  // make_char2first_subseq_index: first index of each char within P[:k+1]
-        for (int j = min(p.k, p.m - 1); j >= 0; j--) sFirst[p.P[j]] = (int16_t)j;
+    if (threadIdx.x == 0)
         for (int j = 0; j < p.m; j++) sClass[p.P[j]] = 1;
-    }
-    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    uint32_t *A = scratch + tid * 2 * (int64_t)cap, *B = A + cap;
-    if (p.k >= p.m) {  // levenshtein.py:62-65: an empty match (i,i,m) at every index 0..N
-        const int64_t hi = (p.own_hi == p.N) ? p.N + 1 : p.own_hi;
-        for (int64_t i = p.own_lo + tid; i < hi; i += stride) emit(out, ocap, counters, i, i, i, p.m, 1);
-        return;
-    }
     const int64_t hi = min(p.own_hi, p.N);
     const int ahead = p.m + p.k + 1;
     const int win = p.m + p.k, need = p.m - p.k;
@@ -178,21 +166,43 @@ k_lev_lp(const ScanParams p, uint32_t *scratch, int cap, RawRec *out, uint32_t o
         const int nload = (int)(load_hi - tile_lo);
         const int nwords = (nload + 3) >> 2;  // tile_lo is a multiple of 16: aligned words
         const uint32_t *src = reinterpret_cast<const uint32_t *>(p.H + (tile_lo - p.buf_lo));
-        __syncthreads();  // previous tile fully consumed (also orders sFirst / sClass on the first pass)
+        __syncthreads();  // previous tile fully consumed (also orders sClass on the first pass)
         for (int w = threadIdx.x; w < nwords; w += blockDim.x) reinterpret_cast<uint32_t *>(sH)[w] = __ldg(src + w);
         if (threadIdx.x == 0) sQn = 0;
         __syncthreads();
         lp_prefix_counts(sH, nload, sClass, sCnt, sWarpTot);
         for (int i = threadIdx.x; i < tile_n; i += blockDim.x)
-            if (sFirst[sH[i]] >= 0 && (int)sCnt[min(i + win, nload)] - (int)sCnt[i] >= need)
+            if (opens(sH[i]) && (int)sCnt[min(i + win, nload)] - (int)sCnt[i] >= need)
                 sQueue[atomicAdd(&sQn, 1u)] = (uint16_t)i;
         __syncthreads();
         const uint32_t qn = sQn;
         const uint8_t *W = sH - tile_lo;  // W[g]: byte at global position g
-        for (uint32_t q = threadIdx.x; q < qn; q += blockDim.x)
-            if (!sim_lev_lp(p, sP, W, tile_lo + sQueue[q], A, B, cap, out, ocap, counters))
-                atomicExch(&counters[CNT_OVERFLOW], 1u);
+        for (uint32_t q = threadIdx.x; q < qn; q += blockDim.x) sim(W, tile_lo + sQueue[q]);
     }
+}
+
+__global__ void __launch_bounds__(kLpThreads)
+k_lev_lp(const ScanParams p, uint32_t *scratch, int cap, RawRec *out, uint32_t ocap, uint32_t *counters) {
+    __shared__ uint8_t sP[256];
+    __shared__ int16_t sFirst[256];
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) {
+        sP[i] = p.P[i];
+        sFirst[i] = -1;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0)  // make_char2first_subseq_index: first index of each char within P[:k+1]
+        for (int j = min(p.k, p.m - 1); j >= 0; j--) sFirst[p.P[j]] = (int16_t)j;
+    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    uint32_t *A = scratch + tid * 2 * (int64_t)cap, *B = A + cap;
+    if (p.k >= p.m) {  // levenshtein.py:62-65: an empty match (i,i,m) at every index 0..N
+        const int64_t hi = (p.own_hi == p.N) ? p.N + 1 : p.own_hi;
+        for (int64_t i = p.own_lo + tid; i < hi; i += stride) emit(out, ocap, counters, i, i, i, p.m, 1);
+        return;
+    }
+    lp_tiles(p, [&](uint8_t c) { return sFirst[c] >= 0; }, [&](const uint8_t *W, int64_t st) {
+        if (!sim_lev_lp(p, sP, W, st, A, B, cap, out, ocap, counters)) atomicExch(&counters[CNT_OVERFLOW], 1u);
+    });
 }
 
 // ---- streaming form of the Levenshtein LP search -------------------------------------------------------------
@@ -214,6 +224,22 @@ constexpr int kLpsFlush = 1024;
 constexpr int kLpsBuf = kLpsFlush + kLpsCtaBytes;
 constexpr int kLpsMaxWin = 48;                                      // m + k: 15 + 48 <= 63 bits of look-ahead
 enum { CNT_LPLIST = 7, CNT_LPWORK = 8 };                            // (the hit-list slots of the dense route)
+
+// Moves the n entries of a CTA's shared-memory buffer sBuf to a global list: one atomicAdd on *list_n reserves
+// their slots (entries at or beyond cap are dropped; the count still tells the host that the list overflowed),
+// then the buffer count *sN is reset.  All nthreads threads of the CTA call it with the same n; sBase is a
+// __shared__ word for the reserved base.  The caller orders the reset before the next append.
+__device__ __forceinline__ void flush_cta_buffer(const unsigned long long *sBuf, uint32_t *sN, uint32_t n,
+                                                 uint32_t *sBase, unsigned long long *list, uint32_t cap,
+                                                 uint32_t *list_n, int nthreads) {
+    if (threadIdx.x == 0) *sBase = atomicAdd(list_n, n);
+    __syncthreads();
+    const uint32_t b0 = *sBase;
+    for (uint32_t i = threadIdx.x; i < n; i += nthreads)
+        if (b0 + i < cap) list[b0 + i] = sBuf[i];
+    __syncthreads();
+    if (threadIdx.x == 0) *sN = 0;
+}
 
 __global__ void __launch_bounds__(kLpsThreads)
 k_lp_scan(const ScanParams p, unsigned long long *list, uint32_t list_cap) {
@@ -275,26 +301,13 @@ k_lp_scan(const ScanParams p, unsigned long long *list, uint32_t list_cap) {
         // an iteration ahead, and the warps of the CTA must agree both on taking this branch (it contains barriers)
         // and on n.  Inside the branch nobody appends, so sN is stable.
         if (__syncthreads_or(full)) {
-            const uint32_t n = sN;
-            if (threadIdx.x == 0) sBase = atomicAdd(&p.counters[CNT_LPLIST], n);
-            __syncthreads();
-            const uint32_t b0 = sBase;
-            for (uint32_t i = threadIdx.x; i < n; i += blockDim.x)
-                if (b0 + i < list_cap) list[b0 + i] = sBuf[i];
-            __syncthreads();
-            if (threadIdx.x == 0) sN = 0;
+            flush_cta_buffer(sBuf, &sN, sN, &sBase, list, list_cap, &p.counters[CNT_LPLIST], blockDim.x);
             __syncthreads();
         }
     }
     __syncthreads();
     const uint32_t n = sN;
-    if (n) {
-        if (threadIdx.x == 0) sBase = atomicAdd(&p.counters[CNT_LPLIST], n);
-        __syncthreads();
-        const uint32_t b0 = sBase;
-        for (uint32_t i = threadIdx.x; i < n; i += blockDim.x)
-            if (b0 + i < list_cap) list[b0 + i] = sBuf[i];
-    }
+    if (n) flush_cta_buffer(sBuf, &sN, n, &sBase, list, list_cap, &p.counters[CNT_LPLIST], blockDim.x);
 }
 
 // Does the candidate born at `start` accept anywhere?  (see the header comment above; m <= 31, k <= K)
@@ -502,51 +515,66 @@ __device__ bool sim_generic(const ScanParams &p, const uint8_t *sP, const uint8_
 __global__ void __launch_bounds__(kLpThreads)
 k_generic_lp(const ScanParams p, uint32_t *scratch, int cap, RawRec *out, uint32_t ocap, uint32_t *counters) {
     __shared__ uint8_t sP[256];
-    __shared__ uint8_t sClass[256];
-    __shared__ __align__(16) uint8_t sH[kLpTile + kLpHalo];
-    __shared__ uint16_t sCnt[kLpTile + kLpHalo + 2];
-    __shared__ uint16_t sQueue[kLpTile];
-    __shared__ uint32_t sQn;
-    __shared__ uint32_t sWarpTot[kLpThreads / 32];
-    for (int i = threadIdx.x; i < 256; i += blockDim.x) {
-        sP[i] = p.P[i];
-        sClass[i] = 0;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0)
-        for (int j = 0; j < p.m; j++) sClass[p.P[j]] = 1;
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) sP[i] = p.P[i];
     const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t *A = scratch + tid * 2 * (int64_t)cap, *B = A + cap;
-    const int64_t hi = min(p.own_hi, p.N);
-    const int ahead = p.m + p.k + 1;
-    const int win = p.m + p.k, need = p.m - p.k;  // p.k = max_l
-    for (int64_t tile_lo = p.own_lo + (int64_t)blockIdx.x * kLpTile; tile_lo < hi; tile_lo += (int64_t)gridDim.x * kLpTile) {
-        const int tile_n = (int)min((int64_t)kLpTile, hi - tile_lo);
-        const int64_t load_hi = min(min(tile_lo + tile_n + ahead, p.N), p.buf_lo + p.buf_len);
-        const int nload = (int)(load_hi - tile_lo);
-        const int nwords = (nload + 3) >> 2;
-        const uint32_t *src = reinterpret_cast<const uint32_t *>(p.H + (tile_lo - p.buf_lo));
-        __syncthreads();
-        for (int w = threadIdx.x; w < nwords; w += blockDim.x) reinterpret_cast<uint32_t *>(sH)[w] = __ldg(src + w);
-        if (threadIdx.x == 0) sQn = 0;
-        __syncthreads();
-        lp_prefix_counts(sH, nload, sClass, sCnt, sWarpTot);
-        for (int i = threadIdx.x; i < tile_n; i += blockDim.x)
-            if ((int)sCnt[min(i + win, nload)] - (int)sCnt[i] >= need) sQueue[atomicAdd(&sQn, 1u)] = (uint16_t)i;
-        __syncthreads();
-        const uint32_t qn = sQn;
-        const uint8_t *W = sH - tile_lo;  // W[g]: byte at global position g
-        for (uint32_t q = threadIdx.x; q < qn; q += blockDim.x) {
-            const int64_t st = tile_lo + sQueue[q];
-            if (!sim_generic(p, sP, W, st, p.N, A, B, cap, st, 1, out, ocap, counters))
-                atomicExch(&counters[CNT_OVERFLOW], 1u);
-        }
-    }
+    lp_tiles(p, [](uint8_t) { return true; }, [&](const uint8_t *W, int64_t st) {  // (p.k = max_l)
+        if (!sim_generic(p, sP, W, st, p.N, A, B, cap, st, 1, out, ocap, counters))
+            atomicExch(&counters[CNT_OVERFLOW], 1u);
+    });
 }
 
 // Generic n-gram route: one warp per marked granule.  Phase 1: lane <-> anchor position, exact
 // n-gram test (generic_search.py:221-227).  Phase 2: for every hit, the lanes of the warp split
 // the starts of the clipped window (:229-237) and run the NFA.
+__device__ __forceinline__ void verify_granule_generic(const ScanParams &p, const uint8_t *sP, uint32_t *sWin,
+                                                       int64_t granule, int lane, uint32_t *A, uint32_t *B, int cap,
+                                                       RawRec *out, uint32_t ocap, uint32_t *counters) {
+    const int m = p.m, k = p.k, L = p.L;
+    const int64_t N = p.N;
+    const int64_t gbase = p.buf_lo + (granule << kGranuleShift);
+    const int64_t alo = stage_window(p, gbase, m + k, lane, sWin);
+    const uint8_t *W = reinterpret_cast<const uint8_t *>(sWin) - alo;  // W[g]: byte at global g
+    for (int half = 0; half < kGranule / 32; half++) {
+        const int64_t idx = gbase + half * 32 + lane;
+        const bool owned = idx >= p.own_lo && idx < p.own_hi;
+        for (int j = 0; j < p.n_ngrams; j++) {
+            const int s = j * L;
+            bool hit = false;
+            if (owned) {
+                int64_t ws = max((int64_t)0, (int64_t)(s - k));  // :223
+                int64_t we = min(N, N - m + s + L + k);          // :224
+                if (we > ws) {                                   // :225-226
+                    ws = max((int64_t)0, min(ws, N));
+                    we = max(ws, min(we, N));
+                    if (idx >= ws && idx + L <= we) {
+                        const uint8_t *h = W + idx;
+                        hit = true;
+                        for (int i = 0; i < L; i++)
+                            if (h[i] != sP[s + i]) {
+                                hit = false;
+                                break;
+                            }
+                    }
+                }
+            }
+            unsigned hits = __ballot_sync(0xFFFFFFFFu, hit);
+            while (hits) {
+                const int hl = __ffs(hits) - 1;
+                hits &= hits - 1;
+                const int64_t hidx = gbase + half * 32 + hl;
+                const int64_t p0 = hidx - s;
+                const int64_t wlo = max((int64_t)0, p0 - k);  // :231
+                const int64_t whi = min(N, p0 + m + k);
+                for (int64_t st = wlo + lane; st < whi; st += 32)
+                    if (!sim_generic(p, sP, W, st, whi, A, B, cap, hidx, j, out, ocap, counters))
+                        atomicExch(&counters[CNT_OVERFLOW], 1u);
+            }
+        }
+    }
+}
+
+// Sweeps the whole bitmap (the host launches it once per search, without a work list).
 __global__ void __launch_bounds__(kLpThreads)
 k_verify_generic(const ScanParams p, uint64_t bitmap_words, uint32_t *scratch, int cap, RawRec *out,
                  uint32_t ocap, uint32_t *counters) {
@@ -558,66 +586,9 @@ k_verify_generic(const ScanParams p, uint64_t bitmap_words, uint32_t *scratch, i
     uint32_t *sWin = sWinAll[threadIdx.x >> 5];
     const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t *A = scratch + tid * 2 * (int64_t)cap, *B = A + cap;
-    const uint64_t gwarp = (uint64_t)tid >> 5;
-    const uint64_t nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
-    const int m = p.m, k = p.k, L = p.L;
-    const int64_t N = p.N;
-    for (uint64_t wbase = gwarp * 32; wbase < bitmap_words; wbase += nwarps * 32) {
-        const uint64_t wi = wbase + lane;
-        uint32_t bits = wi < bitmap_words ? p.bitmap[wi] : 0u;
-        if (bits) p.bitmap[wi] = 0u;  // consumed: the bitmap is all-zero again when the kernel ends
-        unsigned active = __ballot_sync(0xFFFFFFFFu, bits != 0);
-        while (active) {
-            const int src = __ffs(active) - 1;
-            active &= active - 1;
-            uint32_t b = __shfl_sync(0xFFFFFFFFu, bits, src);
-            if (lane == 0) atomicAdd(&counters[CNT_CAND], (uint32_t)__popc(b));
-            while (b) {
-                const int bit = __ffs(b) - 1;
-                b &= b - 1;
-                const int64_t gbase = p.buf_lo + (((int64_t)(wbase + src) * 32 + bit) << kGranuleShift);
-                const int64_t alo = stage_window(p, gbase, m + k, lane, sWin);
-                const uint8_t *W = reinterpret_cast<const uint8_t *>(sWin) - alo;  // W[g]: byte at global g
-                for (int half = 0; half < kGranule / 32; half++) {
-                    const int64_t idx = gbase + half * 32 + lane;
-                    const bool owned = idx >= p.own_lo && idx < p.own_hi;
-                    for (int j = 0; j < p.n_ngrams; j++) {
-                        const int s = j * L;
-                        bool hit = false;
-                        if (owned) {
-                            int64_t ws = max((int64_t)0, (int64_t)(s - k));  // :223
-                            int64_t we = min(N, N - m + s + L + k);          // :224
-                            if (we > ws) {                                   // :225-226
-                                ws = max((int64_t)0, min(ws, N));
-                                we = max(ws, min(we, N));
-                                if (idx >= ws && idx + L <= we) {
-                                    const uint8_t *h = W + idx;
-                                    hit = true;
-                                    for (int i = 0; i < L; i++)
-                                        if (h[i] != sP[s + i]) {
-                                            hit = false;
-                                            break;
-                                        }
-                                }
-                            }
-                        }
-                        unsigned hits = __ballot_sync(0xFFFFFFFFu, hit);
-                        while (hits) {
-                            const int hl = __ffs(hits) - 1;
-                            hits &= hits - 1;
-                            const int64_t hidx = gbase + half * 32 + hl;
-                            const int64_t p0 = hidx - s;
-                            const int64_t wlo = max((int64_t)0, p0 - k);      // :231
-                            const int64_t whi = min(N, p0 + m + k);
-                            for (int64_t st = wlo + lane; st < whi; st += 32)
-                                if (!sim_generic(p, sP, W, st, whi, A, B, cap, hidx, j, out, ocap, counters))
-                                    atomicExch(&counters[CNT_OVERFLOW], 1u);
-                        }
-                    }
-                }
-            }
-        }
-    }
+    for_each_marked_granule(p.bitmap, bitmap_words, nullptr, 0, 1, counters, [&](int64_t g) {
+        verify_granule_generic(p, sP, sWin, g, lane, A, B, cap, out, ocap, counters);
+    });
 }
 
 }  // namespace fzb

@@ -1,8 +1,8 @@
 // CPU check of the Hamming counting filter's recurrences (fuzzysearch_b200/csrc/ham_recur.h), exactly as
 // k_hamming_count applies them: one "thread" per 128-byte row, 7 warm-up words from the previous row, candidates
 // tracked over the row's own 32 words, flagged rows mark a range of start positions.  For random texts with
-// planted near-matches, EVERY start p with Hamming(P, H[p:p+m]) <= k must fall inside a marked range -- for
-// the nibble-field layout and for the bit-sliced ones (three slices; two slices where Wc - k <= 4).  Prints the number of flagged rows of each (selectivity).
+// planted near-matches, EVERY start p with Hamming(P, H[p:p+m]) <= k must fall inside a marked range -- with three
+// slices, and with two slices where Wc - k <= 4.  Prints the number of flagged rows of each (selectivity).
 // Build + run: tests/test_ham_recurrence.py (g++ -O2).
 #include <cstdio>
 #include <cstdlib>
@@ -27,7 +27,7 @@ struct Range {
 
 int main() {
     const char *alphabets[] = {"ACGT", "ab", "abcdefghijklmnopqrstuvwxyz"};
-    long flagged_n = 0, flagged_s = 0, checked = 0, rows_total = 0, flagged_2 = 0, flagged_s_two = 0, n_two = 0;
+    long flagged_s = 0, checked = 0, rows_total = 0, flagged_2 = 0, flagged_s_two = 0, n_two = 0;
     for (int trial = 0; trial < 400; trial++) {
         const char *alpha = alphabets[trial % 3];
         const int alen = (int)strlen(alpha);
@@ -51,14 +51,9 @@ int main() {
             printf("bad parameters m=%d k=%d\n", m, k);
             return 1;
         }
-        // tables
-        std::vector<uint32_t> Tn(kHcBuckets * 4, (uint32_t)bias), Ts(kHcBuckets, 0u);
+        std::vector<uint32_t> Ts(kHcBuckets, 0u);  // the table
         for (int o0 = 0; o0 < 4; o0++)
-            for (int i = 0; i < Wc; i++) {
-                const uint32_t w = hc_gram(P.data(), o0 + 4 * i);
-                Tn[hc_bucket(w) * 4 + o0] += 1u << (4 * i);
-                Ts[hc_bucket(w)] |= 1u << (8 * o0 + i);
-            }
+            for (int i = 0; i < Wc; i++) Ts[hc_bucket(hc_gram(P.data(), o0 + 4 * i))] |= 1u << (8 * o0 + i);
         const long nrows = (n + 127) / 128;
         std::vector<uint8_t> buf((size_t)(nrows + 1) * 128 + 128, 0);  // row -1 (zeros) + rows + padding
         memcpy(&buf[128], H.data(), n);
@@ -68,27 +63,23 @@ int main() {
         };
         const uint32_t B0 = (bias & 1) ? 0x01010101u : 0u, B1 = (bias & 2) ? 0x01010101u : 0u,
                        B2 = (bias & 4) ? 0x01010101u : 0u;
-        const uint32_t flag_bit = 8u << (4 * (Wc - 1));
         const bool two = Wc - k <= 4;  // the two-slice layout applies
         const int bias2 = 4 - (Wc - k);
         const uint32_t C0 = (two && (bias2 & 1)) ? 0x01010101u : 0u, C1 = (two && (bias2 & 2)) ? 0x01010101u : 0u;
-        std::vector<Range> marks_n, marks_s, marks_2;
+        std::vector<Range> marks_s, marks_2;
         for (long r = 0; r < nrows; r++) {
-            uint32_t S[4] = {0, 0, 0, 0}, acc_n = 0, acc_s = 0, acc_2 = 0;
+            uint32_t acc_s = 0, acc_2 = 0;
             HamSliced cnt{0, 0, 0};
             HamSliced2 cnt2{0, 0};
             for (long t = r * 32 - 7; t < r * 32 + 32; t++) {
                 const uint32_t w = word(t);
                 const bool track = t >= r * 32;
-                for (int c = 0; c < 4; c++) S[c] = S[c] * 16u + Tn[hc_bucket(w) * 4 + c];
-                if (track) acc_n |= S[0] | S[1] | S[2] | S[3];
                 const uint32_t carry = ham_sliced_step(cnt, Ts[hc_bucket(w)], B0, B1, B2);
                 if (track) acc_s |= carry;
                 const uint32_t carry2 = two ? ham_sliced2_step(cnt2, Ts[hc_bucket(w)], C0, C1) : 0u;
                 if (track) acc_2 |= carry2;
             }
             const long pr_lo = 4 * (r * 32 - Wc + 1) - 3;
-            if (acc_n & flag_bit) marks_n.push_back({pr_lo < 0 ? 0 : pr_lo, 4 * (r * 32 + 31 - (Wc - 1))});
             if (acc_s) marks_s.push_back({pr_lo < 0 ? 0 : pr_lo, 4 * (r * 32 + 31)});
             if (acc_2) marks_2.push_back({pr_lo < 0 ? 0 : pr_lo, 4 * (r * 32 + 31)});
         }
@@ -97,7 +88,6 @@ int main() {
             flagged_2 += (long)marks_2.size();
             flagged_s_two += (long)marks_s.size();
         }
-        flagged_n += (long)marks_n.size();
         flagged_s += (long)marks_s.size();
         rows_total += nrows;
         for (long p = 0; p + m <= n; p++) {
@@ -105,19 +95,16 @@ int main() {
             for (int i = 0; i < m && nd <= k; i++) nd += H[p + i] != P[i];
             if (nd > k) continue;
             checked++;
-            bool in_n = false, in_s = false, in_2 = !two;
-            for (auto &g : marks_n) in_n |= (p >= g.lo && p <= g.hi);
+            bool in_s = false, in_2 = !two;
             for (auto &g : marks_s) in_s |= (p >= g.lo && p <= g.hi);
             for (auto &g : marks_2) in_2 |= (p >= g.lo && p <= g.hi);
-            if (!in_n || !in_s || !in_2) {
-                printf("MISS trial=%d m=%d k=%d Wc=%d p=%ld nibble=%d sliced=%d two=%d\n", trial, m, k, Wc, p, in_n, in_s,
-                       in_2);
+            if (!in_s || !in_2) {
+                printf("MISS trial=%d m=%d k=%d Wc=%d p=%ld three=%d two=%d\n", trial, m, k, Wc, p, in_s, in_2);
                 return 1;
             }
         }
     }
-    printf("ok: %ld true matches covered; flagged rows nibble=%ld sliced=%ld of %ld; two-slice layout in %ld trials: "
-           "%ld flagged rows (three slices: %ld)\n", checked, flagged_n, flagged_s, rows_total, n_two, flagged_2,
-           flagged_s_two);
+    printf("ok: %ld true matches covered; flagged rows with three slices=%ld of %ld; two-slice layout in %ld trials: "
+           "%ld flagged rows (three slices: %ld)\n", checked, flagged_s, rows_total, n_two, flagged_2, flagged_s_two);
     return 0;
 }
