@@ -329,6 +329,8 @@ static int check_shard(uint64_t buf_len, uint64_t buf_lo, uint64_t global_len, u
         (own_lo < own_hi && (own_lo < buf_lo || own_hi > buf_lo + buf_len)))
         return fail(FZB_E_INVALID, "inconsistent shard geometry");
     if (buf_lo % 16 != 0) return fail(FZB_E_INVALID, "buf_lo must be a multiple of 16");
+    // the batch passes pack buffer-relative positions into 40 bits (MdenseParams::hits, LpMultiParams::list)
+    if (buf_len >= (1ull << 40)) return fail(FZB_E_INVALID, "buf_len must be below 2^40");
     return FZB_OK;
 }
 
@@ -1850,6 +1852,12 @@ constexpr uint32_t kGtabSlots = 1u << 17;     // gram table (open addressing, <=
 constexpr uint32_t kMaxBatchGrams = 60000;    // distinct grams of one pass
 constexpr uint32_t kMaxBatchPostings = 1u << 20;
 constexpr uint32_t kMaxBatchPats = 4096;      // patterns of one pass
+// FZB_F_TINY_LIST (testing) shrinks, for that call only, the q-sample work list, the dense pass's hit list and the LP
+// survivor list to these capacities, and scans the LP starts in chunks of kTinyLpChunk (not a multiple of a tile or
+// of 128: every chunk seam falls inside a tile), so that tests reach the overflow fallbacks and the chunk seams
+constexpr uint32_t kTinyBatchCap = 8;
+constexpr uint32_t kTinyLpListCap = 1024;
+constexpr uint64_t kTinyLpChunk = 3000;
 
 static int ensure_batch_buffers(fzb_haystack *h) {
     if (h->d_mbits) return FZB_OK;
@@ -1965,8 +1973,9 @@ static int split_batch(const std::vector<RawRec> &raw, const std::vector<uint32_
 // the pass overflowed a device structure (the caller then searches these patterns one by one).
 // dense = false: the q-sample scan (k_filter_multi / k_verify_multi) over the 4-grams of the patterns;
 // dense = true: the n-gram-prefix scan at every position (k_filter_mdense / k_verify_mhits).
+// tiny: the capacities of FZB_F_TINY_LIST.
 static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, const uint32_t *ks,
-                      const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, bool dense) {
+                      const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, bool dense, bool tiny) {
     const uint32_t cnt = (uint32_t)ids.size();
     std::vector<BatchPat> pats(cnt);
     std::vector<uint32_t> pinfo(cnt);
@@ -2042,15 +2051,16 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
     mp.set = h->d_mset;
     mp.set_mask = h->mset_slots - 1;
     mp.work = h->d_mwork;
-    mp.work_cap = h->mwork_cap;
+    mp.work_cap = tiny ? std::min(h->mwork_cap, kTinyBatchCap) : h->mwork_cap;
     mp.counters = h->d_counters;
+    const uint32_t hits_cap = tiny ? std::min(h->mhits_cap, kTinyBatchCap) : h->mhits_cap;
     const int64_t nvec = (int64_t)(round_up(h->buf_len, 16) / 16);
     const int64_t ntiles = (nvec + kMultiTileVecs - 1) / kMultiTileVecs;
     std::vector<RawRec> raw;
     uint32_t cnts[CNT_COUNT];
     fzb_stats pass{};
     rc = run_batch_pass(h, [&]() -> int {
-        MdenseParams dp{mp, h->d_bpats, h->d_mhits, h->mhits_cap};
+        MdenseParams dp{mp, h->d_bpats, h->d_mhits, hits_cap};
         if (ntiles > 0) {
             const int grid = (int)std::min<int64_t>(ntiles, h->sm_count);
             if (dense)
@@ -2083,7 +2093,7 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
 // One shared scan for up to 64 LP-route patterns (k_lp_scan_multi / k_lp_verify_multi).  Same return convention
 // as batch_pass.
 static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, const uint32_t *ks,
-                         const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum) {
+                         const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, bool tiny) {
     const uint32_t cnt = (uint32_t)ids.size();
     std::vector<BatchPat> pats(cnt);
     std::vector<ulonglong2> lut(256, make_ulonglong2(0ull, 0ull));
@@ -2135,7 +2145,7 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
     lp.pats = h->d_bpats;
     lp.pm32 = d_pm32;
     lp.list = h->d_lmlist;
-    lp.list_cap = h->lmlist_cap;
+    lp.list_cap = tiny ? std::min(h->lmlist_cap, kTinyLpListCap) : h->lmlist_cap;
     lp.counters = h->d_counters;
     int per_sm = 2;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lp_scan_multi, kLmThreads, kLmSmem));
@@ -2143,7 +2153,7 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
     const int vgrid = h->sm_count * 4, sim_cap = 256;
     rc = ensure_scratch(h, (uint64_t)vgrid * kLpThreads * 2 * sim_cap);
     if (rc) return rc;
-    const uint64_t chunk = 256ull << 20;  // starts per scan: bounds the survivor list
+    const uint64_t chunk = tiny ? kTinyLpChunk : 256ull << 20;  // starts per scan: bounds the survivor list
     std::vector<RawRec> raw;
     uint32_t cnts[CNT_COUNT];
     fzb_stats pass{};
@@ -2213,9 +2223,12 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
         return rc < 0 ? rc : FZB_OK;
     };
     // patterns the shared scan can take: n-gram route, q-sample lemma holds, 4-grams selective on this haystack,
-    // short enough for the 64-bit match table; no special flags (forced routes, raw-only, multi-GPU reduction)
+    // short enough for the 64-bit match table; no special flags (forced routes, raw-only, multi-GPU reduction) other
+    // than FZB_F_TINY_LIST, which shrinks the capacities of the shared passes
+    const bool tiny = (flags & FZB_F_TINY_LIST) != 0;
+    const bool share = (flags & ~FZB_F_TINY_LIST) == 0 && h->buf_len > 0;
     std::vector<uint32_t> shared;
-    if (flags == 0 && h->buf_len > 0) {
+    if (share) {
         for (uint32_t i = 0; i < count; i++) {
             const uint32_t m = offsets[i + 1] - offsets[i], k = max_l_dist[i];
             if (m == 0 || m > (uint32_t)kBatchMaxM || k == 0 || k >= m) continue;
@@ -2240,12 +2253,12 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
             done -= ids.size();
             break;
         }
-        const int rc = settle(batch_pass(h, patterns, offsets, max_l_dist, ids, out, &sum, false), ids);
+        const int rc = settle(batch_pass(h, patterns, offsets, max_l_dist, ids, out, &sum, false, tiny), ids);
         if (rc) return rc;
     }
     // the n-gram-route patterns the lemma does not cover share a scan of their own (n-gram prefixes at every position)
     std::vector<uint32_t> dense_ids;
-    if (flags == 0 && h->buf_len > 0 && sample_collision_prob(h) == FZB_OK) {
+    if (share && sample_collision_prob(h) == FZB_OK) {
         double expect = 0.0;  // expected prefix hits per haystack position
         uint32_t dense_grams = 0;
         const double c3 = h->coll_prob * h->coll_prob * h->coll_prob;
@@ -2264,12 +2277,12 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
         }
     }
     if (dense_ids.size() >= 2) {
-        const int rc = settle(batch_pass(h, patterns, offsets, max_l_dist, dense_ids, out, &sum, true), dense_ids);
+        const int rc = settle(batch_pass(h, patterns, offsets, max_l_dist, dense_ids, out, &sum, true, tiny), dense_ids);
         if (rc) return rc;
     }
     // LP-route patterns (m // (k+1) < 3) share scans of 64 patterns each (bit-sliced window counters)
     std::vector<uint32_t> lp_ids;
-    if (flags == 0 && h->buf_len > 0) {
+    if (share) {
         for (uint32_t i = 0; i < count; i++) {
             if (out[i]) continue;
             const uint32_t m = offsets[i + 1] - offsets[i], k = max_l_dist[i];
@@ -2282,7 +2295,7 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
     for (size_t first = 0; first + 2 <= lp_ids.size(); first += 64) {
         std::vector<uint32_t> ids(lp_ids.begin() + first, lp_ids.begin() + std::min(lp_ids.size(), first + 64));
         if (ids.size() < 2) break;
-        const int rc = settle(batch_pass_lp(h, patterns, offsets, max_l_dist, ids, out, &sum), ids);
+        const int rc = settle(batch_pass_lp(h, patterns, offsets, max_l_dist, ids, out, &sum, tiny), ids);
         if (rc) return rc;
     }
     for (uint32_t i = 0; i < count; i++) {

@@ -181,7 +181,7 @@ enum { CNT_MHITS = 7, CNT_MHITWORK = 8 };
 struct MdenseParams {
     MultiParams mp;             // table pointers as for k_filter_multi (gtab keyed by the 3-byte prefix, postings pid << 8 | j)
     const BatchPat *pats;
-    unsigned long long *hits;   // idx | j << 40 | pid << 48
+    unsigned long long *hits;   // (idx - buf_lo) | j << 40 | pid << 48: buffer-relative, so buf_len < 2^40 (check_shard)
     uint32_t hits_cap;
 };
 
@@ -223,7 +223,7 @@ __device__ __noinline__ bool mdense_confirm(const MdenseParams &p, unsigned long
                         eq = false;
                         break;
                     }
-                if (eq) full |= mdense_append(p, sBuf, sN, (unsigned long long)g | ((unsigned long long)j << 40) | ((unsigned long long)pid << 48));
+                if (eq) full |= mdense_append(p, sBuf, sN, (unsigned long long)(g - p.mp.buf_lo) | ((unsigned long long)j << 40) | ((unsigned long long)pid << 48));
             }
         }
         slot = (slot + 1) & p.mp.gtab_mask;
@@ -319,7 +319,7 @@ k_verify_mhits(const __grid_constant__ MdenseParams p, RawRec *out, uint32_t cap
         int j = 0, tag = 0;
         if (valid) {
             const unsigned long long hv = p.hits[item];
-            idx = (int64_t)(hv & ((1ull << 40) - 1));
+            idx = p.mp.buf_lo + (int64_t)(hv & ((1ull << 40) - 1));
             j = (int)((hv >> 40) & 0xFFu);
             const uint32_t pid = (uint32_t)(hv >> 48);
             tag = (int)(pid << 8);
@@ -369,7 +369,8 @@ struct LpMultiParams {
     int wmax;                                      // longest m + k of the pass
     const BatchPat *pats;
     const uint32_t *pm32;                          // per pattern: 256 match masks {j : P[j] == c} (k_lp_verify_multi)
-    unsigned long long *list;                      // start | pattern << 40
+    unsigned long long *list;                      // (start - buf_lo) | pattern << 40: buffer-relative, so
+                                                   // buf_len < 2^40 (check_shard)
     uint32_t list_cap;
     uint32_t *counters;
 };
@@ -432,7 +433,7 @@ k_lp_scan_multi(const __grid_constant__ LpMultiParams p) {
                 while (surv) {
                     const int pid = __ffsll((long long)surv) - 1;
                     surv &= surv - 1;
-                    const unsigned long long ent = (unsigned long long)s | ((unsigned long long)pid << 40);
+                    const unsigned long long ent = (unsigned long long)(s - p.buf_lo) | ((unsigned long long)pid << 40);
                     if (slot < (uint32_t)kLmBuf) {
                         sBuf[slot] = ent;
                     } else {  // CTA buffer full: straight to the list
@@ -488,7 +489,7 @@ k_lm_refine(const __grid_constant__ LpMultiParams p, unsigned long long *kept, u
         const uint32_t i = base + threadIdx.x;
         if (i < n) {
             const unsigned long long ent = p.list[i];
-            const int64_t st = (int64_t)(ent & ((1ull << 40) - 1));
+            const int64_t st = p.buf_lo + (int64_t)(ent & ((1ull << 40) - 1));
             const uint32_t pid = (uint32_t)(ent >> 40);
             const BatchPat *bp = p.pats + pid;
             const int m = bp->m, k = bp->k, win = m + k, need = m - k;
@@ -594,7 +595,7 @@ k_lp_verify_multi(const __grid_constant__ LpMultiParams p, const unsigned long l
                     drained = true;
                 } else {
                     const unsigned long long ent = sorted[idx];
-                    st = (int64_t)(ent & ((1ull << 40) - 1));
+                    st = p.buf_lo + (int64_t)(ent & ((1ull << 40) - 1));
                     pid = (uint32_t)(ent >> 40);
                     const BatchPat *bp = p.pats + pid;
                     c.m = bp->m;

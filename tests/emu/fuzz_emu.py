@@ -3,7 +3,8 @@
     python tests/emu/fuzz_emu.py --seed 1 --trials 400 [--routes world,lev,ham,generic,exact,shard,batch,has]
 
 Far more geometry than the `-m gpu` suite can afford on a GPU budget: tiny and empty sequences, every pattern
-length, forced filters, capped work lists (overflow paths), shards with arbitrary seams, grid sizes (FZB_EMU_SMS),
+length, forced filters, capped work lists (overflow paths), shards with arbitrary seams (batches too, at global
+offsets up to 2^44), more than 64 LP patterns in one batch, grid sizes (FZB_EMU_SMS),
 both counter layouts of the Hamming filter (two or three slices, as the threshold selects them).  Every mismatch
 prints a reproducer line and the run exits non-zero.
 """
@@ -260,10 +261,18 @@ def batch_trial(rng):
     if rng.integers(3) == 0 and pats:
         pats.append(pats[0])  # duplicate pattern
         ks.append(ks[0])
+    if n >= 100 and rng.integers(4) == 0:  # past one LP pass: more than 64 LP-route patterns (m + k <= 31)
+        for _ in range(int(rng.integers(60, 140))):
+            k = int(rng.integers(1, 4 if len(alphabet) > 8 else 2))
+            pats.append(bytes(al[r2.integers(0, len(al), size=int(r2.integers(k + 1, min(3 * k + 2, 31 - k) + 1)))]))
+            ks.append(k)
+    flags = F.F_TINY_LIST if rng.integers(3) == 0 else 0  # small lists and LP chunks: overflow fallbacks, seams
+    if n >= 100 and rng.integers(2) == 0:
+        return batch_shards(rng, hay, pats, ks, flags, ("batch-shards", seed, len(alphabet), n, len(pats), flags))
     hs = F.Haystack.from_host(hay)
-    ctx = ("batch", seed, len(alphabet), n, len(pats))
+    ctx = ("batch", seed, len(alphabet), n, len(pats), flags)
     try:
-        results, _ = hs.search_levenshtein_batch(pats, ks)
+        results, _ = hs.search_levenshtein_batch(pats, ks, flags)
     except F.UnsupportedError:
         hs.close()
         return
@@ -282,6 +291,51 @@ def batch_trial(rng):
             fail("batch-raw-k0", ctx + (i, len(p)))
         res.close()
     hs.close()
+
+
+def batch_shards(rng, hay, pats, ks, flags, ctx):
+    """The batch on 1..5 shards with random 16-aligned seams (halo >= every m + k), at global offset 0 or as the
+    interior of a longer sequence at an offset up to 2^44: the union of the shards' raw streams, shifted back, is
+    the oracle's raw stream of the records whose owner -- n-gram occurrence, or start on the LP and exact routes --
+    lies in the shards' own range."""
+    n = len(hay)
+    halo = max(len(p) + k for p, k in zip(pats, ks))
+    shift = int(rng.choice([0, 1 << 32, (1 << 40) - 4096, 1 << 40, 1 << 44])) + 16 * int(rng.integers(0, 1 << 20))
+    a, b = (0, n) if shift == 0 else ((halo + 15) // 16 * 16, n - halo)
+    if a >= b:
+        return
+    cuts = sorted(set(int(x) // 16 * 16 for x in rng.integers(a + 1, b, size=int(rng.integers(0, 5)))))
+    bounds = [a] + [c for c in cuts if a < c < b] + [b]
+    ctx = ctx + (bounds, shift)
+    union = [[] for _ in pats]
+    for i in range(len(bounds) - 1):
+        lo, hi = bounds[i], bounds[i + 1]
+        blo = max(0, lo - halo) // 16 * 16
+        bhi = min(n, hi + halo)
+        hs = F.Haystack.from_host(hay[blo:bhi], buf_lo=shift + blo, global_len=shift + n + (1 << 20 if shift else 0),
+                                  own_lo=shift + lo, own_hi=shift + hi)
+        try:
+            results, _ = hs.search_levenshtein_batch(pats, ks, flags)
+        except F.UnsupportedError:
+            hs.close()
+            return
+        except Exception as e:  # noqa: BLE001
+            fail("batch-shards-exception %r" % (e,), ctx + (i,))
+            hs.close()
+            return
+        for q, res in enumerate(results):
+            union[q] += [(s - shift, e - shift, d) for s, e, d in res.triples(F.RAW)]
+            res.close()
+        hs.close()
+    for q, (p, k) in enumerate(zip(pats, ks)):
+        if k and len(p) // (k + 1) >= 3:
+            raw, _, owner = oracle.levenshtein_ngrams_raw(p, hay, k, with_anchor=True)
+        else:
+            raw = oracle.levenshtein_raw(p, hay, k)
+            owner = [r[0] for r in raw]
+        want = sorted(t for t, o in zip(tup(raw), owner) if a <= o < b)
+        if sorted(union[q]) != want:
+            fail("batch-shards", ctx + (q, len(p), k, len(union[q]), len(want)))
 
 
 def has_trial(rng):

@@ -21,6 +21,7 @@ import pytest
 
 import conftest
 import test_gpu_batch
+import test_gpu_batch_edges
 import test_gpu_expand
 import test_gpu_file
 import test_gpu_fuzz
@@ -120,6 +121,18 @@ def test_emu_batches(emu_device):
     test_gpu_batch.test_batch_shared_scan_edge_cases(emu_device)
     test_gpu_batch.test_batch_lp_pass_with_large_budgets(emu_device)
     test_gpu_batch.test_batch_dense_pass_flushes_and_overflows_its_cta_buffer(emu_device)
+
+
+def test_emu_batch_edges(emu_device):
+    """Batches on shards at 64-bit offsets, sharded unions, past the pass limits, through the overflow fallbacks
+    and across the LP chunk seams (the 600 MiB seam test needs a real GPU)."""
+    test_gpu_batch_edges.test_batch_at_64_bit_offsets(emu_device)
+    _run(test_gpu_batch_edges.test_batch_sharded_union_equals_whole, emu_device)
+    _run(test_gpu_batch_edges.test_batch_lp_pass_limits, emu_device)
+    test_gpu_batch_edges.test_batch_two_q_sample_passes(emu_device)
+    test_gpu_batch_edges.test_batch_gram_with_more_than_255_postings(emu_device)
+    test_gpu_batch_edges.test_batch_overflow_fallbacks(emu_device)
+    test_gpu_batch_edges.test_batch_lp_chunk_seams(emu_device)
 
 
 def test_emu_file_search(emu_device, tmp_path):
