@@ -1625,20 +1625,29 @@ static int ensure_scratch(fzb_haystack *h, uint64_t words) {
     return FZB_OK;
 }
 
+// FZB_F_TINY_LIST (testing) caps the survivor list of the streaming LP search (and of the batch LP pass) at this many
+// entries for that call only, so that tests reach its overflow fallback
+constexpr uint32_t kTinyLpListCap = 1024;
+
+// Per-thread candidate capacities of the LP-style searches: 256, 2 048, then kLpMaxCap entries per list.  The slab
+// is threads x 2 lists x cap x 4 B: 17.7 GB at 16 384 with 132 SMs (4 CTAs of 256 threads each), 141 GB at the next
+// step, so a start with more live candidates than kLpMaxCap fails the search.
+constexpr int kLpMaxCap = 16384;
+
 // Runs an LP-style search with growing per-thread candidate capacity until no list overflowed.
 // `enqueue(grid, cap)` must put every kernel of one attempt on the stream.
 template <class F>
 static int run_lp(fzb_haystack *h, fzb_result *res, F enqueue, PostPlan post = PostPlan()) {
     const int grid = h->sm_count * 4;
     const uint64_t threads = (uint64_t)grid * kLpThreads;
-    for (int cap = 256; cap <= (1 << 16); cap *= 8) {
+    for (int cap = 256; cap <= kLpMaxCap; cap *= 8) {
         int rc = ensure_scratch(h, threads * 2 * (uint64_t)cap);
         if (rc) return rc;
         rc = run_emitting(h, res, [&]() -> int { return enqueue(grid, cap); }, post);
         if (rc) return rc;
         if (!h->h_counters[CNT_OVERFLOW]) return FZB_OK;
     }
-    return fail(FZB_E_UNSUPPORTED, "candidate explosion: more than 65536 live candidates for one start");
+    return fail(FZB_E_UNSUPPORTED, "candidate explosion: more than 16384 live candidates for one start");
 }
 
 static int search_lev_lp(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t k, uint32_t flags,
@@ -1661,11 +1670,12 @@ static int search_lev_lp(fzb_haystack *h, const uint8_t *pattern, uint32_t m, ui
     }
     const PostPlan plan{post_mode, post_mode != 0 && (flags & FZB_F_GLOBAL) != 0};
     if (streaming) {
+        const uint32_t list_cap = (flags & FZB_F_TINY_LIST) ? std::min(h->lplist_cap, kTinyLpListCap) : h->lplist_cap;
         rc = run_lp(h, res, [&](int grid, int cap) -> int {
-            k_lp_scan<<<h->sm_count * 4, kLpsThreads, 0, h->stream>>>(p, h->d_lplist, h->lplist_cap);
+            k_lp_scan<<<h->sm_count * 4, kLpsThreads, 0, h->stream>>>(p, h->d_lplist, list_cap);
             CK(cudaEventRecord(h->ev[1], h->stream));
             h->ev1_recorded = true;
-            k_lp_verify<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_lplist, h->lplist_cap, h->d_scratch, cap, h->d_out,
+            k_lp_verify<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_lplist, list_cap, h->d_scratch, cap, h->d_out,
                                                             h->out_cap, h->d_counters);
             res->stats.n_launches += 2;
             return FZB_OK;
@@ -1852,11 +1862,11 @@ constexpr uint32_t kGtabSlots = 1u << 17;     // gram table (open addressing, <=
 constexpr uint32_t kMaxBatchGrams = 60000;    // distinct grams of one pass
 constexpr uint32_t kMaxBatchPostings = 1u << 20;
 constexpr uint32_t kMaxBatchPats = 4096;      // patterns of one pass
-// FZB_F_TINY_LIST (testing) shrinks, for that call only, the q-sample work list, the dense pass's hit list and the LP
-// survivor list to these capacities, and scans the LP starts in chunks of kTinyLpChunk (not a multiple of a tile or
-// of 128: every chunk seam falls inside a tile), so that tests reach the overflow fallbacks and the chunk seams
+// FZB_F_TINY_LIST (testing) shrinks, for that call only, the q-sample work list and the dense pass's hit list to
+// kTinyBatchCap, the batch LP survivor list to kTinyLpListCap, and scans the LP starts in chunks of kTinyLpChunk (not
+// a multiple of a tile or of 128: every chunk seam falls inside a tile), so that tests reach the overflow fallbacks
+// and the chunk seams
 constexpr uint32_t kTinyBatchCap = 8;
-constexpr uint32_t kTinyLpListCap = 1024;
 constexpr uint64_t kTinyLpChunk = 3000;
 
 static int ensure_batch_buffers(fzb_haystack *h) {

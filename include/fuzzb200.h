@@ -57,8 +57,9 @@ extern "C" {
 #define FZB_F_FORCE_DENSE 2u  /* force the every-position candidate filter (testing) */
 #define FZB_F_FORCE_LP 4u     /* Levenshtein/generic: force the "linear programming" route */
 #define FZB_F_FORCE_NGRAMS 8u /* Levenshtein/generic/Hamming: force the n-gram route */
-#define FZB_F_TINY_LIST 16u   /* testing: cap the granule work list and the hit list at 8 entries (overflow paths);
-                                 batches: small work, hit and survivor lists and 3 000-start LP chunks */
+#define FZB_F_TINY_LIST 16u   /* testing: cap the granule work list and the hit list at 8 entries and the LP
+                                 survivor list at 1 024 (overflow paths); batches: small work, hit and survivor
+                                 lists and 3 000-start LP chunks */
 #define FZB_F_FORCE_SAMPLED 64u /* testing: use the sampled filter whenever its lemma holds, even if the
                                  byte statistics say it is not selective */
 #define FZB_F_GLOBAL 32u      /* multi-GPU: FINAL becomes the GLOBAL consolidated list of all shards: every rank

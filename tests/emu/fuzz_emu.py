@@ -4,7 +4,8 @@
 
 Far more geometry than the `-m gpu` suite can afford on a GPU budget: tiny and empty sequences, every pattern
 length, forced filters, capped work lists (overflow paths), shards with arbitrary seams (batches too, at global
-offsets up to 2^44), more than 64 LP patterns in one batch, grid sizes (FZB_EMU_SMS),
+offsets up to 2^44), more than 64 LP patterns in one batch, LP budgets up to 12 and windows up to 60, generic limits
+up to 63 in linear shapes, grid sizes (FZB_EMU_SMS),
 both counter layouts of the Hamming filter (two or three slices, as the threshold selects them).  Every mismatch
 prints a reproducer line and the run exits non-zero.
 """
@@ -63,7 +64,8 @@ def lev_trial(rng):
     m = len(pat)
     k = int(rng.integers(0, min(m, 6) + 1)) if rng.integers(4) else int(rng.integers(0, min(m + 2, 41)))
     if k > 0 and m // (k + 1) < 3:  # LP route: exponential candidate lists on repetitive text (reference too)
-        k = min(k, 3)
+        # budgets up to 12 and windows m + k up to 60 on text (every k_lp_verify mode, streaming and tile windows)
+        k = min(k, 12, max(60 - m, 1)) if len(alphabet) > 8 and rng.integers(2) else min(k, 3)
         hay = hay[:3000 if len(alphabet) <= 8 else 30000]
     if len(alphabet) <= 8 and k > 3:
         hay = hay[:3000]
@@ -135,10 +137,20 @@ def ham_trial(rng):
 
 
 def generic_trial(rng):
-    alphabet, pat, hay, seed = random_case(rng, mmax=64)
+    linear = rng.integers(3) == 0  # one limit up to 63, the others 0: the NFA stays linear, any length is cheap
+    alphabet, pat, hay, seed = random_case(rng, mmax=255 if linear else 64)
     m = len(pat)
-    subs, ins, dels = (int(x) for x in rng.integers(0, 4, size=3))
-    l = int(rng.integers(0, 5)) if rng.integers(3) else None
+    if linear:
+        lim = [0, 0, 0]
+        lim[int(rng.integers(3))] = int(rng.integers(1, 64))
+        subs, ins, dels = lim
+        l = max(lim) if rng.integers(2) else None
+    else:
+        subs, ins, dels = (int(x) for x in rng.integers(0, 4, size=3))
+        l = int(rng.integers(0, 5)) if rng.integers(3) else None
+        if m // ((l or 0) + 1) < 3 and rng.integers(2):  # LP route: windows m + max_l up to 60
+            subs, ins, dels = (int(x) for x in rng.integers(0, 7, size=3))
+            l = int(rng.integers(0, min(12, max(60 - m, 1)) + 1))
     try:
         subs, ins, dels, l = oracle.normalize_params(subs, ins, dels, l)
     except Exception:  # noqa: BLE001

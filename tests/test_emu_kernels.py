@@ -27,6 +27,7 @@ import test_gpu_file
 import test_gpu_fuzz
 import test_gpu_global
 import test_gpu_golden
+import test_gpu_lp_generic_edges
 import test_gpu_oracle
 import test_gpu_python_api
 import test_gpu_symbols
@@ -133,6 +134,22 @@ def test_emu_batch_edges(emu_device):
     test_gpu_batch_edges.test_batch_gram_with_more_than_255_postings(emu_device)
     test_gpu_batch_edges.test_batch_overflow_fallbacks(emu_device)
     test_gpu_batch_edges.test_batch_lp_chunk_seams(emu_device)
+
+
+def test_emu_lp_generic_edges(emu_device):
+    """The LP and generic routes at their limits: every k_lp_verify mode, streaming windows 47-50, the survivor-list
+    overflow (FZB_F_TINY_LIST), candidate-list growth and the 16 384 limit, 6-bit counters at 63, clipped n-gram
+    windows, sharded unions and offsets up to 2^44."""
+    _run(test_gpu_lp_generic_edges.test_lp_verify_and_window_boundaries, emu_device)
+    _run(test_gpu_lp_generic_edges.test_lp_scan_look_ahead, emu_device)
+    test_gpu_lp_generic_edges.test_lp_survivor_list_overflow(emu_device)
+    _run(test_gpu_lp_generic_edges.test_candidate_list_growth, emu_device)
+    test_gpu_lp_generic_edges.test_candidate_limit(emu_device)
+    _run(test_gpu_lp_generic_edges.test_generic_counters_at_63, emu_device)
+    test_gpu_lp_generic_edges.test_generic_lowering_rule(emu_device)
+    _run(test_gpu_lp_generic_edges.test_generic_ngram_windows_at_global_ends, emu_device)
+    _run(test_gpu_lp_generic_edges.test_lp_generic_sharded_union_equals_whole, emu_device)
+    test_gpu_lp_generic_edges.test_lp_generic_at_64_bit_offsets(emu_device)
 
 
 def test_emu_file_search(emu_device, tmp_path):
