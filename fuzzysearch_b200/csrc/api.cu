@@ -325,7 +325,10 @@ static int haystack_common_init(fzb_haystack *h) {
 
 static int check_shard(uint64_t buf_len, uint64_t buf_lo, uint64_t global_len, uint64_t own_lo,
                        uint64_t own_hi) {
-    if (buf_lo + buf_len > global_len || own_lo > own_hi || own_hi > global_len ||
+    // k_post's canonical keys and k_merge's winner scores hold a position in 46 bits; the LP route's empty match
+    // (N, N, m) is one of them, so N itself must fit
+    if (global_len >= (1ull << 46)) return fail(FZB_E_INVALID, "global_len must be below 2^46");
+    if (buf_lo > global_len || buf_len > global_len - buf_lo || own_lo > own_hi || own_hi > global_len ||
         (own_lo < own_hi && (own_lo < buf_lo || own_hi > buf_lo + buf_len)))
         return fail(FZB_E_INVALID, "inconsistent shard geometry");
     if (buf_lo % 16 != 0) return fail(FZB_E_INVALID, "buf_lo must be a multiple of 16");

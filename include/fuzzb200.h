@@ -88,6 +88,8 @@ int fzb_haystack_create(const uint8_t *host, uint64_t n, int device, fzb_haystac
  * own_hi + halo) with halo = len(pattern) + max_l_dist of the searches to be run (checked per
  * search).  Window clipping rules of the reference apply at 0 and global_len only, never at shard
  * seams, so the union of the shards' raw streams equals the single-device raw stream.
+ * global_len must be below 2^46 (FZB_E_INVALID otherwise): the on-device ordering and the multi-GPU merge keep a
+ * position in 46 bits.
  */
 int fzb_haystack_create_shard(const uint8_t *host, uint64_t buf_len, uint64_t buf_lo,
                               uint64_t global_len, uint64_t own_lo, uint64_t own_hi, int device,

@@ -3,7 +3,8 @@
     python tests/emu/fuzz_emu.py --seed 1 --trials 400 [--routes world,lev,ham,generic,exact,shard,batch,has]
 
 Far more geometry than the `-m gpu` suite can afford on a GPU budget: tiny and empty sequences, every pattern
-length, forced filters, capped work lists (overflow paths), shards with arbitrary seams (batches too, at global
+length, forced filters, capped work lists (overflow paths), occurrences at the q-sample lemma's margin, shards with
+arbitrary seams and copies anchored at them (batches too, at global
 offsets up to 2^44), more than 64 LP patterns in one batch, LP budgets up to 12 and windows up to 60, generic limits
 up to 63 in linear shapes, grid sizes (FZB_EMU_SMS),
 both counter layouts of the Hamming filter (two or three slices, as the threshold selects them).  Every mismatch
@@ -26,6 +27,7 @@ from conftest import load_emulated_library  # noqa: E402
 from corpus import ASCII, DNA, make_corpus  # noqa: E402
 from fuzzysearch_b200 import _native as F  # noqa: E402
 from parity import tup  # noqa: E402
+from test_gpu_ngram_edges import one_word_plant  # noqa: E402
 
 ALPHABETS = [b"a", b"ab", DNA, b"abcdefgh", ASCII, bytes(range(256))]
 if os.environ.get("FZB_FUZZ_ZEROS"):  # the buffers are zero-padded: patterns and text made of zero bytes
@@ -72,6 +74,13 @@ def lev_trial(rng):
     if len(alphabet) <= 2:
         hay = hay[:1500]
         k = min(k, 2)
+    if k > 0 and m >= k + 3 and (m - k - 3) // 4 >= k + 1 and len(hay) > 4 * m and rng.integers(2):
+        # occurrences at the q-sample lemma's margin: k deletions, each in a different aligned word
+        for _ in range(int(rng.integers(1, 9))):
+            r = int(rng.integers(4))
+            occ, _ = one_word_plant(rng, pat, k, r)
+            s0 = int(rng.integers(0, len(hay) - len(occ) + 1)) // 4 * 4 + r
+            hay[s0:s0 + len(occ)] = np.frombuffer(occ, dtype=np.uint8)[:len(hay) - s0]
     cpu = oracle.levenshtein_raw(pat, hay, k)
     if len(cpu) > 300000:
         return
@@ -218,9 +227,16 @@ def shard_trial(rng):
         n = len(hay)
         k = min(k, 2)
     nshards = int(rng.integers(2, 6))
-    cuts = sorted(set(int(x) // 16 * 16 for x in rng.integers(1, n, size=nshards - 1)))
+    # seams at 16-byte multiples and at offsets 1, 15 (mod 16) and 63 (mod 64)
+    cuts = sorted(set(int(x) // 64 * 64 + int(rng.choice([0, 16, 1, 15, 63])) for x in rng.integers(1, n, size=nshards - 1)))
     bounds = [0] + [c for c in cuts if 0 < c < n] + [n]
     halo = m + k
+    if k > 0 and m // (k + 1) > 0 and rng.integers(2):  # copies anchored at own_hi - 1 / own_lo through any n-gram
+        L = m // (k + 1)
+        for b in bounds[1:-1]:
+            p0 = b - 1 + int(rng.integers(2)) - int(rng.integers(m // L)) * L
+            if 0 <= p0 <= n - m:
+                hay[p0:p0 + m] = np.frombuffer(pat, dtype=np.uint8)
     whole = sorted(tup(oracle.levenshtein_raw(pat, hay, k)))
     if len(whole) > 200000:
         return

@@ -28,6 +28,7 @@ import test_gpu_fuzz
 import test_gpu_global
 import test_gpu_golden
 import test_gpu_lp_generic_edges
+import test_gpu_ngram_edges
 import test_gpu_oracle
 import test_gpu_python_api
 import test_gpu_symbols
@@ -150,6 +151,19 @@ def test_emu_lp_generic_edges(emu_device):
     _run(test_gpu_lp_generic_edges.test_generic_ngram_windows_at_global_ends, emu_device)
     _run(test_gpu_lp_generic_edges.test_lp_generic_sharded_union_equals_whole, emu_device)
     test_gpu_lp_generic_edges.test_lp_generic_at_64_bit_offsets(emu_device)
+
+
+def test_emu_ngram_edges(emu_device):
+    """The n-gram Levenshtein route at its margins: the q-sample lemma, every byte offset of the dense filters, the
+    verify modes and the hit slot, the hand-over to the host and to a larger output buffer, sharded unions."""
+    _run(test_gpu_ngram_edges.test_sampled_filter_at_the_lemma_margin, emu_device)
+    _run(test_gpu_ngram_edges.test_dense_filters_at_every_byte_offset, emu_device)
+    _run(test_gpu_ngram_edges.test_verify_kernels_at_their_limits, emu_device)
+    test_gpu_ngram_edges.test_same_match_through_several_ngrams(emu_device)
+    _run(test_gpu_ngram_edges.test_post_hand_over, emu_device)
+    _run(test_gpu_ngram_edges.test_post_groups_across_rounds, emu_device)
+    _run(test_gpu_ngram_edges.test_output_buffer_growth, emu_device)
+    _run(test_gpu_ngram_edges.test_ngram_sharded_union_equals_whole, emu_device)
 
 
 def test_emu_file_search(emu_device, tmp_path):

@@ -243,3 +243,26 @@ def test_positions_are_64_bit_everywhere(cuda_device):
             rb.close()
         a.close()
         b.close()
+    # the last positions a handle can hold: k_post's keys and k_merge's scores keep a position in 46 bits, so a shard
+    # may end at global_len = 2^46 - 1 (the LP route's empty match (N, N, m) included) and no further
+    top = (1 << 46) - 1
+    n = 4095  # the shard's buf_lo = top - n is a multiple of 16
+    pat, hay, _ = make_corpus(46, n, ASCII, 20, 10, 3)
+    a = F.Haystack.from_host(hay, buf_lo=0, global_len=n, own_lo=256, own_hi=n)
+    b = F.Haystack.from_host(hay, buf_lo=top - n, global_len=top, own_lo=top - n + 256, own_hi=top)
+    calls = [lambda h: h.search_levenshtein(pat, 2), lambda h: h.search_levenshtein(pat, 2, F.F_FORCE_DENSE),
+             lambda h: h.search_levenshtein(pat, 2, F.F_TINY_LIST), lambda h: h.search_hamming(pat, 3),
+             lambda h: h.search_exact(pat), lambda h: h.search_generic(pat, 2, 1, 1, 2),
+             lambda h: h.search_levenshtein(pat[:8], 3), lambda h: h.search_levenshtein(pat[:4], 4)]  # LP, LP k >= m
+    for ci, call in enumerate(calls):
+        ra, rb = call(a), call(b)
+        for which in (F.RAW, F.FINAL):
+            ta, tb = sorted(ra.triples(which)), sorted(rb.triples(which))
+            assert ta and [(s + top - n, e + top - n, d) for s, e, d in ta] == tb, (ci, which)
+        ra.close()
+        rb.close()
+    a.close()
+    b.close()
+    for glen, blo in (((1 << 46), (1 << 46) - 4096), ((1 << 46), 0), ((1 << 64) - 1, 0)):
+        with pytest.raises(ValueError, match="global_len must be below 2"):
+            F.Haystack.from_host(hay, buf_lo=blo, global_len=glen, own_lo=blo, own_hi=blo + n)
