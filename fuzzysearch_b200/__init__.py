@@ -50,20 +50,41 @@ def has_near_match(subsequence, sequence, max_substitutions=None, max_insertions
         return hay.has_near_match(pat, min(subs, big), min(ins, big), min(dels, big), l)
 
 
-def find_near_matches_batch(subsequences, sequence, max_l_dist):
+def find_near_matches_batch(subsequences, sequence, max_l_dist=None, *, max_substitutions=None,
+                            max_insertions=None, max_deletions=None):
     """Many patterns over one sequence (uploaded once): -> list of find_near_matches(...) results.
 
-    `max_l_dist` is one int or one per pattern.  Equivalent to
-    ``[find_near_matches(p, sequence, max_l_dist=k) for p, k in zip(subsequences, ks)]``."""
+    Each limit is None, one int, or one value per pattern.  Equivalent to
+    ``[find_near_matches(p, sequence, max_substitutions=s, max_insertions=i, max_deletions=d, max_l_dist=l)
+    for p, s, i, d, l in zip(subsequences, ...)]``: exact and Levenshtein searches share passes over the
+    sequence (fzb_search_levenshtein_batch), substitutions-only searches too (fzb_search_hamming_batch), and
+    searches with other limits run one by one on the same uploaded sequence."""
     from . import _native
     subsequences = list(subsequences)
-    ks = [max_l_dist] * len(subsequences) if isinstance(max_l_dist, int) else list(max_l_dist)
-    if len(ks) != len(subsequences):
-        raise ValueError("one max_l_dist per subsequence expected")
-    for p, k in zip(subsequences, ks):
-        LevenshteinSearchParams(None, None, None, k)  # same validation as find_near_matches
+    n = len(subsequences)
+
+    def per_pattern(name, value):
+        if value is None or isinstance(value, int):
+            return [value] * n
+        try:
+            value = list(value)
+        except TypeError:  # not a limit: LevenshteinSearchParams rejects it as find_near_matches does
+            return [value] * n
+        if len(value) != n:
+            raise ValueError("one %s per subsequence expected" % name)
+        return value
+
+    limits = list(zip(per_pattern("max_substitutions", max_substitutions),
+                      per_pattern("max_insertions", max_insertions),
+                      per_pattern("max_deletions", max_deletions), per_pattern("max_l_dist", max_l_dist)))
+    params, classes = [], []
+    for p, lim in zip(subsequences, limits):
+        sp = LevenshteinSearchParams(*lim)  # same validation as find_near_matches
+        cls = choose_search_class(sp)
         if len(p) == 0:
-            raise ValueError("Given subsequence is empty!")
+            raise ValueError("subsequence must not be empty" if cls is ExactSearch else "Given subsequence is empty!")
+        params.append(sp)
+        classes.append(cls)
     if not subsequences:
         return []
     from .search import AlphabetTooLarge, _lock_for, _prepare_many
@@ -73,13 +94,27 @@ def find_near_matches_batch(subsequences, sequence, max_l_dist):
         except AlphabetTooLarge:
             # wide symbols and more than 255 distinct ones over all the patterns: no common byte alphabet,
             # so the patterns go one by one (each reduces the sequence to its own alphabet)
-            return [find_near_matches(p, sequence, max_l_dist=k) for p, k in zip(subsequences, ks)]
-        results, _ = hay.search_levenshtein_batch(pats, ks)
+            return [find_near_matches(p, sequence, *lim) for p, lim in zip(subsequences, limits)]
+        results = [None] * n
+        lev = [i for i in range(n) if classes[i] in (ExactSearch, LevenshteinSearch)]
+        ham = [i for i in range(n) if classes[i] is SubstitutionsOnlySearch]
+        if lev:
+            rs, _ = hay.search_levenshtein_batch([pats[i] for i in lev], [params[i].max_l_dist for i in lev])
+            for i, r in zip(lev, rs):
+                results[i] = r
+        if ham:  # the limit SubstitutionsOnlySearch.search applies
+            ks = [min(x for x in (params[i].max_l_dist, params[i].max_substitutions) if x is not None) for i in ham]
+            rs, _ = hay.search_hamming_batch([pats[i] for i in ham], ks)
+            for i, r in zip(ham, rs):
+                results[i] = r
+        for i in range(n):
+            if classes[i] is GenericSearch:
+                results[i] = hay.search_generic(pats[i], *params[i].unpacked)
         out = []
-        for res, k in zip(results, ks):
-            # max_l_dist == 0 selects ExactSearch in find_near_matches (__init__.py:65-66), whose result is
-            # the unconsolidated occurrence list (search_exact.py:80-89): the RAW stream of the k == 0 route
-            s, e, d = res.arrays(_native.RAW if k == 0 else _native.FINAL)
+        for res, cls in zip(results, classes):
+            # ExactSearch does not consolidate (search_exact.py:80-89): its list is the RAW stream of the k == 0
+            # route; the Hamming results have FINAL == RAW
+            s, e, d = res.arrays(_native.RAW if cls is ExactSearch else _native.FINAL)
             out.append([Match(a, b, c, matched=slicer(a, b)) for a, b, c in zip(s.tolist(), e.tolist(), d.tolist())])
             res.close()
     return out

@@ -26,6 +26,7 @@
 #include "post_kernels.cuh"
 #include "p2p_kernels.cuh"
 #include "batch_kernels.cuh"
+#include "ham_batch_kernels.cuh"
 #include "sym_kernels.cuh"
 #include <unordered_map>
 #include "debug_kernels.cuh"
@@ -1214,11 +1215,13 @@ static int check_halo(const fzb_haystack *h, uint64_t halo) {
     return FZB_OK;
 }
 
+constexpr uint64_t kMaxRawRecs = 1ull << 27;  // raw records of one search (or one shared batch pass)
+
 static int ensure_out_cap(fzb_haystack *h, uint64_t need) {
     if (need <= h->out_cap) return FZB_OK;
     uint64_t cap = h->out_cap;
     while (cap < need) cap *= 2;
-    if (cap > (1ull << 27)) return fail(FZB_E_UNSUPPORTED, "more than 2^27 raw matches in one search");
+    if (cap > kMaxRawRecs) return fail(FZB_E_UNSUPPORTED, "more than 2^27 raw matches in one search");
     CK(cudaFree(h->d_out));
     h->d_out = nullptr;
     CK(cudaMalloc(&h->d_out, (size_t)cap * (sizeof(RawRec) + sizeof(uint64_t))));
@@ -1905,8 +1908,8 @@ static void add_stats(fzb_stats *sum, const fzb_stats &s) {
 
 // The attempt loop of a batch pass.  `enqueue()` puts the kernels of one attempt on h->stream (behind h->ev[0]) and
 // returns FZB_OK, an error, or +1 when a device structure of the pass overflowed.  Returns the same, +1 also when a
-// kernel raised CNT_OVERFLOW; an attempt whose raw records did not fit the output buffer is redone with a larger
-// one.  On FZB_OK `raw` holds the records, `cnts` the counters, and `pass` the time and the bytes scanned.
+// kernel raised CNT_OVERFLOW or the pass emitted more than kMaxRawRecs records; an attempt whose raw records did not
+// fit the output buffer is redone with a larger one.  On FZB_OK `raw` holds the records, `cnts` the counters, and `pass` the time and the bytes scanned.
 template <class F>
 static int run_batch_pass(fzb_haystack *h, F enqueue, std::vector<RawRec> &raw, uint32_t cnts[CNT_COUNT],
                           fzb_stats &pass) {
@@ -1922,6 +1925,9 @@ static int run_batch_pass(fzb_haystack *h, F enqueue, std::vector<RawRec> &raw, 
         if (rc) return rc;
         if (cnts[CNT_OVERFLOW]) return 1;
         const uint32_t n = cnts[CNT_OUT];
+        // more records than one search may return, over all the patterns of the pass: they go one by one, where
+        // each pattern only has to stay within the limit on its own
+        if (n > kMaxRawRecs) return 1;
         if (n > h->out_cap) {
             rc = ensure_out_cap(h, n);
             if (rc) return rc;
@@ -1942,10 +1948,11 @@ static int run_batch_pass(fzb_haystack *h, F enqueue, std::vector<RawRec> &raw, 
 }
 
 // Splits the raw records of a pass over the patterns ids[] (`ngram` = pattern ordinal << 8 | n-gram) into the results
-// out[ids[i]], consolidates each list, and adds the pass to `sum`.  Every result carries the pass's route, the first
-// one its other stats (the haystack is read once for the whole pass).
+// out[ids[i]], consolidates each list (unconsolidated: FINAL is the raw list in canonical order, as the Hamming
+// search returns it), and adds the pass to `sum`.  Every result carries the pass's route, the first one its other
+// stats (the haystack is read once for the whole pass).
 static int split_batch(const std::vector<RawRec> &raw, const std::vector<uint32_t> &ids, const fzb_stats &pass,
-                       int raw_order, fzb_result **out, fzb_stats *sum) {
+                       int raw_order, bool unconsolidated, fzb_result **out, fzb_stats *sum) {
     const uint32_t cnt = (uint32_t)ids.size();
     std::vector<uint32_t> per(cnt, 0);
     for (const RawRec &r : raw) per[(uint32_t)r.ngram >> 8]++;
@@ -1970,7 +1977,11 @@ static int split_batch(const std::vector<RawRec> &raw, const std::vector<uint32_
         for (uint32_t i = next.fetch_add(1); i < cnt; i = next.fetch_add(1)) {
             fzb_result *res = out[ids[i]];
             res->raw_n = (uint32_t)res->raw.size();
-            consolidate_recs(res->raw, res->fin, &res->hulls);
+            res->unconsolidated = unconsolidated;
+            if (unconsolidated)
+                finalize_on_host(res, 2);
+            else
+                consolidate_recs(res->raw, res->fin, &res->hulls);
             res->have_fin = true;
         }
     };
@@ -1980,6 +1991,56 @@ static int split_batch(const std::vector<RawRec> &raw, const std::vector<uint32_
     for (auto &t : pool) t.join();
     add_stats(sum, pass);
     return FZB_OK;
+}
+
+// Builds the posting table of a pass -- open addressing on the key (key * kGramMul), each slot the key and its first
+// posting | count << 24, a key with more than 255 postings spilling into further slots -- lets `mark(key)` set the
+// key's bits in `bits`, and uploads bits, table, postings, pinfo and the patterns.
+template <class F>
+static int upload_pass_tables(fzb_haystack *h, const std::unordered_map<uint32_t, std::vector<uint32_t>> &grams,
+                              const std::vector<uint32_t> &bits, const std::vector<uint32_t> &pinfo,
+                              const std::vector<BatchPat> &pats, F mark) {
+    std::vector<uint32_t> postings;
+    std::vector<uint2> gtab(kGtabSlots, make_uint2(0, 0));
+    for (auto &g : grams) {
+        const uint32_t w = g.first;
+        mark(w);
+        for (size_t first = 0; first < g.second.size(); first += 255) {
+            const uint32_t c = (uint32_t)std::min<size_t>(255, g.second.size() - first);
+            uint32_t slot = (w * kGramMul) & (kGtabSlots - 1);
+            while (gtab[slot].y != 0u) slot = (slot + 1) & (kGtabSlots - 1);
+            gtab[slot] = make_uint2(w, (uint32_t)postings.size() | (c << 24));
+            postings.insert(postings.end(), g.second.begin() + first, g.second.begin() + first + c);
+        }
+    }
+    int rc = ensure_batch_buffers(h);
+    if (rc) return rc;
+    CK(cudaSetDevice(h->device));
+    CK(cudaMemcpyAsync(h->d_mbits, bits.data(), bits.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_gtab, gtab.data(), gtab.size() * sizeof(uint2), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_postings, postings.data(), postings.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_pinfo, pinfo.data(), pinfo.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    // (pageable sources: each copy has left its host vector when it returns)
+    CK(cudaMemcpyAsync(h->d_bpats, pats.data(), pats.size() * sizeof(BatchPat), cudaMemcpyHostToDevice, h->stream));
+    return FZB_OK;
+}
+
+// The handle's geometry and the uploaded tables as the pass kernels see them.
+static MultiParams pass_params(const fzb_haystack *h) {
+    MultiParams mp{};
+    mp.H = h->d;
+    mp.buf_lo = (int64_t)h->buf_lo;
+    mp.buf_len = (int64_t)h->buf_len;
+    mp.N = (int64_t)h->global_len;
+    mp.own_lo = (int64_t)h->own_lo;
+    mp.own_hi = (int64_t)h->own_hi;
+    mp.bits = h->d_mbits;
+    mp.gtab = h->d_gtab;
+    mp.gtab_mask = kGtabSlots - 1;
+    mp.postings = h->d_postings;
+    mp.pinfo = h->d_pinfo;
+    mp.counters = h->d_counters;
+    return mp;
 }
 
 // One pass over the haystack for the patterns ids[0..cnt): fills out[ids[i]].  Returns FZB_OK, an error, or +1 if
@@ -2018,54 +2079,27 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
             }
         }
     }
-    std::vector<uint32_t> bits(kMultiTblWords + (dense ? 0 : kMulti2Words), 0), postings;
-    std::vector<uint2> gtab(kGtabSlots, make_uint2(0, 0));
-    for (auto &g : grams) {
-        const uint32_t w = g.first, hb = (w * kHashMul) >> (32 - kMultiTblBits);
+    std::vector<uint32_t> bits(kMultiTblWords + (dense ? 0 : kMulti2Words), 0);
+    int rc = upload_pass_tables(h, grams, bits, pinfo, pats, [&](uint32_t w) {
+        const uint32_t hb = (w * kHashMul) >> (32 - kMultiTblBits);
         bits[hb >> 5] |= 1u << (hb & 31u);
         if (!dense) {
             const uint32_t h2 = multi_hash2(w);
             bits[kMultiTblWords + (h2 >> 5)] |= 1u << (h2 & 31u);
         }
-        for (size_t first = 0; first < g.second.size(); first += 255) {
-            const uint32_t c = (uint32_t)std::min<size_t>(255, g.second.size() - first);
-            uint32_t slot = (w * kGramMul) & (kGtabSlots - 1);
-            while (gtab[slot].y != 0u) slot = (slot + 1) & (kGtabSlots - 1);
-            gtab[slot] = make_uint2(w, (uint32_t)postings.size() | (c << 24));
-            postings.insert(postings.end(), g.second.begin() + first, g.second.begin() + first + c);
-        }
-    }
-    int rc = ensure_batch_buffers(h);
+    });
     if (rc) return rc;
-    CK(cudaSetDevice(h->device));
     if (dense && !h->d_mhits) {
         h->mhits_cap = 1u << 23;
         CK(cudaMalloc(&h->d_mhits, (size_t)h->mhits_cap * sizeof(unsigned long long)));
         CK(cudaFuncSetAttribute(k_filter_mdense, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMdenseSmem));
     }
-    CK(cudaMemcpyAsync(h->d_mbits, bits.data(), bits.size() * 4, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_gtab, gtab.data(), gtab.size() * sizeof(uint2), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_postings, postings.data(), postings.size() * 4, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_pinfo, pinfo.data(), pinfo.size() * 4, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_bpats, pats.data(), pats.size() * sizeof(BatchPat), cudaMemcpyHostToDevice, h->stream));
-    MultiParams mp{};
-    mp.H = h->d;
-    mp.buf_lo = (int64_t)h->buf_lo;
-    mp.buf_len = (int64_t)h->buf_len;
-    mp.N = (int64_t)h->global_len;
-    mp.own_lo = (int64_t)h->own_lo;
-    mp.own_hi = (int64_t)h->own_hi;
-    mp.bits = h->d_mbits;
+    MultiParams mp = pass_params(h);
     mp.bits2 = dense ? nullptr : h->d_mbits + kMultiTblWords;
-    mp.gtab = h->d_gtab;
-    mp.gtab_mask = kGtabSlots - 1;
-    mp.postings = h->d_postings;
-    mp.pinfo = h->d_pinfo;
     mp.set = h->d_mset;
     mp.set_mask = h->mset_slots - 1;
     mp.work = h->d_mwork;
     mp.work_cap = tiny ? std::min(h->mwork_cap, kTinyBatchCap) : h->mwork_cap;
-    mp.counters = h->d_counters;
     const uint32_t hits_cap = tiny ? std::min(h->mhits_cap, kTinyBatchCap) : h->mhits_cap;
     const int64_t nvec = (int64_t)(round_up(h->buf_len, 16) / 16);
     const int64_t ntiles = (nvec + kMultiTileVecs - 1) / kMultiTileVecs;
@@ -2100,7 +2134,7 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
     pass.filter_ms = filter_ms;
     pass.n_candidates = cnts[CNT_CAND];
     pass.n_launches = 2;
-    return split_batch(raw, ids, pass, 0, out, sum);
+    return split_batch(raw, ids, pass, 0, false, out, sum);
 }
 
 // One shared scan for up to 64 LP-route patterns (k_lp_scan_multi / k_lp_verify_multi).  Same return convention
@@ -2210,7 +2244,21 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
     pass.route = 3;
     pass.filter_ms = scan_ms;
     pass.n_candidates = n_work;
-    return split_batch(raw, ids, pass, 1, out, sum);
+    return split_batch(raw, ids, pass, 1, false, out, sum);
+}
+
+// The outcome `rc` of a shared pass over the patterns ids[] of a batch of `count` results: an error drops every
+// result; an overflow (+1) drops the pass's results, leaving its patterns to the one-by-one path.
+static int settle_pass(int rc, const std::vector<uint32_t> &ids, fzb_result **out, uint32_t count) {
+    auto drop = [&](uint32_t j) {
+        if (out[j]) fzb_result_destroy(out[j]);
+        out[j] = nullptr;
+    };
+    if (rc < 0)
+        for (uint32_t j = 0; j < count; j++) drop(j);
+    if (rc > 0)
+        for (uint32_t id : ids) drop(id);
+    return rc < 0 ? rc : FZB_OK;
 }
 
 extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
@@ -2222,19 +2270,7 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
     for (uint32_t i = 0; i < count; i++)
         if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
     fzb_stats sum{};
-    auto drop = [&](uint32_t j) {
-        if (out[j]) fzb_result_destroy(out[j]);
-        out[j] = nullptr;
-    };
-    // the outcome of a shared pass: an error drops every result; an overflow leaves the pass's patterns to the
-    // one-by-one path below
-    auto settle = [&](int rc, const std::vector<uint32_t> &ids) -> int {
-        if (rc < 0)
-            for (uint32_t j = 0; j < count; j++) drop(j);
-        if (rc > 0)
-            for (uint32_t id : ids) drop(id);
-        return rc < 0 ? rc : FZB_OK;
-    };
+    auto settle = [&](int rc, const std::vector<uint32_t> &ids) { return settle_pass(rc, ids, out, count); };
     // patterns the shared scan can take: n-gram route, q-sample lemma holds, 4-grams selective on this haystack,
     // short enough for the 64-bit match table; no special flags (forced routes, raw-only, multi-GPU reduction) other
     // than FZB_F_TINY_LIST, which shrinks the capacities of the shared passes
@@ -2499,6 +2535,200 @@ extern "C" int fzb_search_hamming(fzb_haystack *h, const uint8_t *pattern, uint3
         res->raw_order = 1;
         return FZB_OK;
     });
+}
+
+// ------------------------------------------------------------------------------------------------
+// Substitutions-only batches: one scan for many patterns (ham_batch_kernels.cuh)
+// ------------------------------------------------------------------------------------------------
+// Bounds on the postings walked per haystack position (expected piece hits, from the sampled byte statistics).
+// Measured on an H100 80GB HBM3 (400 W power limit), 4 GiB of DNA, 1 024 patterns (tools/probe_ham_batch.py): three
+// passes walked 2.21e9 postings in 85 ms of scan, 0.039 ns per posting, against 1.6 ms for one scan of the haystack.
+// A pattern whose postings cost more than one scan (0.01 per position on 4 GiB) is searched on its own; a pass is
+// closed at 0.25 per position (at most 0.25 x 4.29e9 x 0.039 ns = 42 ms of verification behind one 1.6 ms read of
+// 4 GiB; the three measured passes averaged 28 ms).
+constexpr double kHamBatchPatExpect = 0.01;
+constexpr double kHamBatchExpect = 0.25;
+constexpr uint32_t kMaxHamBatchPostings = kMaxBatchGrams;  // postings of one pass (so <= that many distinct keys)
+
+// Key width of pattern (m, k) in a pass, in symbols: 2-bit keys are always 8 symbols wide (a piece of 5..7 symbols
+// is entered under every completion); text keys are the first min(L, 4) bytes of a piece, one width per pass.  0 when
+// no pass can take the pattern: too long for the pass's pattern slots, every start matches, or a piece too short for
+// a selective key.
+static uint32_t ham_batch_key(uint32_t m, uint32_t k, bool two_bit) {
+    if (m > (uint32_t)kBatchMaxM || k >= m) return 0;
+    const uint32_t L = m / (k + 1);
+    if (two_bit) return L >= 5 ? (uint32_t)kHbKeySyms : 0;
+    return L >= 3 ? std::min<uint32_t>(L, 4) : 0;
+}
+
+// Postings of pattern (m, k) in a pass: one per piece, or per completion of a 2-bit key shorter than 8 symbols.
+static uint32_t ham_batch_postings(uint32_t m, uint32_t k, bool two_bit) {
+    const uint32_t L = m / (k + 1);
+    return (k + 1) * (two_bit && L < (uint32_t)kHbKeySyms ? 1u << (2 * (kHbKeySyms - L)) : 1u);
+}
+
+// Expected postings per haystack position of pattern (m, k) in a pass with keys of `key` symbols.
+static double ham_batch_cost(const fzb_haystack *h, uint32_t m, uint32_t k, uint32_t key, bool two_bit) {
+    const uint32_t L = m / (k + 1);
+    const double c = two_bit ? std::max(h->coll_prob, 0.25) : h->coll_prob;  // (2-bit keys see at most 4 codes)
+    return (k + 1) * std::pow(c, (double)std::min(L, key));
+}
+
+// One k_ham_batch_scan pass for the patterns ids[]; same return convention as batch_pass.  two_bit: the 2-bit keys of
+// low-entropy haystacks, else text keys of key_bytes (4 or 3) bytes.
+static int batch_pass_ham(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, const uint32_t *ks,
+                          const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, bool two_bit,
+                          uint32_t key_bytes, bool tiny) {
+    const uint32_t cnt = (uint32_t)ids.size();
+    std::vector<BatchPat> pats(cnt);
+    std::vector<uint32_t> pinfo(cnt);
+    HamBatchParams hp{};
+    hp.key_mask = key_bytes == 4 ? 0xFFFFFFFFu : 0x00FFFFFFu;
+    if (two_bit) {  // the four most frequent pattern bytes of the pass get codes 0..3, every other byte code 0
+        uint64_t freq[256] = {0};
+        for (uint32_t id : ids)
+            for (uint32_t b = offsets[id]; b < offsets[id + 1]; b++) freq[patterns[b]]++;
+        int order[256];
+        for (int c = 0; c < 256; c++) order[c] = c;
+        std::stable_sort(order, order + 256, [&](int a, int b) { return freq[a] > freq[b]; });
+        for (int r = 0; r < 4; r++) hp.code[order[r]] = (uint8_t)r;
+    }
+    std::unordered_map<uint32_t, std::vector<uint32_t>> keys;  // key -> postings pattern << 8 | piece
+    keys.reserve(cnt * 8);
+    for (uint32_t i = 0; i < cnt; i++) {
+        const uint32_t id = ids[i], m = offsets[id + 1] - offsets[id], k = ks[id], L = m / (k + 1);
+        BatchPat &bp = pats[i];
+        memset(&bp, 0, sizeof bp);
+        memcpy(bp.P, patterns + offsets[id], m);
+        bp.m = (int)m;
+        bp.k = (int)k;
+        bp.L = (int)L;
+        bp.n_ngrams = (int)k + 1;
+        pinfo[i] = m | (k << 8) | (L << 16);
+        for (uint32_t j = 0; j <= k; j++) {
+            const uint8_t *s = bp.P + j * L;
+            if (two_bit) {  // codes of the first min(L, 8) symbols, under every completion of the remaining ones
+                const uint32_t n = std::min<uint32_t>(L, kHbKeySyms);
+                uint32_t key = 0;
+                for (uint32_t q = 0; q < n; q++) key |= (uint32_t)hp.code[s[q]] << (2 * q);
+                for (uint32_t x = 0; x < (1u << (2 * (kHbKeySyms - n))); x++) keys[key | (x << (2 * n))].push_back((i << 8) | j);
+            } else {
+                uint32_t w;
+                memcpy(&w, s, 4);  // (P is zero-padded to kBatchMaxM bytes)
+                keys[w & hp.key_mask].push_back((i << 8) | j);
+            }
+        }
+    }
+    std::vector<uint32_t> bits(two_bit ? kHbKeyWords : kMultiTblWords + kMulti2Words, 0);
+    int rc = upload_pass_tables(h, keys, bits, pinfo, pats, [&](uint32_t w) {
+        const uint32_t b = two_bit ? w : (w * kHashMul) >> (32 - kMultiTblBits);
+        bits[b >> 5] |= 1u << (b & 31u);
+        if (!two_bit) {
+            const uint32_t h2 = multi_hash2(w);
+            bits[kMultiTblWords + (h2 >> 5)] |= 1u << (h2 & 31u);
+        }
+    });
+    if (rc) return rc;
+    hp.mp = pass_params(h);
+    hp.mp.bits2 = two_bit ? nullptr : h->d_mbits + kMultiTblWords;
+    hp.pats = h->d_bpats;
+    const size_t smem = two_bit ? kHbSmem2 : kMultiSmem;
+    const void *fn = two_bit ? (const void *)k_ham_batch_scan<true> : (const void *)k_ham_batch_scan<false>;
+    CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 1;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kMultiThreads, smem));
+    per_sm = std::max(per_sm, 1);
+    const int64_t nvec = (int64_t)(round_up(h->buf_len, 16) / 16);
+    const int64_t ntiles = (nvec + kMultiTileVecs - 1) / kMultiTileVecs;
+    std::vector<RawRec> raw;
+    uint32_t cnts[CNT_COUNT];
+    fzb_stats pass{};
+    rc = run_batch_pass(h, [&]() -> int {
+        hp.out = h->d_out;  // (the output buffer may have grown since the last attempt)
+        hp.cap = h->out_cap;
+        if (ntiles > 0) {
+            const int grid = (int)std::min<int64_t>(ntiles, (int64_t)h->sm_count * per_sm);
+            if (two_bit)
+                k_ham_batch_scan<true><<<grid, kMultiThreads, smem, h->stream>>>(hp, nvec, ntiles);
+            else
+                k_ham_batch_scan<false><<<grid, kMultiThreads, smem, h->stream>>>(hp, nvec, ntiles);
+        }
+        CK(cudaGetLastError());
+        return FZB_OK;
+    }, raw, cnts, pass);
+    if (rc) return rc;
+    if (tiny && raw.size() > kTinyBatchCap) return 1;  // FZB_F_TINY_LIST: the pass's record list holds kTinyBatchCap
+    pass.route = 8;
+    pass.filter_ms = pass.gpu_ms;
+    pass.n_candidates = cnts[CNT_CAND];
+    pass.n_launches = 1;
+    return split_batch(raw, ids, pass, 1, true, out, sum);
+}
+
+extern "C" int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
+                                        const uint32_t *max_subs, uint32_t count, uint32_t flags, fzb_result **out,
+                                        fzb_stats *total) {
+    HandleLock handle_lock(h);
+    if (!h || !out || (count && (!patterns || !offsets || !max_subs))) return fail(FZB_E_INVALID, "NULL argument");
+    for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
+    for (uint32_t i = 0; i < count; i++)
+        if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
+    // a pattern the single search refuses fails the whole call, with the single search's error, before any work
+    for (uint32_t i = 0; i < count; i++) {
+        const uint32_t m = offsets[i + 1] - offsets[i];
+        int rc = check_pattern(h, patterns + offsets[i], m, flags);
+        if (rc == FZB_OK) rc = check_halo(h, m);
+        if (rc) return rc;
+    }
+    fzb_stats sum{};
+    auto settle = [&](int rc, const std::vector<uint32_t> &ids) { return settle_pass(rc, ids, out, count); };
+    // the shared scan takes no flags other than FZB_F_TINY_LIST (forced routes, multi-GPU reduction: one by one)
+    const bool tiny = (flags & FZB_F_TINY_LIST) != 0;
+    if ((flags & ~FZB_F_TINY_LIST) == 0 && h->buf_len > 0 && count >= 2 && sample_collision_prob(h) == FZB_OK) {
+        const bool two_bit = h->coll_prob >= 0.15;  // the boundary of k_filter_dense2
+        std::vector<uint32_t> ids;
+        uint32_t key = 0;
+        double expect = 0.0;
+        uint64_t npost = 0;
+        auto run_pass = [&]() -> int {
+            const int rc = ids.size() >= 2 ? settle(batch_pass_ham(h, patterns, offsets, max_subs, ids, out, &sum, two_bit,
+                                                                   key, tiny), ids)
+                                           : FZB_OK;  // (a pass of one pattern is not worth it)
+            ids.clear();
+            expect = 0.0;
+            npost = 0;
+            return rc;
+        };
+        // one group of passes per key width: 8 symbols (2-bit); 4 bytes, then 3 bytes (text)
+        for (key = two_bit ? (uint32_t)kHbKeySyms : 4u; key >= (two_bit ? (uint32_t)kHbKeySyms : 3u); key--) {
+            for (uint32_t i = 0; i < count; i++) {
+                const uint32_t m = offsets[i + 1] - offsets[i], k = max_subs[i];
+                if (ham_batch_key(m, k, two_bit) != key) continue;
+                const double cost = ham_batch_cost(h, m, k, key, two_bit);
+                if (cost > kHamBatchPatExpect) continue;
+                const uint32_t np = ham_batch_postings(m, k, two_bit);
+                if (ids.size() == kMaxBatchPats || expect + cost > kHamBatchExpect || npost + np > kMaxHamBatchPostings) {
+                    const int rc = run_pass();
+                    if (rc) return rc;
+                }
+                ids.push_back(i);
+                expect += cost;
+                npost += np;
+            }
+            const int rc = run_pass();
+            if (rc) return rc;
+        }
+    }
+    for (uint32_t i = 0; i < count; i++) {
+        if (out[i]) continue;
+        const int rc = settle(fzb_search_hamming(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_subs[i],
+                                                 flags, &out[i]), {});
+        if (rc) return rc;
+        add_stats(&sum, out[i]->stats);
+    }
+    sum.route = 7;  // batch
+    if (total) *total = sum;
+    return FZB_OK;
 }
 
 extern "C" int fzb_search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t max_subs,

@@ -59,7 +59,7 @@ extern "C" {
 #define FZB_F_FORCE_NGRAMS 8u /* Levenshtein/generic/Hamming: force the n-gram route */
 #define FZB_F_TINY_LIST 16u   /* testing: cap the granule work list and the hit list at 8 entries and the LP
                                  survivor list at 1 024 (overflow paths); batches: small work, hit and survivor
-                                 lists and 3 000-start LP chunks */
+                                 lists and 3 000-start LP chunks; a Hamming batch pass holds 8 records */
 #define FZB_F_FORCE_SAMPLED 64u /* testing: use the sampled filter whenever its lemma holds, even if the
                                  byte statistics say it is not selective */
 #define FZB_F_GLOBAL 32u      /* multi-GPU: FINAL becomes the GLOBAL consolidated list of all shards: every rank
@@ -217,6 +217,19 @@ int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patterns, const
                                  const uint32_t *max_l_dist, uint32_t count, uint32_t flags,
                                  fzb_result **out, struct fzb_stats_s *total);
 
+/*
+ * Batch of substitutions-only searches over ONE resident haystack: the patterns as for
+ * fzb_search_levenshtein_batch, each with its own max_subs[i].  The patterns of at most 64 bytes with
+ * max_subs < length whose k+1 pieces (pigeonhole filter) have selective keys on this haystack share
+ * scans (DESIGN.md section 5.8; their results report route 8); the others are searched one by one.
+ * Each out[i] is exactly what fzb_search_hamming would return for pattern i (FINAL == RAW, ascending).
+ * A pattern the single search refuses fails the whole call with its error; on error nothing is
+ * returned.  Flags other than FZB_F_TINY_LIST send every pattern one by one with those flags.
+ */
+int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
+                             const uint32_t *max_subs, uint32_t count, uint32_t flags,
+                             fzb_result **out, struct fzb_stats_s *total);
+
 /* ExactSearch.search (search_exact.py:80-85): all (overlapping) occurrences. FINAL == RAW. */
 int fzb_search_exact(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
                      fzb_result **out);
@@ -271,7 +284,8 @@ typedef struct fzb_stats_s {
     uint64_t n_candidates;  /* granules / windows handed to the verify stage */
     uint32_t n_launches;    /* kernels launched */
     uint32_t route;         /* 0 exact, 1 n-grams (sampled filter), 2 n-grams (dense filter), 3 LP,
-                               4 hamming, 5 generic n-grams, 6 generic LP */
+                               4 hamming, 5 generic n-grams, 6 generic LP, 7 batch (summed statistics),
+                               8 hamming batch scan */
 } fzb_stats;
 int fzb_result_stats(const fzb_result *r, fzb_stats *out);
 void fzb_result_destroy(fzb_result *r);
