@@ -14,6 +14,7 @@
 #include <sched.h>
 #include <unistd.h>
 #include <condition_variable>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <new>
@@ -54,6 +55,106 @@ static int fail(int code, const char *fmt, ...) {
         if (e_ != cudaSuccess)                                                            \
             return fail(FZB_E_CUDA, "%s failed: %s", #call, cudaGetErrorString(e_));      \
     } while (0)
+
+#define TRY(call)                                                                         \
+    do {                                                                                  \
+        const int rc_ = (call);                                                           \
+        if (rc_) return rc_;                                                              \
+    } while (0)
+
+// ------------------------------------------------------------------------------------------------
+// owned allocations
+// ------------------------------------------------------------------------------------------------
+enum class Mem { Device, Pinned, Mapped };  // cudaMalloc; cudaHostAlloc, page-locked; ... and mapped for the device
+
+// One device or pinned host allocation of size() elements of T, freed (cudaFree / cudaFreeHost) when the object dies
+// or takes another allocation.  alloc() allocates into a temporary and replaces the current allocation only on
+// success: a failed allocation or growth leaves the object, and whatever holds it, as it was.
+template <class T, Mem kMem>
+class Buf {
+  public:
+    Buf() = default;
+    Buf(Buf &&o) noexcept : p_(o.p_), n_(o.n_) {
+        o.p_ = nullptr;
+        o.n_ = 0;
+    }
+    Buf &operator=(Buf o) noexcept {  // (`o` takes the previous allocation with it)
+        std::swap(p_, o.p_);
+        std::swap(n_, o.n_);
+        return *this;
+    }
+    ~Buf() {
+        if (p_) (void)(kMem == Mem::Device ? cudaFree(p_) : cudaFreeHost(p_));
+    }
+    T *get() const { return p_; }
+    uint64_t size() const { return n_; }
+    explicit operator bool() const { return p_ != nullptr; }
+    T &operator[](uint64_t i) const {
+        static_assert(kMem != Mem::Device, "device memory is not addressable from the host");
+        return p_[i];
+    }
+    // n elements; `bytes` instead of n * sizeof(T) when the allocation also holds a trailing array of another type
+    int alloc(uint64_t n, uint64_t bytes = 0) {
+        Buf b;
+        if (!bytes) bytes = n * sizeof(T);
+        const unsigned flags = kMem == Mem::Mapped ? cudaHostAllocMapped | cudaHostAllocPortable : cudaHostAllocDefault;
+        const cudaError_t e = kMem == Mem::Device ? cudaMalloc(&b.p_, bytes) : cudaHostAlloc(&b.p_, bytes, flags);
+        if (e != cudaSuccess)
+            return fail(FZB_E_CUDA, "%s(%llu bytes) failed: %s", kMem == Mem::Device ? "cudaMalloc" : "cudaHostAlloc",
+                        (unsigned long long)bytes, cudaGetErrorString(e));
+        b.n_ = n;
+        *this = std::move(b);
+        return FZB_OK;
+    }
+
+  private:
+    T *p_ = nullptr;
+    uint64_t n_ = 0;
+};
+template <class T> using DevBuf = Buf<T, Mem::Device>;
+template <class T> using PinnedBuf = Buf<T, Mem::Pinned>;
+template <class T> using MappedBuf = Buf<T, Mem::Mapped>;
+
+// The buffer groups a handle allocates on first use, each built whole or not at all (ensure_group).
+struct BatchBufs {  // the tables of the shared batch passes (batch_kernels.cuh, ham_batch_kernels.cuh)
+    DevBuf<uint32_t> d_mbits;  // first + second level key tables
+    DevBuf<uint2> d_gtab;
+    DevBuf<uint32_t> d_postings, d_pinfo;
+    DevBuf<BatchPat> d_bpats;
+    DevBuf<unsigned long long> d_mset;  // (pattern, granule) set of the q-sample pass: all-zero between passes
+    DevBuf<WorkItem> d_mwork;
+};
+struct LpBatchBufs {  // the LP batch pass
+    DevBuf<ulonglong2> d_lmlut;           // per-byte pattern-set vectors [256], then the match masks u32 [64][256]
+    DevBuf<unsigned long long> d_lmlist;  // survivor list (after the sort: grouped by pattern)
+    DevBuf<unsigned long long> d_lmkept;  // the survivors of the exact per-pattern window test
+    DevBuf<uint32_t> d_lmhist;            // per-pattern counts [64] + kept total [1] | cursors [64]
+};
+struct PeerBufs {  // the peer-memory reduction (p2p_kernels.cuh)
+    DevBuf<uint8_t> d_p2p;  // my receive area: [2 parities][world] slots + flags
+    DevBuf<MergeScratch> d_ms;
+    DevBuf<unsigned long long> d_mscore;
+    DevBuf<uint32_t> d_mpos;
+    MappedBuf<int64_t> h_grows;  // global final rows of the last global search (16 bytes each)
+    MappedBuf<uint32_t> h_ghdr;  // status, count, epoch
+};
+struct GatherBufs {  // the staged NCCL all-gather
+    uint32_t cap = 0;  // rows per rank
+    DevBuf<int64_t> d_send, d_recv;
+    PinnedBuf<int64_t> h_send, h_recv;
+};
+
+// Gives `slot` its group unless it has one.  `init` allocates and sets up the whole group in a local, which `slot`
+// takes only when all of it succeeded: a failure leaves the slot empty, never holding part of a group.
+template <class G, class F>
+static int ensure_group(std::unique_ptr<G> &slot, F init) {
+    if (slot) return FZB_OK;
+    std::unique_ptr<G> g(new (std::nothrow) G());
+    if (!g) return fail(FZB_E_CUDA, "out of host memory");
+    TRY(init(*g));
+    slot = std::move(g);
+    return FZB_OK;
+}
 
 extern "C" int fzb_version(void) { return FZB_VERSION; }
 
@@ -123,23 +224,21 @@ struct fzb_haystack {
     std::recursive_mutex mu;  // one search / upload at a time per handle (HandleLock); recursive: has_near_match and
                               // the windowed exact search call the search entry points on their own handle
     int device = 0;
-    uint8_t *d = nullptr;  // H[0] == global position buf_lo
-    bool owned = true;
+    // Every buffer below is freed with the handle (fzb_haystack_destroy makes its device current first).
+    uint8_t *d = nullptr;       // H[0] == global position buf_lo: owned_buf's bytes, an adopted buffer or a view
+    DevBuf<uint8_t> owned_buf;  // the handle's own sequence buffer (size(): its capacity); empty when adopted
     uint64_t buf_len = 0, buf_lo = 0, global_len = 0, own_lo = 0, own_hi = 0;
     uint64_t padded_len = 0;
-    uint64_t capacity = 0;  // bytes allocated at d (owned buffers)
     cudaEvent_t ev_stop = nullptr;
     cudaStream_t stream = nullptr;
-    uint32_t *d_bitmap = nullptr;
-    uint64_t bitmap_words = 0;
-    RawRec *d_out = nullptr;
-    uint32_t out_cap = 0;
-    uint32_t *d_counters = nullptr;
+    DevBuf<uint32_t> d_bitmap;
+    DevBuf<RawRec> d_out;  // size() raw records, then their size() packed keys (alloc_out)
+    DevBuf<uint32_t> d_counters;
     // k_post writes these straight into MAPPED pinned host memory (no copy operations per search)
-    uint32_t *h_counters = nullptr;  // CNT_COUNT counters
-    int64_t *h_fin = nullptr;        // final rows (kPostMax x kFinCols)
-    int64_t *d_fin = nullptr;        // device copy of the final rows (input of the multi-GPU reduction)
-    uint64_t *d_sorted = nullptr;    // k_post scratch: the sorted canonical keys
+    MappedBuf<uint32_t> h_counters;  // CNT_COUNT counters
+    MappedBuf<int64_t> h_fin;        // final rows (kPostMax x kFinCols)
+    DevBuf<int64_t> d_fin;           // device copy of the final rows (input of the multi-GPU reduction)
+    DevBuf<uint64_t> d_sorted;       // k_post scratch: the sorted canonical keys
     fzb_result *pending = nullptr;   // the last result, while its raw records still sit in d_out only
     bool ev1_recorded = false;
     bool filter_attrs_set = false;
@@ -147,7 +246,7 @@ struct fzb_haystack {
     // multi-GPU reduction (FZB_F_GLOBAL): peer-memory world (p2p_kernels.cuh) + NCCL for bootstrap / staged fallback
     bool p2p = false;               // every rank of the world can store into every other rank's receive area
     bool local_world = false;       // the world lives in this process (fzb_comm_init_local): no NCCL
-    uint8_t *d_p2p = nullptr;       // my receive area: [2 parities][world] slots + flags
+    std::unique_ptr<PeerBufs> peer;  // allocated when the handle joins a world (p2p_alloc)
     uint8_t *peer_base[kMaxWorld] = {};
     bool peer_opened[kMaxWorld] = {};
     uint32_t p2p_cap = 4096;        // group rows per slot
@@ -156,42 +255,21 @@ struct fzb_haystack {
     bool counters_clean = false;    // the device counters are all zero (the last search's final kernel left them so)
     uint32_t seq = 0;               // number of search attempts enqueued: the last kernel of each writes it to mapped
                                     // memory as its final store and the host polls for it (wait_done)
-    MergeScratch *d_ms = nullptr;
-    unsigned long long *d_mscore = nullptr;
-    uint32_t *d_mpos = nullptr;
-    int64_t *h_grows = nullptr;     // mapped: global final rows of the last global search (16 bytes each)
-    uint32_t *h_ghdr = nullptr;     // mapped: status, count, epoch
     void *comm = nullptr;  // ncclComm_t
     int rank = 0, world = 1;
     uint32_t gather_cap = 4096;     // rows per rank in one all-gather slot
-    int64_t *d_send = nullptr, *d_recv = nullptr;
-    int64_t *h_send = nullptr, *h_recv = nullptr;  // pinned
-    uint32_t gather_alloc = 0;
+    std::unique_ptr<GatherBufs> gather;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     int sm_count = 132;
-    uint64_t *d_hits = nullptr;     // dense route: list of confirmed n-gram hits
-    uint32_t hits_cap = 0;
-    uint32_t *d_glist = nullptr;    // compacted list of marked granules
-    uint32_t glist_cap = 0;
-    uint32_t *d_scratch = nullptr;  // candidate lists of the LP / generic kernels
-    uint64_t scratch_words = 0;
-    unsigned long long *d_lplist = nullptr;  // streaming LP route: starts that survived the scan
-    uint32_t lplist_cap = 0;
+    DevBuf<uint64_t> d_hits;        // dense route: list of confirmed n-gram hits (allocated on first use)
+    DevBuf<uint32_t> d_glist;       // compacted list of marked granules
+    uint32_t glist_cap = 0;         // (d_glist has max(glist_cap, 1) entries)
+    DevBuf<uint32_t> d_scratch;     // candidate lists of the LP / generic kernels
+    DevBuf<unsigned long long> d_lplist;  // streaming LP route: starts that survived the scan (allocated on first use)
     // single-pass multi-pattern batches (batch_kernels.cuh), allocated on first use
-    uint32_t *d_mbits = nullptr;
-    uint2 *d_gtab = nullptr;
-    uint32_t *d_postings = nullptr, *d_pinfo = nullptr;
-    BatchPat *d_bpats = nullptr;
-    unsigned long long *d_mset = nullptr;
-    WorkItem *d_mwork = nullptr;
-    uint32_t mset_slots = 0, mwork_cap = 0;
-    unsigned long long *d_mhits = nullptr;  // dense batch pass: (pattern, n-gram, position) hits
-    uint32_t mhits_cap = 0;
-    ulonglong2 *d_lmlut = nullptr;          // LP batch pass: per-byte pattern-set vectors
-    unsigned long long *d_lmlist = nullptr; // ... its survivor list (after the sort: grouped by pattern)
-    unsigned long long *d_lmkept = nullptr; // ... the survivors of the exact per-pattern window test
-    uint32_t *d_lmhist = nullptr;
-    uint32_t lmlist_cap = 0;
+    std::unique_ptr<BatchBufs> batch;
+    DevBuf<unsigned long long> d_mhits;  // dense batch pass: (pattern, n-gram, position) hits
+    std::unique_ptr<LpBatchBufs> lpb;
 };
 
 struct fzb_result {
@@ -208,7 +286,7 @@ struct fzb_result {
     bool device_post = false;  // the final list came from the device (k_post)
     bool raw_ordered = false;  // raw is already in its reference order
     bool has_global = false;   // FZB_F_GLOBAL: gfin is the global consolidated list of all shards
-    bool global_on_device = false;  // ... produced by k_merge; its rows sit in owner->h_grows until fetched
+    bool global_on_device = false;  // ... produced by k_merge; its rows sit in owner->peer->h_grows until fetched
     bool fused_issued = false;      // a k_push / k_merge pair ran for this search
     uint32_t fused_status = 0;      // MS_* of that merge
     uint32_t gcount = 0;
@@ -259,7 +337,7 @@ void fzb_result::fetch_raw() {
         raw.resize(raw_n);
         if (raw_n) {
             cudaSetDevice(owner->device);
-            if (cudaMemcpyAsync(raw.data(), owner->d_out, (size_t)raw_n * sizeof(RawRec), cudaMemcpyDeviceToHost,
+            if (cudaMemcpyAsync(raw.data(), owner->d_out.get(), (size_t)raw_n * sizeof(RawRec), cudaMemcpyDeviceToHost,
                                 owner->stream) != cudaSuccess ||
                 cudaStreamSynchronize(owner->stream) != cudaSuccess) {
                 cudaGetLastError();
@@ -272,7 +350,7 @@ void fzb_result::fetch_raw() {
     if (global_on_device) {  // rows: start, (end - start) << 32 | dist
         gfin.resize(gcount);
         for (uint32_t i = 0; i < gcount; i++) {
-            const int64_t s0 = owner->h_grows[2 * (size_t)i], v = owner->h_grows[2 * (size_t)i + 1];
+            const int64_t s0 = owner->peer->h_grows[2 * (size_t)i], v = owner->peer->h_grows[2 * (size_t)i + 1];
             gfin[i] = make_rec(s0, s0 + (v >> 32), v & 0xFFFFFFFF);
         }
         global_on_device = false;
@@ -288,7 +366,7 @@ void fzb_result::discard_attempt() {  // a search attempt that has to be redone:
     fin.clear();
 }
 
-static void detach_pending(fzb_haystack *h) {  // before h->d_out / h->h_grows are overwritten or freed
+static void detach_pending(fzb_haystack *h) {  // before h->d_out / h->peer->h_grows are overwritten or freed
     fzb_result *r;
     {
         std::lock_guard<std::mutex> lock(g_pending_mutex);
@@ -296,6 +374,9 @@ static void detach_pending(fzb_haystack *h) {  // before h->d_out / h->h_grows a
     }
     if (r) r->fetch_raw();
 }
+
+// d_out: `cap` raw records, then their `cap` packed canonical keys (k_post)
+static int alloc_out(fzb_haystack *h, uint64_t cap) { return h->d_out.alloc(cap, cap * (sizeof(RawRec) + sizeof(uint64_t))); }
 
 static int haystack_common_init(fzb_haystack *h) {
     CK(cudaSetDevice(h->device));
@@ -306,22 +387,18 @@ static int haystack_common_init(fzb_haystack *h) {
     CK(cudaGetDeviceProperties(&prop, h->device));
     h->sm_count = prop.multiProcessorCount;
     uint64_t granules = (h->padded_len >> kGranuleShift) + 2;
-    h->bitmap_words = round_up((granules + 31) / 32, 32);
-    CK(cudaMalloc(&h->d_bitmap, h->bitmap_words * sizeof(uint32_t)));
-    CK(cudaMalloc(&h->d_counters, CNT_COUNT * sizeof(uint32_t)));
-    const unsigned hflags = cudaHostAllocMapped | cudaHostAllocPortable;
-    CK(cudaHostAlloc(&h->h_counters, CNT_COUNT * sizeof(uint32_t), hflags));
-    memset(h->h_counters, 0, CNT_COUNT * sizeof(uint32_t));  // the sequence word the host polls must not hold a stale value
-    CK(cudaHostAlloc(&h->h_fin, (size_t)kPostMax * kFinCols * sizeof(int64_t), hflags));
-    CK(cudaMalloc(&h->d_fin, (size_t)kPostMax * kFinCols * sizeof(int64_t)));
-    CK(cudaMalloc(&h->d_sorted, (size_t)kPostMax * sizeof(uint64_t)));
+    TRY(h->d_bitmap.alloc(round_up((granules + 31) / 32, 32)));
+    TRY(h->d_counters.alloc(CNT_COUNT));
+    TRY(h->h_counters.alloc(CNT_COUNT));
+    memset(h->h_counters.get(), 0, CNT_COUNT * sizeof(uint32_t));  // the sequence word the host polls must not hold a stale value
+    TRY(h->h_fin.alloc((uint64_t)kPostMax * kFinCols));
+    TRY(h->d_fin.alloc((uint64_t)kPostMax * kFinCols));
+    TRY(h->d_sorted.alloc(kPostMax));
     CK(cudaFuncSetAttribute(k_post, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPostSmem));
-    CK(cudaMemset(h->d_bitmap, 0, h->bitmap_words * sizeof(uint32_t)));  // stays all-zero between searches
+    CK(cudaMemset(h->d_bitmap.get(), 0, h->d_bitmap.size() * sizeof(uint32_t)));  // stays all-zero between searches
     h->glist_cap = (uint32_t)std::min<uint64_t>(granules, 1u << 20);
-    CK(cudaMalloc(&h->d_glist, (size_t)std::max<uint32_t>(h->glist_cap, 1) * sizeof(uint32_t)));
-    h->out_cap = 1u << 16;
-    CK(cudaMalloc(&h->d_out, (size_t)h->out_cap * (sizeof(RawRec) + sizeof(uint64_t))));  // records + their keys
-    return FZB_OK;
+    TRY(h->d_glist.alloc(std::max<uint32_t>(h->glist_cap, 1)));
+    return alloc_out(h, 1u << 16);
 }
 
 static int check_shard(uint64_t buf_len, uint64_t buf_lo, uint64_t global_len, uint64_t own_lo,
@@ -340,13 +417,13 @@ static int check_shard(uint64_t buf_len, uint64_t buf_lo, uint64_t global_len, u
 
 static int alloc_buffer(fzb_haystack *h) {
     CK(cudaSetDevice(h->device));
-    CK(cudaMalloc(&h->d, h->padded_len));
-    h->capacity = h->padded_len;
+    TRY(h->owned_buf.alloc(h->padded_len));
+    h->d = h->owned_buf.get();
     CK(cudaMemset(h->d + h->buf_len, 0, h->padded_len - h->buf_len));
     return FZB_OK;
 }
 
-static void p2p_free(fzb_haystack *h);
+static void close_peers(fzb_haystack *h);
 static int upload_bytes(fzb_haystack *h, uint64_t dst_off, const uint8_t *host, uint64_t n);
 
 extern "C" void fzb_haystack_destroy(fzb_haystack *h) {
@@ -354,41 +431,13 @@ extern "C" void fzb_haystack_destroy(fzb_haystack *h) {
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     detach_pending(h);
-    if (h->owned && h->d) cudaFree(h->d);
-    if (h->d_bitmap) cudaFree(h->d_bitmap);
-    if (h->d_out) cudaFree(h->d_out);
-    if (h->d_counters) cudaFree(h->d_counters);
-    if (h->d_scratch) cudaFree(h->d_scratch);
-    if (h->d_lplist) cudaFree(h->d_lplist);
-    if (h->d_mbits) cudaFree(h->d_mbits);
-    if (h->d_gtab) cudaFree(h->d_gtab);
-    if (h->d_postings) cudaFree(h->d_postings);
-    if (h->d_pinfo) cudaFree(h->d_pinfo);
-    if (h->d_bpats) cudaFree(h->d_bpats);
-    if (h->d_mset) cudaFree(h->d_mset);
-    if (h->d_mwork) cudaFree(h->d_mwork);
-    if (h->d_mhits) cudaFree(h->d_mhits);
-    if (h->d_lmlut) cudaFree(h->d_lmlut);
-    if (h->d_lmlist) cudaFree(h->d_lmlist);
-    if (h->d_lmkept) cudaFree(h->d_lmkept);
-    if (h->d_lmhist) cudaFree(h->d_lmhist);
-    if (h->d_glist) cudaFree(h->d_glist);
-    if (h->d_hits) cudaFree(h->d_hits);
-    if (h->d_send) cudaFree(h->d_send);
-    if (h->d_recv) cudaFree(h->d_recv);
-    if (h->h_send) cudaFreeHost(h->h_send);
-    if (h->h_recv) cudaFreeHost(h->h_recv);
     if (h->comm) nccl_comm_destroy(h->comm);
-    p2p_free(h);
-    if (h->h_counters) cudaFreeHost(h->h_counters);
-    if (h->h_fin) cudaFreeHost(h->h_fin);
-    if (h->d_fin) cudaFree(h->d_fin);
-    if (h->d_sorted) cudaFree(h->d_sorted);
+    close_peers(h);
     for (auto &e : h->ev)
         if (e) cudaEventDestroy(e);
     if (h->ev_stop) cudaEventDestroy(h->ev_stop);
     if (h->stream) cudaStreamDestroy(h->stream);
-    delete h;
+    delete h;  // (frees its buffers, on the device made current above)
 }
 
 // The constructors' common part.  `arg_error`: the caller's own argument check failed (reported after the `out`
@@ -407,7 +456,6 @@ static int haystack_new(const char *arg_error, const uint8_t *host, const void *
     fzb_haystack *h = new (std::nothrow) fzb_haystack();
     if (!h) return fail(FZB_E_CUDA, "out of host memory");
     h->device = device;
-    h->owned = !dev_ptr;
     h->d = (uint8_t *)dev_ptr;
     h->buf_len = buf_len;
     h->buf_lo = buf_lo;
@@ -415,7 +463,7 @@ static int haystack_new(const char *arg_error, const uint8_t *host, const void *
     h->own_lo = own_lo;
     h->own_hi = own_hi;
     h->padded_len = round_up(buf_len, 128) + 128;
-    rc = h->owned ? alloc_buffer(h) : FZB_OK;
+    rc = dev_ptr ? FZB_OK : alloc_buffer(h);
     if (rc == FZB_OK) rc = haystack_common_init(h);
     if (rc == FZB_OK && host) rc = upload_bytes(h, 0, host, buf_len);
     if (rc) {
@@ -465,20 +513,19 @@ extern "C" int fzb_haystack_fill_synthetic(fzb_haystack *h, const uint8_t *alpha
                                            uint64_t seed) {
     HandleLock handle_lock(h);
     if (!h || !alphabet || alphabet_len == 0 || alphabet_len > 256) return fail(FZB_E_INVALID, "bad arguments");
-    if (!h->owned) return fail(FZB_E_INVALID, "cannot fill an adopted buffer");
+    if (!h->owned_buf) return fail(FZB_E_INVALID, "cannot fill an adopted buffer");
     CK(cudaSetDevice(h->device));
-    uint8_t *d_alpha = nullptr;
-    CK(cudaMalloc(&d_alpha, 256));
-    CK(cudaMemcpyAsync(d_alpha, alphabet, alphabet_len, cudaMemcpyHostToDevice, h->stream));
+    DevBuf<uint8_t> d_alpha;
+    TRY(d_alpha.alloc(256));
+    CK(cudaMemcpyAsync(d_alpha.get(), alphabet, alphabet_len, cudaMemcpyHostToDevice, h->stream));
     int64_t nwords = (int64_t)(round_up(h->buf_len, 4) / 4);
-    k_fill_synth<<<h->sm_count * 8, 256, 0, h->stream>>>(h->d, (int64_t)h->buf_lo, nwords, seed, d_alpha,
+    k_fill_synth<<<h->sm_count * 8, 256, 0, h->stream>>>(h->d, (int64_t)h->buf_lo, nwords, seed, d_alpha.get(),
                                                         alphabet_len);
     CK(cudaGetLastError());
     // bytes past buf_len must stay zero (the last word may have spilled over)
     if (h->buf_len % 4)
         CK(cudaMemsetAsync(h->d + h->buf_len, 0, 4 - h->buf_len % 4, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    CK(cudaFree(d_alpha));
     h->coll_prob = -1.0;
     return FZB_OK;
 }
@@ -644,8 +691,8 @@ static bool is_whole_sequence(const fzb_haystack *h) {
 extern "C" int fzb_haystack_upload(fzb_haystack *h, const uint8_t *host, uint64_t n) {
     HandleLock handle_lock(h);
     if (!h || (!host && n)) return fail(FZB_E_INVALID, "bad arguments");
-    if (!h->owned) return fail(FZB_E_INVALID, "upload needs an owned handle");
-    if (round_up(n, 128) + 128 > h->capacity) return fail(FZB_E_INVALID, "upload larger than the handle's capacity");
+    if (!h->owned_buf) return fail(FZB_E_INVALID, "upload needs an owned handle");
+    if (round_up(n, 128) + 128 > h->owned_buf.size()) return fail(FZB_E_INVALID, "upload larger than the handle's capacity");
     CK(cudaSetDevice(h->device));
     if (!is_whole_sequence(h)) {  // a shard keeps its geometry: the new bytes replace the same window of the global sequence
         if (n != h->buf_len) return fail(FZB_E_INVALID, "a shard upload must supply exactly buf_len bytes");
@@ -669,8 +716,8 @@ extern "C" int fzb_haystack_upload_symbols(fzb_haystack *h, const void *host, ui
     if (n_alpha > (uint32_t)kMaxPattern) return fail(FZB_E_UNSUPPORTED, "more than %d distinct pattern symbols", kMaxPattern);
     for (uint32_t i = 1; i < n_alpha; i++)
         if (alphabet[i - 1] >= alphabet[i]) return fail(FZB_E_INVALID, "the alphabet must be strictly ascending");
-    if (!h->owned) return fail(FZB_E_INVALID, "upload needs an owned handle");
-    if (round_up(n, 128) + 128 > h->capacity) return fail(FZB_E_INVALID, "upload larger than the handle's capacity");
+    if (!h->owned_buf) return fail(FZB_E_INVALID, "upload needs an owned handle");
+    if (round_up(n, 128) + 128 > h->owned_buf.size()) return fail(FZB_E_INVALID, "upload larger than the handle's capacity");
     if (!is_whole_sequence(h)) return fail(FZB_E_INVALID, "symbol uploads replace a whole (unsharded) sequence");
     CK(cudaSetDevice(h->device));
     h->buf_len = h->global_len = h->own_hi = n;
@@ -683,42 +730,27 @@ extern "C" int fzb_haystack_upload_symbols(fzb_haystack *h, const void *host, ui
     }
     constexpr uint64_t kChunk = 16u << 20;  // symbols per chunk (a multiple of 4: the kernel stores 32-bit words)
     const uint64_t chunk = std::min<uint64_t>(kChunk, round_up(n, 4));
-    uint8_t *d_tmp = nullptr;   // every operation below is on h->stream: a chunk's copy is ordered behind the
-    uint32_t *d_alpha = nullptr;  // reduction of the previous chunk, so one scratch buffer is enough
-    int rc = FZB_OK;
-    auto cleanup = [&]() {
-        if (d_tmp) cudaFree(d_tmp);
-        if (d_alpha) cudaFree(d_alpha);
-    };
-#define SYMCK(call)                                                                                \
-    do {                                                                                           \
-        cudaError_t e_ = (call);                                                                   \
-        if (e_ != cudaSuccess) {                                                                   \
-            rc = fail(FZB_E_CUDA, "%s failed: %s", #call, cudaGetErrorString(e_));                 \
-            cudaStreamSynchronize(h->stream);                                                      \
-            cleanup();                                                                             \
-            return rc;                                                                             \
-        }                                                                                          \
-    } while (0)
-    SYMCK(cudaMalloc(&d_alpha, 256 * sizeof(uint32_t)));
-    if (n_alpha) SYMCK(cudaMemcpyAsync(d_alpha, alphabet, n_alpha * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
-    SYMCK(cudaMalloc(&d_tmp, chunk * width));
+    // every operation below is on h->stream: a chunk's copy is ordered behind the reduction of the previous chunk, so
+    // one scratch buffer is enough.  (On an error return, freeing the buffers waits for the work queued on them.)
+    DevBuf<uint32_t> d_alpha;
+    DevBuf<uint8_t> d_tmp;
+    TRY(d_alpha.alloc(256));
+    if (n_alpha) CK(cudaMemcpyAsync(d_alpha.get(), alphabet, n_alpha * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+    TRY(d_tmp.alloc(chunk * width));
     const uint8_t *src = static_cast<const uint8_t *>(host);
     for (uint64_t off = 0; off < n; off += chunk) {
         const uint64_t cnt = std::min<uint64_t>(chunk, n - off);
-        SYMCK(cudaMemcpyAsync(d_tmp, src + off * width, cnt * width, cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(d_tmp.get(), src + off * width, cnt * width, cudaMemcpyHostToDevice, h->stream));
         const int grid = (int)std::min<uint64_t>((uint64_t)h->sm_count * 8, (cnt / 4 + kSymThreads - 1) / kSymThreads + 1);
         if (width == 4)
-            k_reduce_symbols<uint32_t><<<grid, kSymThreads, 0, h->stream>>>(reinterpret_cast<const uint32_t *>(d_tmp), cnt,
-                                                                            d_alpha, n_alpha, h->d + off);
+            k_reduce_symbols<uint32_t><<<grid, kSymThreads, 0, h->stream>>>(reinterpret_cast<const uint32_t *>(d_tmp.get()),
+                                                                            cnt, d_alpha.get(), n_alpha, h->d + off);
         else
-            k_reduce_symbols<uint16_t><<<grid, kSymThreads, 0, h->stream>>>(reinterpret_cast<const uint16_t *>(d_tmp), cnt,
-                                                                            d_alpha, n_alpha, h->d + off);
-        SYMCK(cudaGetLastError());
+            k_reduce_symbols<uint16_t><<<grid, kSymThreads, 0, h->stream>>>(reinterpret_cast<const uint16_t *>(d_tmp.get()),
+                                                                            cnt, d_alpha.get(), n_alpha, h->d + off);
+        CK(cudaGetLastError());
     }
-    SYMCK(cudaStreamSynchronize(h->stream));
-#undef SYMCK
-    cleanup();
+    CK(cudaStreamSynchronize(h->stream));
     return FZB_OK;
 }
 
@@ -732,9 +764,7 @@ extern "C" void *fzb_host_alloc(uint64_t n) {
     return p;
 }
 
-extern "C" void fzb_host_free(void *p) {
-    if (p) cudaFreeHost(p);
-}
+extern "C" void fzb_host_free(void *p) { cudaFreeHost(p); }  // (a no-op for NULL)
 
 extern "C" int fzb_timer_start(fzb_haystack *h) {
     if (!h) return fail(FZB_E_INVALID, "NULL handle");
@@ -764,20 +794,21 @@ extern "C" int fzb_nccl_unique_id(uint8_t id[FZB_NCCL_ID_BYTES]) {
     return FZB_OK;
 }
 
+// The staging buffers of the all-gather, grown to `cap` rows per rank: the new ones are allocated before the old ones
+// are released, so a failure leaves the handle with its previous buffers.
 static int ensure_gather_buffers(fzb_haystack *h, uint32_t cap) {
-    if (cap <= h->gather_alloc) return FZB_OK;
-    if (h->d_send) cudaFree(h->d_send);
-    if (h->d_recv) cudaFree(h->d_recv);
-    if (h->h_send) cudaFreeHost(h->h_send);
-    if (h->h_recv) cudaFreeHost(h->h_recv);
-    h->d_send = h->d_recv = h->h_send = h->h_recv = nullptr;
-    h->gather_alloc = 0;
-    const size_t slot = (size_t)(cap + 1) * kFinCols * sizeof(int64_t);
-    CK(cudaMalloc(&h->d_send, slot));
-    CK(cudaMalloc(&h->d_recv, slot * h->world));
-    CK(cudaMallocHost(&h->h_send, slot));
-    CK(cudaMallocHost(&h->h_recv, slot * h->world));
-    h->gather_alloc = cap;
+    if (h->gather && cap <= h->gather->cap) return FZB_OK;
+    const uint64_t slot = (uint64_t)(cap + 1) * kFinCols;
+    std::unique_ptr<GatherBufs> grown;
+    TRY(ensure_group(grown, [&](GatherBufs &g) -> int {
+        TRY(g.d_send.alloc(slot));
+        TRY(g.d_recv.alloc(slot * h->world));
+        TRY(g.h_send.alloc(slot));
+        TRY(g.h_recv.alloc(slot * h->world));
+        g.cap = cap;
+        return FZB_OK;
+    }));
+    h->gather = std::move(grown);
     return FZB_OK;
 }
 
@@ -788,20 +819,19 @@ static int p2p_alloc(fzb_haystack *h) {
     h->slot_bytes = ((uint64_t)kHdrWords + (uint64_t)h->p2p_cap * kFinCols) * 8;
     h->flags_off = round_up(2 * (uint64_t)h->world * h->slot_bytes, 256);
     const size_t bytes = h->flags_off + 2 * kMaxWorld * sizeof(uint32_t) + 256;
-    if (!h->d_p2p) {
-        CK(cudaMalloc(&h->d_p2p, bytes));
-        CK(cudaMemset(h->d_p2p, 0, bytes));
-        CK(cudaMalloc(&h->d_ms, sizeof(MergeScratch)));
-        CK(cudaMemset(h->d_ms, 0, sizeof(MergeScratch)));
-        const size_t rows = (size_t)h->world * h->p2p_cap;
-        CK(cudaMalloc(&h->d_mscore, rows * sizeof(unsigned long long)));
-        CK(cudaMalloc(&h->d_mpos, rows * sizeof(uint32_t)));
-        const unsigned hflags = cudaHostAllocMapped | cudaHostAllocPortable;
-        CK(cudaHostAlloc(&h->h_grows, rows * 2 * sizeof(int64_t), hflags));
-        CK(cudaHostAlloc(&h->h_ghdr, 16 * sizeof(uint32_t), hflags));
-        memset(h->h_ghdr, 0, 16 * sizeof(uint32_t));
-    }
-    return FZB_OK;
+    const uint64_t rows = (uint64_t)h->world * h->p2p_cap;
+    return ensure_group(h->peer, [&](PeerBufs &pb) -> int {
+        TRY(pb.d_p2p.alloc(bytes));
+        CK(cudaMemset(pb.d_p2p.get(), 0, bytes));
+        TRY(pb.d_ms.alloc(1));
+        CK(cudaMemset(pb.d_ms.get(), 0, sizeof(MergeScratch)));
+        TRY(pb.d_mscore.alloc(rows));
+        TRY(pb.d_mpos.alloc(rows));
+        TRY(pb.h_grows.alloc(rows * 2));
+        TRY(pb.h_ghdr.alloc(16));
+        memset(pb.h_ghdr.get(), 0, 16 * sizeof(uint32_t));
+        return FZB_OK;
+    });
 }
 
 static void close_peers(fzb_haystack *h) {
@@ -813,19 +843,9 @@ static void close_peers(fzb_haystack *h) {
 }
 
 static void p2p_free(fzb_haystack *h) {
+    detach_pending(h);  // the last result's global rows may still sit in h_grows
     close_peers(h);
-    if (h->d_p2p) cudaFree(h->d_p2p);
-    if (h->d_ms) cudaFree(h->d_ms);
-    if (h->d_mscore) cudaFree(h->d_mscore);
-    if (h->d_mpos) cudaFree(h->d_mpos);
-    if (h->h_grows) cudaFreeHost(h->h_grows);
-    if (h->h_ghdr) cudaFreeHost(h->h_ghdr);
-    h->d_p2p = nullptr;
-    h->d_ms = nullptr;
-    h->d_mscore = nullptr;
-    h->d_mpos = nullptr;
-    h->h_grows = nullptr;
-    h->h_ghdr = nullptr;
+    h->peer.reset();
     h->p2p = false;
 }
 
@@ -850,8 +870,7 @@ extern "C" int fzb_haystack_comm_init(fzb_haystack *h, const uint8_t id[FZB_NCCL
     NcclId nid;
     memcpy(nid.b, id, FZB_NCCL_ID_BYTES);
     NCCLCK(g_nccl.CommInitRank(&h->comm, world_size, nid, rank));
-    rc = ensure_gather_buffers(h, h->gather_cap);
-    if (rc) return rc;
+    TRY(ensure_gather_buffers(h, h->gather_cap));
     // Peer-memory world: every rank exports its receive area through CUDA IPC; the handles travel over the
     // fresh NCCL communicator (bootstrap only).  Any failure on any rank (no IPC in this container, no peer
     // access between two GPUs) leaves p2p = false on ALL ranks and FZB_F_GLOBAL searches use the staged path.
@@ -864,19 +883,20 @@ extern "C" int fzb_haystack_comm_init(fzb_haystack *h, const uint8_t id[FZB_NCCL
     const size_t rec = 128;
     Hello me{};
     me.ok = world_size <= kMaxWorld && p2p_alloc(h) == FZB_OK &&
-            cudaIpcGetMemHandle(&me.handle, h->d_p2p) == cudaSuccess;
+            cudaIpcGetMemHandle(&me.handle, h->peer->d_p2p.get()) == cudaSuccess;
     cudaGetLastError();
     me.device = h->device;
     me.pid = (long long)getpid();
     std::vector<uint8_t> all(rec * world_size);
+    GatherBufs &g = *h->gather;
     auto exchange = [&](const void *mine) -> int {  // all-gather one 128-byte record per rank
-        memset(h->h_send, 0, rec);
-        memcpy(h->h_send, mine, sizeof(Hello));
-        CK(cudaMemcpyAsync(h->d_send, h->h_send, rec, cudaMemcpyHostToDevice, h->stream));
-        NCCLCK(g_nccl.AllGather(h->d_send, h->d_recv, rec, /*ncclInt8*/ 0, h->comm, h->stream));
-        CK(cudaMemcpyAsync(h->h_recv, h->d_recv, rec * world_size, cudaMemcpyDeviceToHost, h->stream));
+        memset(g.h_send.get(), 0, rec);
+        memcpy(g.h_send.get(), mine, sizeof(Hello));
+        CK(cudaMemcpyAsync(g.d_send.get(), g.h_send.get(), rec, cudaMemcpyHostToDevice, h->stream));
+        NCCLCK(g_nccl.AllGather(g.d_send.get(), g.d_recv.get(), rec, /*ncclInt8*/ 0, h->comm, h->stream));
+        CK(cudaMemcpyAsync(g.h_recv.get(), g.d_recv.get(), rec * world_size, cudaMemcpyDeviceToHost, h->stream));
         CK(cudaStreamSynchronize(h->stream));
-        memcpy(all.data(), h->h_recv, rec * world_size);
+        memcpy(all.data(), g.h_recv.get(), rec * world_size);
         return FZB_OK;
     };
     rc = exchange(&me);
@@ -887,7 +907,7 @@ extern "C" int fzb_haystack_comm_init(fzb_haystack *h, const uint8_t id[FZB_NCCL
         for (int r = 0; r < world_size && ok; r++) {
             const Hello *peer = reinterpret_cast<const Hello *>(all.data() + rec * r);
             if (r == rank) {
-                h->peer_base[r] = h->d_p2p;
+                h->peer_base[r] = h->peer->d_p2p.get();
             } else {
                 void *ptr = nullptr;
                 if (cudaIpcOpenMemHandle(&ptr, peer->handle, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) {
@@ -917,14 +937,13 @@ extern "C" int fzb_comm_init_local(fzb_haystack **handles, int world_size) {
     for (int r = 0; r < world_size; r++) {
         fzb_haystack *h = handles[r];
         reset_world(h, r, world_size, true);
-        int rc = p2p_alloc(h);
-        if (rc) return rc;
+        TRY(p2p_alloc(h));
     }
     for (int r = 0; r < world_size; r++) {
         fzb_haystack *h = handles[r];
         CK(cudaSetDevice(h->device));
         for (int q = 0; q < world_size; q++) {
-            h->peer_base[q] = handles[q]->d_p2p;
+            h->peer_base[q] = handles[q]->peer->d_p2p.get();
             if (handles[q]->device != h->device) {
                 int can = 0;
                 CK(cudaDeviceCanAccessPeer(&can, h->device, handles[q]->device));
@@ -950,20 +969,19 @@ extern "C" int fzb_p2p_export(fzb_haystack *h, int rank, int world_size, uint8_t
     static_assert(sizeof(cudaIpcMemHandle_t) == FZB_IPC_HANDLE_BYTES, "IPC handle size");
     CK(cudaSetDevice(h->device));
     reset_world(h, rank, world_size, false);
-    int rc = p2p_alloc(h);
-    if (rc) return rc;
+    TRY(p2p_alloc(h));
     cudaIpcMemHandle_t mine;
-    CK(cudaIpcGetMemHandle(&mine, h->d_p2p));
+    CK(cudaIpcGetMemHandle(&mine, h->peer->d_p2p.get()));
     memcpy(handle, &mine, sizeof mine);
     return FZB_OK;
 }
 
 extern "C" int fzb_p2p_connect(fzb_haystack *h, const uint8_t *handles) {
-    if (!h || !handles || !h->d_p2p) return fail(FZB_E_INVALID, "fzb_p2p_export first");
+    if (!h || !handles || !h->peer) return fail(FZB_E_INVALID, "fzb_p2p_export first");
     CK(cudaSetDevice(h->device));
     for (int r = 0; r < h->world; r++) {
         if (r == h->rank) {
-            h->peer_base[r] = h->d_p2p;
+            h->peer_base[r] = h->peer->d_p2p.get();
             continue;
         }
         cudaIpcMemHandle_t peer;
@@ -1158,25 +1176,25 @@ static int allgather_groups_staged(fzb_haystack *h, const std::vector<int64_t> &
     const uint64_t n = rows.size() / kFinCols;
     for (;;) {
         const uint32_t cap = h->gather_cap;
-        int rc = ensure_gather_buffers(h, cap);
-        if (rc) return rc;
+        TRY(ensure_gather_buffers(h, cap));
+        GatherBufs &g = *h->gather;
         const size_t slot_rows = (size_t)cap + 1, slot = slot_rows * kFinCols * sizeof(int64_t);
-        h->h_send[0] = (int64_t)n;
-        h->h_send[1] = n <= cap;
-        h->h_send[2] = h->h_send[3] = h->h_send[4] = 0;
-        if (n <= cap && n) memcpy(h->h_send + kFinCols, rows.data(), n * kFinCols * sizeof(int64_t));
-        CK(cudaMemcpyAsync(h->d_send, h->h_send, (1 + (n <= cap ? n : 0)) * kFinCols * sizeof(int64_t),
+        g.h_send[0] = (int64_t)n;
+        g.h_send[1] = n <= cap;
+        g.h_send[2] = g.h_send[3] = g.h_send[4] = 0;
+        if (n <= cap && n) memcpy(g.h_send.get() + kFinCols, rows.data(), n * kFinCols * sizeof(int64_t));
+        CK(cudaMemcpyAsync(g.d_send.get(), g.h_send.get(), (1 + (n <= cap ? n : 0)) * kFinCols * sizeof(int64_t),
                            cudaMemcpyHostToDevice, h->stream));
-        NCCLCK(g_nccl.AllGather(h->d_send, h->d_recv, slot, /*ncclInt8*/ 0, h->comm, h->stream));
-        CK(cudaMemcpyAsync(h->h_recv, h->d_recv, slot * h->world, cudaMemcpyDeviceToHost, h->stream));
+        NCCLCK(g_nccl.AllGather(g.d_send.get(), g.d_recv.get(), slot, /*ncclInt8*/ 0, h->comm, h->stream));
+        CK(cudaMemcpyAsync(g.h_recv.get(), g.d_recv.get(), slot * h->world, cudaMemcpyDeviceToHost, h->stream));
         CK(cudaStreamSynchronize(h->stream));
         uint64_t top = 0;
-        for (int r = 0; r < h->world; r++) top = std::max<uint64_t>(top, (uint64_t)h->h_recv[(size_t)r * slot_rows * kFinCols]);
+        for (int r = 0; r < h->world; r++) top = std::max<uint64_t>(top, (uint64_t)g.h_recv[(size_t)r * slot_rows * kFinCols]);
         if (top <= cap) {
             all.clear();
             counts.clear();
             for (int r = 0; r < h->world; r++) {
-                const int64_t *base = h->h_recv + (size_t)r * slot_rows * kFinCols;
+                const int64_t *base = g.h_recv.get() + (size_t)r * slot_rows * kFinCols;
                 all.insert(all.end(), base + kFinCols, base + kFinCols + (size_t)base[0] * kFinCols);
                 counts.push_back((uint64_t)base[0]);
             }
@@ -1197,10 +1215,10 @@ static void fill_params(const fzb_haystack *h, const uint8_t *pattern, uint32_t 
     p.N = (int64_t)h->global_len;
     p.own_lo = (int64_t)h->own_lo;
     p.own_hi = (int64_t)h->own_hi;
-    p.bitmap = h->d_bitmap;
-    p.glist = h->d_glist;
+    p.bitmap = h->d_bitmap.get();
+    p.glist = h->d_glist.get();
     p.glist_cap = h->glist_cap;
-    p.counters = h->d_counters;
+    p.counters = h->d_counters.get();
     p.m = (int)m;
     memcpy(p.P, pattern, m);
 }
@@ -1217,16 +1235,15 @@ static int check_halo(const fzb_haystack *h, uint64_t halo) {
 
 constexpr uint64_t kMaxRawRecs = 1ull << 27;  // raw records of one search (or one shared batch pass)
 
+// Grows d_out to hold `need` records.  The new buffer is allocated before the old one is released, so a failure leaves
+// the handle with its previous buffer and size; the price is a transient peak of 1.5x the new size during the growth
+// (at the 2^27-record limit, 40 B per record: 5.4 GB + 2.7 GB).
 static int ensure_out_cap(fzb_haystack *h, uint64_t need) {
-    if (need <= h->out_cap) return FZB_OK;
-    uint64_t cap = h->out_cap;
+    if (need <= h->d_out.size()) return FZB_OK;
+    uint64_t cap = h->d_out.size();
     while (cap < need) cap *= 2;
     if (cap > kMaxRawRecs) return fail(FZB_E_UNSUPPORTED, "more than 2^27 raw matches in one search");
-    CK(cudaFree(h->d_out));
-    h->d_out = nullptr;
-    CK(cudaMalloc(&h->d_out, (size_t)cap * (sizeof(RawRec) + sizeof(uint64_t))));
-    h->out_cap = (uint32_t)cap;
-    return FZB_OK;
+    return alloc_out(h, cap);
 }
 
 // Runs one search attempt after another until the output buffer was large enough.  `enqueue` must
@@ -1274,7 +1291,7 @@ template <class F>
 static int run_emitting(fzb_haystack *h, fzb_result *res, F enqueue, PostPlan post = PostPlan()) {
     detach_pending(h);  // k_post is about to overwrite the staging buffer an earlier result may still point at
     for (int attempt = 0; attempt < 8; attempt++) {
-        if (!h->counters_clean) CK(cudaMemsetAsync(h->d_counters, 0, CNT_COUNT * sizeof(uint32_t), h->stream));
+        if (!h->counters_clean) CK(cudaMemsetAsync(h->d_counters.get(), 0, CNT_COUNT * sizeof(uint32_t), h->stream));
         h->counters_clean = false;
         CK(cudaEventRecord(h->ev[0], h->stream));
         h->ev1_recorded = false;
@@ -1282,8 +1299,8 @@ static int run_emitting(fzb_haystack *h, fzb_result *res, F enqueue, PostPlan po
         if (rc) return rc;
         CK(cudaGetLastError());
         h->seq++;
-        PostArgs pa{reinterpret_cast<const uint64_t *>(h->d_out + h->out_cap), h->out_cap, post.mode,
-                    h->d_sorted, h->d_fin, h->h_fin, h->h_counters, h->d_counters, h->seq, 0};
+        PostArgs pa{reinterpret_cast<const uint64_t *>(h->d_out.get() + h->d_out.size()), (uint32_t)h->d_out.size(), post.mode,
+                    h->d_sorted.get(), h->d_fin.get(), h->h_fin.get(), h->h_counters.get(), h->d_counters.get(), h->seq, 0};
         // fused multi-GPU reduction over peer memory (below): k_push reads the counters after k_post, and clears them
         pa.clear = !(post.global && attempt == 0 && h->p2p && !res->fused_issued);
         k_post<<<h->sm_count, kPostThreads, kPostSmem, h->stream>>>(pa);
@@ -1303,26 +1320,26 @@ static int run_emitting(fzb_haystack *h, fzb_result *res, F enqueue, PostPlan po
             w.slot_bytes = h->slot_bytes;
             w.flags_off = h->flags_off;
             for (int r = 0; r < h->world; r++) w.peer[r] = h->peer_base[r];
-            k_push<<<kPushCtas, kPushThreads, 0, h->stream>>>(w, h->d_fin, h->d_counters, post.mode, h->d_ms);
-            MergeOut mo{h->d_mscore, h->d_mpos, h->h_grows, h->h_ghdr, h->seq};
-            k_merge<<<h->world, kPostThreads, 0, h->stream>>>(w, h->d_ms, mo);
+            PeerBufs &pb = *h->peer;
+            k_push<<<kPushCtas, kPushThreads, 0, h->stream>>>(w, h->d_fin.get(), h->d_counters.get(), post.mode, pb.d_ms.get());
+            MergeOut mo{pb.d_mscore.get(), pb.d_mpos.get(), pb.h_grows.get(), pb.h_ghdr.get(), h->seq};
+            k_merge<<<h->world, kPostThreads, 0, h->stream>>>(w, pb.d_ms.get(), mo);
             CK(cudaGetLastError());
             res->stats.n_launches += 2;
         }
         CK(cudaEventRecord(h->ev[2], h->stream));
-        rc = wait_done(h, fused ? h->h_ghdr + 7 : h->h_counters + CNT_SEQ);
+        rc = wait_done(h, fused ? h->peer->h_ghdr.get() + 7 : h->h_counters.get() + CNT_SEQ);
         if (rc) return rc;
         const uint32_t n = h->h_counters[CNT_OUT];
         res->stats.n_candidates = h->h_counters[CNT_CAND];
         if (fused) {
             res->fused_issued = true;
-            res->fused_status = h->h_ghdr[0];
-            res->gcount = h->h_ghdr[1];
-            if (h->h_ghdr[2] != h->epoch && res->fused_status == MS_OK) res->fused_status = MS_TIMEOUT;
+            res->fused_status = h->peer->h_ghdr[0];
+            res->gcount = h->peer->h_ghdr[1];
+            if (h->peer->h_ghdr[2] != h->epoch && res->fused_status == MS_OK) res->fused_status = MS_TIMEOUT;
         }
-        if (n > h->out_cap) {  // output buffer too small: grow and redo the whole attempt
-            rc = ensure_out_cap(h, n);
-            if (rc) return rc;
+        if (n > h->d_out.size()) {  // output buffer too small: grow and redo the whole attempt
+            TRY(ensure_out_cap(h, n));
             continue;
         }
         const bool posted = h->h_counters[CNT_POST_DONE] != 0;
@@ -1332,7 +1349,7 @@ static int run_emitting(fzb_haystack *h, fzb_result *res, F enqueue, PostPlan po
         res->raw_n = n;
         res->raw_ordered = false;
         if (posted || (res->fused_issued && res->fused_status == MS_OK)) {
-            // the raw records are in h->d_out, the global rows in h->h_grows: copied out lazily (fetch_raw)
+            // the raw records are in h->d_out, the global rows in h->peer->h_grows: copied out lazily (fetch_raw)
             std::lock_guard<std::mutex> lock(g_pending_mutex);
             res->raw_in_stage = posted;
             res->owner = h;
@@ -1340,7 +1357,7 @@ static int run_emitting(fzb_haystack *h, fzb_result *res, F enqueue, PostPlan po
         }
         if (!posted && n) {  // list too long for k_post: fetch it, the host orders and consolidates
             res->raw.resize(n);
-            CK(cudaMemcpyAsync(res->raw.data(), h->d_out, (size_t)n * sizeof(RawRec), cudaMemcpyDeviceToHost, h->stream));
+            CK(cudaMemcpyAsync(res->raw.data(), h->d_out.get(), (size_t)n * sizeof(RawRec), cudaMemcpyDeviceToHost, h->stream));
             CK(cudaStreamSynchronize(h->stream));
         }
         res->fin.clear();
@@ -1556,10 +1573,8 @@ static int search_lev_ngrams(fzb_haystack *h, const uint8_t *pattern, uint32_t m
     // hit must fit a lane's shared-memory slot); the list overflowing triggers one retry in granule mode
     const int vm = verify_mode((int)m, p.L);
     bool use_hits = !sampled && k > 0 && (m + 2 * k + 8 <= (uint32_t)kHitSlotBytes);
-    if (use_hits && !h->d_hits) {
-        h->hits_cap = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(1u << 20, h->capacity / 256), 1u << 28);
-        CK(cudaMalloc(&h->d_hits, (size_t)h->hits_cap * sizeof(uint64_t)));
-    }
+    if (use_hits && !h->d_hits)
+        TRY(h->d_hits.alloc(std::min<uint64_t>(std::max<uint64_t>(1u << 20, h->owned_buf.size() / 256), 1u << 28)));
     bool fuse_gather = post_mode != 0 && (flags & FZB_F_GLOBAL) != 0;
     bool bitmap_mode = false;
     if (flags & FZB_F_TINY_LIST) p.glist_cap = std::min(h->glist_cap, 8u);
@@ -1568,11 +1583,11 @@ static int search_lev_ngrams(fzb_haystack *h, const uint8_t *pattern, uint32_t m
         if (r2) return r2;
         if (use_hits) {
             if (vm == 0)
-                k_verify_hits<0><<<h->sm_count * 8, kHitThreads, 0, h->stream>>>(p, h->d_out, h->out_cap, h->d_counters);
+                k_verify_hits<0><<<h->sm_count * 8, kHitThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(), h->d_counters.get());
             else if (vm == 1)
-                k_verify_hits<1><<<h->sm_count * 8, kHitThreads, 0, h->stream>>>(p, h->d_out, h->out_cap, h->d_counters);
+                k_verify_hits<1><<<h->sm_count * 8, kHitThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(), h->d_counters.get());
             else
-                k_verify_hits<2><<<h->sm_count * 8, kHitThreads, 0, h->stream>>>(p, h->d_out, h->out_cap, h->d_counters);
+                k_verify_hits<2><<<h->sm_count * 8, kHitThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(), h->d_counters.get());
             res->stats.n_launches++;
             return FZB_OK;
         }
@@ -1580,21 +1595,22 @@ static int search_lev_ngrams(fzb_haystack *h, const uint8_t *pattern, uint32_t m
             const int scan_mode = bitmap_mode ? 1 : 0;
             const int grid = h->sm_count * kVerifyCtasPerSm;
             if (vm == 0)
-                k_verify_lev<0><<<grid, kVerifyThreads, 0, h->stream>>>(p, h->bitmap_words, h->d_glist, p.glist_cap,
-                                                                        scan_mode, h->d_out, h->out_cap, h->d_counters);
+                k_verify_lev<0><<<grid, kVerifyThreads, 0, h->stream>>>(p, h->d_bitmap.size(), h->d_glist.get(), p.glist_cap,
+                                                                        scan_mode, h->d_out.get(), h->d_out.size(), h->d_counters.get());
             else if (vm == 1)
-                k_verify_lev<1><<<grid, kVerifyThreads, 0, h->stream>>>(p, h->bitmap_words, h->d_glist, p.glist_cap,
-                                                                        scan_mode, h->d_out, h->out_cap, h->d_counters);
+                k_verify_lev<1><<<grid, kVerifyThreads, 0, h->stream>>>(p, h->d_bitmap.size(), h->d_glist.get(), p.glist_cap,
+                                                                        scan_mode, h->d_out.get(), h->d_out.size(), h->d_counters.get());
             else
-                k_verify_lev<2><<<grid, kVerifyThreads, 0, h->stream>>>(p, h->bitmap_words, h->d_glist, p.glist_cap,
-                                                                        scan_mode, h->d_out, h->out_cap, h->d_counters);
+                k_verify_lev<2><<<grid, kVerifyThreads, 0, h->stream>>>(p, h->d_bitmap.size(), h->d_glist.get(), p.glist_cap,
+                                                                        scan_mode, h->d_out.get(), h->d_out.size(), h->d_counters.get());
         }
         res->stats.n_launches += 1;
         return FZB_OK;
     };
     for (;;) {
-        p.hits = use_hits ? h->d_hits : nullptr;
-        p.hits_cap = use_hits ? ((flags & FZB_F_TINY_LIST) ? std::min(h->hits_cap, 8u) : h->hits_cap) : 0;
+        p.hits = use_hits ? h->d_hits.get() : nullptr;
+        const uint32_t hits_cap = (uint32_t)h->d_hits.size();
+        p.hits_cap = use_hits ? ((flags & FZB_F_TINY_LIST) ? std::min(hits_cap, 8u) : hits_cap) : 0;
         // (the raw stream's order (n-gram, hit index) is restored lazily)
         rc = run_emitting(h, res, enqueue, PostPlan{post_mode, fuse_gather});
         if (rc) return rc;
@@ -1621,14 +1637,10 @@ static int search_lev_ngrams(fzb_haystack *h, const uint8_t *pattern, uint32_t m
 // ------------------------------------------------------------------------------------------------
 // LP / generic routes (lp_kernels.cuh)
 // ------------------------------------------------------------------------------------------------
+// Grows the candidate lists to `words`: the new slab is allocated before the old one is released, so a failure leaves
+// the handle with its previous slab.
 static int ensure_scratch(fzb_haystack *h, uint64_t words) {
-    if (words <= h->scratch_words) return FZB_OK;
-    if (h->d_scratch) CK(cudaFree(h->d_scratch));
-    h->d_scratch = nullptr;
-    h->scratch_words = 0;
-    CK(cudaMalloc(&h->d_scratch, words * sizeof(uint32_t)));
-    h->scratch_words = words;
-    return FZB_OK;
+    return words <= h->d_scratch.size() ? FZB_OK : h->d_scratch.alloc(words);
 }
 
 // FZB_F_TINY_LIST (testing) caps the survivor list of the streaming LP search (and of the batch LP pass) at this many
@@ -1647,10 +1659,8 @@ static int run_lp(fzb_haystack *h, fzb_result *res, F enqueue, PostPlan post = P
     const int grid = h->sm_count * 4;
     const uint64_t threads = (uint64_t)grid * kLpThreads;
     for (int cap = 256; cap <= kLpMaxCap; cap *= 8) {
-        int rc = ensure_scratch(h, threads * 2 * (uint64_t)cap);
-        if (rc) return rc;
-        rc = run_emitting(h, res, [&]() -> int { return enqueue(grid, cap); }, post);
-        if (rc) return rc;
+        TRY(ensure_scratch(h, threads * 2 * (uint64_t)cap));
+        TRY(run_emitting(h, res, [&]() -> int { return enqueue(grid, cap); }, post));
         if (!h->h_counters[CNT_OVERFLOW]) return FZB_OK;
     }
     return fail(FZB_E_UNSUPPORTED, "candidate explosion: more than 16384 live candidates for one start");
@@ -1670,19 +1680,18 @@ static int search_lev_lp(fzb_haystack *h, const uint8_t *pattern, uint32_t m, ui
     // streaming form (k_lp_scan + k_lp_verify) when the look-ahead masks cover the window; the list of surviving
     // starts overflowing (low-entropy data: most starts survive) falls back to the tile kernel
     bool streaming = k < m && m + k <= (uint32_t)kLpsMaxWin && !(flags & FZB_F_FORCE_DENSE) && h->buf_len > 0;
-    if (streaming && !h->d_lplist) {
-        h->lplist_cap = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(1u << 20, h->capacity / 64), 1u << 26);
-        CK(cudaMalloc(&h->d_lplist, (size_t)h->lplist_cap * sizeof(unsigned long long)));
-    }
+    if (streaming && !h->d_lplist)
+        TRY(h->d_lplist.alloc(std::min<uint64_t>(std::max<uint64_t>(1u << 20, h->owned_buf.size() / 64), 1u << 26)));
     const PostPlan plan{post_mode, post_mode != 0 && (flags & FZB_F_GLOBAL) != 0};
     if (streaming) {
-        const uint32_t list_cap = (flags & FZB_F_TINY_LIST) ? std::min(h->lplist_cap, kTinyLpListCap) : h->lplist_cap;
+        const uint32_t list_cap = (flags & FZB_F_TINY_LIST) ? std::min<uint32_t>(h->d_lplist.size(), kTinyLpListCap)
+                                                            : (uint32_t)h->d_lplist.size();
         rc = run_lp(h, res, [&](int grid, int cap) -> int {
-            k_lp_scan<<<h->sm_count * 4, kLpsThreads, 0, h->stream>>>(p, h->d_lplist, list_cap);
+            k_lp_scan<<<h->sm_count * 4, kLpsThreads, 0, h->stream>>>(p, h->d_lplist.get(), list_cap);
             CK(cudaEventRecord(h->ev[1], h->stream));
             h->ev1_recorded = true;
-            k_lp_verify<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_lplist, list_cap, h->d_scratch, cap, h->d_out,
-                                                            h->out_cap, h->d_counters);
+            k_lp_verify<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_lplist.get(), list_cap, h->d_scratch.get(), cap, h->d_out.get(),
+                                                            h->d_out.size(), h->d_counters.get());
             res->stats.n_launches += 2;
             return FZB_OK;
         }, plan);
@@ -1694,7 +1703,7 @@ static int search_lev_lp(fzb_haystack *h, const uint8_t *pattern, uint32_t m, ui
         res->discard_attempt();  // list overflow: nothing was verified (and the fused reduction saw an invalid shard)
     }
     rc = run_lp(h, res, [&](int grid, int cap) -> int {
-        k_lev_lp<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_scratch, cap, h->d_out, h->out_cap, h->d_counters);
+        k_lev_lp<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_scratch.get(), cap, h->d_out.get(), h->d_out.size(), h->d_counters.get());
         res->stats.n_launches++;
         return FZB_OK;
     }, plan);
@@ -1734,8 +1743,8 @@ static int search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, u
     if (!ngrams) {
         res->stats.route = 6;
         rc = run_lp(h, res, [&](int grid, int cap) -> int {
-            k_generic_lp<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_scratch, cap, h->d_out, h->out_cap,
-                                                             h->d_counters);
+            k_generic_lp<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_scratch.get(), cap, h->d_out.get(), h->d_out.size(),
+                                                             h->d_counters.get());
             res->stats.n_launches++;
             return FZB_OK;
         }, PostPlan{post_mode, post_mode != 0 && (flags & FZB_F_GLOBAL) != 0});
@@ -1755,8 +1764,8 @@ static int search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, u
     rc = run_lp(h, res, [&](int grid, int cap) -> int {
         int r2 = enqueue_filter(h, p, sampled, res);
         if (r2) return r2;
-        k_verify_generic<<<grid, kLpThreads, 0, h->stream>>>(p, h->bitmap_words, h->d_scratch, cap, h->d_out,
-                                                             h->out_cap, h->d_counters);
+        k_verify_generic<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_bitmap.size(), h->d_scratch.get(), cap, h->d_out.get(),
+                                                             h->d_out.size(), h->d_counters.get());
         res->stats.n_launches++;
         return FZB_OK;
     }, PostPlan{post_mode, post_mode != 0 && (flags & FZB_F_GLOBAL) != 0});
@@ -1876,24 +1885,23 @@ constexpr uint32_t kTinyBatchCap = 8;
 constexpr uint64_t kTinyLpChunk = 3000;
 
 static int ensure_batch_buffers(fzb_haystack *h) {
-    if (h->d_mbits) return FZB_OK;
     CK(cudaSetDevice(h->device));
-    CK(cudaMalloc(&h->d_mbits, (kMultiTblWords + kMulti2Words) * sizeof(uint32_t)));  // first + second level tables
-    CK(cudaMalloc(&h->d_gtab, kGtabSlots * sizeof(uint2)));
-    CK(cudaMalloc(&h->d_postings, kMaxBatchPostings * sizeof(uint32_t)));
-    CK(cudaMalloc(&h->d_pinfo, kMaxBatchPats * sizeof(uint32_t)));
-    CK(cudaMalloc(&h->d_bpats, kMaxBatchPats * sizeof(BatchPat)));
-    h->mset_slots = 1u << 22;
-    h->mwork_cap = 1u << 21;
-    CK(cudaMalloc(&h->d_mset, (size_t)h->mset_slots * sizeof(unsigned long long)));
-    CK(cudaMemset(h->d_mset, 0, (size_t)h->mset_slots * sizeof(unsigned long long)));
-    CK(cudaMalloc(&h->d_mwork, (size_t)h->mwork_cap * sizeof(WorkItem)));
-    CK(cudaFuncSetAttribute(k_filter_multi, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMultiSmem));
-    return FZB_OK;
+    return ensure_group(h->batch, [](BatchBufs &b) -> int {
+        TRY(b.d_mbits.alloc(kMultiTblWords + kMulti2Words));  // first + second level tables
+        TRY(b.d_gtab.alloc(kGtabSlots));
+        TRY(b.d_postings.alloc(kMaxBatchPostings));
+        TRY(b.d_pinfo.alloc(kMaxBatchPats));
+        TRY(b.d_bpats.alloc(kMaxBatchPats));
+        TRY(b.d_mset.alloc(1u << 22));
+        CK(cudaMemset(b.d_mset.get(), 0, b.d_mset.size() * sizeof(unsigned long long)));
+        TRY(b.d_mwork.alloc(1u << 21));
+        CK(cudaFuncSetAttribute(k_filter_multi, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMultiSmem));
+        return FZB_OK;
+    });
 }
 
 static int read_counters(fzb_haystack *h, uint32_t cnts[CNT_COUNT]) {
-    CK(cudaMemcpyAsync(cnts, h->d_counters, CNT_COUNT * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(cnts, h->d_counters.get(), CNT_COUNT * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return FZB_OK;
 }
@@ -1916,7 +1924,7 @@ static int run_batch_pass(fzb_haystack *h, F enqueue, std::vector<RawRec> &raw, 
     detach_pending(h);  // the kernels are about to overwrite the output buffer an earlier result may still point at
     for (int attempt = 0; attempt < 8; attempt++) {
         h->counters_clean = false;  // (a batch pass leaves its counters behind)
-        CK(cudaMemsetAsync(h->d_counters, 0, CNT_COUNT * sizeof(uint32_t), h->stream));
+        CK(cudaMemsetAsync(h->d_counters.get(), 0, CNT_COUNT * sizeof(uint32_t), h->stream));
         CK(cudaEventRecord(h->ev[0], h->stream));
         int rc = enqueue();
         if (rc) return rc;
@@ -1928,14 +1936,13 @@ static int run_batch_pass(fzb_haystack *h, F enqueue, std::vector<RawRec> &raw, 
         // more records than one search may return, over all the patterns of the pass: they go one by one, where
         // each pattern only has to stay within the limit on its own
         if (n > kMaxRawRecs) return 1;
-        if (n > h->out_cap) {
-            rc = ensure_out_cap(h, n);
-            if (rc) return rc;
+        if (n > h->d_out.size()) {
+            TRY(ensure_out_cap(h, n));
             continue;
         }
         raw.resize(n);
         if (n) {
-            CK(cudaMemcpyAsync(raw.data(), h->d_out, (size_t)n * sizeof(RawRec), cudaMemcpyDeviceToHost, h->stream));
+            CK(cudaMemcpyAsync(raw.data(), h->d_out.get(), (size_t)n * sizeof(RawRec), cudaMemcpyDeviceToHost, h->stream));
             CK(cudaStreamSynchronize(h->stream));
         }
         float ms = 0.f;
@@ -2013,15 +2020,14 @@ static int upload_pass_tables(fzb_haystack *h, const std::unordered_map<uint32_t
             postings.insert(postings.end(), g.second.begin() + first, g.second.begin() + first + c);
         }
     }
-    int rc = ensure_batch_buffers(h);
-    if (rc) return rc;
-    CK(cudaSetDevice(h->device));
-    CK(cudaMemcpyAsync(h->d_mbits, bits.data(), bits.size() * 4, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_gtab, gtab.data(), gtab.size() * sizeof(uint2), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_postings, postings.data(), postings.size() * 4, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_pinfo, pinfo.data(), pinfo.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    TRY(ensure_batch_buffers(h));  // (makes the handle's device current)
+    BatchBufs &b = *h->batch;
+    CK(cudaMemcpyAsync(b.d_mbits.get(), bits.data(), bits.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(b.d_gtab.get(), gtab.data(), gtab.size() * sizeof(uint2), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(b.d_postings.get(), postings.data(), postings.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(b.d_pinfo.get(), pinfo.data(), pinfo.size() * 4, cudaMemcpyHostToDevice, h->stream));
     // (pageable sources: each copy has left its host vector when it returns)
-    CK(cudaMemcpyAsync(h->d_bpats, pats.data(), pats.size() * sizeof(BatchPat), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(b.d_bpats.get(), pats.data(), pats.size() * sizeof(BatchPat), cudaMemcpyHostToDevice, h->stream));
     return FZB_OK;
 }
 
@@ -2034,12 +2040,12 @@ static MultiParams pass_params(const fzb_haystack *h) {
     mp.N = (int64_t)h->global_len;
     mp.own_lo = (int64_t)h->own_lo;
     mp.own_hi = (int64_t)h->own_hi;
-    mp.bits = h->d_mbits;
-    mp.gtab = h->d_gtab;
+    mp.bits = h->batch->d_mbits.get();
+    mp.gtab = h->batch->d_gtab.get();
     mp.gtab_mask = kGtabSlots - 1;
-    mp.postings = h->d_postings;
-    mp.pinfo = h->d_pinfo;
-    mp.counters = h->d_counters;
+    mp.postings = h->batch->d_postings.get();
+    mp.pinfo = h->batch->d_pinfo.get();
+    mp.counters = h->d_counters.get();
     return mp;
 }
 
@@ -2089,25 +2095,27 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
         }
     });
     if (rc) return rc;
-    if (dense && !h->d_mhits) {
-        h->mhits_cap = 1u << 23;
-        CK(cudaMalloc(&h->d_mhits, (size_t)h->mhits_cap * sizeof(unsigned long long)));
+    if (dense && !h->d_mhits) {  // taken by the handle only together with its kernel's attribute
+        DevBuf<unsigned long long> hits;
+        TRY(hits.alloc(1u << 23));
         CK(cudaFuncSetAttribute(k_filter_mdense, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMdenseSmem));
+        h->d_mhits = std::move(hits);
     }
+    BatchBufs &b = *h->batch;
     MultiParams mp = pass_params(h);
-    mp.bits2 = dense ? nullptr : h->d_mbits + kMultiTblWords;
-    mp.set = h->d_mset;
-    mp.set_mask = h->mset_slots - 1;
-    mp.work = h->d_mwork;
-    mp.work_cap = tiny ? std::min(h->mwork_cap, kTinyBatchCap) : h->mwork_cap;
-    const uint32_t hits_cap = tiny ? std::min(h->mhits_cap, kTinyBatchCap) : h->mhits_cap;
+    mp.bits2 = dense ? nullptr : b.d_mbits.get() + kMultiTblWords;
+    mp.set = b.d_mset.get();
+    mp.set_mask = (uint32_t)b.d_mset.size() - 1;
+    mp.work = b.d_mwork.get();
+    mp.work_cap = tiny ? std::min<uint32_t>(b.d_mwork.size(), kTinyBatchCap) : (uint32_t)b.d_mwork.size();
+    const uint32_t hits_cap = tiny ? std::min<uint32_t>(h->d_mhits.size(), kTinyBatchCap) : (uint32_t)h->d_mhits.size();
     const int64_t nvec = (int64_t)(round_up(h->buf_len, 16) / 16);
     const int64_t ntiles = (nvec + kMultiTileVecs - 1) / kMultiTileVecs;
     std::vector<RawRec> raw;
     uint32_t cnts[CNT_COUNT];
     fzb_stats pass{};
     rc = run_batch_pass(h, [&]() -> int {
-        MdenseParams dp{mp, h->d_bpats, h->d_mhits, hits_cap};
+        MdenseParams dp{mp, b.d_bpats.get(), h->d_mhits.get(), hits_cap};
         if (ntiles > 0) {
             const int grid = (int)std::min<int64_t>(ntiles, h->sm_count);
             if (dense)
@@ -2117,14 +2125,15 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
         }
         CK(cudaEventRecord(h->ev[1], h->stream));
         if (dense)
-            k_verify_mhits<<<h->sm_count * 8, kMhThreads, 0, h->stream>>>(dp, h->d_out, h->out_cap, h->d_counters);
+            k_verify_mhits<<<h->sm_count * 8, kMhThreads, 0, h->stream>>>(dp, h->d_out.get(), h->d_out.size(), h->d_counters.get());
         else
-            k_verify_multi<<<h->sm_count * 8, kVmThreads, 0, h->stream>>>(mp, h->d_bpats, h->d_out, h->out_cap, h->d_counters);
+            k_verify_multi<<<h->sm_count * 8, kVmThreads, 0, h->stream>>>(mp, b.d_bpats.get(), h->d_out.get(), h->d_out.size(),
+                                                                          h->d_counters.get());
         CK(cudaGetLastError());
         return FZB_OK;
     }, raw, cnts, pass);
     if (rc > 0 && !dense) {  // work list / set too small for this batch: clean up, let the caller go one by one
-        CK(cudaMemsetAsync(h->d_mset, 0, (size_t)h->mset_slots * sizeof(unsigned long long), h->stream));
+        CK(cudaMemsetAsync(b.d_mset.get(), 0, b.d_mset.size() * sizeof(unsigned long long), h->stream));
         CK(cudaStreamSynchronize(h->stream));
     }
     if (rc) return rc;
@@ -2168,66 +2177,65 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
         wmax = std::max(wmax, (int)(m + k));
         kmax = std::max(kmax, k);
     }
-    int rc = ensure_batch_buffers(h);
-    if (rc) return rc;
-    CK(cudaSetDevice(h->device));
-    if (!h->d_lmlut) {
-        CK(cudaMalloc(&h->d_lmlut, 256 * sizeof(ulonglong2) + 64 * 256 * sizeof(uint32_t)));  // vectors + match masks
-        h->lmlist_cap = (uint32_t)std::min<uint64_t>(1u << 26, std::max<uint64_t>(1u << 22, h->capacity / 16));
-        CK(cudaMalloc(&h->d_lmlist, (size_t)h->lmlist_cap * sizeof(unsigned long long)));
-        CK(cudaMalloc(&h->d_lmkept, (size_t)h->lmlist_cap * sizeof(unsigned long long)));
-        CK(cudaMalloc(&h->d_lmhist, 256 * sizeof(uint32_t)));  // per-pattern counts [64] + kept total [1] | cursors [64]
+    TRY(ensure_batch_buffers(h));  // (makes the handle's device current)
+    TRY(ensure_group(h->lpb, [&](LpBatchBufs &l) -> int {
+        TRY(l.d_lmlut.alloc(256, 256 * sizeof(ulonglong2) + 64 * 256 * sizeof(uint32_t)));  // vectors + match masks
+        const uint64_t list_cap = std::min<uint64_t>(1u << 26, std::max<uint64_t>(1u << 22, h->owned_buf.size() / 16));
+        TRY(l.d_lmlist.alloc(list_cap));
+        TRY(l.d_lmkept.alloc(list_cap));
+        TRY(l.d_lmhist.alloc(256));
         CK(cudaFuncSetAttribute(k_lp_scan_multi, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLmSmem));
-    }
-    CK(cudaMemcpyAsync(h->d_lmlut, lut.data(), 256 * sizeof(ulonglong2), cudaMemcpyHostToDevice, h->stream));
-    uint32_t *d_pm32 = reinterpret_cast<uint32_t *>(h->d_lmlut + 256);
+        return FZB_OK;
+    }));
+    LpBatchBufs &lb = *h->lpb;
+    CK(cudaMemcpyAsync(lb.d_lmlut.get(), lut.data(), 256 * sizeof(ulonglong2), cudaMemcpyHostToDevice, h->stream));
+    uint32_t *d_pm32 = reinterpret_cast<uint32_t *>(lb.d_lmlut.get() + 256);
     CK(cudaMemcpyAsync(d_pm32, pm32.data(), pm32.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_bpats, pats.data(), pats.size() * sizeof(BatchPat), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->batch->d_bpats.get(), pats.data(), pats.size() * sizeof(BatchPat), cudaMemcpyHostToDevice, h->stream));
     lp.H = h->d;
     lp.buf_lo = (int64_t)h->buf_lo;
     lp.buf_len = (int64_t)h->buf_len;
     lp.N = (int64_t)h->global_len;
-    lp.lut = h->d_lmlut;
+    lp.lut = lb.d_lmlut.get();
     lp.wmax = wmax;
-    lp.pats = h->d_bpats;
+    lp.pats = h->batch->d_bpats.get();
     lp.pm32 = d_pm32;
-    lp.list = h->d_lmlist;
-    lp.list_cap = tiny ? std::min(h->lmlist_cap, kTinyLpListCap) : h->lmlist_cap;
-    lp.counters = h->d_counters;
+    lp.list = lb.d_lmlist.get();
+    lp.list_cap = tiny ? std::min<uint32_t>(lb.d_lmlist.size(), kTinyLpListCap) : (uint32_t)lb.d_lmlist.size();
+    lp.counters = h->d_counters.get();
     int per_sm = 2;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lp_scan_multi, kLmThreads, kLmSmem));
     per_sm = std::max(per_sm, 1);
     const int vgrid = h->sm_count * 4, sim_cap = 256;
-    rc = ensure_scratch(h, (uint64_t)vgrid * kLpThreads * 2 * sim_cap);
-    if (rc) return rc;
+    TRY(ensure_scratch(h, (uint64_t)vgrid * kLpThreads * 2 * sim_cap));
     const uint64_t chunk = tiny ? kTinyLpChunk : 256ull << 20;  // starts per scan: bounds the survivor list
     std::vector<RawRec> raw;
     uint32_t cnts[CNT_COUNT];
     fzb_stats pass{};
     float scan_ms = 0.f;
     uint64_t n_work = 0;
-    rc = run_batch_pass(h, [&]() -> int {
+    int rc = run_batch_pass(h, [&]() -> int {
         scan_ms = 0.f;
         n_work = 0;
         for (uint64_t lo = h->own_lo; lo < h->own_hi; lo += chunk) {
             lp.own_lo = (int64_t)lo;
             lp.own_hi = (int64_t)std::min<uint64_t>(h->own_hi, lo + chunk);
-            CK(cudaMemsetAsync(h->d_counters + CNT_LMLIST, 0, 2 * sizeof(uint32_t), h->stream));  // list length + flag
-            CK(cudaMemsetAsync(h->d_counters + CNT_LMNEXT, 0, sizeof(uint32_t), h->stream));       // verify work counter
+            CK(cudaMemsetAsync(h->d_counters.get() + CNT_LMLIST, 0, 2 * sizeof(uint32_t), h->stream));  // list length + flag
+            CK(cudaMemsetAsync(h->d_counters.get() + CNT_LMNEXT, 0, sizeof(uint32_t), h->stream));       // verify work counter
             CK(cudaEventRecord(h->ev[1], h->stream));
             k_lp_scan_multi<<<h->sm_count * per_sm, kLmThreads, kLmSmem, h->stream>>>(lp);
             CK(cudaEventRecord(h->ev[2], h->stream));
             // exact per-pattern windows, then a counting sort by pattern: the scan's list becomes the sorted output
-            CK(cudaMemsetAsync(h->d_lmhist, 0, 256 * sizeof(uint32_t), h->stream));
-            k_lm_refine<<<h->sm_count * 8, kLmSortThreads, 0, h->stream>>>(lp, h->d_lmkept, h->d_lmhist);
-            k_lm_scatter<<<h->sm_count * 8, kLmSortThreads, 0, h->stream>>>(h->d_lmkept, h->d_lmhist, h->d_lmhist + 128,
-                                                                              h->d_lmlist);
+            CK(cudaMemsetAsync(lb.d_lmhist.get(), 0, 256 * sizeof(uint32_t), h->stream));
+            k_lm_refine<<<h->sm_count * 8, kLmSortThreads, 0, h->stream>>>(lp, lb.d_lmkept.get(), lb.d_lmhist.get());
+            k_lm_scatter<<<h->sm_count * 8, kLmSortThreads, 0, h->stream>>>(lb.d_lmkept.get(), lb.d_lmhist.get(),
+                                                                              lb.d_lmhist.get() + 128, lb.d_lmlist.get());
             if (kmax <= 4)
-                k_lp_verify_multi<4><<<vgrid, kLpThreads, 0, h->stream>>>(lp, h->d_lmlist, h->d_lmhist, h->d_scratch, sim_cap,
-                                                                          h->d_out, h->out_cap, h->d_counters);
+                k_lp_verify_multi<4><<<vgrid, kLpThreads, 0, h->stream>>>(lp, lb.d_lmlist.get(), lb.d_lmhist.get(), h->d_scratch.get(),
+                                                                          sim_cap, h->d_out.get(), h->d_out.size(), h->d_counters.get());
             else
-                k_lp_verify_multi<8><<<vgrid, kLpThreads, 0, h->stream>>>(lp, h->d_lmlist, h->d_lmhist, h->d_scratch, sim_cap,
-                                                                          h->d_out, h->out_cap, h->d_counters);
+                k_lp_verify_multi<8><<<vgrid, kLpThreads, 0, h->stream>>>(lp, lb.d_lmlist.get(), lb.d_lmhist.get(), h->d_scratch.get(),
+                                                                          sim_cap, h->d_out.get(), h->d_out.size(), h->d_counters.get());
             CK(cudaGetLastError());
             const int r2 = read_counters(h, cnts);
             if (r2) return r2;
@@ -2512,12 +2520,12 @@ extern "C" int fzb_search_hamming(fzb_haystack *h, const uint8_t *pattern, uint3
                 h->ev1_recorded = true;
                 // one verify launch: the granule work list -- or, after it overflowed, the whole bitmap
                 k_verify_ham<<<h->sm_count * 4, kVerifyThreads, 0, h->stream>>>(
-                    p, h->bitmap_words, h->d_glist, p.glist_cap, bitmap_mode ? 1 : 0, h->d_out, h->out_cap,
-                    h->d_counters);
+                    p, h->d_bitmap.size(), h->d_glist.get(), p.glist_cap, bitmap_mode ? 1 : 0, h->d_out.get(), h->d_out.size(),
+                    h->d_counters.get());
                 res->stats.n_launches += 1;
             } else {
-                k_hamming_scan<<<h->sm_count * 8, kHamThreads, 0, h->stream>>>(p, h->d_out, h->out_cap,
-                                                                               h->d_counters);
+                k_hamming_scan<<<h->sm_count * 8, kHamThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(),
+                                                                               h->d_counters.get());
             }
             res->stats.n_launches++;
             return FZB_OK;
@@ -2630,8 +2638,8 @@ static int batch_pass_ham(fzb_haystack *h, const uint8_t *patterns, const uint32
     });
     if (rc) return rc;
     hp.mp = pass_params(h);
-    hp.mp.bits2 = two_bit ? nullptr : h->d_mbits + kMultiTblWords;
-    hp.pats = h->d_bpats;
+    hp.mp.bits2 = two_bit ? nullptr : h->batch->d_mbits.get() + kMultiTblWords;
+    hp.pats = h->batch->d_bpats.get();
     const size_t smem = two_bit ? kHbSmem2 : kMultiSmem;
     const void *fn = two_bit ? (const void *)k_ham_batch_scan<true> : (const void *)k_ham_batch_scan<false>;
     CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -2644,8 +2652,8 @@ static int batch_pass_ham(fzb_haystack *h, const uint8_t *patterns, const uint32
     uint32_t cnts[CNT_COUNT];
     fzb_stats pass{};
     rc = run_batch_pass(h, [&]() -> int {
-        hp.out = h->d_out;  // (the output buffer may have grown since the last attempt)
-        hp.cap = h->out_cap;
+        hp.out = h->d_out.get();  // (the output buffer may have grown since the last attempt)
+        hp.cap = h->d_out.size();
         if (ntiles > 0) {
             const int grid = (int)std::min<int64_t>(ntiles, (int64_t)h->sm_count * per_sm);
             if (two_bit)
@@ -2779,7 +2787,7 @@ extern "C" int fzb_find_near_matches(const uint8_t *pattern, uint32_t m, const u
         return fail(FZB_E_CUDA, "CUDA device %d not available (%d devices)", device, fzb_device_count());
     std::lock_guard<std::mutex> lock(g_ws_mutex);
     fzb_haystack *&h = g_ws[device];
-    if (!h || round_up(n, 128) + 128 > h->capacity) {
+    if (!h || round_up(n, 128) + 128 > h->owned_buf.size()) {
         if (h) fzb_haystack_destroy(h);
         h = nullptr;
         const uint64_t cap = std::max<uint64_t>(n + n / 8, 1u << 20);  // head-room: repeated calls with growing inputs
@@ -2835,8 +2843,8 @@ extern "C" int fzb_has_near_match(fzb_haystack *h, const uint8_t *pattern, uint3
 extern "C" int fzb_debug_counters(const fzb_haystack *h, uint32_t out[32]) {
     if (!h || !out) return fail(FZB_E_INVALID, "NULL argument");
     memset(out, 0, 32 * sizeof(uint32_t));
-    memcpy(out, h->h_counters, CNT_COUNT * sizeof(uint32_t));
-    if (h->h_ghdr) memcpy(out + 16, h->h_ghdr, 16 * sizeof(uint32_t));
+    memcpy(out, h->h_counters.get(), CNT_COUNT * sizeof(uint32_t));
+    if (h->peer) memcpy(out + 16, h->peer->h_ghdr.get(), 16 * sizeof(uint32_t));
     return FZB_OK;
 }
 
@@ -2857,37 +2865,27 @@ extern "C" int fzb_debug_expand(const uint8_t *subs, const uint32_t *sub_off, co
         if (variant[i] < 0 || variant[i] > 2 || max_l[i] < 0) return fail(FZB_E_INVALID, "bad variant / budget");
     }
     CK(cudaSetDevice(device));
-    uint8_t *d_subs = nullptr, *d_seqs = nullptr;
-    uint32_t *d_so = nullptr, *d_qo = nullptr;
-    int32_t *d_k = nullptr, *d_v = nullptr, *d_out = nullptr;
     const size_t nsub = std::max<size_t>(sub_off[count], 1), nseq = std::max<size_t>(seq_off[count], 1);
-    int rc = [&]() -> int {
-        CK(cudaMalloc(&d_subs, nsub));
-        CK(cudaMalloc(&d_seqs, nseq));
-        CK(cudaMalloc(&d_so, (count + 1) * sizeof(uint32_t)));
-        CK(cudaMalloc(&d_qo, (count + 1) * sizeof(uint32_t)));
-        CK(cudaMalloc(&d_k, count * sizeof(int32_t)));
-        CK(cudaMalloc(&d_v, count * sizeof(int32_t)));
-        CK(cudaMalloc(&d_out, (size_t)count * 8 * sizeof(int32_t)));
-        CK(cudaMemcpy(d_subs, subs, sub_off[count], cudaMemcpyHostToDevice));
-        CK(cudaMemcpy(d_seqs, seqs, seq_off[count], cudaMemcpyHostToDevice));
-        CK(cudaMemcpy(d_so, sub_off, (count + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice));
-        CK(cudaMemcpy(d_qo, seq_off, (count + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice));
-        CK(cudaMemcpy(d_k, max_l, count * sizeof(int32_t), cudaMemcpyHostToDevice));
-        CK(cudaMemcpy(d_v, variant, count * sizeof(int32_t), cudaMemcpyHostToDevice));
-        k_debug_expand<<<count, 32>>>(d_subs, d_so, d_seqs, d_qo, d_k, d_v, d_out);
-        CK(cudaGetLastError());
-        CK(cudaMemcpy(out, d_out, (size_t)count * 8 * sizeof(int32_t), cudaMemcpyDeviceToHost));
-        return FZB_OK;
-    }();
-    cudaFree(d_subs);
-    cudaFree(d_seqs);
-    cudaFree(d_so);
-    cudaFree(d_qo);
-    cudaFree(d_k);
-    cudaFree(d_v);
-    cudaFree(d_out);
-    return rc;
+    DevBuf<uint8_t> d_subs, d_seqs;
+    DevBuf<uint32_t> d_so, d_qo;
+    DevBuf<int32_t> d_k, d_v, d_out;
+    TRY(d_subs.alloc(nsub));
+    TRY(d_seqs.alloc(nseq));
+    TRY(d_so.alloc(count + 1));
+    TRY(d_qo.alloc(count + 1));
+    TRY(d_k.alloc(count));
+    TRY(d_v.alloc(count));
+    TRY(d_out.alloc((uint64_t)count * 8));
+    CK(cudaMemcpy(d_subs.get(), subs, sub_off[count], cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_seqs.get(), seqs, seq_off[count], cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_so.get(), sub_off, (count + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_qo.get(), seq_off, (count + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_k.get(), max_l, count * sizeof(int32_t), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d_v.get(), variant, count * sizeof(int32_t), cudaMemcpyHostToDevice));
+    k_debug_expand<<<count, 32>>>(d_subs.get(), d_so.get(), d_seqs.get(), d_qo.get(), d_k.get(), d_v.get(), d_out.get());
+    CK(cudaGetLastError());
+    CK(cudaMemcpy(out, d_out.get(), (size_t)count * 8 * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return FZB_OK;
 }
 
 // ------------------------------------------------------------------------------------------------

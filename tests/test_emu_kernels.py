@@ -267,6 +267,135 @@ def test_emu_allocation_failures_surface_cleanly(emu_device, monkeypatch):
     assert "FZB_EMU_FAIL_ALLOC" in os.environ
 
 
+def _alloc_failure_scenarios():
+    """name -> (open() -> state, call(state) -> comparable answer).  Each call reaches allocations a handle makes
+    after it was created: lazily allocated buffer groups and grow paths."""
+    import numpy as np
+
+    from corpus import ASCII, DNA, make_corpus
+    from fuzzysearch_b200.sharding import init_local_world, search_all, shard_bounds
+    F = _native
+    rng = np.random.default_rng(7)
+    dna = bytes(rng.choice(np.frombuffer(DNA, np.uint8), size=1 << 17))
+    _, text, _ = make_corpus(8, 1 << 13, ASCII, 20, 8, 3)
+    text = text.tobytes()
+    lp_pat, lp_hay, _ = make_corpus(2, 300, DNA, 16, 4, 8)  # > 256 live candidates at some start (test_gpu_lp_generic_edges)
+
+    def routes(results):
+        return [(r.stats()["route"], r.triples(F.FINAL)) for r in results[0]]
+
+    def lev_batch(hs):  # two q-sample patterns, two for the dense pass, two for the LP pass
+        pats = [text[100:130], text[300:330], text[500:511], text[700:710], text[900:908], text[1100:1109]]
+        return routes(hs.search_levenshtein_batch(pats, [1, 2, 1, 1, 3, 3]))
+
+    def ham_batch(hay, m, k):
+        return lambda hs: routes(hs.search_hamming_batch([hay[p:p + m] for p in range(64, 64 + 6 * 97, 97)], [k] * 6))
+
+    def world_open():
+        shards = []
+        for r in range(2):
+            blo, bhi, lo, hi = shard_bounds(len(text), 2, r, 64)
+            shards.append(F.Haystack.from_host(text[blo:bhi], buf_lo=blo, global_len=len(text), own_lo=lo, own_hi=hi))
+        return shards
+
+    def world_call(shards):
+        init_local_world(shards)
+        return search_all(shards, lambda h: h.search_levenshtein(text[2000:2020], 2, F.F_GLOBAL).triples(F.FINAL))
+
+    def symbols(hs):
+        hs.upload_symbols(np.arange(3000, dtype=np.uint32) % 97 + 70000, [70001, 70005, 70020])
+        return hs.read(0, len(hs))
+
+    def synthetic(hs):
+        hs.fill_synthetic(b"ACGT", 11)
+        return hs.read(0, len(hs))
+
+    one = lambda hay: lambda: F.Haystack.from_host(hay)  # noqa: E731
+    return {
+        "output growth": (one(dna), lambda hs: (hs.search_levenshtein(b"ACGTAC", 3).count(F.RAW),
+                                                 hs.search_levenshtein(b"ACGTAC", 3).triples(F.FINAL))),
+        "lp scratch growth": (one(lp_hay), lambda hs: hs.search_levenshtein(lp_pat, 7, F.F_FORCE_LP).triples(F.FINAL)),
+        "levenshtein batch": (one(text), lev_batch),
+        "hamming batch text": (one(text), ham_batch(text, 20, 2)),
+        "hamming batch dna": (one(dna[:1 << 14]), ham_batch(dna, 32, 3)),
+        "has_near_match": (one(text), lambda hs: [hs.has_near_match(text[40:60], 0, 0, 2, 2),
+                                                  hs.has_near_match(b"qqqqqqqqqqqqqq", 1, 1, 1, 2)]),
+        "local world": (world_open, world_call),
+        "upload_symbols": (lambda: F.Haystack.alloc(4096), symbols),
+        "fill_synthetic": (lambda: F.Haystack.alloc(1000), synthetic),
+    }
+
+
+def _replay_allocation_failures(name, upto):
+    """Child-process side of test_emu_allocation_failures_leave_the_handle_usable: for nth = 1 .. upto - 1, make the
+    scenario's call on a handle that outlives the failure with the nth allocation failing, repeat it on that handle
+    without the failure, close it and count what is still allocated.  Prints one line per nth."""
+    import os
+
+    F = _native
+    F._lib = conftest.load_emulated_library()
+    live = F._lib.fzb_emu_live_allocations
+    live.restype = ctypes.c_long
+    open_, call = _alloc_failure_scenarios()[name]
+
+    def close(state):
+        for h in state if isinstance(state, list) else [state]:
+            h.close()
+
+    state = open_()
+    good = call(state)
+    close(state)
+    gc.collect()
+    baseline = live()
+    for nth in range(1, upto):
+        state = open_()
+        os.environ["FZB_EMU_FAIL_ALLOC"] = str(nth)
+        try:
+            failed, got = False, call(state)
+        except F.CudaError:
+            failed, got = True, None
+        finally:
+            os.environ["FZB_EMU_FAIL_ALLOC"] = ""
+        assert failed or got == good, (name, nth, "wrong answer")
+        assert call(state) == good, (name, nth, "wrong answer on the handle that saw the failure")
+        close(state)
+        gc.collect()
+        assert live() == baseline, (name, nth, "leak")
+        print("%s nth=%d %s" % (name, nth, "raised" if failed else "ok"), flush=True)
+
+
+@pytest.mark.parametrize("name,upto,failing", [
+    ("output growth", 5, 3),        # LP list, candidate lists, the output buffer grown past 65 536 records
+    ("lp scratch growth", 5, 3),    # LP list, candidate lists at 256, grown to 2 048 entries
+    ("levenshtein batch", 15, 13),  # batch tables (7), dense hit list, LP batch buffers (4), candidate lists
+    ("hamming batch text", 9, 7),   # batch tables
+    ("hamming batch dna", 9, 7),
+    ("has_near_match", 3, 1),
+    ("local world", 14, 12),        # the peer-memory buffers of both handles
+    ("upload_symbols", 4, 2),       # alphabet, chunk buffer
+    ("fill_synthetic", 3, 1),       # alphabet
+])
+def test_emu_allocation_failures_leave_the_handle_usable(emu_lib, name, upto, failing):
+    """A failed allocation in a call on a live handle (FZB_EMU_FAIL_ALLOC=N, for every N the call reaches) comes back
+    as CudaError, and the same call on the same handle then returns the right answer: no buffer group is left half
+    built and no grown buffer is lost.  Each scenario replays in a child process, so a handle left pointing at
+    missing memory fails this test by name instead of killing the session.  `failing`: allocations the call makes;
+    the last N makes none fail."""
+    import os
+    import subprocess
+    import sys
+    code = "import sys; sys.path[:0] = %r; import test_emu_kernels as t; t._replay_allocation_failures(%r, %d)" % (
+        [conftest.ROOT, os.path.join(conftest.ROOT, "tests")], name, upto)
+    env = dict(os.environ, FZB_EMU_SMS="2", FZB_EMU_FAIL_ALLOC="")
+    p = subprocess.run([sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code], env=env,
+                       capture_output=True, text=True, timeout=1800)
+    lines = p.stdout.split("\n")
+    assert p.returncode == 0, (name, "exit %d" % p.returncode, lines[-6:], p.stderr[-3000:])
+    raised = [ln for ln in lines if ln.endswith(" raised")]
+    assert len(raised) == failing, (name, lines)
+    assert lines[-2].endswith("nth=%d ok" % (upto - 1)), (name, lines)  # the scenario's last allocation was reached
+
+
 def test_emulator_racecheck_sees_a_missing_barrier():
     """tests/emu/selftest: under the emulator's ThreadSanitizer mode a kernel without its __syncthreads() and one
     whose threads all store to one global word are reported; the correct twins (__syncthreads, __syncwarp within a
