@@ -57,8 +57,8 @@ def find_near_matches_batch(subsequences, sequence, max_l_dist=None, *, max_subs
     Each limit is None, one int, or one value per pattern.  Equivalent to
     ``[find_near_matches(p, sequence, max_substitutions=s, max_insertions=i, max_deletions=d, max_l_dist=l)
     for p, s, i, d, l in zip(subsequences, ...)]``: exact and Levenshtein searches share passes over the
-    sequence (fzb_search_levenshtein_batch), substitutions-only searches too (fzb_search_hamming_batch), and
-    searches with other limits run one by one on the same uploaded sequence."""
+    sequence (fzb_search_levenshtein_batch), substitutions-only searches too (fzb_search_hamming_batch), and so do
+    searches with other (generic) limits (fzb_search_generic_batch); all of them use the same uploaded sequence."""
     from . import _native
     subsequences = list(subsequences)
     n = len(subsequences)
@@ -107,9 +107,13 @@ def find_near_matches_batch(subsequences, sequence, max_l_dist=None, *, max_subs
             rs, _ = hay.search_hamming_batch([pats[i] for i in ham], ks)
             for i, r in zip(ham, rs):
                 results[i] = r
-        for i in range(n):
-            if classes[i] is GenericSearch:
-                results[i] = hay.search_generic(pats[i], *params[i].unpacked)
+        gen = [i for i in range(n) if classes[i] is GenericSearch]
+        if len(gen) == 1:  # (nothing to share)
+            results[gen[0]] = hay.search_generic(pats[gen[0]], *params[gen[0]].unpacked)
+        elif gen:  # the normalised limits GenericSearch.search applies
+            rs, _ = hay.search_generic_batch([pats[i] for i in gen], *zip(*[params[i].unpacked for i in gen]))
+            for i, r in zip(gen, rs):
+                results[i] = r
         out = []
         for res, cls in zip(results, classes):
             # ExactSearch does not consolidate (search_exact.py:80-89): its list is the RAW stream of the k == 0

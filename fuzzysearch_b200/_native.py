@@ -22,7 +22,8 @@ RAW, FINAL = 0, 1
 F_NO_FINAL, F_FORCE_DENSE, F_FORCE_LP, F_FORCE_NGRAMS, F_TINY_LIST, F_GLOBAL, F_FORCE_SAMPLED = 1, 2, 4, 8, 16, 32, 64
 
 ROUTE_NAMES = {7: "batch", 0: "exact", 1: "ngrams/sampled-filter", 2: "ngrams/dense-filter", 3: "lp",
-               4: "hamming", 5: "generic-ngrams", 6: "generic-lp", 8: "hamming/batch-scan"}
+               4: "hamming", 5: "generic-ngrams", 6: "generic-lp", 8: "hamming/batch-scan",
+               9: "generic-ngrams/batch-scan", 10: "generic-lp/batch-scan"}
 
 
 class NativeLibraryMissing(ImportError):
@@ -82,6 +83,7 @@ SYMBOLS = {
     "fzb_search_exact_window": (_i32, [_vp, _u8p, _u32, _u64, _u64, _u32, _vpp]),
     "fzb_search_levenshtein_batch": (_i32, [_vp, _u8p, _vp, _vp, _u32, _u32, _vpp, ctypes.POINTER(Stats)]),
     "fzb_search_hamming_batch": (_i32, [_vp, _u8p, _vp, _vp, _u32, _u32, _vpp, ctypes.POINTER(Stats)]),
+    "fzb_search_generic_batch": (_i32, [_vp, _u8p, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _vpp, ctypes.POINTER(Stats)]),
     "fzb_find_near_matches": (_i32, [_u8p, _u32, _u8p, _u64, _u32, _u32, _u32, _u32, _i32, _vpp]),
     "fzb_has_near_match": (_i32, [_vp, _u8p, _u32, _u32, _u32, _u32, _u32, ctypes.POINTER(ctypes.c_int)]),
     "fzb_release_workspace": (None, []),
@@ -348,22 +350,29 @@ class Haystack(object):
 
     def search_levenshtein_batch(self, patterns, ks, flags=0):
         """-> (list of Result, one per pattern; summed stats dict)."""
-        return self._batch(lib().fzb_search_levenshtein_batch, patterns, ks, flags)
+        return self._batch(lib().fzb_search_levenshtein_batch, patterns, [ks], flags)
 
     def search_hamming_batch(self, patterns, ks, flags=0):
         """Substitutions-only searches, ks[i] = max substitutions of patterns[i] -> (list of Result, one per
         pattern; summed stats dict)."""
-        return self._batch(lib().fzb_search_hamming_batch, patterns, ks, flags)
+        return self._batch(lib().fzb_search_hamming_batch, patterns, [ks], flags)
 
-    def _batch(self, fn, patterns, ks, flags):
+    def search_generic_batch(self, patterns, max_subs, max_ins, max_dels, max_l, flags=0):
+        """Generic searches, one normalised limit of each kind per pattern (as search_generic takes them) -> (list of
+        Result, one per pattern; summed stats dict)."""
+        return self._batch(lib().fzb_search_generic_batch, patterns, [max_subs, max_ins, max_dels, max_l], flags)
+
+    def _batch(self, fn, patterns, limits, flags):
+        """limits: the C-ABI's per-pattern limit arrays, in its order (one value per pattern each)."""
         pats = [as_u8(p) for p in patterns]
         blob = np.concatenate(pats) if pats else np.zeros(0, np.uint8)
         offsets = np.zeros(len(pats) + 1, dtype=np.uint32)
         offsets[1:] = np.cumsum([p.size for p in pats])
-        ks = np.ascontiguousarray(ks, dtype=np.uint32)
+        limits = [np.ascontiguousarray(ks, dtype=np.uint32) for ks in limits]
         out = (ctypes.c_void_p * max(len(pats), 1))()
         st = Stats()
-        check(fn(self._h, ptr(blob), ptr(offsets), ptr(ks), len(pats), flags, out, ctypes.byref(st)))
+        check(fn(self._h, ptr(blob), ptr(offsets), *[ptr(ks) for ks in limits], len(pats), flags, out,
+                 ctypes.byref(st)))
         results = [Result(ctypes.c_void_p(out[i])) for i in range(len(pats))]
         return results, {"gpu_ms": st.gpu_ms, "filter_ms": st.filter_ms, "bytes_scanned": st.bytes_scanned,
                          "n_candidates": st.n_candidates, "n_launches": st.n_launches, "route": "batch"}

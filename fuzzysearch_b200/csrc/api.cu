@@ -28,6 +28,7 @@
 #include "p2p_kernels.cuh"
 #include "batch_kernels.cuh"
 #include "ham_batch_kernels.cuh"
+#include "generic_batch_kernels.cuh"
 #include "sym_kernels.cuh"
 #include <unordered_map>
 #include "debug_kernels.cuh"
@@ -129,6 +130,9 @@ struct LpBatchBufs {  // the LP batch pass
     DevBuf<unsigned long long> d_lmlist;  // survivor list (after the sort: grouped by pattern)
     DevBuf<unsigned long long> d_lmkept;  // the survivors of the exact per-pattern window test
     DevBuf<uint32_t> d_lmhist;            // per-pattern counts [64] + kept total [1] | cursors [64]
+};
+struct GenericBatchBufs {  // the generic batch passes (generic_batch_kernels.cuh)
+    DevBuf<uint32_t> d_glim;  // per pattern of a pass: max_subs | max_ins << 8 | max_dels << 16
 };
 struct PeerBufs {  // the peer-memory reduction (p2p_kernels.cuh)
     DevBuf<uint8_t> d_p2p;  // my receive area: [2 parities][world] slots + flags
@@ -270,6 +274,7 @@ struct fzb_haystack {
     std::unique_ptr<BatchBufs> batch;
     DevBuf<unsigned long long> d_mhits;  // dense batch pass: (pattern, n-gram, position) hits
     std::unique_ptr<LpBatchBufs> lpb;
+    std::unique_ptr<GenericBatchBufs> gbatch;
 };
 
 struct fzb_result {
@@ -1712,6 +1717,11 @@ static int search_lev_lp(fzb_haystack *h, const uint8_t *pattern, uint32_t m, ui
     return FZB_OK;
 }
 
+// The total limit the LP route of the generic search works with (see search_generic).
+static uint32_t lp_generic_limit(uint32_t m, uint32_t max_ins, uint32_t max_l) {
+    return (uint32_t)std::min<uint64_t>(max_l, (uint64_t)m + std::min(max_ins, max_l));
+}
+
 static int search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t max_subs, uint32_t max_ins,
                           uint32_t max_dels, uint32_t max_l, bool ngrams, uint32_t flags, fzb_result *res,
                           int post_mode) {
@@ -1722,7 +1732,7 @@ static int search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, u
     // final loop (:172-177) -- and can be lowered to it without changing the raw stream.  (Not so on the n-gram
     // route, where max_l_dist also sets the n-gram length and the windows.)  E.g. max_substitutions=100,
     // max_insertions=1, max_deletions=1 on 20 symbols: 102 -> 21.
-    if (!ngrams) max_l = (uint32_t)std::min<uint64_t>(max_l, (uint64_t)m + std::min(max_ins, max_l));
+    if (!ngrams) max_l = lp_generic_limit(m, max_ins, max_l);
     // the packed candidate of sim_generic keeps 6 bits per counter
     if (max_l > 63) return fail(FZB_E_UNSUPPORTED, "max_l_dist > 63 is not supported by the generic search");
     // no counter can exceed max_l (every operation that increments one costs >= 1), so clamping the
@@ -2049,13 +2059,30 @@ static MultiParams pass_params(const fzb_haystack *h) {
     return mp;
 }
 
+// Entries of each of a lane's two candidate lists in the verify kernels of a generic pass: a start with more live
+// candidates sends the pass's patterns one by one, where the single search grows its lists
+constexpr int kGenericBatchCap = 256;
+
+// A generic pass: uploads the limits glim[id] of the patterns ids[] (max_subs | max_ins << 8 | max_dels << 16) and
+// sizes the candidate lists of `grid` CTAs of the verify kernel.
+static int prepare_generic_pass(fzb_haystack *h, const uint32_t *glim, const std::vector<uint32_t> &ids, int grid) {
+    TRY(ensure_group(h->gbatch, [](GenericBatchBufs &g) -> int { return g.d_glim.alloc(kMaxBatchPats); }));
+    std::vector<uint32_t> lim(ids.size());
+    for (size_t i = 0; i < ids.size(); i++) lim[i] = glim[ids[i]];
+    CK(cudaMemcpyAsync(h->gbatch->d_glim.get(), lim.data(), lim.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    return ensure_scratch(h, (uint64_t)grid * kLpThreads * 2 * kGenericBatchCap);
+}
+
 // One pass over the haystack for the patterns ids[0..cnt): fills out[ids[i]].  Returns FZB_OK, an error, or +1 if
 // the pass overflowed a device structure (the caller then searches these patterns one by one).
 // dense = false: the q-sample scan (k_filter_multi / k_verify_multi) over the 4-grams of the patterns;
 // dense = true: the n-gram-prefix scan at every position (k_filter_mdense / k_verify_mhits).
 // tiny: the capacities of FZB_F_TINY_LIST.
+// glim: nullptr for Levenshtein patterns (ks = max_l_dist); for generic patterns (ks = max_l_dist) their limits as
+// prepare_generic_pass takes them, and the generic verify kernels (k_verify_multi_generic / k_verify_mhits_generic).
 static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, const uint32_t *ks,
-                      const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, bool dense, bool tiny) {
+                      const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, bool dense, bool tiny,
+                      const uint32_t *glim = nullptr) {
     const uint32_t cnt = (uint32_t)ids.size();
     std::vector<BatchPat> pats(cnt);
     std::vector<uint32_t> pinfo(cnt);
@@ -2070,7 +2097,12 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
         bp.k = (int)k;
         bp.L = (int)(m / (k + 1));
         bp.n_ngrams = (int)m / bp.L;
-        pinfo[i] = m | (k << 8) | ((uint32_t)bp.L << 16);
+        // The k of pinfo only sets the anchors k_filter_multi marks around a word hit, [g-o-k, g-o+k+m-L].  A generic
+        // pattern needs 2k there: its verification runs the NFA from every start of the window [p0-k, p0+m+k) of an
+        // n-gram hit, whose end is also the NFA's end of input, so a match that aligns the word with offset o can
+        // start anywhere in [g-o-ins, g-o+dels] and its hit p0 anywhere in [g-o-k-dels, g-o+k+dels] (ins + dels <= k).
+        const uint32_t mark_k = glim ? 2 * k : k;  // (n-gram route, m <= 64: k <= 20)
+        pinfo[i] = m | (mark_k << 8) | ((uint32_t)bp.L << 16);
         if (dense) {  // key: the first 3 bytes of n-gram j; posting: pattern << 8 | j
             for (int j = 0; j < bp.n_ngrams; j++) {
                 uint32_t w = 0;
@@ -2101,6 +2133,8 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
         CK(cudaFuncSetAttribute(k_filter_mdense, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMdenseSmem));
         h->d_mhits = std::move(hits);
     }
+    const int ggrid = h->sm_count * 4;  // generic verify kernels: as many lanes (and candidate lists) as run_lp's
+    if (glim) TRY(prepare_generic_pass(h, glim, ids, ggrid));
     BatchBufs &b = *h->batch;
     MultiParams mp = pass_params(h);
     mp.bits2 = dense ? nullptr : b.d_mbits.get() + kMultiTblWords;
@@ -2124,7 +2158,15 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
                 k_filter_multi<<<grid, kMultiThreads, kMultiSmem, h->stream>>>(mp, nvec, ntiles);
         }
         CK(cudaEventRecord(h->ev[1], h->stream));
-        if (dense)
+        if (glim && dense)
+            k_verify_mhits_generic<<<ggrid, kLpThreads, 0, h->stream>>>(dp, h->gbatch->d_glim.get(), h->d_scratch.get(),
+                                                                       kGenericBatchCap, h->d_out.get(), h->d_out.size(),
+                                                                       h->d_counters.get());
+        else if (glim)
+            k_verify_multi_generic<<<ggrid, kLpThreads, 0, h->stream>>>(mp, b.d_bpats.get(), h->gbatch->d_glim.get(),
+                                                                       h->d_scratch.get(), kGenericBatchCap, h->d_out.get(),
+                                                                       h->d_out.size(), h->d_counters.get());
+        else if (dense)
             k_verify_mhits<<<h->sm_count * 8, kMhThreads, 0, h->stream>>>(dp, h->d_out.get(), h->d_out.size(), h->d_counters.get());
         else
             k_verify_multi<<<h->sm_count * 8, kVmThreads, 0, h->stream>>>(mp, b.d_bpats.get(), h->d_out.get(), h->d_out.size(),
@@ -2139,17 +2181,21 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
     if (rc) return rc;
     float filter_ms = 0.f;
     cudaEventElapsedTime(&filter_ms, h->ev[0], h->ev[1]);
-    pass.route = dense ? 2 : 1;
+    pass.route = glim ? 9 : dense ? 2 : 1;
     pass.filter_ms = filter_ms;
     pass.n_candidates = cnts[CNT_CAND];
     pass.n_launches = 2;
-    return split_batch(raw, ids, pass, 0, false, out, sum);
+    // (the generic n-gram route's raw order: n-gram, hit index, then the window's matches in canonical order)
+    return split_batch(raw, ids, pass, glim ? 2 : 0, false, out, sum);
 }
 
 // One shared scan for up to 64 LP-route patterns (k_lp_scan_multi / k_lp_verify_multi).  Same return convention
-// as batch_pass.
+// as batch_pass.  glim: as for batch_pass (ks = the lowered max_l_dist of the LP route, search_generic); a generic
+// NFA opens a candidate at every start (generic_search.py:81), so the scan applies the counting condition only, and
+// k_lp_verify_multi_generic verifies.
 static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, const uint32_t *ks,
-                         const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, bool tiny) {
+                         const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, bool tiny,
+                         const uint32_t *glim = nullptr) {
     const uint32_t cnt = (uint32_t)ids.size();
     std::vector<BatchPat> pats(cnt);
     std::vector<ulonglong2> lut(256, make_ulonglong2(0ull, 0ull));
@@ -2170,7 +2216,10 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
             lut[bp.P[j]].x |= 1ull << i;
             pm32[(size_t)i * 256 + bp.P[j]] |= 1u << j;
         }
-        for (uint32_t j = 0; j <= std::min(k, m - 1); j++) lut[bp.P[j]].y |= 1ull << i;
+        if (glim)
+            for (int c = 0; c < 256; c++) lut[c].y |= 1ull << i;
+        else
+            for (uint32_t j = 0; j <= std::min(k, m - 1); j++) lut[bp.P[j]].y |= 1ull << i;
         const uint32_t bias = 32 - (m - k);  // need = m - k in [1, 31]
         for (int b = 0; b < 6; b++)
             if ((bias >> b) & 1u) lp.bias[b] |= 1ull << i;
@@ -2207,7 +2256,10 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lp_scan_multi, kLmThreads, kLmSmem));
     per_sm = std::max(per_sm, 1);
     const int vgrid = h->sm_count * 4, sim_cap = 256;
-    TRY(ensure_scratch(h, (uint64_t)vgrid * kLpThreads * 2 * sim_cap));
+    if (glim)
+        TRY(prepare_generic_pass(h, glim, ids, vgrid));
+    else
+        TRY(ensure_scratch(h, (uint64_t)vgrid * kLpThreads * 2 * sim_cap));
     const uint64_t chunk = tiny ? kTinyLpChunk : 256ull << 20;  // starts per scan: bounds the survivor list
     std::vector<RawRec> raw;
     uint32_t cnts[CNT_COUNT];
@@ -2230,7 +2282,12 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
             k_lm_refine<<<h->sm_count * 8, kLmSortThreads, 0, h->stream>>>(lp, lb.d_lmkept.get(), lb.d_lmhist.get());
             k_lm_scatter<<<h->sm_count * 8, kLmSortThreads, 0, h->stream>>>(lb.d_lmkept.get(), lb.d_lmhist.get(),
                                                                               lb.d_lmhist.get() + 128, lb.d_lmlist.get());
-            if (kmax <= 4)
+            if (glim)
+                k_lp_verify_multi_generic<<<vgrid, kLpThreads, 0, h->stream>>>(lp, h->gbatch->d_glim.get(), lb.d_lmlist.get(),
+                                                                               lb.d_lmhist.get(), h->d_scratch.get(),
+                                                                               kGenericBatchCap, h->d_out.get(),
+                                                                               h->d_out.size(), h->d_counters.get());
+            else if (kmax <= 4)
                 k_lp_verify_multi<4><<<vgrid, kLpThreads, 0, h->stream>>>(lp, lb.d_lmlist.get(), lb.d_lmhist.get(), h->d_scratch.get(),
                                                                           sim_cap, h->d_out.get(), h->d_out.size(), h->d_counters.get());
             else
@@ -2249,7 +2306,7 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
         return FZB_OK;
     }, raw, cnts, pass);
     if (rc) return rc;
-    pass.route = 3;
+    pass.route = glim ? 10 : 3;
     pass.filter_ms = scan_ms;
     pass.n_candidates = n_work;
     return split_batch(raw, ids, pass, 1, false, out, sum);
@@ -2752,6 +2809,127 @@ extern "C" int fzb_search_generic(fzb_haystack *h, const uint8_t *pattern, uint3
         if (flags & FZB_F_FORCE_LP) ngrams = false;
         return search_generic(h, pattern, m, max_subs, max_ins, max_dels, max_l, ngrams, flags, res, post_mode);
     });
+}
+
+extern "C" int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
+                                        const uint32_t *max_subs, const uint32_t *max_ins, const uint32_t *max_dels,
+                                        const uint32_t *max_l_dist, uint32_t count, uint32_t flags, fzb_result **out,
+                                        fzb_stats *total) {
+    HandleLock handle_lock(h);
+    if (!h || !out || (count && (!patterns || !offsets || !max_subs || !max_ins || !max_dels || !max_l_dist)))
+        return fail(FZB_E_INVALID, "NULL argument");
+    for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
+    for (uint32_t i = 0; i < count; i++)
+        if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
+    // Per pattern, as fzb_search_generic would search it: the route, the total limit it works with (the LP route
+    // lowers it, search_generic) and the per-operation limits clamped to that total.  A pattern the single search
+    // refuses (check_pattern, max_l_dist > 63, the halo, an n-gram length of 0) fails the whole call, with the single
+    // search's error, before any work.
+    std::vector<uint32_t> kl(count, 0), glim(count, 0);
+    std::vector<uint8_t> ngram_route(count, 0);
+    for (uint32_t i = 0; i < count; i++) {
+        const uint32_t m = offsets[i + 1] - offsets[i], l = max_l_dist[i];
+        int rc = check_pattern(h, patterns + offsets[i], m, flags);
+        if (rc) return rc;
+        bool ngrams = m / ((uint64_t)l + 1) >= 3;
+        if (flags & FZB_F_FORCE_NGRAMS) ngrams = true;
+        if (flags & FZB_F_FORCE_LP) ngrams = false;
+        if (l == 0 && !(flags & (FZB_F_FORCE_LP | FZB_F_FORCE_NGRAMS))) {
+            rc = check_halo(h, m);  // (the exact route)
+        } else {
+            const uint32_t lk = ngrams ? l : lp_generic_limit(m, max_ins[i], l);
+            if (lk > 63) return fail(FZB_E_UNSUPPORTED, "max_l_dist > 63 is not supported by the generic search");
+            rc = check_halo(h, (uint64_t)m + lk);
+            if (rc == FZB_OK && ngrams && m / (lk + 1) == 0)  // (only under FZB_F_FORCE_NGRAMS)
+                rc = fail(FZB_E_NGRAM_ZERO, "the subsequence length must be greater than max_l_dist");
+            kl[i] = lk;
+            glim[i] = std::min(max_subs[i], lk) | std::min(max_ins[i], lk) << 8 | std::min(max_dels[i], lk) << 16;
+        }
+        if (rc) return rc;
+        ngram_route[i] = ngrams;
+    }
+    fzb_stats sum{};
+    auto settle = [&](int rc, const std::vector<uint32_t> &ids) { return settle_pass(rc, ids, out, count); };
+    // the shared scans take no flags other than FZB_F_TINY_LIST (forced routes, raw-only, multi-GPU reduction: one by
+    // one), no exact-route pattern (max_l_dist == 0) and no pattern longer than a BatchPat holds
+    const bool tiny = (flags & FZB_F_TINY_LIST) != 0;
+    const bool share = (flags & ~FZB_F_TINY_LIST) == 0 && h->buf_len > 0;
+    auto shareable = [&](uint32_t i) {
+        const uint32_t m = offsets[i + 1] - offsets[i];
+        return share && !out[i] && max_l_dist[i] > 0 && m <= (uint32_t)kBatchMaxM;
+    };
+    // n-gram route, q-sample lemma holds and its 4-grams are selective on this haystack: q-sample passes, bounded as
+    // in the Levenshtein batch (gram table / posting capacity)
+    std::vector<uint32_t> shared;
+    for (uint32_t i = 0; i < count; i++) {
+        if (!shareable(i) || !ngram_route[i]) continue;
+        const uint32_t m = offsets[i + 1] - offsets[i], k = kl[i], L = m / (k + 1);
+        if (!sampled_filter_applies(m, k, 0) || !sampled_is_selective(h, m, k, (int)L, (int)(m / L))) continue;
+        shared.push_back(i);
+    }
+    size_t done = 0;
+    while (done < shared.size()) {
+        std::vector<uint32_t> ids;
+        uint64_t ngr = 0;
+        while (done < shared.size() && ids.size() < kMaxBatchPats) {
+            const uint32_t m = offsets[shared[done] + 1] - offsets[shared[done]];
+            if (ngr + (m - 3) > kMaxBatchGrams) break;
+            ngr += m - 3;
+            ids.push_back(shared[done++]);
+        }
+        if (ids.size() < 2) break;  // (a pass of one pattern is not worth it)
+        const int rc = settle(batch_pass(h, patterns, offsets, kl.data(), ids, out, &sum, false, tiny, glim.data()), ids);
+        if (rc) return rc;
+    }
+    // the other n-gram-route patterns: one n-gram-prefix pass, under the Levenshtein batch's bound on the expected
+    // prefix hits per position and the prefix table's capacity; a hit's window must fit a warp's slot in
+    // k_verify_mhits_generic
+    std::vector<uint32_t> dense_ids;
+    if (share && sample_collision_prob(h) == FZB_OK) {
+        double expect = 0.0;
+        uint32_t dense_grams = 0;
+        const double c3 = h->coll_prob * h->coll_prob * h->coll_prob;
+        for (uint32_t i = 0; i < count && dense_ids.size() < kMaxBatchPats; i++) {
+            if (!shareable(i) || !ngram_route[i]) continue;
+            const uint32_t m = offsets[i + 1] - offsets[i], k = kl[i], L = m / (k + 1);
+            if (m + 2 * k + 8 > (uint32_t)kMhgSlotBytes) continue;
+            if (expect + (m / L) * c3 > 0.02) continue;  // (low-entropy text: prefixes hit everywhere -> one by one)
+            if (dense_grams + m / L > kMaxBatchGrams) continue;
+            expect += (m / L) * c3;
+            dense_grams += m / L;
+            dense_ids.push_back(i);
+        }
+    }
+    if (dense_ids.size() >= 2) {
+        const int rc = settle(batch_pass(h, patterns, offsets, kl.data(), dense_ids, out, &sum, true, tiny, glim.data()),
+                              dense_ids);
+        if (rc) return rc;
+    }
+    // LP route (after the lowering of search_generic): passes of at most 64 patterns (6-bit window counters, 32-bit masks)
+    std::vector<uint32_t> lp_ids;
+    for (uint32_t i = 0; i < count; i++) {
+        if (!shareable(i) || ngram_route[i]) continue;
+        const uint32_t m = offsets[i + 1] - offsets[i], k = kl[i];
+        if (m > 31 || m + k > 31 || k >= m) continue;
+        lp_ids.push_back(i);
+    }
+    // (the passes are balanced, so that none is left with a single pattern: 65 patterns make passes of 33 and 32)
+    const size_t nlp = (lp_ids.size() + 63) / 64;
+    for (size_t q = 0; q < nlp && lp_ids.size() >= 2; q++) {
+        std::vector<uint32_t> ids(lp_ids.begin() + lp_ids.size() * q / nlp, lp_ids.begin() + lp_ids.size() * (q + 1) / nlp);
+        const int rc = settle(batch_pass_lp(h, patterns, offsets, kl.data(), ids, out, &sum, tiny, glim.data()), ids);
+        if (rc) return rc;
+    }
+    for (uint32_t i = 0; i < count; i++) {
+        if (out[i]) continue;
+        const int rc = settle(fzb_search_generic(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_subs[i],
+                                                 max_ins[i], max_dels[i], max_l_dist[i], flags, &out[i]), {});
+        if (rc) return rc;
+        add_stats(&sum, out[i]->stats);
+    }
+    sum.route = 7;  // batch
+    if (total) *total = sum;
+    return FZB_OK;
 }
 
 // choose_search_class (__init__.py:60-83) on normalised limits

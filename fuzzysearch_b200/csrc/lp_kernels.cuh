@@ -442,7 +442,10 @@ __device__ __forceinline__ bool g_push(uint32_t *list, int &n, int cap, uint32_t
 // Candidates born at `start`, over the sequence that ends (exclusive) at `seq_end` (both global).
 // anchor_idx / anchor_ngram tag the emitted records (n-gram hit that opened the window, or start).
 // H[g] must be the haystack byte at global position g (global memory, or the staged window).
-__device__ bool sim_generic(const ScanParams &p, const uint8_t *sP, const uint8_t *H, int64_t start,
+// PT: anything with m, k (= max_l_dist), max_subs, max_ins, max_dels (ScanParams, or the per-pattern context of the
+// batch kernels, generic_batch_kernels.cuh).
+template <class PT>
+__device__ bool sim_generic(const PT &p, const uint8_t *sP, const uint8_t *H, int64_t start,
                             int64_t seq_end, uint32_t *A, uint32_t *B, int cap, int64_t anchor_idx,
                             int anchor_ngram, RawRec *out, uint32_t ocap, uint32_t *counters) {
     const int m = p.m, max_l = p.k, max_subs = p.max_subs, max_ins = p.max_ins, max_dels = p.max_dels;
@@ -526,10 +529,12 @@ k_generic_lp(const ScanParams p, uint32_t *scratch, int cap, RawRec *out, uint32
 
 // Generic n-gram route: one warp per marked granule.  Phase 1: lane <-> anchor position, exact
 // n-gram test (generic_search.py:221-227).  Phase 2: for every hit, the lanes of the warp split
-// the starts of the clipped window (:229-237) and run the NFA.
-__device__ __forceinline__ void verify_granule_generic(const ScanParams &p, const uint8_t *sP, uint32_t *sWin,
+// the starts of the clipped window (:229-237) and run the NFA.  PT as for sim_generic, plus the geometry, L and
+// n_ngrams; `tag` is OR-ed into the records' n-gram field (pattern number << 8 in a batch).
+template <class PT>
+__device__ __forceinline__ void verify_granule_generic(const PT &p, const uint8_t *sP, uint32_t *sWin,
                                                        int64_t granule, int lane, uint32_t *A, uint32_t *B, int cap,
-                                                       RawRec *out, uint32_t ocap, uint32_t *counters) {
+                                                       RawRec *out, uint32_t ocap, uint32_t *counters, int tag = 0) {
     const int m = p.m, k = p.k, L = p.L;
     const int64_t N = p.N;
     const int64_t gbase = p.buf_lo + (granule << kGranuleShift);
@@ -567,7 +572,7 @@ __device__ __forceinline__ void verify_granule_generic(const ScanParams &p, cons
                 const int64_t wlo = max((int64_t)0, p0 - k);  // :231
                 const int64_t whi = min(N, p0 + m + k);
                 for (int64_t st = wlo + lane; st < whi; st += 32)
-                    if (!sim_generic(p, sP, W, st, whi, A, B, cap, hidx, j, out, ocap, counters))
+                    if (!sim_generic(p, sP, W, st, whi, A, B, cap, hidx, j | tag, out, ocap, counters))
                         atomicExch(&counters[CNT_OVERFLOW], 1u);
             }
         }

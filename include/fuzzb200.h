@@ -230,6 +230,21 @@ int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns, const uin
                              const uint32_t *max_subs, uint32_t count, uint32_t flags,
                              fzb_result **out, struct fzb_stats_s *total);
 
+/*
+ * Batch of generic searches over ONE resident haystack: the patterns as for fzb_search_levenshtein_batch,
+ * each with its own limits, normalised as for fzb_search_generic.  The patterns of at most 64 bytes with
+ * max_l_dist > 0 share the scans of the Levenshtein batch (DESIGN.md section 5.9): q-sample passes and one
+ * n-gram-prefix pass for the n-gram route (their results report route 9), passes of 64 patterns for the
+ * LP route (route 10); the others are searched one by one.  Each out[i] is exactly what
+ * fzb_search_generic would return for pattern i.  A pattern the single search refuses fails the whole
+ * call with its error; on error nothing is returned.  Flags other than FZB_F_TINY_LIST send every
+ * pattern one by one with those flags.
+ */
+int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
+                             const uint32_t *max_subs, const uint32_t *max_ins, const uint32_t *max_dels,
+                             const uint32_t *max_l_dist, uint32_t count, uint32_t flags, fzb_result **out,
+                             struct fzb_stats_s *total);
+
 /* ExactSearch.search (search_exact.py:80-85): all (overlapping) occurrences. FINAL == RAW. */
 int fzb_search_exact(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
                      fzb_result **out);
@@ -285,7 +300,8 @@ typedef struct fzb_stats_s {
     uint32_t n_launches;    /* kernels launched */
     uint32_t route;         /* 0 exact, 1 n-grams (sampled filter), 2 n-grams (dense filter), 3 LP,
                                4 hamming, 5 generic n-grams, 6 generic LP, 7 batch (summed statistics),
-                               8 hamming batch scan */
+                               8 hamming batch scan, 9 generic n-grams batch scan, 10 generic LP batch
+                               scan */
 } fzb_stats;
 int fzb_result_stats(const fzb_result *r, fzb_stats *out);
 void fzb_result_destroy(fzb_result *r);
