@@ -70,6 +70,7 @@ SYMBOLS = {
     "fzb_p2p_disable": (None, [_vp]),
     "fzb_haystack_upload": (_i32, [_vp, _u8p, _u64]),
     "fzb_haystack_upload_symbols": (_i32, [_vp, _vp, _u64, _u32, _vp, _u32]),
+    "fzb_haystack_set_records": (_i32, [_vp, _vp, _u64]),
     "fzb_host_alloc": (_vp, [_u64]),
     "fzb_host_free": (None, [_vp]),
     "fzb_timer_start": (_i32, [_vp]),
@@ -298,6 +299,15 @@ class Haystack(object):
         alpha = np.ascontiguousarray(alphabet, dtype=np.uint32)
         check(lib().fzb_haystack_upload_symbols(self._h, ptr(units), units.size, units.dtype.itemsize, ptr(alpha),
                                                 alpha.size))
+
+    def set_records(self, offsets):
+        """Declare a record set: record i is [offsets[i], offsets[i+1] - 1), followed by one separator position
+        (fzb_haystack_set_records).  None or an empty list removes it."""
+        off = np.ascontiguousarray([] if offsets is None else offsets, dtype=np.uint64).reshape(-1)
+        if off.size == 1:
+            raise ValueError("record offsets need at least two entries (or none, to remove the record set)")
+        count = max(off.size - 1, 0)
+        check(lib().fzb_haystack_set_records(self._h, ptr(off) if count else None, count))
 
     def debug_counters(self):
         out = np.zeros(32, dtype=np.uint32)

@@ -19,6 +19,7 @@
 #include <thread>
 #include <new>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "kernels.cuh"
@@ -141,6 +142,10 @@ struct PeerBufs {  // the peer-memory reduction (p2p_kernels.cuh)
     DevBuf<uint32_t> d_mpos;
     MappedBuf<int64_t> h_grows;  // global final rows of the last global search (16 bytes each)
     MappedBuf<uint32_t> h_ghdr;  // status, count, epoch
+};
+struct RecBufs {  // a record set (fzb_haystack_set_records, DESIGN.md section 5.10)
+    DevBuf<uint64_t> d_off;    // the count + 1 record offsets
+    DevBuf<uint32_t> d_first;  // per 64-byte granule: the record holding its first position (k_rec_first)
 };
 struct GatherBufs {  // the staged NCCL all-gather
     uint32_t cap = 0;  // rows per rank
@@ -275,6 +280,7 @@ struct fzb_haystack {
     DevBuf<unsigned long long> d_mhits;  // dense batch pass: (pattern, n-gram, position) hits
     std::unique_ptr<LpBatchBufs> lpb;
     std::unique_ptr<GenericBatchBufs> gbatch;
+    std::unique_ptr<RecBufs> recs;  // the record set, if any (cleared by every upload)
 };
 
 struct fzb_result {
@@ -699,6 +705,7 @@ extern "C" int fzb_haystack_upload(fzb_haystack *h, const uint8_t *host, uint64_
     if (!h->owned_buf) return fail(FZB_E_INVALID, "upload needs an owned handle");
     if (round_up(n, 128) + 128 > h->owned_buf.size()) return fail(FZB_E_INVALID, "upload larger than the handle's capacity");
     CK(cudaSetDevice(h->device));
+    h->recs.reset();
     if (!is_whole_sequence(h)) {  // a shard keeps its geometry: the new bytes replace the same window of the global sequence
         if (n != h->buf_len) return fail(FZB_E_INVALID, "a shard upload must supply exactly buf_len bytes");
     } else {
@@ -725,6 +732,7 @@ extern "C" int fzb_haystack_upload_symbols(fzb_haystack *h, const void *host, ui
     if (round_up(n, 128) + 128 > h->owned_buf.size()) return fail(FZB_E_INVALID, "upload larger than the handle's capacity");
     if (!is_whole_sequence(h)) return fail(FZB_E_INVALID, "symbol uploads replace a whole (unsharded) sequence");
     CK(cudaSetDevice(h->device));
+    h->recs.reset();
     h->buf_len = h->global_len = h->own_hi = n;
     h->padded_len = round_up(n, 128) + 128;
     h->coll_prob = -1.0;
@@ -757,6 +765,58 @@ extern "C" int fzb_haystack_upload_symbols(fzb_haystack *h, const void *host, ui
     }
     CK(cudaStreamSynchronize(h->stream));
     return FZB_OK;
+}
+
+// Record sets (DESIGN.md section 5.10): the offsets and the per-granule lookup table of the exact stages, built whole
+// in a new group that replaces the handle's only on success.
+extern "C" int fzb_haystack_set_records(fzb_haystack *h, const uint64_t *offsets, uint64_t count) {
+    HandleLock handle_lock(h);
+    if (!h) return fail(FZB_E_INVALID, "haystack handle is NULL");
+    if (!is_whole_sequence(h)) return fail(FZB_E_INVALID, "record sets need a whole (unsharded) sequence");
+    if (count == 0) {
+        h->recs.reset();
+        return FZB_OK;
+    }
+    if (!offsets) return fail(FZB_E_INVALID, "offsets is NULL");
+    if (count >= (1ull << 32)) return fail(FZB_E_INVALID, "a record set holds fewer than 2^32 records");
+    if (offsets[0] != 0 || offsets[count] != h->global_len)
+        return fail(FZB_E_INVALID, "record offsets must run from 0 to the sequence length");
+    for (uint64_t i = 0; i < count; i++)
+        if (offsets[i + 1] <= offsets[i]) return fail(FZB_E_INVALID, "record offsets must be strictly increasing");
+    CK(cudaSetDevice(h->device));
+    const uint64_t ngran = (h->global_len + kGranule - 1) >> kGranuleShift;
+    std::unique_ptr<RecBufs> recs;
+    TRY(ensure_group(recs, [&](RecBufs &b) -> int {
+        TRY(b.d_off.alloc(count + 1));
+        TRY(b.d_first.alloc(ngran));
+        CK(cudaMemcpyAsync(b.d_off.get(), offsets, (count + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+        const int grid = (int)std::min<uint64_t>((uint64_t)h->sm_count * 8, (ngran + 255) / 256);
+        k_rec_first<<<grid, 256, 0, h->stream>>>(b.d_off.get(), count, b.d_first.get(), ngran);
+        CK(cudaGetLastError());
+        CK(cudaStreamSynchronize(h->stream));
+        return FZB_OK;
+    }));
+    h->recs = std::move(recs);
+    return FZB_OK;
+}
+
+// The record set the exact stages of a search on `h` take (null pointers without one) and its compile-time switch:
+// with_recs(h, f) calls f(std::true_type) on a handle with a record set, f(std::false_type) otherwise.
+static RecSet rec_set(const fzb_haystack *h) {
+    return h->recs ? RecSet{h->recs->d_off.get(), h->recs->d_first.get()} : RecSet{nullptr, nullptr};
+}
+
+template <class F>
+static void with_recs(const fzb_haystack *h, F f) {
+    if (h->recs)
+        f(std::true_type{});
+    else
+        f(std::false_type{});
+}
+
+// The entry points outside a record set's scope (batches, has_near_match, windows, FZB_F_GLOBAL) refuse to run on one.
+static int refuse_records(const fzb_haystack *h, const char *what) {
+    return h && h->recs ? fail(FZB_E_UNSUPPORTED, "%s does not support record sets", what) : FZB_OK;
 }
 
 extern "C" void *fzb_host_alloc(uint64_t n) {
@@ -1583,31 +1643,44 @@ static int search_lev_ngrams(fzb_haystack *h, const uint8_t *pattern, uint32_t m
     bool fuse_gather = post_mode != 0 && (flags & FZB_F_GLOBAL) != 0;
     bool bitmap_mode = false;
     if (flags & FZB_F_TINY_LIST) p.glist_cap = std::min(h->glist_cap, 8u);
+    const RecSet rs = rec_set(h);
     auto enqueue = [&]() -> int {
         int r2 = enqueue_filter(h, p, sampled, res);
         if (r2) return r2;
         if (use_hits) {
-            if (vm == 0)
-                k_verify_hits<0><<<h->sm_count * 8, kHitThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(), h->d_counters.get());
-            else if (vm == 1)
-                k_verify_hits<1><<<h->sm_count * 8, kHitThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(), h->d_counters.get());
-            else
-                k_verify_hits<2><<<h->sm_count * 8, kHitThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(), h->d_counters.get());
+            with_recs(h, [&](auto rec) {
+                constexpr bool R = decltype(rec)::value;
+                if (vm == 0)
+                    k_verify_hits<0, R><<<h->sm_count * 8, kHitThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(),
+                                                                                         h->d_counters.get(), rs);
+                else if (vm == 1)
+                    k_verify_hits<1, R><<<h->sm_count * 8, kHitThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(),
+                                                                                         h->d_counters.get(), rs);
+                else
+                    k_verify_hits<2, R><<<h->sm_count * 8, kHitThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(),
+                                                                                         h->d_counters.get(), rs);
+            });
             res->stats.n_launches++;
             return FZB_OK;
         }
         {   // one verify launch: the granule work list -- or, second attempt after the list overflowed, the whole bitmap
             const int scan_mode = bitmap_mode ? 1 : 0;
             const int grid = h->sm_count * kVerifyCtasPerSm;
-            if (vm == 0)
-                k_verify_lev<0><<<grid, kVerifyThreads, 0, h->stream>>>(p, h->d_bitmap.size(), h->d_glist.get(), p.glist_cap,
-                                                                        scan_mode, h->d_out.get(), h->d_out.size(), h->d_counters.get());
-            else if (vm == 1)
-                k_verify_lev<1><<<grid, kVerifyThreads, 0, h->stream>>>(p, h->d_bitmap.size(), h->d_glist.get(), p.glist_cap,
-                                                                        scan_mode, h->d_out.get(), h->d_out.size(), h->d_counters.get());
-            else
-                k_verify_lev<2><<<grid, kVerifyThreads, 0, h->stream>>>(p, h->d_bitmap.size(), h->d_glist.get(), p.glist_cap,
-                                                                        scan_mode, h->d_out.get(), h->d_out.size(), h->d_counters.get());
+            with_recs(h, [&](auto rec) {
+                constexpr bool R = decltype(rec)::value;
+                if (vm == 0)
+                    k_verify_lev<0, R><<<grid, kVerifyThreads, 0, h->stream>>>(p, h->d_bitmap.size(), h->d_glist.get(),
+                                                                               p.glist_cap, scan_mode, h->d_out.get(),
+                                                                               h->d_out.size(), h->d_counters.get(), rs);
+                else if (vm == 1)
+                    k_verify_lev<1, R><<<grid, kVerifyThreads, 0, h->stream>>>(p, h->d_bitmap.size(), h->d_glist.get(),
+                                                                               p.glist_cap, scan_mode, h->d_out.get(),
+                                                                               h->d_out.size(), h->d_counters.get(), rs);
+                else
+                    k_verify_lev<2, R><<<grid, kVerifyThreads, 0, h->stream>>>(p, h->d_bitmap.size(), h->d_glist.get(),
+                                                                               p.glist_cap, scan_mode, h->d_out.get(),
+                                                                               h->d_out.size(), h->d_counters.get(), rs);
+            });
         }
         res->stats.n_launches += 1;
         return FZB_OK;
@@ -1688,6 +1761,7 @@ static int search_lev_lp(fzb_haystack *h, const uint8_t *pattern, uint32_t m, ui
     if (streaming && !h->d_lplist)
         TRY(h->d_lplist.alloc(std::min<uint64_t>(std::max<uint64_t>(1u << 20, h->owned_buf.size() / 64), 1u << 26)));
     const PostPlan plan{post_mode, post_mode != 0 && (flags & FZB_F_GLOBAL) != 0};
+    const RecSet rs = rec_set(h);
     if (streaming) {
         const uint32_t list_cap = (flags & FZB_F_TINY_LIST) ? std::min<uint32_t>(h->d_lplist.size(), kTinyLpListCap)
                                                             : (uint32_t)h->d_lplist.size();
@@ -1695,8 +1769,11 @@ static int search_lev_lp(fzb_haystack *h, const uint8_t *pattern, uint32_t m, ui
             k_lp_scan<<<h->sm_count * 4, kLpsThreads, 0, h->stream>>>(p, h->d_lplist.get(), list_cap);
             CK(cudaEventRecord(h->ev[1], h->stream));
             h->ev1_recorded = true;
-            k_lp_verify<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_lplist.get(), list_cap, h->d_scratch.get(), cap, h->d_out.get(),
-                                                            h->d_out.size(), h->d_counters.get());
+            with_recs(h, [&](auto rec) {
+                constexpr bool R = decltype(rec)::value;
+                k_lp_verify<R><<<grid, kLpThreads, 0, h->stream>>>(p, h->d_lplist.get(), list_cap, h->d_scratch.get(), cap,
+                                                                   h->d_out.get(), h->d_out.size(), h->d_counters.get(), rs);
+            });
             res->stats.n_launches += 2;
             return FZB_OK;
         }, plan);
@@ -1708,7 +1785,11 @@ static int search_lev_lp(fzb_haystack *h, const uint8_t *pattern, uint32_t m, ui
         res->discard_attempt();  // list overflow: nothing was verified (and the fused reduction saw an invalid shard)
     }
     rc = run_lp(h, res, [&](int grid, int cap) -> int {
-        k_lev_lp<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_scratch.get(), cap, h->d_out.get(), h->d_out.size(), h->d_counters.get());
+        with_recs(h, [&](auto rec) {
+            constexpr bool R = decltype(rec)::value;
+            k_lev_lp<R><<<grid, kLpThreads, 0, h->stream>>>(p, h->d_scratch.get(), cap, h->d_out.get(), h->d_out.size(),
+                                                            h->d_counters.get(), rs);
+        });
         res->stats.n_launches++;
         return FZB_OK;
     }, plan);
@@ -1750,11 +1831,15 @@ static int search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, u
     if (rc) return rc;
     CK(cudaSetDevice(h->device));
     res->stats.bytes_scanned = h->buf_len;
+    const RecSet rs = rec_set(h);
     if (!ngrams) {
         res->stats.route = 6;
         rc = run_lp(h, res, [&](int grid, int cap) -> int {
-            k_generic_lp<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_scratch.get(), cap, h->d_out.get(), h->d_out.size(),
-                                                             h->d_counters.get());
+            with_recs(h, [&](auto rec) {
+                constexpr bool R = decltype(rec)::value;
+                k_generic_lp<R><<<grid, kLpThreads, 0, h->stream>>>(p, h->d_scratch.get(), cap, h->d_out.get(),
+                                                                    h->d_out.size(), h->d_counters.get(), rs);
+            });
             res->stats.n_launches++;
             return FZB_OK;
         }, PostPlan{post_mode, post_mode != 0 && (flags & FZB_F_GLOBAL) != 0});
@@ -1774,8 +1859,11 @@ static int search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, u
     rc = run_lp(h, res, [&](int grid, int cap) -> int {
         int r2 = enqueue_filter(h, p, sampled, res);
         if (r2) return r2;
-        k_verify_generic<<<grid, kLpThreads, 0, h->stream>>>(p, h->d_bitmap.size(), h->d_scratch.get(), cap, h->d_out.get(),
-                                                             h->d_out.size(), h->d_counters.get());
+        with_recs(h, [&](auto rec) {
+            constexpr bool R = decltype(rec)::value;
+            k_verify_generic<R><<<grid, kLpThreads, 0, h->stream>>>(p, h->d_bitmap.size(), h->d_scratch.get(), cap,
+                                                                    h->d_out.get(), h->d_out.size(), h->d_counters.get(), rs);
+        });
         res->stats.n_launches++;
         return FZB_OK;
     }, PostPlan{post_mode, post_mode != 0 && (flags & FZB_F_GLOBAL) != 0});
@@ -1832,6 +1920,7 @@ static int make_result(fzb_result **out, fzb_result **res) {
 
 static int check_pattern(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags) {
     if (!h) return fail(FZB_E_INVALID, "haystack handle is NULL");
+    if (flags & FZB_F_GLOBAL) TRY(refuse_records(h, "FZB_F_GLOBAL"));
     if ((flags & FZB_F_GLOBAL) && !h->comm && !h->local_world)
         return fail(FZB_E_INVALID, "FZB_F_GLOBAL needs fzb_haystack_comm_init / fzb_comm_init_local on this handle");
     if (!pattern || m == 0) return fail(FZB_E_INVALID, "Given subsequence is empty!");
@@ -2332,6 +2421,7 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
     HandleLock handle_lock(h);
     if (!h || !out || (count && (!patterns || !offsets || !max_l_dist))) return fail(FZB_E_INVALID, "NULL argument");
     for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
+    TRY(refuse_records(h, "a batch search"));
     for (uint32_t i = 0; i < count; i++)
         if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
     fzb_stats sum{};
@@ -2474,6 +2564,7 @@ extern "C" int fzb_search_exact_window(fzb_haystack *h, const uint8_t *pattern, 
     HandleLock handle_lock(h);
     if (!h || !out) return fail(FZB_E_INVALID, "NULL argument");
     *out = nullptr;
+    TRY(refuse_records(h, "the windowed exact search"));
     if (flags & FZB_F_GLOBAL) return fail(FZB_E_INVALID, "windowed exact search is per handle");
     if (!is_whole_sequence(h)) return fail(FZB_E_INVALID, "windowed exact search needs a whole (unsharded) sequence");
     // clamp (search_exact.py:29-30): start into [0, n], end into [start, n]
@@ -2544,6 +2635,7 @@ extern "C" int fzb_search_hamming(fzb_haystack *h, const uint8_t *pattern, uint3
         ScanParams p;
         fill_params(h, pattern, m, p);
         p.k = (int)std::min<uint32_t>(k, m);
+        const RecSet rs = rec_set(h);
         CK(cudaSetDevice(h->device));
         res->stats.route = 4;
         res->stats.bytes_scanned = h->buf_len;
@@ -2576,13 +2668,19 @@ extern "C" int fzb_search_hamming(fzb_haystack *h, const uint8_t *pattern, uint3
                 CK(cudaEventRecord(h->ev[1], h->stream));
                 h->ev1_recorded = true;
                 // one verify launch: the granule work list -- or, after it overflowed, the whole bitmap
-                k_verify_ham<<<h->sm_count * 4, kVerifyThreads, 0, h->stream>>>(
-                    p, h->d_bitmap.size(), h->d_glist.get(), p.glist_cap, bitmap_mode ? 1 : 0, h->d_out.get(), h->d_out.size(),
-                    h->d_counters.get());
+                with_recs(h, [&](auto rec) {
+                    constexpr bool R = decltype(rec)::value;
+                    k_verify_ham<R><<<h->sm_count * 4, kVerifyThreads, 0, h->stream>>>(
+                        p, h->d_bitmap.size(), h->d_glist.get(), p.glist_cap, bitmap_mode ? 1 : 0, h->d_out.get(),
+                        h->d_out.size(), h->d_counters.get(), rs);
+                });
                 res->stats.n_launches += 1;
             } else {
-                k_hamming_scan<<<h->sm_count * 8, kHamThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(),
-                                                                               h->d_counters.get());
+                with_recs(h, [&](auto rec) {
+                    constexpr bool R = decltype(rec)::value;
+                    k_hamming_scan<R><<<h->sm_count * 8, kHamThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(),
+                                                                                      h->d_counters.get(), rs);
+                });
             }
             res->stats.n_launches++;
             return FZB_OK;
@@ -2736,6 +2834,7 @@ extern "C" int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns
     HandleLock handle_lock(h);
     if (!h || !out || (count && (!patterns || !offsets || !max_subs))) return fail(FZB_E_INVALID, "NULL argument");
     for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
+    TRY(refuse_records(h, "a batch search"));
     for (uint32_t i = 0; i < count; i++)
         if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
     // a pattern the single search refuses fails the whole call, with the single search's error, before any work
@@ -2819,6 +2918,7 @@ extern "C" int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns
     if (!h || !out || (count && (!patterns || !offsets || !max_subs || !max_ins || !max_dels || !max_l_dist)))
         return fail(FZB_E_INVALID, "NULL argument");
     for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
+    TRY(refuse_records(h, "a batch search"));
     for (uint32_t i = 0; i < count; i++)
         if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
     // Per pattern, as fzb_search_generic would search it: the route, the total limit it works with (the LP route
@@ -2992,6 +3092,7 @@ extern "C" int fzb_has_near_match(fzb_haystack *h, const uint8_t *pattern, uint3
     HandleLock handle_lock(h);
     if (!h || !found) return fail(FZB_E_INVALID, "NULL argument");
     *found = 0;
+    TRY(refuse_records(h, "has_near_match"));
     int rc = check_pattern(h, pattern, m, 0);
     if (rc) return rc;
     CK(cudaSetDevice(h->device));

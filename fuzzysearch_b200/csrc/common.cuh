@@ -44,6 +44,39 @@ struct ScanParams {
 enum { CNT_OUT = 0, CNT_CAND = 1, CNT_OVERFLOW = 2, CNT_GRAN = 3, CNT_WORK = 4, /* 5,6: post_kernels.cuh */
        CNT_HITS = 7, CNT_HITWORK = 8, /* 9: post_kernels.cuh */ CNT_KEYS = 14, CNT_COUNT = 16 };
 
+// A record set (fzb_haystack_set_records, DESIGN.md section 5.10): record r of a whole-sequence buffer is
+// [off[r], off[r+1] - 1), followed by one separator position off[r+1] - 1.  first[g] is the record that holds position
+// 64 g.  Only the exact stages read it, through rec_bounds; kernels take it as a trailing argument and ignore it in
+// their REC == false instantiations.
+struct RecSet {
+    const uint64_t *off;
+    const uint32_t *first;
+};
+
+// [lo, hi) of the record holding buffer position x (x < N); false if x is that record's separator (x == hi).  A
+// 64-position granule holds at most 64 record starts, so the walk from first[] takes at most 64 steps.
+__device__ __forceinline__ bool rec_bounds(const RecSet &rs, int64_t x, int64_t &lo, int64_t &hi) {
+    uint32_t r = rs.first[x >> kGranuleShift];
+    while ((int64_t)rs.off[r + 1] <= x) r++;
+    lo = (int64_t)rs.off[r];
+    hi = (int64_t)rs.off[r + 1] - 1;
+    return x < hi;
+}
+
+// first[g] for every granule g < ngran: the largest r with off[r] <= 64 g (binary search over the count + 1 offsets)
+__global__ void k_rec_first(const uint64_t *off, uint64_t count, uint32_t *first, uint64_t ngran) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < ngran; g += stride) {
+        const uint64_t x = g << kGranuleShift;
+        uint64_t lo = 0, hi = count;  // off[lo] <= x < off[hi]
+        while (hi - lo > 1) {
+            const uint64_t mid = (lo + hi) / 2;
+            if (off[mid] <= x) lo = mid; else hi = mid;
+        }
+        first[g] = (uint32_t)lo;
+    }
+}
+
 __host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
     x += 0x9E3779B97F4A7C15ull;
     x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;

@@ -40,8 +40,18 @@ __device__ __forceinline__ int ham_mismatches(Text text, const uint8_t *sP, int 
     return nd;
 }
 
+// REC: does the occurrence [pos, pos + m) lie inside one record of `rs`?  (Asked of the few starts that pass the
+// mismatch count only.)
+template <bool REC>
+__device__ __forceinline__ bool ham_in_record(const RecSet &rs, int64_t pos, int m) {
+    if (!REC) return true;
+    int64_t lo, hi;
+    return rec_bounds(rs, pos, lo, hi) && pos + m <= hi;
+}
+
+template <bool REC>
 __global__ void __launch_bounds__(kHamThreads)
-k_hamming_scan(const ScanParams p, RawRec *out, uint32_t cap, uint32_t *counters) {
+k_hamming_scan(const ScanParams p, RawRec *out, uint32_t cap, uint32_t *counters, const RecSet rs) {
     __shared__ uint8_t sP[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) sP[i] = p.P[i];
     __syncthreads();
@@ -51,7 +61,7 @@ k_hamming_scan(const ScanParams p, RawRec *out, uint32_t cap, uint32_t *counters
     for (int64_t pos = p.own_lo + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pos < last; pos += stride) {
         const uint8_t *h = p.H + (pos - p.buf_lo);
         const int nd = ham_mismatches([&](int i) { return __ldg(h + i); }, sP, m, k);
-        if (nd <= k) emit(out, cap, counters, pos, pos + m, pos, nd, 0);
+        if (nd <= k && ham_in_record<REC>(rs, pos, m)) emit(out, cap, counters, pos, pos + m, pos, nd, 0);
     }
 }
 
@@ -223,9 +233,10 @@ k_hamming_count(const ScanParams p, const HamCountParams hp, const __grid_consta
 }
 
 // ---- exact verification of the marked granules (same work-list scheme as k_verify_lev) -------------
+template <bool REC>
 __device__ __forceinline__ void verify_granule_ham(const ScanParams &p, const uint8_t *sP, uint32_t *sWin,
                                                    int64_t granule, int lane, RawRec *out, uint32_t cap,
-                                                   uint32_t *counters) {
+                                                   uint32_t *counters, const RecSet &rs) {
     const int m = p.m, k = p.k;
     const int64_t gbase = p.buf_lo + (granule << kGranuleShift);
     const int64_t alo = stage_window(p, gbase, m, lane, sWin);
@@ -235,13 +246,14 @@ __device__ __forceinline__ void verify_granule_ham(const ScanParams &p, const ui
         const int64_t pos = gbase + half * 32 + lane;
         if (pos < p.own_lo || pos >= p.own_hi || pos + m > p.N) continue;
         const int nd = ham_mismatches([&](int i) { return W[pos + i]; }, sP, m, k);
-        if (nd <= k) emit(out, cap, counters, pos, pos + m, pos, nd, 0);
+        if (nd <= k && ham_in_record<REC>(rs, pos, m)) emit(out, cap, counters, pos, pos + m, pos, nd, 0);
     }
 }
 
+template <bool REC>
 __global__ void __launch_bounds__(kVerifyThreads)
 k_verify_ham(const ScanParams p, uint64_t bitmap_words, const uint32_t *glist, uint32_t glist_cap, int scan_mode,
-             RawRec *out, uint32_t cap, uint32_t *counters) {
+             RawRec *out, uint32_t cap, uint32_t *counters, const RecSet rs) {
     __shared__ uint8_t sP[256];
     __shared__ uint32_t sWinAll[kVerifyThreads / 32][kWinWords];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) sP[i] = p.P[i];
@@ -249,7 +261,7 @@ k_verify_ham(const ScanParams p, uint64_t bitmap_words, const uint32_t *glist, u
     const int lane = threadIdx.x & 31;
     uint32_t *sWin = sWinAll[threadIdx.x >> 5];
     for_each_marked_granule(p.bitmap, bitmap_words, glist, glist_cap, scan_mode, counters, [&](int64_t g) {
-        verify_granule_ham(p, sP, sWin, g, lane, out, cap, counters);
+        verify_granule_ham<REC>(p, sP, sWin, g, lane, out, cap, counters, rs);
     });
 }
 

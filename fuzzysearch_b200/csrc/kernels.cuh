@@ -838,18 +838,24 @@ __device__ __forceinline__ int64_t stage_window(const PT &p, int64_t gbase, int 
     return alo;
 }
 
-// One lane's window for a hit whose occurrence would start at p0: H[max(p0-k, 0) : min(p0+m+k, N)), clipped to the
-// buffer, copied into the lane's private slot.  Returns the global position of slot[0].
+// One lane's window for a hit whose occurrence would start at p0: H[max(p0-k, lo) : min(p0+m+k, hi)), clipped to the
+// buffer, copied into the lane's private slot; [lo, hi) is the sequence (or record) of the hit.  Returns the global
+// position of slot[0].
 template <class PT>
-__device__ __forceinline__ int64_t stage_lane_window(const PT &p, int64_t p0, uint8_t *slot) {
-    const int64_t wlo = max(max(p0 - p.k, (int64_t)0), p.buf_lo);
-    const int64_t whi = min(min(p0 + p.m + p.k, p.N), p.buf_lo + p.buf_len);
+__device__ __forceinline__ int64_t stage_lane_window(const PT &p, int64_t p0, uint8_t *slot, int64_t lo, int64_t hi) {
+    const int64_t wlo = max(max(p0 - p.k, lo), p.buf_lo);
+    const int64_t whi = min(min(p0 + p.m + p.k, hi), p.buf_lo + p.buf_len);
     const int64_t alo = wlo & ~(int64_t)3;
     const int nwords = (int)((whi - alo + 3) >> 2);
     const uint32_t *src = reinterpret_cast<const uint32_t *>(p.H + (alo - p.buf_lo));
     uint32_t *dst = reinterpret_cast<uint32_t *>(slot);
     for (int w = 0; w < nwords; w++) dst[w] = __ldg(src + w);
     return alo;
+}
+
+template <class PT>
+__device__ __forceinline__ int64_t stage_lane_window(const PT &p, int64_t p0, uint8_t *slot) {
+    return stage_lane_window(p, p0, slot, 0, p.N);
 }
 
 // All lanes of the warp call this together (lanes without an anchor pass valid = false).  Each lane
@@ -865,23 +871,30 @@ struct VerifyCtx {
     int32_t m, k, L, n_ngrams;
 };
 
-template <int VM, class PT>
+// REC: the sequence of the anchor is its own record [rec_lo, rec_hi) of a record set (the caller looked it up and
+// passes valid = false for an anchor on a separator) in place of [0, N).
+template <int VM, bool REC = false, class PT>
 __device__ void verify_anchor_lev(const PT &p, const uint8_t *sP, const unsigned long long *sPM,
                                   const uint8_t *W, int64_t idx, bool valid, DpScratch *S, RawRec *out, uint32_t cap,
-                                  uint32_t *counters, int j_lo, int j_hi, int tag = 0) {
+                                  uint32_t *counters, int j_lo, int j_hi, int tag = 0, int64_t rec_lo = 0,
+                                  int64_t rec_hi = 0) {
     // W[g] is the haystack byte at global position g (shared-memory window); n-grams j_lo..j_hi-1
     const int m = p.m, k = p.k, L = p.L;
-    const int64_t N = p.N;
+    int64_t lo = 0, hi = p.N;
+    if constexpr (REC) {
+        lo = rec_lo;
+        hi = rec_hi;
+    }
     const uint8_t *h = W + idx;
     int j = valid ? j_lo : j_hi;
     for (;;) {
         for (; j < j_hi; j++) {  // next n-gram hit at this anchor
             const int s = j * L;  // :170
-            // search window of n-gram j, clamped like search_exact.py:29-30   (:174-176)
-            int64_t ws = max((int64_t)0, (int64_t)(s - k));
-            int64_t we = min(N, N - m + s + L + k);
-            ws = max((int64_t)0, min(ws, N));
-            we = max(ws, min(we, N));
+            // search window of n-gram j, clamped like search_exact.py:29-30   (:174-176), relative to the sequence
+            int64_t ws = lo + max((int64_t)0, (int64_t)(s - k));
+            int64_t we = min(hi, hi - m + s + L + k);
+            ws = max(lo, min(ws, hi));
+            we = max(ws, min(we, hi));
             if (idx < ws || idx + L > we) continue;
             bool eq = true;
             for (int i = 0; i < L; i++) {
@@ -900,7 +913,7 @@ __device__ void verify_anchor_lev(const PT &p, const uint8_t *sP, const unsigned
         int dr = 0, rs = 0, dl = 0, ls = 0;
         bool ok = have;
         if (ok) {
-            const int64_t rhi = min(N, p0 + m + k);
+            const int64_t rhi = min(hi, p0 + m + k);
             const int rlen = (int)max((int64_t)0, rhi - (idx + L));
             if (VM == 3)  // per-lane patterns: Eq on the fly (m - L <= 32)
                 ok = expand_bp<uint32_t, 1>(EqOtf<1>{sP + s + L, m - s - L}, m - s - L, h + L, rlen, k, dr, rs);
@@ -913,7 +926,7 @@ __device__ void verify_anchor_lev(const PT &p, const uint8_t *sP, const unsigned
         }
         // left: _expand(P[:s][::-1], H[max(0,p0-(k-dr)) : idx][::-1], k-dr)   (:185-189)
         if (ok) {
-            const int64_t llo = max((int64_t)0, p0 - (k - dr));
+            const int64_t llo = max(lo, p0 - (k - dr));
             const int llen = (int)max((int64_t)0, idx - llo);
             if (VM == 3)
                 ok = expand_bp<uint32_t, -1>(EqOtf<-1>{sP + s - 1, s}, s, h - 1, llen, k - dr, dl, ls);
@@ -989,26 +1002,31 @@ __device__ __forceinline__ void for_each_marked_granule(uint32_t *bitmap, uint64
     }
 }
 
-template <int VM, class PT>
+template <int VM, bool REC = false, class PT>
 __device__ __forceinline__ void verify_granule_lev(const PT &p, const uint8_t *sP,
                                                    const unsigned long long *sPM, uint32_t *sWin, int64_t granule,
                                                    int lane, DpScratch *S, RawRec *out, uint32_t cap,
-                                                   uint32_t *counters, int tag = 0) {
+                                                   uint32_t *counters, int tag = 0, const RecSet &rs = RecSet{}) {
     const int64_t gbase = p.buf_lo + (granule << kGranuleShift);
     const int64_t alo = stage_window(p, gbase, p.m + p.k, lane, sWin);
     const uint8_t *W = reinterpret_cast<const uint8_t *>(sWin) - alo;
 #pragma unroll 1
     for (int half = 0; half < kGranule / 32; half++) {
         const int64_t idx = gbase + half * 32 + lane;
-        verify_anchor_lev<VM>(p, sP, sPM, W, idx, idx >= p.own_lo && idx < p.own_hi, S, out, cap, counters, 0,
-                              p.n_ngrams, tag);
+        bool valid = idx >= p.own_lo && idx < p.own_hi;
+        int64_t lo = 0, hi = 0;
+        if constexpr (REC) {
+            if (valid) valid = rec_bounds(rs, idx, lo, hi);
+        }
+        verify_anchor_lev<VM, REC>(p, sP, sPM, W, idx, valid, S, out, cap, counters, 0, p.n_ngrams, tag, lo, hi);
     }
 }
 
-template <int VM>
+// REC: the handle holds a record set `rs` (its instantiations with REC == false never read rs)
+template <int VM, bool REC>
 __global__ void __launch_bounds__(kVerifyThreads)
 k_verify_lev(const ScanParams p, uint64_t bitmap_words, const uint32_t *glist, uint32_t glist_cap, int scan_mode,
-             RawRec *out, uint32_t cap, uint32_t *counters) {
+             RawRec *out, uint32_t cap, uint32_t *counters, const RecSet rs) {
     __shared__ uint8_t sP[256];
     __shared__ unsigned long long sPM[VM < 2 ? 256 : 1];
     __shared__ uint32_t sWinAll[kVerifyThreads / 32][kWinWords];
@@ -1020,7 +1038,7 @@ k_verify_lev(const ScanParams p, uint64_t bitmap_words, const uint32_t *glist, u
     const int lane = threadIdx.x & 31;
     uint32_t *sWin = sWinAll[threadIdx.x >> 5];
     for_each_marked_granule(p.bitmap, bitmap_words, glist, glist_cap, scan_mode, counters, [&](int64_t g) {
-        verify_granule_lev<VM>(p, sP, sPM, sWin, g, lane, S, out, cap, counters);
+        verify_granule_lev<VM, REC>(p, sP, sPM, sWin, g, lane, S, out, cap, counters, 0, rs);
     });
 }
 
@@ -1033,9 +1051,9 @@ k_verify_lev(const ScanParams p, uint64_t bitmap_words, const uint32_t *glist, u
 constexpr int kHitSlotBytes = 144;  // per-lane window slot: m + 2k + alignment slack must fit
 constexpr int kHitThreads = 128;
 
-template <int VM>
+template <int VM, bool REC>
 __global__ void __launch_bounds__(kHitThreads)
-k_verify_hits(const ScanParams p, RawRec *out, uint32_t cap, uint32_t *counters) {
+k_verify_hits(const ScanParams p, RawRec *out, uint32_t cap, uint32_t *counters, const RecSet rs) {
     __shared__ uint8_t sP[256];
     __shared__ unsigned long long sPM[VM < 2 ? 256 : 1];
     __shared__ __align__(16) uint8_t slots[kHitThreads][kHitSlotBytes];
@@ -1057,16 +1075,21 @@ k_verify_hits(const ScanParams p, RawRec *out, uint32_t cap, uint32_t *counters)
         base = __shfl_sync(0xFFFFFFFFu, base, 0);
         if (base >= nhits) break;
         const uint32_t item = base + lane;
-        const bool valid = item < nhits;
-        int64_t idx = 0, alo = 0;
+        bool valid = item < nhits;
+        int64_t idx = 0, alo = 0, lo = 0, hi = 0;
         int j = 0;
         if (valid) {
             const uint64_t hv = p.hits[item];
             idx = (int64_t)(hv >> 8);
             j = (int)(hv & 0xFFu);
-            alo = stage_lane_window(p, idx - (int64_t)j * p.L, slot);
+            if constexpr (REC) {  // the hit's own record; a hit on a separator is dropped
+                valid = rec_bounds(rs, idx, lo, hi);
+                if (valid) alo = stage_lane_window(p, idx - (int64_t)j * p.L, slot, lo, hi);
+            } else {
+                alo = stage_lane_window(p, idx - (int64_t)j * p.L, slot);
+            }
         }
-        verify_anchor_lev<VM>(p, sP, sPM, slot - alo, idx, valid, S, out, cap, counters, j, j + 1);  // whole warp
+        verify_anchor_lev<VM, REC>(p, sP, sPM, slot - alo, idx, valid, S, out, cap, counters, j, j + 1, 0, lo, hi);  // whole warp
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&counters[CNT_CAND], nhits);
 }

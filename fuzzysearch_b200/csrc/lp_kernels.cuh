@@ -181,8 +181,18 @@ __device__ __forceinline__ void lp_tiles(const ScanParams &p, Opens opens, Sim s
     }
 }
 
+// What sim_lev_lp needs when the sequence of a start is one record of a record set: N = that record's end.
+struct LpSeq {
+    int32_t m, k;
+    int64_t N;
+};
+
+// REC: the starts of a record set `rs` (see k_verify_lev): a start on a separator is dropped, the others run to the end
+// of their own record.
+template <bool REC>
 __global__ void __launch_bounds__(kLpThreads)
-k_lev_lp(const ScanParams p, uint32_t *scratch, int cap, RawRec *out, uint32_t ocap, uint32_t *counters) {
+k_lev_lp(const ScanParams p, uint32_t *scratch, int cap, RawRec *out, uint32_t ocap, uint32_t *counters,
+         const RecSet rs) {
     __shared__ uint8_t sP[256];
     __shared__ int16_t sFirst[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) {
@@ -196,12 +206,21 @@ k_lev_lp(const ScanParams p, uint32_t *scratch, int cap, RawRec *out, uint32_t o
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     uint32_t *A = scratch + tid * 2 * (int64_t)cap, *B = A + cap;
     if (p.k >= p.m) {  // levenshtein.py:62-65: an empty match (i,i,m) at every index 0..N
-        const int64_t hi = (p.own_hi == p.N) ? p.N + 1 : p.own_hi;
+        // (with records: 0..n_r of every record, i.e. every buffer position, separators included, but not N)
+        const int64_t hi = (p.own_hi == p.N) ? p.N + (REC ? 0 : 1) : p.own_hi;
         for (int64_t i = p.own_lo + tid; i < hi; i += stride) emit(out, ocap, counters, i, i, i, p.m, 1);
         return;
     }
     lp_tiles(p, [&](uint8_t c) { return sFirst[c] >= 0; }, [&](const uint8_t *W, int64_t st) {
-        if (!sim_lev_lp(p, sP, W, st, A, B, cap, out, ocap, counters)) atomicExch(&counters[CNT_OVERFLOW], 1u);
+        bool ok;
+        if constexpr (REC) {
+            int64_t lo, hi;
+            if (!rec_bounds(rs, st, lo, hi)) return;
+            ok = sim_lev_lp(LpSeq{p.m, p.k, hi}, sP, W, st, A, B, cap, out, ocap, counters);
+        } else {
+            ok = sim_lev_lp(p, sP, W, st, A, B, cap, out, ocap, counters);
+        }
+        if (!ok) atomicExch(&counters[CNT_OVERFLOW], 1u);
     });
 }
 
@@ -389,9 +408,10 @@ __device__ __forceinline__ bool lp_nfa_any(const uint32_t *sPM32, const uint8_t 
     return lp_nfa_end<K>(R, m, k);
 }
 
+template <bool REC>
 __global__ void __launch_bounds__(kLpThreads)
 k_lp_verify(const ScanParams p, const unsigned long long *list, uint32_t list_cap, uint32_t *scratch, int cap,
-            RawRec *out, uint32_t ocap, uint32_t *counters) {
+            RawRec *out, uint32_t ocap, uint32_t *counters, const RecSet rs) {
     __shared__ uint8_t sP[256];
     __shared__ int16_t sFirst[256];
     __shared__ uint32_t sPM32[256];
@@ -417,13 +437,26 @@ k_lp_verify(const ScanParams p, const unsigned long long *list, uint32_t list_ca
     const bool use_nfa = p.m <= 31 && p.k <= 8;
     for (int64_t i = tid; i < (int64_t)n; i += (int64_t)gridDim.x * blockDim.x) {
         const int64_t st = (int64_t)list[i];
-        if (use_nfa) {
-            const int j0 = sFirst[W[st]];
-            const bool any = p.k <= 4 ? lp_nfa_any<4>(sPM32, W, st, p.N, p.m, p.k, j0)
-                                      : lp_nfa_any<8>(sPM32, W, st, p.N, p.m, p.k, j0);
-            if (!any) continue;
+        if constexpr (REC) {  // the start's own record is the sequence; a separator is no start
+            int64_t lo, end;
+            if (!rec_bounds(rs, st, lo, end)) continue;
+            if (use_nfa) {
+                const int j0 = sFirst[W[st]];
+                const bool any = p.k <= 4 ? lp_nfa_any<4>(sPM32, W, st, end, p.m, p.k, j0)
+                                          : lp_nfa_any<8>(sPM32, W, st, end, p.m, p.k, j0);
+                if (!any) continue;
+            }
+            if (!sim_lev_lp(LpSeq{p.m, p.k, end}, sP, W, st, A, B, cap, out, ocap, counters))
+                atomicExch(&counters[CNT_OVERFLOW], 1u);
+        } else {
+            if (use_nfa) {
+                const int j0 = sFirst[W[st]];
+                const bool any = p.k <= 4 ? lp_nfa_any<4>(sPM32, W, st, p.N, p.m, p.k, j0)
+                                          : lp_nfa_any<8>(sPM32, W, st, p.N, p.m, p.k, j0);
+                if (!any) continue;
+            }
+            if (!sim_lev_lp(p, sP, W, st, A, B, cap, out, ocap, counters)) atomicExch(&counters[CNT_OVERFLOW], 1u);
         }
-        if (!sim_lev_lp(p, sP, W, st, A, B, cap, out, ocap, counters)) atomicExch(&counters[CNT_OVERFLOW], 1u);
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&counters[CNT_CAND], n);
 }
@@ -515,14 +548,18 @@ __device__ bool sim_generic(const PT &p, const uint8_t *sP, const uint8_t *H, in
 // an equal text character costs at least 1 (substitution, deletion, or the insertion+deletion pair of
 // :120-128), and it consumes at most m + max_l text characters -- so H[s : s+m+max_l) must hold at least
 // m - max_l characters that occur in the pattern.
+template <bool REC>
 __global__ void __launch_bounds__(kLpThreads)
-k_generic_lp(const ScanParams p, uint32_t *scratch, int cap, RawRec *out, uint32_t ocap, uint32_t *counters) {
+k_generic_lp(const ScanParams p, uint32_t *scratch, int cap, RawRec *out, uint32_t ocap, uint32_t *counters,
+             const RecSet rs) {
     __shared__ uint8_t sP[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) sP[i] = p.P[i];
     const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t *A = scratch + tid * 2 * (int64_t)cap, *B = A + cap;
     lp_tiles(p, [](uint8_t) { return true; }, [&](const uint8_t *W, int64_t st) {  // (p.k = max_l)
-        if (!sim_generic(p, sP, W, st, p.N, A, B, cap, st, 1, out, ocap, counters))
+        int64_t lo = 0, seq_end = p.N;
+        if (REC && !rec_bounds(rs, st, lo, seq_end)) return;
+        if (!sim_generic(p, sP, W, st, seq_end, A, B, cap, st, 1, out, ocap, counters))
             atomicExch(&counters[CNT_OVERFLOW], 1u);
     });
 }
@@ -579,10 +616,61 @@ __device__ __forceinline__ void verify_granule_generic(const PT &p, const uint8_
     }
 }
 
+// The same for a record set `rs` (k_verify_generic<true>): per anchor, its own record is the sequence, the window
+// arithmetic of :223-226 and :231 taken relative to it and shifted back; anchors on separators are dropped.
+__device__ __forceinline__ void verify_granule_generic_rec(const ScanParams &p, const uint8_t *sP, uint32_t *sWin,
+                                                           int64_t granule, int lane, uint32_t *A, uint32_t *B,
+                                                           int cap, RawRec *out, uint32_t ocap, uint32_t *counters,
+                                                           const RecSet &rs) {
+    const int m = p.m, k = p.k, L = p.L;
+    const int64_t gbase = p.buf_lo + (granule << kGranuleShift);
+    const int64_t alo = stage_window(p, gbase, m + k, lane, sWin);
+    const uint8_t *W = reinterpret_cast<const uint8_t *>(sWin) - alo;  // W[g]: byte at global g
+    for (int half = 0; half < kGranule / 32; half++) {
+        const int64_t idx = gbase + half * 32 + lane;
+        int64_t lo = 0, hi = 0;  // the anchor's record
+        const bool owned = idx >= p.own_lo && idx < p.own_hi && rec_bounds(rs, idx, lo, hi);
+        for (int j = 0; j < p.n_ngrams; j++) {
+            const int s = j * L;
+            bool hit = false;
+            if (owned) {
+                int64_t ws = lo + max((int64_t)0, (int64_t)(s - k));
+                int64_t we = min(hi, hi - m + s + L + k);
+                if (we > ws) {
+                    ws = max(lo, min(ws, hi));
+                    we = max(ws, min(we, hi));
+                    if (idx >= ws && idx + L <= we) {
+                        const uint8_t *h = W + idx;
+                        hit = true;
+                        for (int i = 0; i < L; i++)
+                            if (h[i] != sP[s + i]) {
+                                hit = false;
+                                break;
+                            }
+                    }
+                }
+            }
+            unsigned hits = __ballot_sync(0xFFFFFFFFu, hit);
+            while (hits) {
+                const int hl = __ffs(hits) - 1;
+                hits &= hits - 1;
+                const int64_t hidx = gbase + half * 32 + hl;
+                const int64_t p0 = hidx - s;
+                const int64_t wlo = max((int64_t)__shfl_sync(0xFFFFFFFFu, lo, hl), p0 - k);  // the hit lane's record
+                const int64_t whi = min((int64_t)__shfl_sync(0xFFFFFFFFu, hi, hl), p0 + m + k);
+                for (int64_t st = wlo + lane; st < whi; st += 32)
+                    if (!sim_generic(p, sP, W, st, whi, A, B, cap, hidx, j, out, ocap, counters))
+                        atomicExch(&counters[CNT_OVERFLOW], 1u);
+            }
+        }
+    }
+}
+
 // Sweeps the whole bitmap (the host launches it once per search, without a work list).
+template <bool REC>
 __global__ void __launch_bounds__(kLpThreads)
 k_verify_generic(const ScanParams p, uint64_t bitmap_words, uint32_t *scratch, int cap, RawRec *out,
-                 uint32_t ocap, uint32_t *counters) {
+                 uint32_t ocap, uint32_t *counters, const RecSet rs) {
     __shared__ uint8_t sP[256];
     __shared__ uint32_t sWinAll[kLpThreads / 32][kWinWords];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) sP[i] = p.P[i];
@@ -592,7 +680,10 @@ k_verify_generic(const ScanParams p, uint64_t bitmap_words, uint32_t *scratch, i
     const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t *A = scratch + tid * 2 * (int64_t)cap, *B = A + cap;
     for_each_marked_granule(p.bitmap, bitmap_words, nullptr, 0, 1, counters, [&](int64_t g) {
-        verify_granule_generic(p, sP, sWin, g, lane, A, B, cap, out, ocap, counters);
+        if constexpr (REC)
+            verify_granule_generic_rec(p, sP, sWin, g, lane, A, B, cap, out, ocap, counters, rs);
+        else
+            verify_granule_generic(p, sP, sWin, g, lane, A, B, cap, out, ocap, counters);
     });
 }
 

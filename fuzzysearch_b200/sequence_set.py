@@ -1,0 +1,135 @@
+"""One pattern over many sequences in one device pass: ``find_near_matches_in_each`` and ``DeviceSequenceSet``.
+
+The sequences are joined into one resident buffer, each followed by one separator position, and the buffer is
+declared a record set (fzb_haystack_set_records, DESIGN.md section 5.10): the kernels clip every window at the edges
+of the record it belongs to, so one search returns, in buffer coordinates, what searching each sequence alone would
+return.  The lists are split per sequence on the host by the start of each match."""
+import threading
+
+import numpy as np
+
+from . import _native
+from .common import LevenshteinSearchParams, Match
+from .search import DeviceSequence, ExactSearch, GenericSearch, LevenshteinSearch, _kind, _text
+
+__all__ = ["DeviceSequenceSet", "find_near_matches_in_each"]
+
+
+def _set_kind(sequences):
+    """'str' | 'bytes' for a list of sequences of one kind (Bio.Seq.Seq counts as str)."""
+    kinds = set()
+    for s in sequences:
+        k = _kind(_text(s))
+        if k == "items":
+            raise TypeError("sequences of items (lists / tuples) are not supported in a sequence set")
+        kinds.add(k)
+    if len(kinds) > 1:
+        raise TypeError("the sequences of a set must all be str or all be byte-like")
+    return kinds.pop() if kinds else "bytes"
+
+
+def _slicer(orig, kind):
+    """Match.matched as find_near_matches(pattern, orig) slices it."""
+    if kind == "str" or isinstance(orig, (bytes, bytearray)):
+        return lambda s, e: orig[s:e]
+    mv = memoryview(_native.as_u8(orig))
+    return lambda s, e: bytes(mv[s:e])
+
+
+class DeviceSequenceSet(object):
+    """Many sequences kept resident in HBM as one record set, searched with any number of patterns by
+    ``find_near_matches_in_each(pattern, this_set, ...)``.  ``len()`` is the number of sequences."""
+
+    def __init__(self, sequences, device=0):
+        if not isinstance(sequences, (list, tuple)):
+            raise TypeError("sequences must be a list or tuple")
+        self._lock = threading.RLock()
+        self._orig = list(sequences)
+        self._kind = _set_kind(self._orig)
+        texts = [_text(s) for s in self._orig]
+        lengths = np.fromiter((len(t) for t in texts), dtype=np.uint64, count=len(texts))
+        self.offsets = np.zeros(len(texts) + 1, dtype=np.uint64)
+        np.cumsum(lengths + 1, out=self.offsets[1:])
+        if self._kind == "str":
+            joined = "\0".join(texts) + "\0"
+        else:
+            # byte-like elements go through as_u8: the single-byte, contiguous check find_near_matches applies
+            joined = b"\0".join(t if isinstance(t, (bytes, bytearray)) else _native.as_u8(t) for t in texts) + b"\0"
+        self._seq = DeviceSequence(joined, device=device)
+        self._bound_alphabet = self._seq._alphabet
+        self._seq.haystack.set_records(self.offsets)
+
+    def __len__(self):
+        return len(self._orig)
+
+    def _bind(self, subsequence):
+        """-> the pattern in the resident set's byte alphabet; a re-reduction of a wide-symbol set (a new upload,
+        which clears the record set) is followed by declaring the records again."""
+        pat = self._seq._bind(subsequence)
+        if self._seq._alphabet != self._bound_alphabet:
+            self._seq.haystack.set_records(self.offsets)
+            self._bound_alphabet = self._seq._alphabet
+        return pat
+
+    def close(self):
+        self._seq.close()
+
+
+def find_near_matches_in_each(subsequence, sequences, max_substitutions=None, max_insertions=None,
+                              max_deletions=None, max_l_dist=None):
+    """One pattern over many sequences: -> a list with, for every sequence, exactly
+    ``find_near_matches(subsequence, sequences[i], ...)``.  `sequences` is a list / tuple (uploaded for this call)
+    or a DeviceSequenceSet (resident).  All of them are searched in one device pass.  The limits are validated once
+    for the call, before anything else (also when there are no sequences)."""
+    search_params = LevenshteinSearchParams(max_substitutions, max_insertions, max_deletions, max_l_dist)
+    from . import choose_search_class
+    cls = choose_search_class(search_params)
+    if len(subsequence) == 0:
+        raise ValueError("subsequence must not be empty" if cls is ExactSearch else "Given subsequence is empty!")
+    if isinstance(sequences, DeviceSequenceSet):
+        return _search_set(subsequence, sequences, cls, search_params)
+    if not isinstance(sequences, (list, tuple)):
+        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
+    if not sequences:
+        return []
+    seqset = DeviceSequenceSet(sequences)
+    try:
+        return _search_set(subsequence, seqset, cls, search_params)
+    finally:
+        seqset.close()
+
+
+def _search_set(subsequence, seqset, cls, search_params):
+    if len(seqset) == 0:
+        return []
+    subs, ins, dels, l = search_params.unpacked
+    with seqset._lock:
+        pat = seqset._bind(subsequence)
+        hay = seqset._seq.haystack
+        if cls is ExactSearch:
+            res = hay.search_exact(pat)
+        elif cls is LevenshteinSearch:
+            res = hay.search_levenshtein(pat, l)
+        elif cls is GenericSearch:
+            res = hay.search_generic(pat, subs, ins, dels, l)
+        else:  # the limit SubstitutionsOnlySearch.search applies
+            res = hay.search_hamming(pat, min(x for x in (l, subs) if x is not None))
+        try:
+            # ExactSearch does not consolidate: its list is the RAW stream; the Hamming FINAL list equals RAW
+            s, e, d = res.arrays(_native.RAW if cls is ExactSearch else _native.FINAL)
+        finally:
+            res.close()
+    offsets = seqset.offsets.astype(np.int64)
+    rec = np.searchsorted(offsets, s, side="right") - 1
+    order = np.argsort(rec, kind="stable")  # each record's matches keep their order
+    rec, s, e, d = rec[order], s[order], e[order], d[order]
+    base = offsets[rec]
+    s, e, d = (s - base).tolist(), (e - base).tolist(), d.tolist()
+    out = [[] for _ in range(len(seqset))]
+    # only the records that hold matches are visited (most short sequences hold none)
+    hit_recs, firsts = np.unique(rec, return_index=True)
+    ends = np.append(firsts[1:], len(s))
+    for i, lo, hi in zip(hit_recs.tolist(), firsts.tolist(), ends.tolist()):
+        sl = _slicer(seqset._orig[i], seqset._kind)
+        out[i] = [Match(a, b, c, matched=sl(a, b)) for a, b, c in zip(s[lo:hi], e[lo:hi], d[lo:hi])]
+    return out

@@ -165,6 +165,18 @@ int fzb_haystack_upload(fzb_haystack *h, const uint8_t *host, uint64_t n);
 int fzb_haystack_upload_symbols(fzb_haystack *h, const void *host, uint64_t n, uint32_t width,
                                 const uint32_t *alphabet, uint32_t n_alpha);
 
+/* Declare `h` (a whole-sequence handle) to hold count >= 1 records: record i is
+ * [offsets[i], offsets[i+1] - 1), followed by ONE separator position offsets[i+1] - 1 whose value no search reads
+ * into a match. offsets[0] == 0, offsets[count] == fzb_haystack_len(h), strictly increasing.  Until the next
+ * upload, fzb_search_exact / _hamming / _levenshtein / _generic on `h` return what searching each record alone
+ * would return, in buffer coordinates: every window, start and end-of-sequence rule applies at record edges.
+ * count == 0 (offsets may be NULL) removes the record set.
+ * The record of a match (empty ones included) is the i with offsets[i] <= start < offsets[i+1].  A shard, malformed
+ * offsets or count >= 2^32 are refused with FZB_E_INVALID; with a record set in place the batch searches,
+ * fzb_has_near_match, fzb_search_exact_window and FZB_F_GLOBAL return FZB_E_UNSUPPORTED.  Every refusal leaves the
+ * handle as it was.  Any fzb_haystack_upload* clears the record set; fzb_haystack_write keeps it. */
+int fzb_haystack_set_records(fzb_haystack *h, const uint64_t *offsets, uint64_t count);
+
 /* Page-locked host memory for fast host<->device copies (cudaHostAlloc); NULL on failure. */
 void *fzb_host_alloc(uint64_t n);
 void fzb_host_free(void *p);
