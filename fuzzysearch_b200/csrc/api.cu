@@ -251,6 +251,7 @@ struct fzb_haystack {
     fzb_result *pending = nullptr;   // the last result, while its raw records still sit in d_out only
     bool ev1_recorded = false;
     bool filter_attrs_set = false;
+    int scan_per_sm = 0;      // resident k_filter_sampled CTAs per SM (asked once, after set_filter_attrs)
     double coll_prob = -1.0;  // sum_c p_c^2 of the byte distribution (sampled lazily; < 0 = unknown)
     // multi-GPU reduction (FZB_F_GLOBAL): peer-memory world (p2p_kernels.cuh) + NCCL for bootstrap / staged fallback
     bool p2p = false;               // every rank of the world can store into every other rank's receive area
@@ -1521,7 +1522,6 @@ static int set_filter_attrs(size_t smem) {
     return FZB_OK;
 }
 
-constexpr size_t kFilterSmem = kTblSize + 256 * sizeof(uint32_t);
 constexpr int kVerifyCtasPerSm = 8;  // k_verify_lev is latency bound (one DRAM round trip + a dependent chain per granule)
 
 // The q-sample lemma of k_filter_sampled needs floor((m-k-3)/4) >= k+1 aligned words per occurrence.
@@ -1573,13 +1573,20 @@ static bool sampled_is_selective(fzb_haystack *h, uint32_t m, uint32_t k, int L,
 // Enqueue the one pass over the haystack that marks candidate granules; records ev[1] behind it.
 static int enqueue_filter(fzb_haystack *h, const ScanParams &p, bool sampled, fzb_result *res) {
     const int64_t nvec = (int64_t)(round_up(h->buf_len, 16) / 16);
-    const int64_t ntiles = (nvec + kTileVecs - 1) / kTileVecs;
+    int64_t ntiles = (nvec + kTileVecs - 1) / kTileVecs;
     // dense route on a low-entropy haystack (about six effective symbols or fewer): index the table with 2-bit codes
     bool two_bit = false;
     if (!sampled && h->buf_len > 0 && sample_collision_prob(h) == FZB_OK) two_bit = h->coll_prob >= 0.15;
     if (ntiles > 0) {
         int per_sm = 4;
-        if (two_bit) {
+        if (sampled) {  // the sampled scan strides over its own (larger) tiles
+            ntiles = (nvec + kScanVecs - 1) / kScanVecs;
+            if (h->scan_per_sm == 0) {
+                CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_filter_sampled, kScanThreads, kScanSmem));
+                h->scan_per_sm = std::max(per_sm, 1);
+            }
+            per_sm = h->scan_per_sm;
+        } else if (two_bit) {
             CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_filter_dense2, kFilterThreads, kDense2Smem));
             per_sm = std::max(per_sm, 1);
         } else if (!sampled) {  // persistent grid = exactly the resident CTAs of the chosen instantiation
@@ -1592,7 +1599,7 @@ static int enqueue_filter(fzb_haystack *h, const ScanParams &p, bool sampled, fz
         }
         int grid = (int)std::min<int64_t>(ntiles, (int64_t)h->sm_count * per_sm);
         if (sampled)
-            k_filter_sampled<<<grid, kFilterThreads, kFilterSmem, h->stream>>>(p, nvec, ntiles);
+            k_filter_sampled<<<grid, kScanThreads, kScanSmem, h->stream>>>(p, nvec, ntiles);
         else if (two_bit)
             k_filter_dense2<<<grid, kFilterThreads, kDense2Smem, h->stream>>>(p, nvec, ntiles);
         else if (p.q < 4)
@@ -1630,7 +1637,7 @@ static int search_lev_ngrams(fzb_haystack *h, const uint8_t *pattern, uint32_t m
     res->stats.bytes_scanned = h->buf_len;
     CK(cudaSetDevice(h->device));
     if (!h->filter_attrs_set) {
-        rc = set_filter_attrs(kFilterSmem);
+        rc = set_filter_attrs(kScanSmem);
         if (rc) return rc;
         h->filter_attrs_set = true;
     }
@@ -1854,7 +1861,7 @@ static int search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, u
                          ((flags & FZB_F_FORCE_SAMPLED) || sampled_is_selective(h, m, max_l, p.L, p.n_ngrams));
     p.q = sampled ? 4 : std::min(p.L, 8);
     res->stats.route = 5;
-    rc = set_filter_attrs(kFilterSmem);
+    rc = set_filter_attrs(kScanSmem);
     if (rc) return rc;
     rc = run_lp(h, res, [&](int grid, int cap) -> int {
         int r2 = enqueue_filter(h, p, sampled, res);

@@ -1,5 +1,6 @@
 // common.cuh -- shared declarations for the libfuzzb200 kernels (sm_90a).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -75,6 +76,85 @@ __global__ void k_rec_first(const uint64_t *off, uint64_t count, uint32_t *first
         }
         first[g] = (uint32_t)lo;
     }
+}
+
+// ---- TMA / mbarrier primitives and shared-space loads (sm_90+ PTX) ---------------------------------
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+#ifdef FZB_EMU  // tests/emu: mbarrier / TMA semantics restated in C++ (tests/emu/include/cuda.h)
+__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) { emu::mbar_init(bar, count); }
+__device__ __forceinline__ void mbar_init_fence() {}
+__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) { emu::mbar_expect_tx(bar, bytes); }
+__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) { emu::mbar_wait(bar, parity); }
+__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar) {
+    emu::tma_load_2d(dst, map, c0, c1, bar);
+}
+// cp.async.bulk (1-D): the bytes land, then count against the barrier's expected transaction bytes
+__device__ __forceinline__ void bulk_load_1d(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
+    if ((bytes & 15) || ((uintptr_t)src & 15) || (((uintptr_t)dst - (uintptr_t)emu::smem_base()) & 15))
+        emu::die("bulk copy: size or address not a multiple of 16");
+    memcpy(dst, src, bytes);
+    emu::mbar_tx(bar, -(int64_t)bytes, false);
+}
+#else
+__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+}
+// makes the initialised barriers visible to the async proxy (the bulk copies that complete on them)
+__device__ __forceinline__ void mbar_init_fence() {
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "WAIT_LOOP:\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+        "@p bra WAIT_DONE;\n"
+        "bra WAIT_LOOP;\n"
+        "WAIT_DONE:\n"
+        "}\n" ::"r"(smem_u32(bar)),
+        "r"(parity)
+        : "memory");
+}
+__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
+            smem_u32(dst)),
+        "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
+        : "memory");
+}
+// contiguous copy of `bytes` (a multiple of 16; src and dst 16-byte aligned) global -> shared, completing on bar
+__device__ __forceinline__ void bulk_load_1d(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
+        "l"(src), "r"(bytes), "r"(smem_u32(bar))
+        : "memory");
+}
+#endif
+
+// explicit shared-space loads (32-bit shared address: no generic-address arithmetic)
+__device__ __forceinline__ uint4 lds128(uint32_t saddr) {
+#ifdef FZB_EMU
+    return *reinterpret_cast<const uint4 *>(emu::smem_base() + saddr);
+#else
+    uint4 r;
+    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(saddr));
+    return r;
+#endif
+}
+
+__device__ __forceinline__ uint32_t lds32(uint32_t saddr) {
+#ifdef FZB_EMU
+    return *reinterpret_cast<const uint32_t *>(emu::smem_base() + saddr);
+#else
+    uint32_t r;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(saddr));
+    return r;
+#endif
 }
 
 __host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {

@@ -65,45 +65,6 @@ k_hamming_scan(const ScanParams p, RawRec *out, uint32_t cap, uint32_t *counters
     }
 }
 
-// ---- TMA / mbarrier primitives (sm_90+ PTX) ------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-#ifdef FZB_EMU  // tests/emu: mbarrier / TMA semantics restated in C++ (tests/emu/include/cuda.h)
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) { emu::mbar_init(bar, count); }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) { emu::mbar_expect_tx(bar, bytes); }
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) { emu::mbar_wait(bar, parity); }
-__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar) {
-    emu::tma_load_2d(dst, map, c0, c1, bar);
-}
-#else
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra WAIT_DONE;\n"
-        "bra WAIT_LOOP;\n"
-        "WAIT_DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, int c0, int c1, uint64_t *bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-            smem_u32(dst)),
-        "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
-        : "memory");
-}
-#endif
-
 // ---- counting filter --------------------------------------------------------------------------------
 constexpr int kHcThreads = 256;               // one 128-byte row per thread; 2 CTAs per SM
 constexpr int kHcRowBytes = 128;
@@ -119,30 +80,9 @@ struct HamCountParams {
     int64_t nrows; // rows of the buffer that hold data: ceil(buf_len / 128)
 };
 
-// explicit shared-space 128-bit load (32-bit shared address: no generic-address arithmetic)
-__device__ __forceinline__ uint4 lds128(uint32_t saddr) {
-#ifdef FZB_EMU
-    return *reinterpret_cast<const uint4 *>(emu::smem_base() + saddr);
-#else
-    uint4 r;
-    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(saddr));
-    return r;
-#endif
-}
-
 // swizzled shared address of 16-byte chunk j of local row r (SWIZZLE_128B: chunk index ^= row % 8)
 __device__ __forceinline__ uint32_t hc_chunk(uint32_t stage, int r, int j) {
     return stage + r * kHcRowBytes + ((j ^ (r & 7)) << 4);
-}
-
-__device__ __forceinline__ uint32_t lds32(uint32_t saddr) {
-#ifdef FZB_EMU
-    return *reinterpret_cast<const uint32_t *>(emu::smem_base() + saddr);
-#else
-    uint32_t r;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(saddr));
-    return r;
-#endif
 }
 
 // SLICES = 2 (thresholds Wc - k <= 4) or 3: the bit slices of the counters (ham_recur.h).
@@ -161,9 +101,7 @@ k_hamming_count(const ScanParams p, const HamCountParams hp, const __grid_consta
     for (int i = tid; i < kHcBuckets * 32; i += kHcThreads) table[i] = 0u;
     if (tid == 0) {
         for (int s = 0; s < kHcStages; s++) mbar_init(&full[s], 1);
-#ifndef FZB_EMU
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-#endif
+        mbar_init_fence();
     }
     __syncthreads();
     if (tid < 32) {  // replica `tid` of the table: add the pattern's 4-grams (serial per replica: no races)

@@ -112,11 +112,41 @@ __device__ __forceinline__ void confirm_word(const ScanParams &p, const uint32_t
     }
 }
 
-__global__ void __launch_bounds__(kFilterThreads)
+// The bytes reach the threads through a ring of kScanStages shared-memory stages, one kScanStageBytes tile each,
+// filled by 1-D bulk copies (cp.async.bulk, mbarrier complete_tx) that one elected thread issues: the copies in
+// flight do not depend on what the warps are doing, and the first ones are issued before the table is built.
+// Tile t is buffer bytes [t * kScanStageBytes, (t+1) * kScanStageBytes); the last one is copied up to the
+// 16-byte-rounded end of the buffer (its zero padding), and chunks past that read as zeros.  Thread i reads the
+// 16-byte chunks i + u * kScanThreads of a stage (lane-contiguous: conflict-free).  A stage is refilled after the
+// __syncthreads that ends its tile.
+constexpr int kScanThreads = 512;        // two CTAs per SM
+constexpr int kScanStages = 2;
+constexpr int kScanStageBytes = 32768;
+constexpr int kScanVecs = kScanStageBytes / 16;         // 16-byte chunks per tile
+constexpr int kScanUnroll = kScanVecs / kScanThreads;   // chunks per thread per tile
+static_assert(kScanUnroll * kScanThreads == kScanVecs && 4 * kScanUnroll <= 32, "tile must split evenly");
+constexpr size_t kScanSmem = (size_t)kScanStages * kScanStageBytes + kTblSize + 256 * sizeof(uint32_t) +
+                             kScanStages * sizeof(uint64_t);
+
+__global__ void __launch_bounds__(kScanThreads, 2)
 k_filter_sampled(const ScanParams p, int64_t nvec, int64_t ntiles) {
     extern __shared__ __align__(16) uint8_t smem[];
-    uint8_t *tbl = smem;
-    uint32_t *grams = reinterpret_cast<uint32_t *>(smem + kTblSize);
+    uint8_t *ring = smem;
+    uint8_t *tbl = smem + kScanStages * kScanStageBytes;
+    uint32_t *grams = reinterpret_cast<uint32_t *>(tbl + kTblSize);
+    uint64_t *full = reinterpret_cast<uint64_t *>(grams + 256);
+    auto issue = [&](int64_t t, int s) {  // the elected thread only
+        const int64_t v0 = t * kScanVecs;
+        const uint32_t bytes = (uint32_t)min((int64_t)kScanVecs, nvec - v0) * 16u;
+        mbar_expect_tx(&full[s], bytes);
+        bulk_load_1d(ring + s * kScanStageBytes, p.H + v0 * 16, bytes, &full[s]);
+    };
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < kScanStages; s++) mbar_init(&full[s], 1);
+        mbar_init_fence();
+        for (int s = 0; s < kScanStages; s++)
+            if (blockIdx.x + (int64_t)s * gridDim.x < ntiles) issue(blockIdx.x + (int64_t)s * gridDim.x, s);
+    }
     for (int i = threadIdx.x; i < kTblSize / 16; i += blockDim.x)
         reinterpret_cast<uint4 *>(tbl)[i] = make_uint4(0, 0, 0, 0);
     __syncthreads();
@@ -130,18 +160,22 @@ k_filter_sampled(const ScanParams p, int64_t nvec, int64_t ntiles) {
     __syncthreads();
 
     const int lane = threadIdx.x & 31;
-    const uint4 *base = reinterpret_cast<const uint4 *>(p.H);
+    const uint32_t my_chunk = smem_u32(ring) + 16u * threadIdx.x;
+    int s = 0;
+    uint32_t parity = 0;
     for (int64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        const int64_t v0 = t * kTileVecs + threadIdx.x;
-        uint4 d[kFilterUnroll];
+        mbar_wait(&full[s], parity);
+        const int64_t v0 = t * kScanVecs + threadIdx.x;
+        uint4 d[kScanUnroll];
 #pragma unroll
-        for (int u = 0; u < kFilterUnroll; u++) {
-            int64_t v = v0 + (int64_t)u * kFilterThreads;
-            d[u] = (v < nvec) ? ldg_stream(base + v) : make_uint4(0, 0, 0, 0);
+        for (int u = 0; u < kScanUnroll; u++) {
+            const int64_t v = v0 + (int64_t)u * kScanThreads;
+            d[u] = (v < nvec) ? lds128(my_chunk + s * kScanStageBytes + u * kScanThreads * 16)
+                              : make_uint4(0, 0, 0, 0);
         }
-        uint32_t acc = 0;  // bit (4*kFilterUnroll - 1 - 4u - i) <-> word i of load u
+        uint32_t acc = 0;  // bit (4*kScanUnroll - 1 - 4u - i) <-> word i of chunk u
 #pragma unroll
-        for (int u = 0; u < kFilterUnroll; u++) {
+        for (int u = 0; u < kScanUnroll; u++) {
             acc = acc * 2u + tbl[hash_word(d[u].x)];
             acc = acc * 2u + tbl[hash_word(d[u].y)];
             acc = acc * 2u + tbl[hash_word(d[u].z)];
@@ -152,22 +186,29 @@ k_filter_sampled(const ScanParams p, int64_t nvec, int64_t ntiles) {
             const int src = __ffs(flagged) - 1;
             flagged &= flagged - 1;
             const uint32_t a = __shfl_sync(0xFFFFFFFFu, acc, src);
-            const int64_t vsrc = t * kTileVecs + (threadIdx.x - lane + src);
+            const int64_t vsrc = t * kScanVecs + (threadIdx.x - lane + src);
 #pragma unroll
-            for (int u = 0; u < kFilterUnroll; u++) {
-                if ((a >> (4 * (kFilterUnroll - 1 - u))) & 0xFu) {  // uniform
-                    const int64_t off = (vsrc + (int64_t)u * kFilterThreads) * 16;
+            for (int u = 0; u < kScanUnroll; u++) {
+                if ((a >> (4 * (kScanUnroll - 1 - u))) & 0xFu) {  // uniform
+                    const int64_t off = (vsrc + (int64_t)u * kScanThreads) * 16;
                     const uint32_t wx = __shfl_sync(0xFFFFFFFFu, d[u].x, src);
                     const uint32_t wy = __shfl_sync(0xFFFFFFFFu, d[u].y, src);
                     const uint32_t wz = __shfl_sync(0xFFFFFFFFu, d[u].z, src);
                     const uint32_t ww = __shfl_sync(0xFFFFFFFFu, d[u].w, src);
-                    const uint32_t nib = a >> (4 * (kFilterUnroll - 1 - u));
+                    const uint32_t nib = a >> (4 * (kScanUnroll - 1 - u));
                     if (nib & 8u) confirm_word(p, grams, ngr, lane, wx, off);
                     if (nib & 4u) confirm_word(p, grams, ngr, lane, wy, off + 4);
                     if (nib & 2u) confirm_word(p, grams, ngr, lane, wz, off + 8);
                     if (nib & 1u) confirm_word(p, grams, ngr, lane, ww, off + 12);
                 }
             }
+        }
+        __syncthreads();  // every thread is done with stage s
+        if (threadIdx.x == 0 && t + (int64_t)kScanStages * gridDim.x < ntiles)
+            issue(t + (int64_t)kScanStages * gridDim.x, s);
+        if (++s == kScanStages) {
+            s = 0;
+            parity ^= 1u;
         }
     }
 }
