@@ -10,14 +10,15 @@ Every search runs as hand-written CUDA kernels behind the C-ABI of libfuzzb200.s
 """
 __version__ = "0.1.0"
 
-__all__ = ["find_near_matches", "find_near_matches_batch", "find_near_matches_in_each", "find_near_matches_in_file",
+__all__ = ["find_near_matches", "find_near_matches_batch", "find_near_matches_in_each",
+           "find_near_matches_batch_in_each", "find_near_matches_in_file",
            "has_near_match", "Match", "LevenshteinSearchParams", "DeviceSequence", "DeviceSequenceSet", "ExactSearch", "SubstitutionsOnlySearch", "LevenshteinSearch",
            "GenericSearch", "choose_search_class", "search_exact"]
 
 from .common import LevenshteinSearchParams, Match
 from .search import (DeviceSequence, ExactSearch, GenericSearch, LevenshteinSearch,
                      SubstitutionsOnlySearch, search_exact)
-from .sequence_set import DeviceSequenceSet, find_near_matches_in_each
+from .sequence_set import DeviceSequenceSet, find_near_matches_batch_in_each, find_near_matches_in_each
 
 
 def find_near_matches(subsequence, sequence, max_substitutions=None, max_insertions=None,
@@ -60,7 +61,27 @@ def find_near_matches_batch(subsequences, sequence, max_l_dist=None, *, max_subs
     for p, s, i, d, l in zip(subsequences, ...)]``: exact and Levenshtein searches share passes over the
     sequence (fzb_search_levenshtein_batch), substitutions-only searches too (fzb_search_hamming_batch), and so do
     searches with other (generic) limits (fzb_search_generic_batch); all of them use the same uploaded sequence."""
-    from . import _native
+    subsequences, limits, params, classes = _batch_params(subsequences, max_substitutions, max_insertions,
+                                                          max_deletions, max_l_dist)
+    if not subsequences:
+        return []
+    from .search import AlphabetTooLarge, _lock_for, _prepare_many
+    with _lock_for(sequence):
+        try:
+            pats, hay, slicer = _prepare_many(subsequences, sequence)
+        except AlphabetTooLarge:
+            # wide symbols and more than 255 distinct ones over all the patterns: no common byte alphabet,
+            # so the patterns go one by one (each reduces the sequence to its own alphabet)
+            return [find_near_matches(p, sequence, *lim) for p, lim in zip(subsequences, limits)]
+        out = []
+        for s, e, d in _search_batch(hay, pats, params, classes, 0):
+            out.append([Match(a, b, c, matched=slicer(a, b)) for a, b, c in zip(s.tolist(), e.tolist(), d.tolist())])
+    return out
+
+
+def _batch_params(subsequences, max_substitutions, max_insertions, max_deletions, max_l_dist):
+    """The limits of a batch call, each None, one int or one value per pattern, validated as find_near_matches
+    validates them, before anything is uploaded: -> (patterns, limit tuples, LevenshteinSearchParams, classes)."""
     subsequences = list(subsequences)
     n = len(subsequences)
 
@@ -86,43 +107,45 @@ def find_near_matches_batch(subsequences, sequence, max_l_dist=None, *, max_subs
             raise ValueError("subsequence must not be empty" if cls is ExactSearch else "Given subsequence is empty!")
         params.append(sp)
         classes.append(cls)
-    if not subsequences:
-        return []
-    from .search import AlphabetTooLarge, _lock_for, _prepare_many
-    with _lock_for(sequence):
-        try:
-            pats, hay, slicer = _prepare_many(subsequences, sequence)
-        except AlphabetTooLarge:
-            # wide symbols and more than 255 distinct ones over all the patterns: no common byte alphabet,
-            # so the patterns go one by one (each reduces the sequence to its own alphabet)
-            return [find_near_matches(p, sequence, *lim) for p, lim in zip(subsequences, limits)]
-        results = [None] * n
-        lev = [i for i in range(n) if classes[i] in (ExactSearch, LevenshteinSearch)]
-        ham = [i for i in range(n) if classes[i] is SubstitutionsOnlySearch]
+    return subsequences, limits, params, classes
+
+
+def _search_batch(hay, pats, params, classes, flags):
+    """The patterns `pats` (bound to the handle `hay`) searched by class: exact and Levenshtein patterns in one
+    Levenshtein batch, substitutions-only ones in one Hamming batch, generic ones in one generic batch (a lone
+    generic pattern on its own).  -> per pattern, its (start, end, dist) arrays in the list find_near_matches
+    returns.  The caller holds the handle's lock."""
+    from . import _native
+    n = len(pats)
+    results = [None] * n
+    lev = [i for i in range(n) if classes[i] in (ExactSearch, LevenshteinSearch)]
+    ham = [i for i in range(n) if classes[i] is SubstitutionsOnlySearch]
+    gen = [i for i in range(n) if classes[i] is GenericSearch]
+    try:
         if lev:
-            rs, _ = hay.search_levenshtein_batch([pats[i] for i in lev], [params[i].max_l_dist for i in lev])
+            rs, _ = hay.search_levenshtein_batch([pats[i] for i in lev], [params[i].max_l_dist for i in lev], flags)
             for i, r in zip(lev, rs):
                 results[i] = r
         if ham:  # the limit SubstitutionsOnlySearch.search applies
             ks = [min(x for x in (params[i].max_l_dist, params[i].max_substitutions) if x is not None) for i in ham]
-            rs, _ = hay.search_hamming_batch([pats[i] for i in ham], ks)
+            rs, _ = hay.search_hamming_batch([pats[i] for i in ham], ks, flags)
             for i, r in zip(ham, rs):
                 results[i] = r
-        gen = [i for i in range(n) if classes[i] is GenericSearch]
-        if len(gen) == 1:  # (nothing to share)
+        if len(gen) == 1:  # (nothing to share; the single search needs no flag to honour a record set)
             results[gen[0]] = hay.search_generic(pats[gen[0]], *params[gen[0]].unpacked)
         elif gen:  # the normalised limits GenericSearch.search applies
-            rs, _ = hay.search_generic_batch([pats[i] for i in gen], *zip(*[params[i].unpacked for i in gen]))
+            rs, _ = hay.search_generic_batch([pats[i] for i in gen], *zip(*[params[i].unpacked for i in gen]),
+                                             flags=flags)
             for i, r in zip(gen, rs):
                 results[i] = r
-        out = []
-        for res, cls in zip(results, classes):
-            # ExactSearch does not consolidate (search_exact.py:80-89): its list is the RAW stream of the k == 0
-            # route; the Hamming results have FINAL == RAW
-            s, e, d = res.arrays(_native.RAW if cls is ExactSearch else _native.FINAL)
-            out.append([Match(a, b, c, matched=slicer(a, b)) for a, b, c in zip(s.tolist(), e.tolist(), d.tolist())])
-            res.close()
-    return out
+        # ExactSearch does not consolidate (search_exact.py:80-89): its list is the RAW stream of the k == 0
+        # route; the Hamming results have FINAL == RAW
+        return [res.arrays(_native.RAW if cls is ExactSearch else _native.FINAL)
+                for res, cls in zip(results, classes)]
+    finally:
+        for res in results:
+            if res is not None:
+                res.close()
 
 
 def choose_search_class(search_params):

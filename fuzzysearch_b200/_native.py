@@ -20,6 +20,7 @@ FZB_MAX_PATTERN = 255
 
 RAW, FINAL = 0, 1
 F_NO_FINAL, F_FORCE_DENSE, F_FORCE_LP, F_FORCE_NGRAMS, F_TINY_LIST, F_GLOBAL, F_FORCE_SAMPLED = 1, 2, 4, 8, 16, 32, 64
+F_PER_RECORD = 128  # batches on a handle with a record set: per-record results (DESIGN.md section 5.11)
 
 ROUTE_NAMES = {7: "batch", 0: "exact", 1: "ngrams/sampled-filter", 2: "ngrams/dense-filter", 3: "lp",
                4: "hamming", 5: "generic-ngrams", 6: "generic-lp", 8: "hamming/batch-scan",

@@ -820,6 +820,13 @@ static int refuse_records(const fzb_haystack *h, const char *what) {
     return h && h->recs ? fail(FZB_E_UNSUPPORTED, "%s does not support record sets", what) : FZB_OK;
 }
 
+// The batches take a record set only when the caller asks for per-record results (FZB_F_PER_RECORD), so that a handle
+// passed by accident does not silently change what a batch means; the flag without a record set is an error.
+static int check_batch_records(const fzb_haystack *h, uint32_t flags) {
+    if (!(flags & FZB_F_PER_RECORD)) return refuse_records(h, "a batch search without FZB_F_PER_RECORD");
+    return h->recs ? FZB_OK : fail(FZB_E_INVALID, "FZB_F_PER_RECORD needs a handle with a record set");
+}
+
 extern "C" void *fzb_host_alloc(uint64_t n) {
     void *p = nullptr;
     if (cudaHostAlloc(&p, n ? n : 1, cudaHostAllocDefault) != cudaSuccess) {
@@ -2244,6 +2251,7 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
     std::vector<RawRec> raw;
     uint32_t cnts[CNT_COUNT];
     fzb_stats pass{};
+    const RecSet rs = rec_set(h);  // (the filters only look at content: only the verify kernels take it)
     rc = run_batch_pass(h, [&]() -> int {
         MdenseParams dp{mp, b.d_bpats.get(), h->d_mhits.get(), hits_cap};
         if (ntiles > 0) {
@@ -2254,19 +2262,23 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
                 k_filter_multi<<<grid, kMultiThreads, kMultiSmem, h->stream>>>(mp, nvec, ntiles);
         }
         CK(cudaEventRecord(h->ev[1], h->stream));
-        if (glim && dense)
-            k_verify_mhits_generic<<<ggrid, kLpThreads, 0, h->stream>>>(dp, h->gbatch->d_glim.get(), h->d_scratch.get(),
-                                                                       kGenericBatchCap, h->d_out.get(), h->d_out.size(),
-                                                                       h->d_counters.get());
-        else if (glim)
-            k_verify_multi_generic<<<ggrid, kLpThreads, 0, h->stream>>>(mp, b.d_bpats.get(), h->gbatch->d_glim.get(),
-                                                                       h->d_scratch.get(), kGenericBatchCap, h->d_out.get(),
-                                                                       h->d_out.size(), h->d_counters.get());
-        else if (dense)
-            k_verify_mhits<<<h->sm_count * 8, kMhThreads, 0, h->stream>>>(dp, h->d_out.get(), h->d_out.size(), h->d_counters.get());
-        else
-            k_verify_multi<<<h->sm_count * 8, kVmThreads, 0, h->stream>>>(mp, b.d_bpats.get(), h->d_out.get(), h->d_out.size(),
-                                                                          h->d_counters.get());
+        with_recs(h, [&](auto rec) {
+            constexpr bool R = decltype(rec)::value;
+            if (glim && dense)
+                k_verify_mhits_generic<R><<<ggrid, kLpThreads, 0, h->stream>>>(
+                    dp, h->gbatch->d_glim.get(), h->d_scratch.get(), kGenericBatchCap, h->d_out.get(), h->d_out.size(),
+                    h->d_counters.get(), rs);
+            else if (glim)
+                k_verify_multi_generic<R><<<ggrid, kLpThreads, 0, h->stream>>>(
+                    mp, b.d_bpats.get(), h->gbatch->d_glim.get(), h->d_scratch.get(), kGenericBatchCap, h->d_out.get(),
+                    h->d_out.size(), h->d_counters.get(), rs);
+            else if (dense)
+                k_verify_mhits<R><<<h->sm_count * 8, kMhThreads, 0, h->stream>>>(dp, h->d_out.get(), h->d_out.size(),
+                                                                                    h->d_counters.get(), rs);
+            else
+                k_verify_multi<R><<<h->sm_count * 8, kVmThreads, 0, h->stream>>>(
+                    mp, b.d_bpats.get(), h->d_out.get(), h->d_out.size(), h->d_counters.get(), rs);
+        });
         CK(cudaGetLastError());
         return FZB_OK;
     }, raw, cnts, pass);
@@ -2360,6 +2372,7 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
     std::vector<RawRec> raw;
     uint32_t cnts[CNT_COUNT];
     fzb_stats pass{};
+    const RecSet rs = rec_set(h);  // (verify kernels only)
     float scan_ms = 0.f;
     uint64_t n_work = 0;
     int rc = run_batch_pass(h, [&]() -> int {
@@ -2378,17 +2391,21 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
             k_lm_refine<<<h->sm_count * 8, kLmSortThreads, 0, h->stream>>>(lp, lb.d_lmkept.get(), lb.d_lmhist.get());
             k_lm_scatter<<<h->sm_count * 8, kLmSortThreads, 0, h->stream>>>(lb.d_lmkept.get(), lb.d_lmhist.get(),
                                                                               lb.d_lmhist.get() + 128, lb.d_lmlist.get());
-            if (glim)
-                k_lp_verify_multi_generic<<<vgrid, kLpThreads, 0, h->stream>>>(lp, h->gbatch->d_glim.get(), lb.d_lmlist.get(),
-                                                                               lb.d_lmhist.get(), h->d_scratch.get(),
-                                                                               kGenericBatchCap, h->d_out.get(),
-                                                                               h->d_out.size(), h->d_counters.get());
-            else if (kmax <= 4)
-                k_lp_verify_multi<4><<<vgrid, kLpThreads, 0, h->stream>>>(lp, lb.d_lmlist.get(), lb.d_lmhist.get(), h->d_scratch.get(),
-                                                                          sim_cap, h->d_out.get(), h->d_out.size(), h->d_counters.get());
-            else
-                k_lp_verify_multi<8><<<vgrid, kLpThreads, 0, h->stream>>>(lp, lb.d_lmlist.get(), lb.d_lmhist.get(), h->d_scratch.get(),
-                                                                          sim_cap, h->d_out.get(), h->d_out.size(), h->d_counters.get());
+            with_recs(h, [&](auto rec) {
+                constexpr bool R = decltype(rec)::value;
+                if (glim)
+                    k_lp_verify_multi_generic<R><<<vgrid, kLpThreads, 0, h->stream>>>(
+                        lp, h->gbatch->d_glim.get(), lb.d_lmlist.get(), lb.d_lmhist.get(), h->d_scratch.get(),
+                        kGenericBatchCap, h->d_out.get(), h->d_out.size(), h->d_counters.get(), rs);
+                else if (kmax <= 4)
+                    k_lp_verify_multi<4, R><<<vgrid, kLpThreads, 0, h->stream>>>(
+                        lp, lb.d_lmlist.get(), lb.d_lmhist.get(), h->d_scratch.get(), sim_cap, h->d_out.get(),
+                        h->d_out.size(), h->d_counters.get(), rs);
+                else
+                    k_lp_verify_multi<8, R><<<vgrid, kLpThreads, 0, h->stream>>>(
+                        lp, lb.d_lmlist.get(), lb.d_lmhist.get(), h->d_scratch.get(), sim_cap, h->d_out.get(),
+                        h->d_out.size(), h->d_counters.get(), rs);
+            });
             CK(cudaGetLastError());
             const int r2 = read_counters(h, cnts);
             if (r2) return r2;
@@ -2428,16 +2445,16 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
     HandleLock handle_lock(h);
     if (!h || !out || (count && (!patterns || !offsets || !max_l_dist))) return fail(FZB_E_INVALID, "NULL argument");
     for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
-    TRY(refuse_records(h, "a batch search"));
+    TRY(check_batch_records(h, flags));
     for (uint32_t i = 0; i < count; i++)
         if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
     fzb_stats sum{};
     auto settle = [&](int rc, const std::vector<uint32_t> &ids) { return settle_pass(rc, ids, out, count); };
     // patterns the shared scan can take: n-gram route, q-sample lemma holds, 4-grams selective on this haystack,
     // short enough for the 64-bit match table; no special flags (forced routes, raw-only, multi-GPU reduction) other
-    // than FZB_F_TINY_LIST, which shrinks the capacities of the shared passes
+    // than FZB_F_TINY_LIST, which shrinks the capacities of the shared passes, and FZB_F_PER_RECORD
     const bool tiny = (flags & FZB_F_TINY_LIST) != 0;
-    const bool share = (flags & ~FZB_F_TINY_LIST) == 0 && h->buf_len > 0;
+    const bool share = (flags & ~(FZB_F_TINY_LIST | FZB_F_PER_RECORD)) == 0 && h->buf_len > 0;
     std::vector<uint32_t> shared;
     if (share) {
         for (uint32_t i = 0; i < count; i++) {
@@ -2511,8 +2528,9 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
     }
     for (uint32_t i = 0; i < count; i++) {
         if (out[i]) continue;
+        // (the single search honours a record set by itself)
         const int rc = settle(fzb_search_levenshtein(h, patterns + offsets[i], offsets[i + 1] - offsets[i],
-                                                     max_l_dist[i], flags, &out[i]), {});
+                                                     max_l_dist[i], flags & ~FZB_F_PER_RECORD, &out[i]), {});
         if (rc) return rc;
         add_stats(&sum, out[i]->stats);
     }
@@ -2803,7 +2821,12 @@ static int batch_pass_ham(fzb_haystack *h, const uint8_t *patterns, const uint32
     hp.mp.bits2 = two_bit ? nullptr : h->batch->d_mbits.get() + kMultiTblWords;
     hp.pats = h->batch->d_bpats.get();
     const size_t smem = two_bit ? kHbSmem2 : kMultiSmem;
-    const void *fn = two_bit ? (const void *)k_ham_batch_scan<true> : (const void *)k_ham_batch_scan<false>;
+    const RecSet rs = rec_set(h);  // (the key and table tests only look at content: only the verification takes it)
+    const void *fn = nullptr;
+    with_recs(h, [&](auto rec) {
+        constexpr bool R = decltype(rec)::value;
+        fn = two_bit ? (const void *)k_ham_batch_scan<true, R> : (const void *)k_ham_batch_scan<false, R>;
+    });
     CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 1;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kMultiThreads, smem));
@@ -2818,10 +2841,13 @@ static int batch_pass_ham(fzb_haystack *h, const uint8_t *patterns, const uint32
         hp.cap = h->d_out.size();
         if (ntiles > 0) {
             const int grid = (int)std::min<int64_t>(ntiles, (int64_t)h->sm_count * per_sm);
-            if (two_bit)
-                k_ham_batch_scan<true><<<grid, kMultiThreads, smem, h->stream>>>(hp, nvec, ntiles);
-            else
-                k_ham_batch_scan<false><<<grid, kMultiThreads, smem, h->stream>>>(hp, nvec, ntiles);
+            with_recs(h, [&](auto rec) {
+                constexpr bool R = decltype(rec)::value;
+                if (two_bit)
+                    k_ham_batch_scan<true, R><<<grid, kMultiThreads, smem, h->stream>>>(hp, nvec, ntiles, rs);
+                else
+                    k_ham_batch_scan<false, R><<<grid, kMultiThreads, smem, h->stream>>>(hp, nvec, ntiles, rs);
+            });
         }
         CK(cudaGetLastError());
         return FZB_OK;
@@ -2841,7 +2867,7 @@ extern "C" int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns
     HandleLock handle_lock(h);
     if (!h || !out || (count && (!patterns || !offsets || !max_subs))) return fail(FZB_E_INVALID, "NULL argument");
     for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
-    TRY(refuse_records(h, "a batch search"));
+    TRY(check_batch_records(h, flags));
     for (uint32_t i = 0; i < count; i++)
         if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
     // a pattern the single search refuses fails the whole call, with the single search's error, before any work
@@ -2853,9 +2879,11 @@ extern "C" int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns
     }
     fzb_stats sum{};
     auto settle = [&](int rc, const std::vector<uint32_t> &ids) { return settle_pass(rc, ids, out, count); };
-    // the shared scan takes no flags other than FZB_F_TINY_LIST (forced routes, multi-GPU reduction: one by one)
+    // the shared scan takes no flags other than FZB_F_TINY_LIST and FZB_F_PER_RECORD (forced routes, multi-GPU
+    // reduction: one by one)
     const bool tiny = (flags & FZB_F_TINY_LIST) != 0;
-    if ((flags & ~FZB_F_TINY_LIST) == 0 && h->buf_len > 0 && count >= 2 && sample_collision_prob(h) == FZB_OK) {
+    if ((flags & ~(FZB_F_TINY_LIST | FZB_F_PER_RECORD)) == 0 && h->buf_len > 0 && count >= 2 &&
+        sample_collision_prob(h) == FZB_OK) {
         const bool two_bit = h->coll_prob >= 0.15;  // the boundary of k_filter_dense2
         std::vector<uint32_t> ids;
         uint32_t key = 0;
@@ -2893,7 +2921,7 @@ extern "C" int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns
     for (uint32_t i = 0; i < count; i++) {
         if (out[i]) continue;
         const int rc = settle(fzb_search_hamming(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_subs[i],
-                                                 flags, &out[i]), {});
+                                                 flags & ~FZB_F_PER_RECORD, &out[i]), {});
         if (rc) return rc;
         add_stats(&sum, out[i]->stats);
     }
@@ -2925,7 +2953,7 @@ extern "C" int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns
     if (!h || !out || (count && (!patterns || !offsets || !max_subs || !max_ins || !max_dels || !max_l_dist)))
         return fail(FZB_E_INVALID, "NULL argument");
     for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
-    TRY(refuse_records(h, "a batch search"));
+    TRY(check_batch_records(h, flags));
     for (uint32_t i = 0; i < count; i++)
         if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
     // Per pattern, as fzb_search_generic would search it: the route, the total limit it works with (the LP route
@@ -2957,10 +2985,11 @@ extern "C" int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns
     }
     fzb_stats sum{};
     auto settle = [&](int rc, const std::vector<uint32_t> &ids) { return settle_pass(rc, ids, out, count); };
-    // the shared scans take no flags other than FZB_F_TINY_LIST (forced routes, raw-only, multi-GPU reduction: one by
-    // one), no exact-route pattern (max_l_dist == 0) and no pattern longer than a BatchPat holds
+    // the shared scans take no flags other than FZB_F_TINY_LIST and FZB_F_PER_RECORD (forced routes, raw-only,
+    // multi-GPU reduction: one by one), no exact-route pattern (max_l_dist == 0) and no pattern longer than a BatchPat
+    // holds
     const bool tiny = (flags & FZB_F_TINY_LIST) != 0;
-    const bool share = (flags & ~FZB_F_TINY_LIST) == 0 && h->buf_len > 0;
+    const bool share = (flags & ~(FZB_F_TINY_LIST | FZB_F_PER_RECORD)) == 0 && h->buf_len > 0;
     auto shareable = [&](uint32_t i) {
         const uint32_t m = offsets[i + 1] - offsets[i];
         return share && !out[i] && max_l_dist[i] > 0 && m <= (uint32_t)kBatchMaxM;
@@ -3030,7 +3059,8 @@ extern "C" int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns
     for (uint32_t i = 0; i < count; i++) {
         if (out[i]) continue;
         const int rc = settle(fzb_search_generic(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_subs[i],
-                                                 max_ins[i], max_dels[i], max_l_dist[i], flags, &out[i]), {});
+                                                 max_ins[i], max_dels[i], max_l_dist[i], flags & ~FZB_F_PER_RECORD,
+                                                 &out[i]), {});
         if (rc) return rc;
         add_stats(&sum, out[i]->stats);
     }

@@ -286,8 +286,9 @@ k_filter_mdense(const __grid_constant__ MdenseParams p, int64_t nvec, int64_t nt
 constexpr int kMhThreads = 128;
 constexpr int kMhSlotBytes = 160;  // per-lane window slot: m + 2k + alignment slack (m <= 64, m + 2k + 8 <= 160)
 
+template <bool REC>
 __global__ void __launch_bounds__(kMhThreads)
-k_verify_mhits(const __grid_constant__ MdenseParams p, RawRec *out, uint32_t cap, uint32_t *counters) {
+k_verify_mhits(const __grid_constant__ MdenseParams p, RawRec *out, uint32_t cap, uint32_t *counters, const RecSet rs) {
     __shared__ __align__(16) uint8_t slots[kMhThreads][kMhSlotBytes];
     __shared__ __align__(16) uint8_t pats[kMhThreads][kBatchMaxM];
     const uint32_t nhits = counters[CNT_MHITS];
@@ -304,7 +305,7 @@ k_verify_mhits(const __grid_constant__ MdenseParams p, RawRec *out, uint32_t cap
         base = __shfl_sync(0xFFFFFFFFu, base, 0);
         if (base >= nhits) break;
         const uint32_t item = base + lane;
-        const bool valid = item < nhits;
+        bool valid = item < nhits;
         VerifyCtx c;
         c.H = p.mp.H;
         c.buf_lo = p.mp.buf_lo;
@@ -315,7 +316,7 @@ k_verify_mhits(const __grid_constant__ MdenseParams p, RawRec *out, uint32_t cap
         c.m = c.k = 1;
         c.L = 1;
         c.n_ngrams = 1;
-        int64_t idx = 0, alo = 0;
+        int64_t idx = 0, alo = 0, lo = 0, hi = 0;
         int j = 0, tag = 0;
         if (valid) {
             const unsigned long long hv = p.hits[item];
@@ -330,9 +331,15 @@ k_verify_mhits(const __grid_constant__ MdenseParams p, RawRec *out, uint32_t cap
             c.n_ngrams = bp->n_ngrams;
             for (int w = 0; w < kBatchMaxM / 4; w++)
                 reinterpret_cast<uint32_t *>(myP)[w] = __ldg(reinterpret_cast<const uint32_t *>(bp->P) + w);
-            alo = stage_lane_window(c, idx - (int64_t)j * c.L, slot);
+            if constexpr (REC) {  // the hit's own record; a hit on a separator is dropped
+                valid = rec_bounds(rs, idx, lo, hi);
+                if (valid) alo = stage_lane_window(c, idx - (int64_t)j * c.L, slot, lo, hi);
+            } else {
+                alo = stage_lane_window(c, idx - (int64_t)j * c.L, slot);
+            }
         }
-        verify_anchor_lev<3>(c, myP, nullptr, slot - alo, idx, valid, nullptr, out, cap, counters, j, j + 1, tag);
+        verify_anchor_lev<3, REC>(c, myP, nullptr, slot - alo, idx, valid, nullptr, out, cap, counters, j, j + 1, tag,
+                                  lo, hi);
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&counters[CNT_CAND], nhits);
 }
@@ -555,10 +562,11 @@ struct LpLaneCtx {  // what sim_lev_lp needs
 // step for (almost) all lanes.  An accepting lane runs the literal simulation (rare) and goes back to the pool.
 enum { CNT_LMNEXT = 10 };
 
-template <int K>
+// REC: c.N is the end of the survivor's own record, and a start on a separator opens nothing (as in k_lp_verify).
+template <int K, bool REC>
 __global__ void __launch_bounds__(kLpThreads)
 k_lp_verify_multi(const __grid_constant__ LpMultiParams p, const unsigned long long *sorted, const uint32_t *hist,
-                  uint32_t *scratch, int cap, RawRec *out, uint32_t ocap, uint32_t *counters) {
+                  uint32_t *scratch, int cap, RawRec *out, uint32_t ocap, uint32_t *counters, const RecSet rs) {
     __shared__ __align__(4) uint8_t sPat[kLpThreads][kBatchMaxM / 2];  // LP patterns are at most 31 bytes
     if (counters[CNT_LMLIST] > p.list_cap) {  // the scan's list overflowed: the host searches these patterns one by one
         if (blockIdx.x == 0 && threadIdx.x == 0) counters[CNT_LMWORK] = 1;
@@ -610,6 +618,10 @@ k_lp_verify_multi(const __grid_constant__ LpMultiParams p, const unsigned long l
                             j0 = j;
                             break;
                         }
+                    if constexpr (REC) {
+                        int64_t lo;
+                        if (!rec_bounds(rs, st, lo, c.N)) j0 = -1;
+                    }
                     if (j0 >= 0) {
                         if (j0 + 1 == c.m) {
                             accept = true;  // :78-79
@@ -625,12 +637,12 @@ k_lp_verify_multi(const __grid_constant__ LpMultiParams p, const unsigned long l
         }
         if (__all_sync(0xFFFFFFFFu, drained && !have && !accept)) break;
         if (have) {  // one character
-            if (i >= p.N) {
+            if (i >= (REC ? c.N : p.N)) {
                 accept = lp_nfa_end<K>(R, c.m, c.k);
                 have = false;
             } else {
                 bool alive = true;
-                if (lp_nfa_step<K>(R, __ldg(pm + W[i]), i + 1 < p.N, c.m, c.k, alive)) {
+                if (lp_nfa_step<K>(R, __ldg(pm + W[i]), i + 1 < (REC ? c.N : p.N), c.m, c.k, alive)) {
                     accept = true;
                     have = false;
                 } else if (!alive) {
@@ -649,8 +661,13 @@ k_lp_verify_multi(const __grid_constant__ LpMultiParams p, const unsigned long l
 
 constexpr int kVmThreads = 128;
 
+// REC (here and in the other batch verify kernels): the handle holds a record set `rs` (DESIGN.md section 5.11); each
+// anchor or start is verified inside its own record, as the single-pattern kernels do.  The REC == false
+// instantiations never read rs.
+template <bool REC>
 __global__ void __launch_bounds__(kVmThreads)
-k_verify_multi(const __grid_constant__ MultiParams p, const BatchPat *pats, RawRec *out, uint32_t cap, uint32_t *counters) {
+k_verify_multi(const __grid_constant__ MultiParams p, const BatchPat *pats, RawRec *out, uint32_t cap, uint32_t *counters,
+               const RecSet rs) {
     __shared__ __align__(8) uint8_t sPall[kVmThreads / 32][kBatchMaxM];
     __shared__ unsigned long long sPMall[kVmThreads / 32][256];
     __shared__ uint32_t sWinAll[kVmThreads / 32][kWinWords];
@@ -688,7 +705,8 @@ k_verify_multi(const __grid_constant__ MultiParams p, const BatchPat *pats, RawR
             __syncwarp();
             cur_pid = it.pid;
         }
-        verify_granule_lev<1>(c, sP, sPM, sWin, (int64_t)it.granule, lane, nullptr, out, cap, counters, (int)(it.pid << 8));
+        verify_granule_lev<1, REC>(c, sP, sPM, sWin, (int64_t)it.granule, lane, nullptr, out, cap, counters,
+                                   (int)(it.pid << 8), rs);
         if (lane == 0) p.set[it.slot] = 0ull;  // the set is empty again when the kernel ends
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&counters[CNT_CAND], nitems);

@@ -56,9 +56,12 @@ __device__ __forceinline__ void generic_ctx_pattern(GenericCtx &c, const BatchPa
     c.max_dels = (int)((g >> 16) & 0xFFu);
 }
 
+// REC (all three kernels): the handle holds a record set `rs`; every window and NFA run stays inside the record of
+// its anchor or start, as in the single generic search (k_verify_generic, k_generic_lp).  REC == false never reads rs.
+template <bool REC>
 __global__ void __launch_bounds__(kLpThreads, 1)
 k_verify_multi_generic(const __grid_constant__ MultiParams p, const BatchPat *pats, const uint32_t *glim,
-                       uint32_t *scratch, int cap, RawRec *out, uint32_t ocap, uint32_t *counters) {
+                       uint32_t *scratch, int cap, RawRec *out, uint32_t ocap, uint32_t *counters, const RecSet rs) {
     __shared__ __align__(8) uint8_t sPall[kLpThreads / 32][kBatchMaxM];
     __shared__ uint32_t sWinAll[kLpThreads / 32][kWinWords];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -84,7 +87,11 @@ k_verify_multi_generic(const __grid_constant__ MultiParams p, const BatchPat *pa
             __syncwarp();
             cur_pid = it.pid;
         }
-        verify_granule_generic(c, sP, sWin, (int64_t)it.granule, lane, A, B, cap, out, ocap, counters, (int)(it.pid << 8));
+        if constexpr (REC)
+            verify_granule_generic_rec(c, sP, sWin, (int64_t)it.granule, lane, A, B, cap, out, ocap, counters, rs,
+                                       (int)(it.pid << 8));
+        else
+            verify_granule_generic(c, sP, sWin, (int64_t)it.granule, lane, A, B, cap, out, ocap, counters, (int)(it.pid << 8));
         if (lane == 0) p.set[it.slot] = 0ull;  // the set is empty again when the kernel ends
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&counters[CNT_CAND], nitems);
@@ -94,9 +101,10 @@ k_verify_multi_generic(const __grid_constant__ MultiParams p, const BatchPat *pa
 // m + 2k + 6 bytes; the host admits a pattern when m + 2k + 8 <= kMhgSlotBytes.
 constexpr int kMhgSlotBytes = 128;
 
+template <bool REC>
 __global__ void __launch_bounds__(kLpThreads, 1)
 k_verify_mhits_generic(const __grid_constant__ MdenseParams p, const uint32_t *glim, uint32_t *scratch, int cap,
-                       RawRec *out, uint32_t ocap, uint32_t *counters) {
+                       RawRec *out, uint32_t ocap, uint32_t *counters, const RecSet rs) {
     __shared__ __align__(8) uint8_t sPall[kLpThreads / 32][kBatchMaxM];
     __shared__ uint32_t sWinAll[kLpThreads / 32][kMhgSlotBytes / 4];
     const uint32_t nhits = counters[CNT_MHITS];
@@ -125,16 +133,30 @@ k_verify_mhits_generic(const __grid_constant__ MdenseParams p, const uint32_t *g
         const BatchPat *bp = p.pats + pid;
         generic_ctx_pattern(c, bp, glim, pid);
         const int m = c.m, k = c.k, L = c.L, s = j * L;
-        // the search window of n-gram j (generic_search.py:223-227); the filter already checked the n-gram itself
-        int64_t ws = max((int64_t)0, (int64_t)(s - k));
-        int64_t we = min(N, N - m + s + L + k);
-        if (we <= ws) continue;
-        ws = max((int64_t)0, min(ws, N));
-        we = max(ws, min(we, N));
-        if (idx < ws || idx + L > we) continue;
-        const int64_t p0 = idx - s;
-        const int64_t wlo = max((int64_t)0, p0 - k);  // :231
-        const int64_t whi = min(N, p0 + m + k);
+        int64_t wlo, whi;
+        if constexpr (REC) {  // the same arithmetic with the hit's own record [lo, hi) for [0, N); a separator is dropped
+            int64_t lo, hi;
+            if (!rec_bounds(rs, idx, lo, hi)) continue;
+            int64_t ws = lo + max((int64_t)0, (int64_t)(s - k));
+            int64_t we = min(hi, hi - m + s + L + k);
+            if (we <= ws) continue;
+            ws = max(lo, min(ws, hi));
+            we = max(ws, min(we, hi));
+            if (idx < ws || idx + L > we) continue;
+            wlo = max(lo, idx - s - k);
+            whi = min(hi, idx - s + m + k);
+        } else {
+            // the search window of n-gram j (generic_search.py:223-227); the filter already checked the n-gram itself
+            int64_t ws = max((int64_t)0, (int64_t)(s - k));
+            int64_t we = min(N, N - m + s + L + k);
+            if (we <= ws) continue;
+            ws = max((int64_t)0, min(ws, N));
+            we = max(ws, min(we, N));
+            if (idx < ws || idx + L > we) continue;
+            const int64_t p0 = idx - s;
+            wlo = max((int64_t)0, p0 - k);  // :231
+            whi = min(N, p0 + m + k);
+        }
         const int64_t alo = max(wlo, mp.buf_lo) & ~(int64_t)3;  // buf_lo is a multiple of 16
         const int nwords = (int)((min(whi, mp.buf_lo + mp.buf_len) - alo + 3) >> 2);
         const uint32_t *src = reinterpret_cast<const uint32_t *>(mp.H + (alo - mp.buf_lo));
@@ -153,10 +175,11 @@ k_verify_mhits_generic(const __grid_constant__ MdenseParams p, const uint32_t *g
 // One survivor per lane; a lane that is done takes the next one (its own atomic on the work counter), so lanes whose
 // NFA dies early do not wait for the rest of the warp before they refill.  The survivors are grouped by pattern
 // (k_lm_scatter), so neighbouring lanes mostly run the same pattern.
+template <bool REC>
 __global__ void __launch_bounds__(kLpThreads, 1)
 k_lp_verify_multi_generic(const __grid_constant__ LpMultiParams p, const uint32_t *glim, const unsigned long long *sorted,
                           const uint32_t *hist, uint32_t *scratch, int cap, RawRec *out, uint32_t ocap,
-                          uint32_t *counters) {
+                          uint32_t *counters, const RecSet rs) {
     __shared__ __align__(4) uint8_t sPat[kLpThreads][kBatchMaxM / 2];  // LP patterns are at most 31 bytes
     if (counters[CNT_LMLIST] > p.list_cap) {  // the scan's list overflowed: the host searches these patterns one by one
         if (blockIdx.x == 0 && threadIdx.x == 0) counters[CNT_LMWORK] = 1;
@@ -183,7 +206,9 @@ k_lp_verify_multi_generic(const __grid_constant__ LpMultiParams p, const uint32_
             generic_ctx_pattern(c, bp, glim, pid);
             cur_pid = pid;
         }
-        if (!sim_generic(c, myP, W, st, p.N, A, B, cap, st, 1 | (int)(pid << 8), out, ocap, counters))
+        int64_t lo = 0, seq_end = p.N;
+        if (REC && !rec_bounds(rs, st, lo, seq_end)) continue;  // a separator is no start
+        if (!sim_generic(c, myP, W, st, seq_end, A, B, cap, st, 1 | (int)(pid << 8), out, ocap, counters))
             atomicExch(&counters[CNT_OVERFLOW], 1u);
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&counters[CNT_CAND], counters[CNT_LMLIST]);

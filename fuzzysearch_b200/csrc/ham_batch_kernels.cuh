@@ -43,8 +43,11 @@ __device__ __forceinline__ uint32_t hb_nonzero_nibble(uint32_t x) {
     return (((nz >> 7) * 0x00204081u) >> 21) & 0xFu;
 }
 
-// Position g (global) carries `key`: walk its postings, verify each candidate start; -> candidates verified
-__device__ __noinline__ uint32_t hb_confirm(const HamBatchParams &p, uint32_t key, int64_t g) {
+// Position g (global) carries `key`: walk its postings, verify each candidate start; -> candidates verified.
+// REC: `rs` is the record set (one argument, by value); a start is emitted only if its occurrence lies inside one record.  Without
+// records the pack is empty, so the call passes exactly the arguments it passed before record sets existed.
+template <bool REC, class... Rec>
+__device__ __noinline__ uint32_t hb_confirm(const HamBatchParams &p, uint32_t key, int64_t g, Rec... rs) {
     uint32_t n = 0;
     uint32_t slot = (key * kGramMul) & p.mp.gtab_mask;
     for (;;) {
@@ -84,6 +87,8 @@ __device__ __noinline__ uint32_t hb_confirm(const HamBatchParams &p, uint32_t ke
                 bool first_exact = true;
                 for (int q = 0; q < j; q++)
                     if (!(mm & (piece << (q * L)))) first_exact = false;  // an earlier piece emits this start
+                if constexpr (REC)
+                    if (first_exact) first_exact = ham_in_record<true>(rs..., st, m);
                 if (first_exact) emit(p.out, p.cap, p.mp.counters, st, st + m, st, nd, (int)(pid << 8), false);
             }
         }
@@ -91,9 +96,9 @@ __device__ __noinline__ uint32_t hb_confirm(const HamBatchParams &p, uint32_t ke
     }
 }
 
-template <bool TWO_BIT>
+template <bool TWO_BIT, bool REC>
 __global__ void __launch_bounds__(kMultiThreads, 1)
-k_ham_batch_scan(const __grid_constant__ HamBatchParams p, int64_t nvec, int64_t ntiles) {
+k_ham_batch_scan(const __grid_constant__ HamBatchParams p, int64_t nvec, int64_t ntiles, const RecSet rs) {
     extern __shared__ __align__(16) uint32_t hb_tbl[];
     __shared__ uint8_t sCode[256];
     constexpr int kWords = TWO_BIT ? kHbKeyWords : kMultiTblWords;
@@ -145,7 +150,10 @@ k_ham_batch_scan(const __grid_constant__ HamBatchParams p, int64_t nvec, int64_t
                     const uint32_t h2 = multi_hash2(key);
                     if (!((__ldg(p.mp.bits2 + (h2 >> 5)) >> (h2 & 31u)) & 1u)) continue;
                 }
-                cand += hb_confirm(p, key, p.mp.buf_lo + off + b);
+                if constexpr (REC)
+                    cand += hb_confirm<true>(p, key, p.mp.buf_lo + off + b, rs);
+                else
+                    cand += hb_confirm<false>(p, key, p.mp.buf_lo + off + b);
             }
         }
     }

@@ -617,11 +617,13 @@ __device__ __forceinline__ void verify_granule_generic(const PT &p, const uint8_
 }
 
 // The same for a record set `rs` (k_verify_generic<true>): per anchor, its own record is the sequence, the window
-// arithmetic of :223-226 and :231 taken relative to it and shifted back; anchors on separators are dropped.
-__device__ __forceinline__ void verify_granule_generic_rec(const ScanParams &p, const uint8_t *sP, uint32_t *sWin,
+// arithmetic of :223-226 and :231 taken relative to it and shifted back; anchors on separators are dropped.  PT and
+// `tag` as for verify_granule_generic (k_verify_multi_generic<true> passes its per-pattern context).
+template <class PT>
+__device__ __forceinline__ void verify_granule_generic_rec(const PT &p, const uint8_t *sP, uint32_t *sWin,
                                                            int64_t granule, int lane, uint32_t *A, uint32_t *B,
                                                            int cap, RawRec *out, uint32_t ocap, uint32_t *counters,
-                                                           const RecSet &rs) {
+                                                           const RecSet &rs, int tag = 0) {
     const int m = p.m, k = p.k, L = p.L;
     const int64_t gbase = p.buf_lo + (granule << kGranuleShift);
     const int64_t alo = stage_window(p, gbase, m + k, lane, sWin);
@@ -659,7 +661,7 @@ __device__ __forceinline__ void verify_granule_generic_rec(const ScanParams &p, 
                 const int64_t wlo = max((int64_t)__shfl_sync(0xFFFFFFFFu, lo, hl), p0 - k);  // the hit lane's record
                 const int64_t whi = min((int64_t)__shfl_sync(0xFFFFFFFFu, hi, hl), p0 + m + k);
                 for (int64_t st = wlo + lane; st < whi; st += 32)
-                    if (!sim_generic(p, sP, W, st, whi, A, B, cap, hidx, j, out, ocap, counters))
+                    if (!sim_generic(p, sP, W, st, whi, A, B, cap, hidx, j | tag, out, ocap, counters))
                         atomicExch(&counters[CNT_OVERFLOW], 1u);
             }
         }

@@ -12,7 +12,7 @@ from . import _native
 from .common import LevenshteinSearchParams, Match
 from .search import DeviceSequence, ExactSearch, GenericSearch, LevenshteinSearch, _kind, _text
 
-__all__ = ["DeviceSequenceSet", "find_near_matches_in_each"]
+__all__ = ["DeviceSequenceSet", "find_near_matches_in_each", "find_near_matches_batch_in_each"]
 
 
 def _set_kind(sequences):
@@ -63,13 +63,16 @@ class DeviceSequenceSet(object):
         return len(self._orig)
 
     def _bind(self, subsequence):
-        """-> the pattern in the resident set's byte alphabet; a re-reduction of a wide-symbol set (a new upload,
+        return self._bind_many([subsequence])[0]
+
+    def _bind_many(self, subsequences):
+        """-> the patterns in the resident set's byte alphabet; a re-reduction of a wide-symbol set (a new upload,
         which clears the record set) is followed by declaring the records again."""
-        pat = self._seq._bind(subsequence)
+        pats = self._seq._bind_many(subsequences)
         if self._seq._alphabet != self._bound_alphabet:
             self._seq.haystack.set_records(self.offsets)
             self._bound_alphabet = self._seq._alphabet
-        return pat
+        return pats
 
     def close(self):
         self._seq.close()
@@ -119,17 +122,70 @@ def _search_set(subsequence, seqset, cls, search_params):
             s, e, d = res.arrays(_native.RAW if cls is ExactSearch else _native.FINAL)
         finally:
             res.close()
+    out = [[] for _ in range(len(seqset))]
+    for i, matches in _split_by_record(seqset, s, e, d):
+        out[i] = matches
+    return out
+
+
+def _split_by_record(seqset, s, e, d):
+    """One search's list over the set (buffer coordinates) -> (sequence index, its Match list) for every sequence
+    that holds matches, in sequence order; positions relative to the sequence, `matched` sliced from it."""
     offsets = seqset.offsets.astype(np.int64)
     rec = np.searchsorted(offsets, s, side="right") - 1
     order = np.argsort(rec, kind="stable")  # each record's matches keep their order
     rec, s, e, d = rec[order], s[order], e[order], d[order]
     base = offsets[rec]
     s, e, d = (s - base).tolist(), (e - base).tolist(), d.tolist()
-    out = [[] for _ in range(len(seqset))]
     # only the records that hold matches are visited (most short sequences hold none)
     hit_recs, firsts = np.unique(rec, return_index=True)
     ends = np.append(firsts[1:], len(s))
     for i, lo, hi in zip(hit_recs.tolist(), firsts.tolist(), ends.tolist()):
         sl = _slicer(seqset._orig[i], seqset._kind)
-        out[i] = [Match(a, b, c, matched=sl(a, b)) for a, b, c in zip(s[lo:hi], e[lo:hi], d[lo:hi])]
-    return out
+        yield i, [Match(a, b, c, matched=sl(a, b)) for a, b, c in zip(s[lo:hi], e[lo:hi], d[lo:hi])]
+
+
+def find_near_matches_batch_in_each(subsequences, sequences, max_l_dist=None, *, max_substitutions=None,
+                                    max_insertions=None, max_deletions=None):
+    """Many patterns over many sequences: -> one dict per pattern, mapping the index of every sequence that holds
+    matches to its non-empty list, so that ``out[i].get(r, []) == find_near_matches(subsequences[i], sequences[r],
+    ...)``.  The limits are taken as find_near_matches_batch takes them (None, one int, or one value per pattern)
+    and validated before anything is uploaded.  `sequences` is a list / tuple (uploaded for this call) or a
+    DeviceSequenceSet (resident).  The patterns share passes over the whole set as in find_near_matches_batch
+    (fzb_search_*_batch with FZB_F_PER_RECORD, DESIGN.md section 5.11)."""
+    from . import _batch_params
+    subsequences, limits, params, classes = _batch_params(subsequences, max_substitutions, max_insertions,
+                                                          max_deletions, max_l_dist)
+    if not subsequences:
+        return []
+    if isinstance(sequences, DeviceSequenceSet):
+        return _search_set_batch(subsequences, sequences, limits, params, classes)
+    if not isinstance(sequences, (list, tuple)):
+        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
+    if not sequences:
+        return [{} for _ in subsequences]
+    seqset = DeviceSequenceSet(sequences)
+    try:
+        return _search_set_batch(subsequences, seqset, limits, params, classes)
+    finally:
+        seqset.close()
+
+
+def _search_set_batch(subsequences, seqset, limits, params, classes):
+    if len(seqset) == 0:
+        return [{} for _ in subsequences]
+    from . import _search_batch
+    from .search import AlphabetTooLarge
+    with seqset._lock:
+        try:
+            pats = seqset._bind_many(subsequences)
+        except AlphabetTooLarge:
+            # wide symbols and more than 255 distinct ones over all the patterns: no common byte alphabet, so the
+            # patterns go one by one (each reduces the set to its own alphabet)
+            pats = None
+        if pats is not None:
+            lists = _search_batch(seqset._seq.haystack, pats, params, classes, _native.F_PER_RECORD)
+    if pats is None:
+        return [dict((r, ms) for r, ms in enumerate(find_near_matches_in_each(p, seqset, *lim)) if ms)
+                for p, lim in zip(subsequences, limits)]
+    return [dict(_split_by_record(seqset, s, e, d)) for s, e, d in lists]

@@ -67,6 +67,9 @@ extern "C" {
                                  memory and merges the seams on the device, on the search's own stream, right
                                  behind the kernels (needs fzb_haystack_comm_init / fzb_comm_init_local on every
                                  rank; collective: every rank must issue the same searches in the same order) */
+#define FZB_F_PER_RECORD 128u /* batches: accept a handle that holds a record set (fzb_haystack_set_records) and
+                                 search every record of it; each out[i] is then what the single search of
+                                 pattern i returns on that handle.  Refused on a handle without a record set */
 
 struct fzb_stats_s;
 typedef struct fzb_haystack fzb_haystack; /* a device-resident sequence (or one shard of it) */
@@ -172,9 +175,10 @@ int fzb_haystack_upload_symbols(fzb_haystack *h, const void *host, uint64_t n, u
  * would return, in buffer coordinates: every window, start and end-of-sequence rule applies at record edges.
  * count == 0 (offsets may be NULL) removes the record set.
  * The record of a match (empty ones included) is the i with offsets[i] <= start < offsets[i+1].  A shard, malformed
- * offsets or count >= 2^32 are refused with FZB_E_INVALID; with a record set in place the batch searches,
- * fzb_has_near_match, fzb_search_exact_window and FZB_F_GLOBAL return FZB_E_UNSUPPORTED.  Every refusal leaves the
- * handle as it was.  Any fzb_haystack_upload* clears the record set; fzb_haystack_write keeps it. */
+ * offsets or count >= 2^32 are refused with FZB_E_INVALID; with a record set in place the batch searches return
+ * FZB_E_UNSUPPORTED unless called with FZB_F_PER_RECORD (then out[i] is the single search of pattern i on `h`, per
+ * record, and the shared scans still apply), and fzb_has_near_match, fzb_search_exact_window and FZB_F_GLOBAL
+ * return FZB_E_UNSUPPORTED.  Every refusal leaves the handle as it was.  Any fzb_haystack_upload* clears the record set; fzb_haystack_write keeps it. */
 int fzb_haystack_set_records(fzb_haystack *h, const uint64_t *offsets, uint64_t count);
 
 /* Page-locked host memory for fast host<->device copies (cudaHostAlloc); NULL on failure. */
@@ -224,6 +228,7 @@ int fzb_search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint
  * q-sample lemma covers, ONE for the other n-gram-route patterns, ONE per 64 LP-route patterns; patterns
  * longer than 64 bytes are searched one by one.  Each out[i] is exactly what fzb_search_levenshtein would
  * return for pattern i.  `total` (optional) sums the statistics.  On error nothing is returned.
+ * On a handle with a record set the three batches need FZB_F_PER_RECORD (DESIGN.md section 5.11).
  */
 int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
                                  const uint32_t *max_l_dist, uint32_t count, uint32_t flags,
@@ -236,7 +241,8 @@ int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patterns, const
  * scans (DESIGN.md section 5.8; their results report route 8); the others are searched one by one.
  * Each out[i] is exactly what fzb_search_hamming would return for pattern i (FINAL == RAW, ascending).
  * A pattern the single search refuses fails the whole call with its error; on error nothing is
- * returned.  Flags other than FZB_F_TINY_LIST send every pattern one by one with those flags.
+ * returned.  Flags other than FZB_F_TINY_LIST and FZB_F_PER_RECORD send every pattern one by one with those flags
+ * (FZB_F_PER_RECORD cleared).
  */
 int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
                              const uint32_t *max_subs, uint32_t count, uint32_t flags,
@@ -249,8 +255,8 @@ int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns, const uin
  * n-gram-prefix pass for the n-gram route (their results report route 9), passes of 64 patterns for the
  * LP route (route 10); the others are searched one by one.  Each out[i] is exactly what
  * fzb_search_generic would return for pattern i.  A pattern the single search refuses fails the whole
- * call with its error; on error nothing is returned.  Flags other than FZB_F_TINY_LIST send every
- * pattern one by one with those flags.
+ * call with its error; on error nothing is returned.  Flags other than FZB_F_TINY_LIST and FZB_F_PER_RECORD
+ * send every pattern one by one with those flags (FZB_F_PER_RECORD cleared).
  */
 int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
                              const uint32_t *max_subs, const uint32_t *max_ins, const uint32_t *max_dels,
