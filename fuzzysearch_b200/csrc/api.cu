@@ -2176,6 +2176,41 @@ static int prepare_generic_pass(fzb_haystack *h, const uint32_t *glim, const std
     return ensure_scratch(h, (uint64_t)grid * kLpThreads * 2 * kGenericBatchCap);
 }
 
+// The hit list of the dense passes (k_filter_mdense, k_filter_mdense2), taken by the handle only together with the
+// shared-memory attribute of k_filter_mdense.
+static int ensure_mhits(fzb_haystack *h) {
+    if (h->d_mhits) return FZB_OK;
+    DevBuf<unsigned long long> hits;
+    TRY(hits.alloc(1u << 23));
+    CK(cudaFuncSetAttribute(k_filter_mdense, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMdenseSmem));
+    h->d_mhits = std::move(hits);
+    return FZB_OK;
+}
+
+// 2-bit keys of a pass over a low-entropy haystack (k_ham_batch_scan<true>, k_filter_mdense2): the four most frequent
+// pattern bytes of the pass get codes 0..3, every other byte code 0 (DNA reduced from a wide str arrives as bytes
+// 1..4).  two_bit_key enters `post` under the key of the first min(L, 8) symbols at s, under every completion of
+// the remaining ones.
+static void two_bit_code(const uint8_t *patterns, const uint32_t *offsets, const std::vector<uint32_t> &ids,
+                         uint8_t code[256]) {
+    uint64_t freq[256] = {0};
+    for (uint32_t id : ids)
+        for (uint32_t b = offsets[id]; b < offsets[id + 1]; b++) freq[patterns[b]]++;
+    int order[256];
+    for (int c = 0; c < 256; c++) order[c] = c;
+    std::stable_sort(order, order + 256, [&](int a, int b) { return freq[a] > freq[b]; });
+    for (int c = 0; c < 256; c++) code[c] = 0;
+    for (int r = 0; r < 4; r++) code[order[r]] = (uint8_t)r;
+}
+
+static void two_bit_key(std::unordered_map<uint32_t, std::vector<uint32_t>> &keys, const uint8_t code[256],
+                        const uint8_t *s, uint32_t L, uint32_t post) {
+    const uint32_t n = std::min<uint32_t>(L, kHbKeySyms);
+    uint32_t key = 0;
+    for (uint32_t q = 0; q < n; q++) key |= (uint32_t)code[s[q]] << (2 * q);
+    for (uint32_t x = 0; x < (1u << (2 * (kHbKeySyms - n))); x++) keys[key | (x << (2 * n))].push_back(post);
+}
+
 // One pass over the haystack for the patterns ids[0..cnt): fills out[ids[i]].  Returns FZB_OK, an error, or +1 if
 // the pass overflowed a device structure (the caller then searches these patterns one by one).
 // dense = false: the q-sample scan (k_filter_multi / k_verify_multi) over the 4-grams of the patterns;
@@ -2230,12 +2265,7 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
         }
     });
     if (rc) return rc;
-    if (dense && !h->d_mhits) {  // taken by the handle only together with its kernel's attribute
-        DevBuf<unsigned long long> hits;
-        TRY(hits.alloc(1u << 23));
-        CK(cudaFuncSetAttribute(k_filter_mdense, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMdenseSmem));
-        h->d_mhits = std::move(hits);
-    }
+    if (dense) TRY(ensure_mhits(h));
     const int ggrid = h->sm_count * 4;  // generic verify kernels: as many lanes (and candidate lists) as run_lp's
     if (glim) TRY(prepare_generic_pass(h, glim, ids, ggrid));
     BatchBufs &b = *h->batch;
@@ -2425,6 +2455,129 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
     return split_batch(raw, ids, pass, 1, false, out, sum);
 }
 
+// Admission of n-gram-route Levenshtein patterns to the 2-bit pass (k_filter_mdense2 / k_verify_mhits) on
+// low-entropy haystacks: a pattern rides when its work in the pass costs less than its own search.  Per haystack
+// position it walks n_ngrams * max(c, 1/4)^min(L, 8) postings and verifies n_ngrams * c^L exact n-gram hits
+// (c: collision probability); its own search costs a fixed part, a read of the haystack and a verification per hit.
+// Measured on an H100 80GB HBM3 (700 W power limit) with tools/probe_dna_lev_batch.py (DESIGN.md section 5.12):
+// - in a pass of 1 024 patterns over 4 GiB of DNA: 0.53 ns of scan per posting walked (almost every posting is an
+//   exact hit there, so this includes the byte comparison and the append) and 0.31 ns per hit beyond the scans
+//   (verification and the host turnaround between chunks);
+// - alone: 1.98 ms + 0.29 ns per hit on 4 GiB (least squares over the 1 024 searches) and 0.196 ms per search on
+//   1.5e8 bytes of reads with few hits, i.e. 0.13 ms + 4.3e-4 ns per position.
+// So on 4 GiB a pattern with n-grams of 5 symbols costs more in the pass than alone (measured: 52 such patterns
+// added 773 ms to the pass against 296 ms searched alone), one with n-grams of 6 symbols less (93 ms against 136 ms).
+constexpr double kDnaLevPostNs = 0.53;
+constexpr double kDnaLevHitNs = 0.31;
+constexpr double kDnaLevAloneMs = 0.13;
+constexpr double kDnaLevAloneReadNs = 4.3e-4;
+constexpr double kDnaLevAloneHitNs = 0.29;
+// Not a cost bound: a pass closes at 4 expected hits per position, so that even a chunk of one 64 KiB tile expects at
+// most 2.6e5 hits, far inside the hit list.
+constexpr double kDnaLevPassHits = 4.0;
+constexpr uint32_t kDnaLevMinL = 5;    // n-grams of at least 5 symbols: at most 64 completions of a key
+
+static uint32_t dna_lev_postings(uint32_t m, uint32_t k) {
+    const uint32_t L = m / (k + 1);
+    return (m / L) << (2 * (kHbKeySyms - std::min<uint32_t>(L, kHbKeySyms)));
+}
+
+// expected hits per position of pattern (m, k); `rides` whether it costs less in a pass over `positions` than alone
+static double dna_lev_hits(const fzb_haystack *h, uint32_t m, uint32_t k, double positions, bool *rides) {
+    const uint32_t L = m / (k + 1), n = m / L;
+    const double c = h->coll_prob;
+    const double post = n * std::pow(std::max(c, 0.25), (double)std::min<uint32_t>(L, kHbKeySyms));
+    const double hits = n * std::pow(c, (double)L);
+    const double pass_ns = positions * (kDnaLevPostNs * post + kDnaLevHitNs * hits);
+    const double alone_ns = kDnaLevAloneMs * 1e6 + positions * (kDnaLevAloneReadNs + kDnaLevAloneHitNs * hits);
+    *rides = pass_ns < alone_ns;
+    return hits;
+}
+
+// One 2-bit n-gram pass (k_filter_mdense2 / k_verify_mhits) for the Levenshtein patterns ids[]; same return convention
+// as batch_pass.  The own range is scanned and verified in chunks whose expected hits (hits_per_pos per position)
+// fill at most half the hit list; an overflowing chunk sends the pass's patterns one by one.  tiny
+// (FZB_F_TINY_LIST): kTinyBatchCap hits and chunks of kTinyLpChunk positions.
+static int batch_pass_dna(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, const uint32_t *ks,
+                          const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, double hits_per_pos,
+                          bool tiny) {
+    const uint32_t cnt = (uint32_t)ids.size();
+    std::vector<BatchPat> pats(cnt);
+    std::vector<uint32_t> pinfo(cnt);
+    Mdense2Params p{};
+    two_bit_code(patterns, offsets, ids, p.code);
+    std::unordered_map<uint32_t, std::vector<uint32_t>> keys;  // key -> postings pattern << 8 | n-gram
+    keys.reserve(cnt * 64);
+    for (uint32_t i = 0; i < cnt; i++) {
+        const uint32_t id = ids[i], m = offsets[id + 1] - offsets[id], k = ks[id];
+        BatchPat &bp = pats[i];
+        memset(&bp, 0, sizeof bp);
+        memcpy(bp.P, patterns + offsets[id], m);
+        bp.m = (int)m;
+        bp.k = (int)k;
+        bp.L = (int)(m / (k + 1));
+        bp.n_ngrams = (int)m / bp.L;
+        pinfo[i] = m | (k << 8) | ((uint32_t)bp.L << 16);
+        for (int j = 0; j < bp.n_ngrams; j++) two_bit_key(keys, p.code, bp.P + j * bp.L, bp.L, (i << 8) | (uint32_t)j);
+    }
+    std::vector<uint32_t> bits(kHbKeyWords, 0);
+    int rc = upload_pass_tables(h, keys, bits, pinfo, pats, [&](uint32_t w) { bits[w >> 5] |= 1u << (w & 31u); });
+    if (rc) return rc;
+    TRY(ensure_mhits(h));
+    const uint32_t hits_cap = tiny ? std::min<uint32_t>(h->d_mhits.size(), kTinyBatchCap) : (uint32_t)h->d_mhits.size();
+    p.dp = MdenseParams{pass_params(h), h->batch->d_bpats.get(), h->d_mhits.get(), hits_cap};
+    const uint64_t tile = (uint64_t)kMultiTileVecs * 16;
+    const uint64_t chunk = tiny ? kTinyLpChunk
+                                : std::max(tile, (uint64_t)(hits_cap / 2 / std::max(hits_per_pos, 1e-9)) / tile * tile);
+    const int64_t nvec = (int64_t)(round_up(h->buf_len, 16) / 16);
+    std::vector<RawRec> raw;
+    uint32_t cnts[CNT_COUNT];
+    fzb_stats pass{};
+    const RecSet rs = rec_set(h);  // (verify kernel only)
+    float scan_ms = 0.f;
+    uint32_t nchunks = 0;
+    uint64_t n_hits = 0;  // (over all chunks: more than 2^32 on a large haystack)
+    rc = run_batch_pass(h, [&]() -> int {
+        scan_ms = 0.f;
+        nchunks = 0;
+        n_hits = 0;
+        for (uint64_t lo = h->own_lo; lo < h->own_hi; lo += chunk) {
+            p.scan_lo = (int64_t)lo;
+            p.scan_hi = (int64_t)std::min<uint64_t>(h->own_hi, lo + chunk);
+            const int64_t v0 = (p.scan_lo - (int64_t)h->buf_lo) / 16;
+            const int64_t v1 = (p.scan_hi - (int64_t)h->buf_lo + 15) / 16;
+            const int64_t ntiles = (v1 - v0 + kMultiTileVecs - 1) / kMultiTileVecs;
+            p.dp.mp.counters = h->d_counters.get();
+            CK(cudaMemsetAsync(h->d_counters.get() + CNT_MHITS, 0, 2 * sizeof(uint32_t), h->stream));  // list + work
+            CK(cudaEventRecord(h->ev[1], h->stream));
+            k_filter_mdense2<<<(int)std::min<int64_t>(ntiles, h->sm_count), kMultiThreads, kMdense2Smem, h->stream>>>(
+                p, nvec, v0, ntiles);
+            CK(cudaEventRecord(h->ev[2], h->stream));
+            with_recs(h, [&](auto rec) {
+                constexpr bool R = decltype(rec)::value;
+                k_verify_mhits<R><<<h->sm_count * 8, kMhThreads, 0, h->stream>>>(p.dp, h->d_out.get(), h->d_out.size(),
+                                                                                    h->d_counters.get(), rs);
+            });
+            CK(cudaGetLastError());
+            nchunks++;
+            const int r2 = read_counters(h, cnts);
+            if (r2) return r2;
+            float ms = 0.f;
+            cudaEventElapsedTime(&ms, h->ev[1], h->ev[2]);
+            scan_ms += ms;
+            n_hits += cnts[CNT_MHITS];
+            if (cnts[CNT_OVERFLOW]) return 1;  // the chunk's hits did not fit the list
+        }
+        return FZB_OK;
+    }, raw, cnts, pass);
+    if (rc) return rc;
+    pass.route = 2;
+    pass.filter_ms = scan_ms;
+    pass.n_candidates = n_hits;
+    pass.n_launches = 2 * nchunks;
+    return split_batch(raw, ids, pass, 0, false, out, sum);
+}
+
 // The outcome `rc` of a shared pass over the patterns ids[] of a batch of `count` results: an error drops every
 // result; an overflow (+1) drops the pass's results, leaving its patterns to the one-by-one path.
 static int settle_pass(int rc, const std::vector<uint32_t> &ids, fzb_result **out, uint32_t count) {
@@ -2524,6 +2677,46 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
         std::vector<uint32_t> ids(lp_ids.begin() + first, lp_ids.begin() + std::min(lp_ids.size(), first + 64));
         if (ids.size() < 2) break;
         const int rc = settle(batch_pass_lp(h, patterns, offsets, max_l_dist, ids, out, &sum, tiny), ids);
+        if (rc) return rc;
+    }
+    // on low-entropy haystacks (at the 0.15 boundary of k_filter_dense2) the n-gram-route patterns left over that cost
+    // less in a pass than alone share 2-bit n-gram scans (k_filter_mdense2), in passes bounded by hits and capacity
+    if (share && h->coll_prob >= 0.15) {
+        std::vector<uint32_t> ids;
+        const double positions = (double)(h->own_hi - h->own_lo);
+        double hits = 0.0;
+        uint64_t npost = 0;
+        auto run_pass = [&]() -> int {
+            const int rc = ids.size() >= 2 ? settle(batch_pass_dna(h, patterns, offsets, max_l_dist, ids, out, &sum, hits,
+                                                                   tiny), ids)
+                                           : FZB_OK;  // (a pass of one pattern is not worth it)
+            ids.clear();
+            hits = 0.0;
+            npost = 0;
+            return rc;
+        };
+        for (uint32_t i = 0; i < count; i++) {
+            if (out[i]) continue;
+            const uint32_t m = offsets[i + 1] - offsets[i], k = max_l_dist[i];
+            if (m == 0 || m > (uint32_t)kBatchMaxM || k == 0 || k >= m) continue;
+            const uint32_t L = m / (k + 1);
+            if (L < kDnaLevMinL || m - L > 32 || m + 2 * k + 12 > (uint32_t)kMhSlotBytes) continue;
+            if (check_halo(h, (uint64_t)m + k) != FZB_OK) continue;
+            if (sampled_filter_applies(m, k, 0) && sampled_is_selective(h, m, k, (int)L, (int)(m / L)))
+                continue;  // (its single search takes the sampled route: a q-sample pass that overflowed)
+            bool rides = false;
+            const double phits = dna_lev_hits(h, m, k, positions, &rides);
+            if (!rides || phits > kDnaLevPassHits) continue;
+            const uint32_t np = dna_lev_postings(m, k);
+            if (ids.size() == kMaxBatchPats || hits + phits > kDnaLevPassHits || npost + np > kMaxBatchGrams) {
+                const int rc = run_pass();
+                if (rc) return rc;
+            }
+            ids.push_back(i);
+            hits += phits;
+            npost += np;
+        }
+        const int rc = run_pass();
         if (rc) return rc;
     }
     for (uint32_t i = 0; i < count; i++) {
@@ -2772,15 +2965,7 @@ static int batch_pass_ham(fzb_haystack *h, const uint8_t *patterns, const uint32
     std::vector<uint32_t> pinfo(cnt);
     HamBatchParams hp{};
     hp.key_mask = key_bytes == 4 ? 0xFFFFFFFFu : 0x00FFFFFFu;
-    if (two_bit) {  // the four most frequent pattern bytes of the pass get codes 0..3, every other byte code 0
-        uint64_t freq[256] = {0};
-        for (uint32_t id : ids)
-            for (uint32_t b = offsets[id]; b < offsets[id + 1]; b++) freq[patterns[b]]++;
-        int order[256];
-        for (int c = 0; c < 256; c++) order[c] = c;
-        std::stable_sort(order, order + 256, [&](int a, int b) { return freq[a] > freq[b]; });
-        for (int r = 0; r < 4; r++) hp.code[order[r]] = (uint8_t)r;
-    }
+    if (two_bit) two_bit_code(patterns, offsets, ids, hp.code);
     std::unordered_map<uint32_t, std::vector<uint32_t>> keys;  // key -> postings pattern << 8 | piece
     keys.reserve(cnt * 8);
     for (uint32_t i = 0; i < cnt; i++) {
@@ -2795,11 +2980,8 @@ static int batch_pass_ham(fzb_haystack *h, const uint8_t *patterns, const uint32
         pinfo[i] = m | (k << 8) | (L << 16);
         for (uint32_t j = 0; j <= k; j++) {
             const uint8_t *s = bp.P + j * L;
-            if (two_bit) {  // codes of the first min(L, 8) symbols, under every completion of the remaining ones
-                const uint32_t n = std::min<uint32_t>(L, kHbKeySyms);
-                uint32_t key = 0;
-                for (uint32_t q = 0; q < n; q++) key |= (uint32_t)hp.code[s[q]] << (2 * q);
-                for (uint32_t x = 0; x < (1u << (2 * (kHbKeySyms - n))); x++) keys[key | (x << (2 * n))].push_back((i << 8) | j);
+            if (two_bit) {
+                two_bit_key(keys, hp.code, s, L, (i << 8) | j);
             } else {
                 uint32_t w;
                 memcpy(&w, s, 4);  // (P is zero-padded to kBatchMaxM bytes)

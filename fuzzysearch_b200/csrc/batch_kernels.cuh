@@ -283,6 +283,127 @@ k_filter_mdense(const __grid_constant__ MdenseParams p, int64_t nvec, int64_t nt
     if (n) flush_cta_buffer(sBuf, sN, n, &sBase, p.hits, p.hits_cap, &p.mp.counters[CNT_MHITS], kMultiThreads);
 }
 
+// ------------------------------------------------------------------------------------------------
+// On low-entropy haystacks (DNA) a 3-byte prefix hits about every 64th position, so the prefix scan is no filter.
+//   k_filter_mdense2  finds the same hits with 2-bit keys: at EVERY position the 16-bit key of the 2-bit codes of the
+//        8 symbols there (a 256-entry byte -> code table from the pass's four most frequent pattern bytes) indexes an
+//        exact 64 Ki-bit table in shared memory; an n-gram shorter than 8 symbols is entered under every completion of
+//        its key.  A flagged lane walks the key's postings (pattern, n-gram j) and compares ALL L bytes of n-gram j
+//        with the text (bytes outside the four coded ones alias to code 0), appending exactly the hits k_filter_mdense
+//        appends, for k_verify_mhits unchanged.  One launch scans [scan_lo, scan_hi) only: the host cuts the own range
+//        into chunks whose hits fit the list, and verifies each chunk before scanning the next.
+// ------------------------------------------------------------------------------------------------
+constexpr int kHbKeySyms = 8;                                   // 2-bit key: codes of 8 symbols = 16 bits
+constexpr int kHbKeyWords = 1 << (2 * kHbKeySyms - 5);          // 2048 words = 8 KiB, one bit per key
+constexpr size_t kHbSmem2 = (size_t)kHbKeyWords * 4;
+constexpr size_t kMdense2Smem = kHbSmem2 + (size_t)kMdBuf * 8 + 16;
+
+// 2-bit codes of the 16 bytes of ws[0..3] and the 7 after them: symbol i at bits 2i and 2i+1
+__device__ __forceinline__ unsigned long long key_codes(const uint8_t *sCode, const uint32_t (&ws)[6]) {
+    unsigned long long codes = 0ull;
+#pragma unroll
+    for (int i = 0; i < 16 + kHbKeySyms - 1; i++)
+        codes |= (unsigned long long)sCode[(ws[i >> 2] >> (8 * (i & 3))) & 0xFFu] << (2 * i);
+    return codes;
+}
+
+struct Mdense2Params {
+    MdenseParams dp;           // as for k_filter_mdense, gtab keyed by the 2-bit key (MdenseParams itself stays as
+                               // k_verify_mhits takes it)
+    int64_t scan_lo, scan_hi;  // global positions of this launch
+    uint8_t code[256];         // byte -> 2-bit code
+};
+
+// position `g` (global, inside the scan and own ranges) carries `key`: walk its postings, compare each n-gram in full
+// (-> true when one of its appends brought the CTA buffer to the flush threshold)
+__device__ __noinline__ bool mdense2_confirm(const MdenseParams &p, unsigned long long *sBuf, uint32_t *sN, uint32_t key,
+                                             int64_t g) {
+    bool full = false;
+    uint32_t slot = (key * kGramMul) & p.mp.gtab_mask;
+    for (;;) {
+        const uint2 e = __ldg(p.mp.gtab + slot);
+        if (e.y == 0u) return full;
+        if (e.x == key) {
+            const uint32_t first = e.y & 0xFFFFFFu, cnt = e.y >> 24;
+            for (uint32_t i = 0; i < cnt; i++) {
+                const uint32_t post = __ldg(p.mp.postings + first + i);
+                const uint32_t pid = post >> 8, j = post & 0xFFu;
+                const BatchPat *bp = p.pats + pid;
+                const int L = bp->L, s = (int)j * L;
+                if (g + L > p.mp.N) continue;
+                const uint8_t *t = p.mp.H + (g - p.mp.buf_lo);
+                bool eq = true;
+                for (int b = 0; b < L; b++)
+                    if (__ldg(t + b) != bp->P[s + b]) {
+                        eq = false;
+                        break;
+                    }
+                if (eq) full |= mdense_append(p, sBuf, sN, (unsigned long long)(g - p.mp.buf_lo) | ((unsigned long long)j << 40) | ((unsigned long long)pid << 48));
+            }
+        }
+        slot = (slot + 1) & p.mp.gtab_mask;
+    }
+}
+
+// v0: the first 16-byte vector of the buffer this launch reads (the one holding scan_lo); nvec: vectors of the buffer
+__global__ void __launch_bounds__(kMultiThreads, 1)
+k_filter_mdense2(const __grid_constant__ Mdense2Params p, int64_t nvec, int64_t v0, int64_t ntiles) {
+    extern __shared__ __align__(16) uint32_t md2_tbl[];
+    unsigned long long *sBuf = reinterpret_cast<unsigned long long *>(md2_tbl + kHbKeyWords);
+    uint32_t *sN = reinterpret_cast<uint32_t *>(sBuf + kMdBuf);
+    __shared__ uint32_t sBase;
+    __shared__ uint8_t sCode[256];
+    const MdenseParams &dp = p.dp;
+    for (int i = threadIdx.x; i < kHbKeyWords / 4; i += kMultiThreads)
+        reinterpret_cast<uint4 *>(md2_tbl)[i] = __ldg(reinterpret_cast<const uint4 *>(dp.mp.bits) + i);
+    for (int i = threadIdx.x; i < 256; i += kMultiThreads) sCode[i] = p.code[i];
+    if (threadIdx.x == 0) *sN = 0;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const uint4 *base = reinterpret_cast<const uint4 *>(dp.mp.H);
+    const int64_t lo = max(p.scan_lo, dp.mp.own_lo), hi = min(p.scan_hi, dp.mp.own_hi);  // positions that count
+    for (int64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        bool full = false;
+#pragma unroll 1
+        for (int u = 0; u < kMultiUnroll; u++) {
+            const int64_t v = v0 + t * kMultiTileVecs + (int64_t)u * kMultiThreads + threadIdx.x;
+            const uint4 d = (v < nvec) ? ldg_stream(base + v) : make_uint4(0, 0, 0, 0);
+            uint32_t nx = __shfl_down_sync(0xFFFFFFFFu, d.x, 1);  // the 8 bytes after my 16
+            uint32_t ny = __shfl_down_sync(0xFFFFFFFFu, d.y, 1);
+            if (lane == 31 && v < nvec) {  // padded buffer
+                const uint2 e = __ldg(reinterpret_cast<const uint2 *>(base + v + 1));
+                nx = e.x;
+                ny = e.y;
+            }
+            const uint32_t ws[6] = {d.x, d.y, d.z, d.w, nx, ny};
+            const unsigned long long codes = key_codes(sCode, ws);
+            uint32_t acc = 0;  // bit (15 - b) <-> position b of my vector
+#pragma unroll
+            for (int b = 0; b < 16; b++) {
+                const uint32_t key = (uint32_t)(codes >> (2 * b)) & 0xFFFFu;
+                acc = acc * 2u + ((md2_tbl[key >> 5] >> (key & 31u)) & 1u);
+            }
+            const int64_t g0 = dp.mp.buf_lo + v * 16;
+            while (acc) {
+                const int bit = 31 - __clz(acc);
+                acc &= ~(1u << bit);
+                const int b = 15 - bit;
+                if (g0 + b < lo || g0 + b >= hi) continue;
+                full |= mdense2_confirm(dp, sBuf, sN, (uint32_t)(codes >> (2 * b)) & 0xFFFFu, g0 + b);
+            }
+        }
+        // flush decision reduced inside the barrier, as in k_filter_mdense
+        if (__syncthreads_or(full)) {
+            flush_cta_buffer(sBuf, sN, min(*sN, (uint32_t)kMdBuf), &sBase, dp.hits, dp.hits_cap,
+                             &dp.mp.counters[CNT_MHITS], kMultiThreads);
+            __syncthreads();
+        }
+    }
+    __syncthreads();
+    const uint32_t n = min(*sN, (uint32_t)kMdBuf);
+    if (n) flush_cta_buffer(sBuf, sN, n, &sBase, dp.hits, dp.hits_cap, &dp.mp.counters[CNT_MHITS], kMultiThreads);
+}
+
 constexpr int kMhThreads = 128;
 constexpr int kMhSlotBytes = 160;  // per-lane window slot: m + 2k + alignment slack (m <= 64, m + 2k + 8 <= 160)
 

@@ -23,10 +23,6 @@
 
 namespace fzb {
 
-constexpr int kHbKeySyms = 8;                                   // 2-bit key: codes of 8 symbols = 16 bits
-constexpr int kHbKeyWords = 1 << (2 * kHbKeySyms - 5);          // 2048 words = 8 KiB, one bit per key
-constexpr size_t kHbSmem2 = (size_t)kHbKeyWords * 4;
-
 struct HamBatchParams {
     MultiParams mp;       // H, geometry, key table (bits; text: bits2 too), gtab keyed by the key, postings
                           // pid << 8 | piece, pinfo m | k << 8 | L << 16, counters (CNT_CAND = candidates verified)
@@ -124,11 +120,7 @@ k_ham_batch_scan(const __grid_constant__ HamBatchParams p, int64_t nvec, int64_t
             const uint32_t ws[6] = {d.x, d.y, d.z, d.w, nx, ny};
             uint32_t acc = 0;  // bit (15 - b) <-> position b of my vector
             unsigned long long codes = 0ull;  // 2-bit codes of my 16 bytes and the 7 after them
-            if (TWO_BIT) {
-#pragma unroll
-                for (int i = 0; i < 16 + kHbKeySyms - 1; i++)
-                    codes |= (unsigned long long)sCode[(ws[i >> 2] >> (8 * (i & 3))) & 0xFFu] << (2 * i);
-            }
+            if (TWO_BIT) codes = key_codes(sCode, ws);
 #pragma unroll
             for (int b = 0; b < 16; b++) {
                 uint32_t h;
