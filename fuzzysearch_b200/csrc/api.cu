@@ -2853,6 +2853,7 @@ extern "C" int fzb_search_hamming(fzb_haystack *h, const uint8_t *pattern, uint3
         ScanParams p;
         fill_params(h, pattern, m, p);
         p.k = (int)std::min<uint32_t>(k, m);
+        if (flags & FZB_F_TINY_LIST) p.glist_cap = std::min(h->glist_cap, 8u);  // (testing) reach the bitmap-mode retry
         const RecSet rs = rec_set(h);
         CK(cudaSetDevice(h->device));
         res->stats.route = 4;
