@@ -86,6 +86,8 @@ SYMBOLS = {
     "fzb_search_levenshtein_batch": (_i32, [_vp, _u8p, _vp, _vp, _u32, _u32, _vpp, ctypes.POINTER(Stats)]),
     "fzb_search_hamming_batch": (_i32, [_vp, _u8p, _vp, _vp, _u32, _u32, _vpp, ctypes.POINTER(Stats)]),
     "fzb_search_generic_batch": (_i32, [_vp, _u8p, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _vpp, ctypes.POINTER(Stats)]),
+    "fzb_best_per_record": (_i32, [_vp, _u8p, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                   ctypes.POINTER(Stats)]),
     "fzb_find_near_matches": (_i32, [_u8p, _u32, _u8p, _u64, _u32, _u32, _u32, _u32, _i32, _vpp]),
     "fzb_has_near_match": (_i32, [_vp, _u8p, _u32, _u32, _u32, _u32, _u32, ctypes.POINTER(ctypes.c_int)]),
     "fzb_release_workspace": (None, []),
@@ -223,6 +225,7 @@ class Haystack(object):
     def __init__(self, handle, dev_ptr=None):
         self._h = handle
         self.dev_ptr = dev_ptr
+        self.record_count = 0  # records declared by set_records (an upload clears the set)
 
     @classmethod
     def from_host(cls, data, device=0, buf_lo=0, global_len=None, own_lo=None, own_hi=None):
@@ -290,6 +293,7 @@ class Haystack(object):
     def upload(self, data):
         a = as_u8(data)
         check(lib().fzb_haystack_upload(self._h, ptr(a), a.size))
+        self.record_count = 0
 
     def upload_symbols(self, units, alphabet):
         """units: numpy uint16 / uint32 code units; alphabet: the pattern's distinct symbols, ascending.
@@ -300,6 +304,7 @@ class Haystack(object):
         alpha = np.ascontiguousarray(alphabet, dtype=np.uint32)
         check(lib().fzb_haystack_upload_symbols(self._h, ptr(units), units.size, units.dtype.itemsize, ptr(alpha),
                                                 alpha.size))
+        self.record_count = 0
 
     def set_records(self, offsets):
         """Declare a record set: record i is [offsets[i], offsets[i+1] - 1), followed by one separator position
@@ -309,6 +314,7 @@ class Haystack(object):
             raise ValueError("record offsets need at least two entries (or none, to remove the record set)")
         count = max(off.size - 1, 0)
         check(lib().fzb_haystack_set_records(self._h, ptr(off) if count else None, count))
+        self.record_count = count
 
     def debug_counters(self):
         out = np.zeros(32, dtype=np.uint32)
@@ -387,6 +393,23 @@ class Haystack(object):
         results = [Result(ctypes.c_void_p(out[i])) for i in range(len(pats))]
         return results, {"gpu_ms": st.gpu_ms, "filter_ms": st.filter_ms, "bytes_scanned": st.bytes_scanned,
                          "n_candidates": st.n_candidates, "n_launches": st.n_launches, "route": "batch"}
+
+    def best_per_record(self, patterns, max_subs, max_ins, max_dels, max_l, flags=0):
+        """fzb_best_per_record on a handle with a record set: one normalised limit of each kind per pattern ->
+        ((pattern, start, end, dist, second_pattern, second_dist) arrays with one entry per record, -1 where a record
+        holds no match; summed stats dict)."""
+        pats = [as_u8(p) for p in patterns]
+        blob = np.concatenate(pats) if pats else np.zeros(0, np.uint8)
+        offsets = np.zeros(len(pats) + 1, dtype=np.uint32)
+        offsets[1:] = np.cumsum([p.size for p in pats])
+        limits = [np.ascontiguousarray(ks, dtype=np.uint32) for ks in (max_subs, max_ins, max_dels, max_l)]
+        n = self.record_count
+        cols = [np.empty(n, dtype=t) for t in (np.int32, np.int64, np.int64, np.int32, np.int32, np.int32)]
+        st = Stats()
+        check(lib().fzb_best_per_record(self._h, ptr(blob), ptr(offsets), *[ptr(ks) for ks in limits], len(pats), flags,
+                                        *[ctypes.c_void_p(c.ctypes.data) for c in cols], ctypes.byref(st)))
+        return tuple(cols), {"gpu_ms": st.gpu_ms, "filter_ms": st.filter_ms, "bytes_scanned": st.bytes_scanned,
+                             "n_candidates": st.n_candidates, "n_launches": st.n_launches, "route": "batch"}
 
     def has_near_match(self, pattern, max_subs, max_ins, max_dels, max_l):
         """True iff the search would return at least one match; stops at the first chunk that holds one."""

@@ -30,6 +30,7 @@
 #include "batch_kernels.cuh"
 #include "ham_batch_kernels.cuh"
 #include "generic_batch_kernels.cuh"
+#include "best_kernels.cuh"
 #include "sym_kernels.cuh"
 #include <unordered_map>
 #include "debug_kernels.cuh"
@@ -146,6 +147,17 @@ struct PeerBufs {  // the peer-memory reduction (p2p_kernels.cuh)
 struct RecBufs {  // a record set (fzb_haystack_set_records, DESIGN.md section 5.10)
     DevBuf<uint64_t> d_off;    // the count + 1 record offsets
     DevBuf<uint32_t> d_first;  // per 64-byte granule: the record holding its first position (k_rec_first)
+    uint64_t longest = 0;      // positions of the longest record, its separator included
+};
+struct BestBufs {  // fzb_best_per_record (best_kernels.cuh)
+    DevBuf<uint64_t> d_words;  // best[records], then top2[records]
+    DevBuf<uint32_t> d_ids;    // the pattern ordinals of the pass being reduced
+};
+// fzb_best_per_record in progress on a handle (DESIGN.md section 5.13): the batches it runs reduce the raw records of
+// every pass and of every one-by-one search into these words instead of returning lists.
+struct BestState {
+    uint64_t *best, *top2;    // one word per record each
+    const uint32_t *ordinal;  // pattern i of the batch being run is pattern ordinal[i] of the call
 };
 struct GatherBufs {  // the staged NCCL all-gather
     uint32_t cap = 0;  // rows per rank
@@ -282,6 +294,8 @@ struct fzb_haystack {
     std::unique_ptr<LpBatchBufs> lpb;
     std::unique_ptr<GenericBatchBufs> gbatch;
     std::unique_ptr<RecBufs> recs;  // the record set, if any (cleared by every upload)
+    std::unique_ptr<BestBufs> bestb;
+    BestState *best = nullptr;      // set for the duration of fzb_best_per_record (BestScope)
 };
 
 struct fzb_result {
@@ -795,6 +809,7 @@ extern "C" int fzb_haystack_set_records(fzb_haystack *h, const uint64_t *offsets
         k_rec_first<<<grid, 256, 0, h->stream>>>(b.d_off.get(), count, b.d_first.get(), ngran);
         CK(cudaGetLastError());
         CK(cudaStreamSynchronize(h->stream));
+        for (uint64_t i = 0; i < count; i++) b.longest = std::max(b.longest, offsets[i + 1] - offsets[i]);
         return FZB_OK;
     }));
     h->recs = std::move(recs);
@@ -2030,7 +2045,8 @@ static void add_stats(fzb_stats *sum, const fzb_stats &s) {
 // The attempt loop of a batch pass.  `enqueue()` puts the kernels of one attempt on h->stream (behind h->ev[0]) and
 // returns FZB_OK, an error, or +1 when a device structure of the pass overflowed.  Returns the same, +1 also when a
 // kernel raised CNT_OVERFLOW or the pass emitted more than kMaxRawRecs records; an attempt whose raw records did not
-// fit the output buffer is redone with a larger one.  On FZB_OK `raw` holds the records, `cnts` the counters, and `pass` the time and the bytes scanned.
+// fit the output buffer is redone with a larger one.  On FZB_OK `raw` holds the records (under fzb_best_per_record they stay
+// in h->d_out and `raw` stays empty), `cnts` the counters, and `pass` the time and the bytes scanned.
 template <class F>
 static int run_batch_pass(fzb_haystack *h, F enqueue, std::vector<RawRec> &raw, uint32_t cnts[CNT_COUNT],
                           fzb_stats &pass) {
@@ -2053,8 +2069,8 @@ static int run_batch_pass(fzb_haystack *h, F enqueue, std::vector<RawRec> &raw, 
             TRY(ensure_out_cap(h, n));
             continue;
         }
-        raw.resize(n);
-        if (n) {
+        if (!h->best) raw.resize(n);  // (fzb_best_per_record reduces the records where they are: finish_pass)
+        if (!raw.empty()) {
             CK(cudaMemcpyAsync(raw.data(), h->d_out.get(), (size_t)n * sizeof(RawRec), cudaMemcpyDeviceToHost, h->stream));
             CK(cudaStreamSynchronize(h->stream));
         }
@@ -2110,6 +2126,69 @@ static int split_batch(const std::vector<RawRec> &raw, const std::vector<uint32_
     work();
     for (auto &t : pool) t.join();
     add_stats(sum, pass);
+    return FZB_OK;
+}
+
+// The n raw records in h->d_out reduced into the words of the fzb_best_per_record in progress: those of a shared pass
+// whose pattern j is pattern d_ids[j] of the call, or (d_ids == nullptr) those of a single search of pattern `id`.
+static int best_accumulate(fzb_haystack *h, uint32_t n, const uint32_t *d_ids, uint32_t id) {
+    if (n == 0) return FZB_OK;
+    const int grid = (int)std::min<uint32_t>((n + kBestThreads - 1) / kBestThreads, (uint32_t)h->sm_count * 8);
+    if (d_ids)
+        k_best_accumulate<true><<<grid, kBestThreads, 0, h->stream>>>(h->d_out.get(), n, rec_set(h), d_ids, id,
+                                                                     h->best->best, h->best->top2);
+    else
+        k_best_accumulate<false><<<grid, kBestThreads, 0, h->stream>>>(h->d_out.get(), n, rec_set(h), d_ids, id,
+                                                                      h->best->best, h->best->top2);
+    CK(cudaGetLastError());
+    return FZB_OK;
+}
+
+// What a pass over the patterns ids[] ends with: the per-pattern results of split_batch or, under
+// fzb_best_per_record, its n raw records reduced where they are, each out[ids[i]] then an empty result that marks the
+// pattern as searched and carries the pass's stats.  Every way a pass can still overflow (+1) lies before this point
+// (for the chunked passes: behind the last chunk), so a pass that is redone pattern by pattern has contributed nothing.
+static int finish_pass(fzb_haystack *h, const std::vector<RawRec> &raw, uint32_t n, const std::vector<uint32_t> &ids,
+                       fzb_stats pass, int raw_order, bool unconsolidated, fzb_result **out, fzb_stats *sum) {
+    if (!h->best) return split_batch(raw, ids, pass, raw_order, unconsolidated, out, sum);
+    if (n) {
+        std::vector<uint32_t> ordinals(ids.size());
+        for (size_t j = 0; j < ids.size(); j++) ordinals[j] = h->best->ordinal[ids[j]];
+        // (a pageable source: the copy has left the vector when it returns)
+        CK(cudaMemcpyAsync(h->bestb->d_ids.get(), ordinals.data(), ordinals.size() * sizeof(uint32_t),
+                           cudaMemcpyHostToDevice, h->stream));
+        TRY(best_accumulate(h, n, h->bestb->d_ids.get(), 0));
+        pass.n_launches++;
+    }
+    for (size_t j = 0; j < ids.size(); j++) {
+        fzb_result *res = new (std::nothrow) fzb_result();
+        if (!res) return fail(FZB_E_CUDA, "out of host memory");
+        if (j == 0) res->stats = pass;
+        res->stats.route = pass.route;
+        out[ids[j]] = res;
+    }
+    add_stats(sum, pass);
+    return FZB_OK;
+}
+
+// The flags of a batch's one-by-one searches.  Under fzb_best_per_record they return the raw stream only
+// (best_single reduces it).
+static uint32_t single_flags(const fzb_haystack *h, uint32_t flags) {
+    return (flags & ~FZB_F_PER_RECORD) | (h->best ? FZB_F_NO_FINAL : 0u);
+}
+
+// Under fzb_best_per_record, behind the one-by-one search of pattern i of a batch: its raw records, still in h->d_out,
+// are reduced there and dropped, so that nothing reads them back.
+static int best_single(fzb_haystack *h, fzb_result *res, uint32_t i) {
+    if (!h->best) return FZB_OK;
+    TRY(best_accumulate(h, res->raw_n, nullptr, h->best->ordinal[i]));
+    if (res->raw_n) res->stats.n_launches++;
+    std::lock_guard<std::mutex> lock(g_pending_mutex);
+    if (res->owner) res->owner->pending = nullptr;
+    res->owner = nullptr;
+    res->raw_in_stage = false;
+    res->raw.clear();
+    res->raw_n = 0;
     return FZB_OK;
 }
 
@@ -2324,7 +2403,7 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
     pass.n_candidates = cnts[CNT_CAND];
     pass.n_launches = 2;
     // (the generic n-gram route's raw order: n-gram, hit index, then the window's matches in canonical order)
-    return split_batch(raw, ids, pass, glim ? 2 : 0, false, out, sum);
+    return finish_pass(h, raw, cnts[CNT_OUT], ids, pass, glim ? 2 : 0, false, out, sum);
 }
 
 // One shared scan for up to 64 LP-route patterns (k_lp_scan_multi / k_lp_verify_multi).  Same return convention
@@ -2452,7 +2531,7 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
     pass.route = glim ? 10 : 3;
     pass.filter_ms = scan_ms;
     pass.n_candidates = n_work;
-    return split_batch(raw, ids, pass, 1, false, out, sum);
+    return finish_pass(h, raw, cnts[CNT_OUT], ids, pass, 1, false, out, sum);
 }
 
 // Admission of n-gram-route Levenshtein patterns to the 2-bit pass (k_filter_mdense2 / k_verify_mhits) on
@@ -2575,7 +2654,7 @@ static int batch_pass_dna(fzb_haystack *h, const uint8_t *patterns, const uint32
     pass.filter_ms = scan_ms;
     pass.n_candidates = n_hits;
     pass.n_launches = 2 * nchunks;
-    return split_batch(raw, ids, pass, 0, false, out, sum);
+    return finish_pass(h, raw, cnts[CNT_OUT], ids, pass, 0, false, out, sum);
 }
 
 // The outcome `rc` of a shared pass over the patterns ids[] of a batch of `count` results: an error drops every
@@ -2722,8 +2801,9 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
     for (uint32_t i = 0; i < count; i++) {
         if (out[i]) continue;
         // (the single search honours a record set by itself)
-        const int rc = settle(fzb_search_levenshtein(h, patterns + offsets[i], offsets[i + 1] - offsets[i],
-                                                     max_l_dist[i], flags & ~FZB_F_PER_RECORD, &out[i]), {});
+        int rc = settle(fzb_search_levenshtein(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_l_dist[i],
+                                               single_flags(h, flags), &out[i]), {});
+        if (rc == FZB_OK) rc = settle(best_single(h, out[i], i), {});
         if (rc) return rc;
         add_stats(&sum, out[i]->stats);
     }
@@ -3036,12 +3116,12 @@ static int batch_pass_ham(fzb_haystack *h, const uint8_t *patterns, const uint32
         return FZB_OK;
     }, raw, cnts, pass);
     if (rc) return rc;
-    if (tiny && raw.size() > kTinyBatchCap) return 1;  // FZB_F_TINY_LIST: the pass's record list holds kTinyBatchCap
+    if (tiny && cnts[CNT_OUT] > kTinyBatchCap) return 1;  // FZB_F_TINY_LIST: the pass's record list holds kTinyBatchCap
     pass.route = 8;
     pass.filter_ms = pass.gpu_ms;
     pass.n_candidates = cnts[CNT_CAND];
     pass.n_launches = 1;
-    return split_batch(raw, ids, pass, 1, true, out, sum);
+    return finish_pass(h, raw, cnts[CNT_OUT], ids, pass, 1, true, out, sum);
 }
 
 extern "C" int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
@@ -3103,8 +3183,9 @@ extern "C" int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns
     }
     for (uint32_t i = 0; i < count; i++) {
         if (out[i]) continue;
-        const int rc = settle(fzb_search_hamming(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_subs[i],
-                                                 flags & ~FZB_F_PER_RECORD, &out[i]), {});
+        int rc = settle(fzb_search_hamming(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_subs[i],
+                                           single_flags(h, flags), &out[i]), {});
+        if (rc == FZB_OK) rc = settle(best_single(h, out[i], i), {});
         if (rc) return rc;
         add_stats(&sum, out[i]->stats);
     }
@@ -3241,9 +3322,9 @@ extern "C" int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns
     }
     for (uint32_t i = 0; i < count; i++) {
         if (out[i]) continue;
-        const int rc = settle(fzb_search_generic(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_subs[i],
-                                                 max_ins[i], max_dels[i], max_l_dist[i], flags & ~FZB_F_PER_RECORD,
-                                                 &out[i]), {});
+        int rc = settle(fzb_search_generic(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_subs[i],
+                                           max_ins[i], max_dels[i], max_l_dist[i], single_flags(h, flags), &out[i]), {});
+        if (rc == FZB_OK) rc = settle(best_single(h, out[i], i), {});
         if (rc) return rc;
         add_stats(&sum, out[i]->stats);
     }
@@ -3260,6 +3341,121 @@ static int search_by_class(fzb_haystack *h, const uint8_t *pattern, uint32_t m, 
     if (max_l <= std::min(max_subs, std::min(max_ins, max_dels)))
         return fzb_search_levenshtein(h, pattern, m, max_l, flags, out);
     return fzb_search_generic(h, pattern, m, max_subs, max_ins, max_dels, max_l, flags, out);
+}
+
+// ------------------------------------------------------------------------------------------------
+// fzb_best_per_record (DESIGN.md section 5.13): every record of a set assigned its best-matching pattern
+// ------------------------------------------------------------------------------------------------
+struct BestScope {  // h->best for the duration of a call, cleared on every way out
+    fzb_haystack *h;
+    BestScope(fzb_haystack *h_, BestState *s) : h(h_) { h->best = s; }
+    ~BestScope() { h->best = nullptr; }
+    BestScope(const BestScope &) = delete;
+    BestScope &operator=(const BestScope &) = delete;
+};
+
+extern "C" int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
+                                   const uint32_t *max_subs, const uint32_t *max_ins, const uint32_t *max_dels,
+                                   const uint32_t *max_l_dist, uint32_t count, uint32_t flags, int32_t *pattern,
+                                   int64_t *start, int64_t *end, int32_t *dist, int32_t *second_pattern,
+                                   int32_t *second_dist, fzb_stats *total) {
+    HandleLock handle_lock(h);
+    if (!h || !pattern || !start || !end || !dist || !second_pattern || !second_dist ||
+        (count && (!patterns || !offsets || !max_subs || !max_ins || !max_dels || !max_l_dist)))
+        return fail(FZB_E_INVALID, "NULL argument");
+    if (!h->recs) return fail(FZB_E_INVALID, "fzb_best_per_record needs a handle with a record set");
+    if (flags & ~FZB_F_TINY_LIST) return fail(FZB_E_UNSUPPORTED, "fzb_best_per_record takes no flag other than FZB_F_TINY_LIST");
+    if (count > kBestMaxPatterns)
+        return fail(FZB_E_UNSUPPORTED, "more than %u patterns in one fzb_best_per_record call", kBestMaxPatterns);
+    if (h->recs->longest > (1ull << 31))
+        return fail(FZB_E_UNSUPPORTED, "fzb_best_per_record needs records shorter than 2^31");
+    // every pattern as its single search would take it, before any work; then by class (search_by_class), each class
+    // a batch of its own over its subset of the patterns
+    struct Subset {
+        std::vector<uint8_t> blob;
+        std::vector<uint32_t> offsets{0}, ordinal, lim[4];  // lim: the limit arrays of the class's batch entry point
+    } lev, ham, gen;
+    for (uint32_t i = 0; i < count; i++) {
+        if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
+        const uint8_t *p = patterns + offsets[i];
+        const uint32_t m = offsets[i + 1] - offsets[i], l = max_l_dist[i];
+        TRY(l == 0 ? check_exact_pattern(h, p, m, 0) : check_pattern(h, p, m, 0));
+        Subset *sub = &gen;
+        if (l == 0) {  // (the exact search is the Levenshtein batch's k == 0 route)
+            sub = &lev;
+            sub->lim[0].push_back(0);
+        } else if (max_ins[i] == 0 && max_dels[i] == 0) {
+            sub = &ham;
+            sub->lim[0].push_back(std::min(l, max_subs[i]));
+        } else if (l <= std::min(max_subs[i], std::min(max_ins[i], max_dels[i]))) {
+            sub = &lev;
+            sub->lim[0].push_back(l);
+        } else {
+            const uint32_t lk = m / ((uint64_t)l + 1) >= 3 ? l : lp_generic_limit(m, max_ins[i], l);
+            if (lk > 63) return fail(FZB_E_UNSUPPORTED, "max_l_dist > 63 is not supported by the generic search");
+            const uint32_t lims[4] = {max_subs[i], max_ins[i], max_dels[i], l};
+            for (int q = 0; q < 4; q++) sub->lim[q].push_back(lims[q]);
+        }
+        sub->blob.insert(sub->blob.end(), p, p + m);
+        sub->offsets.push_back((uint32_t)sub->blob.size());
+        sub->ordinal.push_back(i);
+    }
+    CK(cudaSetDevice(h->device));
+    const uint64_t nrec = h->recs->d_off.size() - 1;
+    if (!h->bestb || h->bestb->d_words.size() < 2 * nrec) {  // built whole, beside the one it replaces
+        std::unique_ptr<BestBufs> grown;
+        TRY(ensure_group(grown, [&](BestBufs &b) -> int {
+            TRY(b.d_words.alloc(2 * nrec));
+            return b.d_ids.alloc(kMaxBatchPats);
+        }));
+        h->bestb = std::move(grown);
+    }
+    BestState state{h->bestb->d_words.get(), h->bestb->d_words.get() + nrec, nullptr};
+    BestScope scope(h, &state);
+    fzb_stats sum{};
+    k_best_fill<<<(int)std::min<uint64_t>((2 * nrec + kBestThreads - 1) / kBestThreads, (uint64_t)h->sm_count * 8),
+                  kBestThreads, 0, h->stream>>>(state.best, 2 * nrec);
+    CK(cudaGetLastError());
+    sum.n_launches = 1;
+    for (Subset *sub : {&lev, &ham, &gen}) {
+        const uint32_t n = (uint32_t)sub->ordinal.size();
+        if (n == 0) continue;
+        state.ordinal = sub->ordinal.data();
+        std::vector<fzb_result *> out(n, nullptr);
+        fzb_stats part{};
+        const uint32_t f = flags | FZB_F_PER_RECORD;
+        if (sub->blob.empty()) sub->blob.push_back(0);
+        const int rc = sub == &lev   ? fzb_search_levenshtein_batch(h, sub->blob.data(), sub->offsets.data(),
+                                                                    sub->lim[0].data(), n, f, out.data(), &part)
+                       : sub == &ham ? fzb_search_hamming_batch(h, sub->blob.data(), sub->offsets.data(),
+                                                                sub->lim[0].data(), n, f, out.data(), &part)
+                                     : fzb_search_generic_batch(h, sub->blob.data(), sub->offsets.data(),
+                                                                sub->lim[0].data(), sub->lim[1].data(), sub->lim[2].data(),
+                                                                sub->lim[3].data(), n, f, out.data(), &part);
+        for (fzb_result *r : out)
+            if (r) fzb_result_destroy(r);
+        if (rc) return rc;
+        add_stats(&sum, part);
+    }
+    // one read-back of 16 bytes per record, whatever the number of matches
+    std::vector<uint64_t> words(2 * nrec);
+    CK(cudaMemcpyAsync(words.data(), state.best, 2 * nrec * sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    for (uint64_t r = 0; r < nrec; r++) {
+        const uint64_t b = words[r];
+        const uint32_t second = (uint32_t)words[nrec + r] & kBestPairNone;
+        const bool none = b == kBestEmpty;
+        const int64_t len = kBestMaxLen - (int64_t)((b >> 31) & 0x1FFu);
+        dist[r] = none ? -1 : (int32_t)(b >> 56);
+        pattern[r] = none ? -1 : (int32_t)((b >> 40) & 0xFFFFu);
+        start[r] = none ? -1 : (int64_t)(b & 0x7FFFFFFFu);
+        end[r] = none ? -1 : start[r] + len;
+        second_dist[r] = second == kBestPairNone ? -1 : (int32_t)(second >> 16);
+        second_pattern[r] = second == kBestPairNone ? -1 : (int32_t)(second & 0xFFFFu);
+    }
+    sum.route = 7;  // batch
+    if (total) *total = sum;
+    return FZB_OK;
 }
 
 // One cached workspace per device for the one-shot call: the analogue of the reference's reusable

@@ -12,7 +12,8 @@ from . import _native
 from .common import LevenshteinSearchParams, Match
 from .search import DeviceSequence, ExactSearch, GenericSearch, LevenshteinSearch, _kind, _text
 
-__all__ = ["DeviceSequenceSet", "find_near_matches_in_each", "find_near_matches_batch_in_each"]
+__all__ = ["BestMatches", "DeviceSequenceSet", "best_match_in_each", "find_near_matches_in_each",
+           "find_near_matches_batch_in_each"]
 
 
 def _set_kind(sequences):
@@ -189,3 +190,88 @@ def _search_set_batch(subsequences, seqset, limits, params, classes):
         return [dict((r, ms) for r, ms in enumerate(find_near_matches_in_each(p, seqset, *lim)) if ms)
                 for p, lim in zip(subsequences, limits)]
     return [dict(_split_by_record(seqset, s, e, d)) for s, e, d in lists]
+
+
+class BestMatches(object):
+    """What best_match_in_each returns: six numpy arrays with one entry per sequence, -1 where a sequence holds no
+    match.  ``pattern``: the index of the nearest pattern (the smallest index among equals); ``dist``, ``start``,
+    ``end``: its best match there (the smallest distance, then the longest, then the leftmost), in the sequence's own
+    coordinates; ``second_pattern``, ``second_dist``: the nearest match of any OTHER pattern (the smallest index
+    among equals), for rejecting ambiguous calls by ``second_dist - dist``.  ``best[r]`` is None or
+    ``(pattern index, Match)``, the Match built (and its ``matched`` sliced from the sequence) when asked for."""
+
+    def __init__(self, sequences, kind, columns):
+        self._sequences, self._kind = sequences, kind
+        self.pattern, self.start, self.end, self.dist, self.second_pattern, self.second_dist = columns
+
+    def __len__(self):
+        return len(self.pattern)
+
+    def __getitem__(self, r):
+        if self.pattern[r] < 0:
+            return None
+        s, e = int(self.start[r]), int(self.end[r])
+        matched = _slicer(self._sequences[r], self._kind)(s, e)
+        return int(self.pattern[r]), Match(s, e, int(self.dist[r]), matched=matched)
+
+
+def _no_matches(n):
+    return tuple(np.full(n, -1, dtype=t) for t in (np.int32, np.int64, np.int64, np.int32, np.int32, np.int32))
+
+
+def best_match_in_each(subsequences, sequences, max_l_dist=None, *, max_substitutions=None, max_insertions=None,
+                       max_deletions=None):
+    """Many patterns over many sequences, reduced on the device to one row per sequence: -> BestMatches, the
+    nearest pattern of every sequence, its best match there and the runner-up among the other patterns -- what
+    reducing ``find_near_matches_batch_in_each(...)`` over the patterns gives, without building its lists
+    (fzb_best_per_record, DESIGN.md section 5.13).  Patterns, limits and `sequences` are taken and validated as
+    find_near_matches_batch_in_each takes them."""
+    from . import _batch_params
+    subsequences, limits, params, classes = _batch_params(subsequences, max_substitutions, max_insertions,
+                                                          max_deletions, max_l_dist)
+    if isinstance(sequences, DeviceSequenceSet):
+        return _best_in_set(subsequences, sequences, limits, params)
+    if not isinstance(sequences, (list, tuple)):
+        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
+    if not sequences or not subsequences:
+        return BestMatches(list(sequences), _set_kind(sequences), _no_matches(len(sequences)))
+    seqset = DeviceSequenceSet(sequences)
+    try:
+        return _best_in_set(subsequences, seqset, limits, params)
+    finally:
+        seqset.close()
+
+
+def _best_in_set(subsequences, seqset, limits, params):
+    n = len(seqset)
+    if n == 0 or not subsequences:
+        return BestMatches(seqset._orig, seqset._kind, _no_matches(n))
+    from .search import AlphabetTooLarge
+    big = 1 << 29
+    with seqset._lock:
+        try:
+            pats = seqset._bind_many(subsequences)
+        except AlphabetTooLarge:
+            pats = None  # no common byte alphabet: pattern by pattern, below
+        if pats is not None:
+            lims = zip(*[[big if x is None else min(x, big) for x in p.unpacked] for p in params])
+            columns, _ = seqset._seq.haystack.best_per_record(pats, *lims)
+    if pats is None:
+        columns = _best_on_host(subsequences, seqset, limits)
+    return BestMatches(seqset._orig, seqset._kind, columns)
+
+
+def _best_on_host(subsequences, seqset, limits):
+    """The same rows from find_near_matches_in_each, pattern by pattern (each reduces the set to its own alphabet)."""
+    pat, start, end, dist, pat2, dist2 = columns = _no_matches(len(seqset))
+    for i, (p, lim) in enumerate(zip(subsequences, limits)):
+        for r, matches in enumerate(find_near_matches_in_each(p, seqset, *lim)):
+            if not matches:
+                continue
+            m = min(matches, key=lambda x: (x.dist, x.start - x.end, x.start))
+            if pat[r] < 0 or m.dist < dist[r]:  # (an equal distance leaves the earlier pattern in place)
+                pat2[r], dist2[r] = pat[r], dist[r]
+                pat[r], start[r], end[r], dist[r] = i, m.start, m.end, m.dist
+            elif pat2[r] < 0 or m.dist < dist2[r]:
+                pat2[r], dist2[r] = i, m.dist
+    return columns

@@ -263,6 +263,36 @@ int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns, const uin
                              const uint32_t *max_l_dist, uint32_t count, uint32_t flags, fzb_result **out,
                              struct fzb_stats_s *total);
 
+/*
+ * Every record of a record set assigned its best-matching pattern, reduced on the device (DESIGN.md section 5.13):
+ * what a demultiplexer keeps of the three batches above.  The patterns as for fzb_search_levenshtein_batch, each
+ * with its own limits, normalised as for fzb_find_near_matches; pattern i is searched as its class's search would
+ * search it (max_l_dist == 0 exact, max_ins == max_dels == 0 substitutions-only, max_l_dist <= every other limit
+ * Levenshtein, else generic).  With M(i, r) the list that search returns inside record r, every output array gets
+ * one entry per record, -1 where there is none:
+ *   dist[r]            the smallest dist of any match in any M(i, r);
+ *   pattern[r]         the smallest i whose M(i, r) holds a match at dist[r];
+ *   start[r], end[r]   of the matches of M(pattern[r], r) at dist[r]: the longest, then the smallest start, relative
+ *                      to the start of record r;
+ *   second_dist[r]     the smallest dist of any match in any M(i, r) with i != pattern[r] (another match of
+ *                      pattern[r] itself never counts);
+ *   second_pattern[r]  the smallest such i at second_dist[r].
+ * The patterns share the scans of the three batches under FZB_F_PER_RECORD, with the same admission, passes and
+ * fallbacks; the raw records of each pass are reduced where the kernels left them, no per-pattern list is built,
+ * and the only read-back is 16 bytes per record.  `total` (optional) sums the passes as the batches do and counts
+ * the reducing kernels in n_launches.
+ * Needs a handle with a record set (FZB_E_INVALID otherwise).  Every pattern is checked as its single search checks
+ * it before any work.  FZB_E_UNSUPPORTED: more than 65 535 patterns, a record of 2^31 bytes or more, any flag other
+ * than FZB_F_TINY_LIST.  Every refusal and every error leaves the handle as it was; the arrays then hold nothing
+ * meaningful.
+ */
+int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
+                        const uint32_t *max_subs, const uint32_t *max_ins, const uint32_t *max_dels,
+                        const uint32_t *max_l_dist, uint32_t count, uint32_t flags,
+                        int32_t *pattern, int64_t *start, int64_t *end, int32_t *dist,
+                        int32_t *second_pattern, int32_t *second_dist, /* each: one entry per record */
+                        struct fzb_stats_s *total);
+
 /* ExactSearch.search (search_exact.py:80-85): all (overlapping) occurrences. FINAL == RAW. */
 int fzb_search_exact(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
                      fzb_result **out);
