@@ -12,14 +12,15 @@ __version__ = "0.1.0"
 
 __all__ = ["find_near_matches", "find_near_matches_batch", "find_near_matches_in_each",
            "find_near_matches_batch_in_each", "best_match_in_each", "BestMatches", "find_near_matches_in_file",
+           "nearest_distance", "find_nearest_matches", "nearest_distance_in_each", "NearestDistances",
            "has_near_match", "Match", "LevenshteinSearchParams", "DeviceSequence", "DeviceSequenceSet", "ExactSearch", "SubstitutionsOnlySearch", "LevenshteinSearch",
            "GenericSearch", "choose_search_class", "search_exact"]
 
 from .common import LevenshteinSearchParams, Match
 from .search import (DeviceSequence, ExactSearch, GenericSearch, LevenshteinSearch,
-                     SubstitutionsOnlySearch, search_exact)
-from .sequence_set import (BestMatches, DeviceSequenceSet, best_match_in_each, find_near_matches_batch_in_each,
-                           find_near_matches_in_each)
+                     SubstitutionsOnlySearch, find_nearest_matches, nearest_distance, search_exact)
+from .sequence_set import (BestMatches, DeviceSequenceSet, NearestDistances, best_match_in_each,
+                           find_near_matches_batch_in_each, find_near_matches_in_each, nearest_distance_in_each)
 
 
 def find_near_matches(subsequence, sequence, max_substitutions=None, max_insertions=None,

@@ -24,7 +24,7 @@ F_PER_RECORD = 128  # batches on a handle with a record set: per-record results 
 
 ROUTE_NAMES = {7: "batch", 0: "exact", 1: "ngrams/sampled-filter", 2: "ngrams/dense-filter", 3: "lp",
                4: "hamming", 5: "generic-ngrams", 6: "generic-lp", 8: "hamming/batch-scan",
-               9: "generic-ngrams/batch-scan", 10: "generic-lp/batch-scan"}
+               9: "generic-ngrams/batch-scan", 10: "generic-lp/batch-scan", 11: "nearest/bit-vector-scan"}
 
 
 class NativeLibraryMissing(ImportError):
@@ -88,6 +88,8 @@ SYMBOLS = {
     "fzb_search_generic_batch": (_i32, [_vp, _u8p, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _vpp, ctypes.POINTER(Stats)]),
     "fzb_best_per_record": (_i32, [_vp, _u8p, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp,
                                    ctypes.POINTER(Stats)]),
+    "fzb_nearest_distance": (_i32, [_vp, _u8p, _u32, _u32, _vp, _vp, _vp, ctypes.POINTER(Stats)]),
+    "fzb_nearest_per_record": (_i32, [_vp, _u8p, _u32, _u32, _vp, _vp, ctypes.POINTER(Stats)]),
     "fzb_find_near_matches": (_i32, [_u8p, _u32, _u8p, _u64, _u32, _u32, _u32, _u32, _i32, _vpp]),
     "fzb_has_near_match": (_i32, [_vp, _u8p, _u32, _u32, _u32, _u32, _u32, ctypes.POINTER(ctypes.c_int)]),
     "fzb_release_workspace": (None, []),
@@ -217,6 +219,12 @@ class Result(object):
         return {"gpu_ms": st.gpu_ms, "filter_ms": st.filter_ms, "bytes_scanned": st.bytes_scanned,
                 "n_candidates": st.n_candidates, "n_launches": st.n_launches,
                 "route": ROUTE_NAMES.get(st.route, str(st.route))}
+
+
+def _scan_stats(st):
+    return {"gpu_ms": st.gpu_ms, "filter_ms": st.filter_ms, "bytes_scanned": st.bytes_scanned,
+            "n_candidates": st.n_candidates, "n_launches": st.n_launches,
+            "route": ROUTE_NAMES.get(st.route, str(st.route))}
 
 
 class Haystack(object):
@@ -410,6 +418,25 @@ class Haystack(object):
                                         *[ctypes.c_void_p(c.ctypes.data) for c in cols], ctypes.byref(st)))
         return tuple(cols), {"gpu_ms": st.gpu_ms, "filter_ms": st.filter_ms, "bytes_scanned": st.bytes_scanned,
                              "n_candidates": st.n_candidates, "n_launches": st.n_launches, "route": "batch"}
+
+    def nearest_distance(self, pattern, flags=0):
+        """fzb_nearest_distance: the nearest match of the pattern anywhere in the sequence, without a limit ->
+        (dist, n_ends, first_end, stats dict)."""
+        p, pp, m = self._pat(pattern)
+        dist, n_ends, first_end, st = ctypes.c_uint32(0), ctypes.c_uint64(0), ctypes.c_uint64(0), Stats()
+        check(lib().fzb_nearest_distance(self._h, pp, m, flags, ctypes.byref(dist), ctypes.byref(n_ends),
+                                         ctypes.byref(first_end), ctypes.byref(st)))
+        return dist.value, n_ends.value, first_end.value, _scan_stats(st)
+
+    def nearest_per_record(self, pattern, flags=0):
+        """fzb_nearest_per_record on a handle with a record set -> (dist int32, end int64: one entry per record,
+        the end relative to the record's start; stats dict)."""
+        p, pp, m = self._pat(pattern)
+        dist, end = np.empty(self.record_count, dtype=np.int32), np.empty(self.record_count, dtype=np.int64)
+        st = Stats()
+        check(lib().fzb_nearest_per_record(self._h, pp, m, flags, ctypes.c_void_p(dist.ctypes.data),
+                                           ctypes.c_void_p(end.ctypes.data), ctypes.byref(st)))
+        return dist, end, _scan_stats(st)
 
     def has_near_match(self, pattern, max_subs, max_ins, max_dels, max_l):
         """True iff the search would return at least one match; stops at the first chunk that holds one."""

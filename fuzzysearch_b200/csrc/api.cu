@@ -31,6 +31,7 @@
 #include "ham_batch_kernels.cuh"
 #include "generic_batch_kernels.cuh"
 #include "best_kernels.cuh"
+#include "nearest_kernels.cuh"
 #include "sym_kernels.cuh"
 #include <unordered_map>
 #include "debug_kernels.cuh"
@@ -158,6 +159,10 @@ struct BestBufs {  // fzb_best_per_record (best_kernels.cuh)
 struct BestState {
     uint64_t *best, *top2;    // one word per record each
     const uint32_t *ordinal;  // pattern i of the batch being run is pattern ordinal[i] of the call
+};
+struct NearBufs {  // fzb_nearest_distance / fzb_nearest_per_record (nearest_kernels.cuh)
+    DevBuf<uint64_t> d_head;   // the whole-sequence result (2 words), then the partials of kNearMaxGrid CTAs
+    DevBuf<uint64_t> d_words;  // one word per record
 };
 struct GatherBufs {  // the staged NCCL all-gather
     uint32_t cap = 0;  // rows per rank
@@ -296,6 +301,7 @@ struct fzb_haystack {
     std::unique_ptr<RecBufs> recs;  // the record set, if any (cleared by every upload)
     std::unique_ptr<BestBufs> bestb;
     BestState *best = nullptr;      // set for the duration of fzb_best_per_record (BestScope)
+    std::unique_ptr<NearBufs> nearb;
 };
 
 struct fzb_result {
@@ -3455,6 +3461,131 @@ extern "C" int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, con
     }
     sum.route = 7;  // batch
     if (total) *total = sum;
+    return FZB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// fzb_nearest_distance / fzb_nearest_per_record (DESIGN.md section 5.14): the nearest match without a distance limit
+// ------------------------------------------------------------------------------------------------
+template <int BITS, bool REC>
+static int launch_nearest(fzb_haystack *h, int grid, const NearParams &p, const RecSet &rs) {
+    CK(cudaFuncSetAttribute(k_nearest_scan<BITS, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)near_smem(BITS)));
+    k_nearest_scan<BITS, REC><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
+    CK(cudaGetLastError());
+    return FZB_OK;
+}
+
+// The scan over the whole buffer, per record if `rec`.  It keeps to its own buffer group: the counters, the output
+// area and a pending result of the handle are not touched.  On FZB_OK the answer is in nearb->d_head[0..1] or
+// nearb->d_words, and the stream has drained.
+static int nearest_scan(fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool rec, fzb_stats *stats) {
+    CK(cudaSetDevice(h->device));
+    const uint64_t nrec = rec ? h->recs->d_off.size() - 1 : 0;
+    if (!h->nearb || h->nearb->d_words.size() < nrec) {  // built whole, beside the one it replaces
+        std::unique_ptr<NearBufs> grown;
+        TRY(ensure_group(grown, [&](NearBufs &b) -> int {
+            TRY(b.d_head.alloc(2 + 2 * (uint64_t)kNearMaxGrid));
+            return b.d_words.alloc(std::max<uint64_t>(nrec, 1));
+        }));
+        h->nearb = std::move(grown);
+    }
+    NearParams p{};
+    p.H = h->d;
+    p.N = (int64_t)h->buf_len;
+    p.m = (int)m;
+    // segments long against the 2m warm-up on a long sequence, short enough to fill the SMs on a short one
+    p.seg = (int)std::min<uint64_t>(kNearMaxSeg, std::max<uint64_t>(kNearMinSeg,
+                                    round_up(h->buf_len / ((uint64_t)h->sm_count * 1024) + 1, 16)));
+    p.result = h->nearb->d_head.get();
+    p.partial = p.result + 2;
+    p.words = h->nearb->d_words.get();
+    memcpy(p.P, pattern, m);
+    const int bits = m <= 32 ? 32 : (int)round_up(m, 64);
+    const uint64_t tile = (uint64_t)kNearThreads * p.seg, ntiles = (h->buf_len + tile - 1) / tile;
+    const int per_sm = bits == 32 ? 4 : bits == 64 ? 3 : 2;
+    const int grid = (int)std::min<uint64_t>(ntiles, std::min<uint64_t>((uint64_t)h->sm_count * per_sm, kNearMaxGrid));
+    fzb_stats st{};
+    st.route = 11;
+    st.bytes_scanned = h->buf_len;
+    CK(cudaEventRecord(h->ev[0], h->stream));
+    if (rec) {
+        k_nearest_fill<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
+            p.words, nrec, (uint64_t)m << 32);
+    } else {
+        k_nearest_fill<<<1, 32, 0, h->stream>>>(p.result, 1, (uint64_t)m << 48);
+        CK(cudaMemsetAsync(p.result + 1, 0, sizeof(uint64_t), h->stream));
+    }
+    CK(cudaGetLastError());
+    st.n_launches = 1;
+    if (grid > 0) {
+        const RecSet rs = rec_set(h);
+        int rc = FZB_OK;
+        with_recs(h, [&](auto r) {
+            constexpr bool R = decltype(r)::value;
+            rc = bits == 32    ? launch_nearest<32, R>(h, grid, p, rs)
+                 : bits == 64  ? launch_nearest<64, R>(h, grid, p, rs)
+                 : bits == 128 ? launch_nearest<128, R>(h, grid, p, rs)
+                 : bits == 192 ? launch_nearest<192, R>(h, grid, p, rs)
+                               : launch_nearest<256, R>(h, grid, p, rs);
+        });
+        TRY(rc);
+        st.n_launches++;
+    }
+    CK(cudaEventRecord(h->ev[1], h->stream));
+    if (!rec) {
+        k_nearest_count<<<1, 256, 0, h->stream>>>(p.result, p.partial, (uint32_t)grid, m);
+        CK(cudaGetLastError());
+        st.n_launches++;
+    }
+    CK(cudaEventRecord(h->ev[2], h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, h->ev[0], h->ev[2]));
+    st.gpu_ms = ms;
+    CK(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
+    st.filter_ms = ms;
+    if (stats) *stats = st;
+    return FZB_OK;
+}
+
+extern "C" int fzb_nearest_distance(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
+                                    uint32_t *dist, uint64_t *n_ends, uint64_t *first_end, fzb_stats *stats) {
+    HandleLock handle_lock(h);
+    if (!h || !dist || !n_ends || !first_end) return fail(FZB_E_INVALID, "NULL argument");
+    if (flags) return fail(FZB_E_UNSUPPORTED, "fzb_nearest_distance takes no flags");
+    if (!is_whole_sequence(h) || h->comm || h->local_world || h->peer)
+        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_distance needs a whole (unsharded) sequence outside a world");
+    TRY(refuse_records(h, "fzb_nearest_distance"));
+    TRY(check_pattern(h, pattern, m, 0));
+    TRY(nearest_scan(h, pattern, m, false, stats));
+    uint64_t out[2];
+    CK(cudaMemcpyAsync(out, h->nearb->d_head.get(), sizeof out, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    *dist = (uint32_t)(out[0] >> 48);
+    *first_end = out[0] & kNearNoEnd;
+    *n_ends = out[1];
+    return FZB_OK;
+}
+
+extern "C" int fzb_nearest_per_record(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
+                                      int32_t *dist, int64_t *end, fzb_stats *stats) {
+    HandleLock handle_lock(h);
+    if (!h || !dist || !end) return fail(FZB_E_INVALID, "NULL argument");
+    if (!h->recs) return fail(FZB_E_INVALID, "fzb_nearest_per_record needs a handle with a record set");
+    if (flags) return fail(FZB_E_UNSUPPORTED, "fzb_nearest_per_record takes no flags");
+    if (h->recs->longest > (1ull << 32))
+        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_per_record needs records shorter than 2^32");
+    TRY(check_pattern(h, pattern, m, 0));
+    TRY(nearest_scan(h, pattern, m, true, stats));
+    // one read-back of 8 bytes per record
+    const uint64_t nrec = h->recs->d_off.size() - 1;
+    std::vector<uint64_t> words(nrec);
+    CK(cudaMemcpyAsync(words.data(), h->nearb->d_words.get(), nrec * sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    for (uint64_t r = 0; r < nrec; r++) {
+        dist[r] = (int32_t)(words[r] >> 32);
+        end[r] = (int64_t)(words[r] & 0xFFFFFFFFull);
+    }
     return FZB_OK;
 }
 

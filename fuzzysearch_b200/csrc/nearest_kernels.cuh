@@ -1,0 +1,246 @@
+// nearest_kernels.cuh -- fzb_nearest_distance / fzb_nearest_per_record (DESIGN.md section 5.14): the smallest
+// Levenshtein distance of the pattern to any substring of the sequence, without a distance limit.
+//
+// E(e) = min over s <= e of lev(P, S[s:e]) is the bottom row of Sellers' table with a free start (D[0][j] = 0).
+// k_nearest_scan runs its bit-vector form (Myers 1999, Hyyro 2003): the column is kept as the vertical deltas Pv / Mv,
+// one bit per pattern symbol, and the score follows the horizontal delta at bit m - 1.  Nothing is shifted into the
+// horizontal deltas (the search form; expand_bp in kernels.cuh is the prefix-anchored form, which shifts +1 in).
+//
+// Parallel along the text.  A thread owns a segment [a, b) of the text and first runs the recurrence, untracked, over
+// the 2m bytes before a, from the initial column (Pv all ones, score m).  That is exact, not a heuristic: a column
+// started at w computes E_w(e) = min over w <= s <= e, and for e >= w + 2m the two agree -- E(e) <= m (the empty
+// substring), and a substring at distance d <= m from P is at most m + d <= 2m long, so some optimal s is >= e - 2m >= w.
+// Each later score depends on the text only through these minima, so every score the thread records is E itself.
+//
+// The text is read straight from global memory, 16 bytes per load and lane (the lines of a lane's segment stay in L1
+// between its loads); a segment is `seg` bytes, 512 to 4 096, chosen by the host from the sequence length.  The
+// match masks PM[c] sit in shared memory.  With one word (m <= 64) the table is replicated per lane, entry
+// c * 32 + lane: a 32-bit entry falls into bank `lane`, a 64-bit entry into banks 2 lane and 2 lane + 1 of its half
+// warp, so 32 lanes looking up 32 different bytes never share a bank with different addresses (no conflict for any
+// text).  With 2 to 4 words (m <= 255, correct but not tuned) one table [c][word] serves all lanes.
+//
+// Results.  Whole sequence: a thread keeps (minimum, ends at the minimum, first such end); warps, then the CTA combine
+// them, and the CTA sends one atomicMin of dist << 48 | first_end and stores (minimum, count) as its partial;
+// k_nearest_count adds the counts of the partials at the global minimum.  All of it is min / integer addition: the
+// answer does not depend on thread, CTA or launch order.  Record sets (REC): the column is reset at every record
+// start, a thread finds its first record as rec_bounds does and walks the offsets as its segment crosses separators, and
+// each (record, thread) sends one atomicMin of dist << 32 | end - record start into the record's word, which
+// k_nearest_fill set to the empty record's (m, 0).  The end position 0 (score m) is that initial value in both forms.
+#pragma once
+#include "common.cuh"
+
+namespace fzb {
+
+constexpr int kNearThreads = 256;
+constexpr int kNearMinSeg = 512, kNearMaxSeg = 4096;  // bytes per thread (multiples of 16)
+constexpr int kNearMaxGrid = 1024;                    // CTAs of a scan (partials of the whole-sequence form)
+constexpr uint64_t kNearNoEnd = (1ull << 48) - 1;
+
+struct NearParams {
+    const uint8_t *H;
+    int64_t N;
+    int32_t m, seg;
+    uint64_t *result;   // [0] dist << 48 | first_end, [1] n_ends
+    uint64_t *partial;  // per CTA: its minimum, its count of ends there
+    uint64_t *words;    // REC: dist << 32 | end per record
+    uint8_t P[256];
+};
+
+template <int BITS> struct NearWord { typedef uint64_t type; };
+template <> struct NearWord<32> { typedef uint32_t type; };
+
+__host__ __device__ constexpr int near_words(int bits) { return bits <= 64 ? 1 : bits / 64; }
+__host__ __device__ constexpr size_t near_smem(int bits) { return bits <= 64 ? (size_t)256 * 32 * (bits / 8) : (size_t)256 * (bits / 8); }
+
+__global__ void k_nearest_fill(uint64_t *words, uint64_t n, uint64_t value) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) words[i] = value;
+}
+
+// (minimum, ends at the minimum, first such end) of two disjoint sets of end positions
+__device__ __forceinline__ void near_merge(uint32_t &best, uint64_t &cnt, uint64_t &first, uint32_t ob, uint64_t oc,
+                                           uint64_t of) {
+    if (ob < best) {
+        best = ob;
+        cnt = oc;
+        first = of;
+    } else if (ob == best) {
+        cnt += oc;
+        if (of < first) first = of;
+    }
+}
+
+template <int BITS>
+struct NearCol {  // one column of the table and what the thread has seen of its bottom row
+    typedef typename NearWord<BITS>::type word;
+    static constexpr int NW = near_words(BITS);
+    word Pv[NW], Mv[NW];
+    uint32_t score, top;          // top: the bit of row m - 1 in the last word
+    uint32_t best, cnt, first;    // tracked ends: the minimum below m (else m), its count, the first (as `rel`)
+    const word *pm;               // this lane's view of the table
+
+    __device__ __forceinline__ void reset(uint32_t m) {
+#pragma unroll
+        for (int w = 0; w < NW; w++) {
+            Pv[w] = ~(word)0;
+            Mv[w] = 0;
+        }
+        score = best = m;
+        cnt = 0;
+        first = 0;
+    }
+
+    // the column behind text byte c; rel: the end position it closes, relative to the caller's base
+    template <bool TRACK>
+    __device__ __forceinline__ void step(uint32_t c, uint32_t rel) {
+        int hin = 0;
+#pragma unroll
+        for (int w = 0; w < NW; w++) {
+            word Eq = NW == 1 ? pm[c * 32] : pm[c * NW + w];
+            const word pv = Pv[w], mv = Mv[w];
+            const word Xv = Eq | mv;
+            if (NW > 1) Eq |= (word)(hin < 0);
+            const word Xh = (((Eq & pv) + pv) ^ pv) | Eq;
+            word Ph = mv | ~(Xh | pv);
+            word Mh = pv & Xh;
+            const uint32_t bit = w == NW - 1 ? top : (uint32_t)(sizeof(word) * 8 - 1);
+            const int hout = (int)((Ph >> bit) & 1) - (int)((Mh >> bit) & 1);
+            Ph <<= 1;
+            Mh <<= 1;
+            if (NW > 1) {
+                Ph |= (word)(hin > 0);
+                Mh |= (word)(hin < 0);
+            }
+            Pv[w] = Mh | ~(Xv | Ph);
+            Mv[w] = Ph & Xv;
+            hin = hout;
+        }
+        score += (uint32_t)hin;
+        if (TRACK) {
+            if (score < best) {
+                best = score;
+                cnt = 1;
+                first = rel;
+            } else if (score == best) {
+                cnt++;
+            }
+        }
+    }
+
+    // text bytes [x, end); rel: the end position behind H[x], relative to the caller's base
+    template <bool TRACK>
+    __device__ __forceinline__ void run(const uint8_t *H, int64_t x, int64_t end, uint32_t rel) {
+        for (; x < end && (x & 15); x++) step<TRACK>(H[x], rel++);
+        for (; x + 16 <= end; x += 16) {
+            const uint4 v = __ldg(reinterpret_cast<const uint4 *>(H + x));
+            const uint32_t q[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int j = 0; j < 16; j++) step<TRACK>((q[j >> 2] >> (8 * (j & 3))) & 0xFFu, rel++);
+        }
+        for (; x < end; x++) step<TRACK>(H[x], rel++);
+    }
+};
+
+template <int BITS, bool REC>
+__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : BITS == 64 ? 3 : 2)
+k_nearest_scan(NearParams p, RecSet rs) {
+    typedef typename NearWord<BITS>::type word;
+    constexpr int NW = near_words(BITS);
+    extern __shared__ __align__(16) uint64_t near_smem_raw[];
+    __shared__ uint32_t s_best[kNearThreads / 32];
+    __shared__ uint64_t s_cnt[kNearThreads / 32], s_first[kNearThreads / 32];
+    word *pm = reinterpret_cast<word *>(near_smem_raw);
+    const uint32_t m = (uint32_t)p.m, lane = threadIdx.x & 31u;
+
+    {  // thread c builds the masks of byte c
+        const uint32_t c = threadIdx.x;
+        word mask[NW];
+#pragma unroll
+        for (int w = 0; w < NW; w++) mask[w] = 0;
+        for (uint32_t i = 0; i < m; i++)
+            if (p.P[i] == c) {
+#pragma unroll
+                for (int w = 0; w < NW; w++)
+                    if ((int)(i / (sizeof(word) * 8)) == w) mask[w] |= (word)1 << (i % (sizeof(word) * 8));
+            }
+        if (NW == 1) {
+            for (int l = 0; l < 32; l++) pm[c * 32 + l] = mask[0];
+        } else {
+#pragma unroll
+            for (int w = 0; w < NW; w++) pm[c * NW + w] = mask[w];
+        }
+    }
+    __syncthreads();
+
+    NearCol<BITS> col;
+    col.pm = NW == 1 ? pm + lane : pm;
+    col.top = (m - 1) % (uint32_t)(sizeof(word) * 8);
+    uint32_t tbest = m;  // whole sequence: over all tiles of this thread
+    uint64_t tcnt = 0, tfirst = kNearNoEnd;
+
+    const int64_t tile = (int64_t)kNearThreads * p.seg;
+    for (int64_t base = (int64_t)blockIdx.x * tile; base < p.N; base += (int64_t)gridDim.x * tile) {
+        const int64_t a = base + (int64_t)threadIdx.x * p.seg;
+        if (a >= p.N) continue;
+        const int64_t b = a + p.seg < p.N ? a + p.seg : p.N;
+        int64_t lo = 0, hi = p.N;  // the record around the column: [lo, hi), its separator at hi
+        uint32_t r = 0;
+        if (REC) {
+            r = rs.first[a >> kGranuleShift];
+            while ((int64_t)rs.off[r + 1] <= a) r++;
+            lo = (int64_t)rs.off[r];
+            hi = (int64_t)rs.off[r + 1] - 1;
+        }
+        col.reset(m);
+        const int64_t w = a - 2 * (int64_t)m > lo ? a - 2 * (int64_t)m : lo;
+        col.template run<false>(p.H, w, a, 0);
+        if (!REC) {
+            col.template run<true>(p.H, a, b, 1);
+            near_merge(tbest, tcnt, tfirst, col.best, col.cnt, col.best < m ? (uint64_t)a + col.first : kNearNoEnd);
+        } else {
+            int64_t x = a;
+            for (;;) {
+                const int64_t stop = b < hi ? b : hi;
+                if (x < stop) col.template run<true>(p.H, x, stop, (uint32_t)(x + 1 - lo));
+                if (col.best < m)
+                    atomicMin((unsigned long long *)&p.words[r], (unsigned long long)col.best << 32 | col.first);
+                if (hi + 1 >= b) break;  // (the record behind the separator starts in another segment, or nowhere)
+                r++;
+                lo = hi + 1;
+                hi = (int64_t)rs.off[r + 1] - 1;
+                x = lo;
+                col.reset(m);
+            }
+        }
+    }
+    if (!REC) {  // the CTA's (minimum, count, first end): warps by shuffle, then thread 0 over the warps
+        for (int d = 16; d > 0; d >>= 1) {
+            const uint32_t ob = __shfl_down_sync(0xFFFFFFFFu, tbest, d);
+            const uint64_t oc = __shfl_down_sync(0xFFFFFFFFu, tcnt, d), of = __shfl_down_sync(0xFFFFFFFFu, tfirst, d);
+            near_merge(tbest, tcnt, tfirst, ob, oc, of);
+        }
+        if (lane == 0) {
+            s_best[threadIdx.x >> 5] = tbest;
+            s_cnt[threadIdx.x >> 5] = tcnt;
+            s_first[threadIdx.x >> 5] = tfirst;
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            for (int i = 1; i < kNearThreads / 32; i++) near_merge(tbest, tcnt, tfirst, s_best[i], s_cnt[i], s_first[i]);
+            if (tbest < m) atomicMin((unsigned long long *)&p.result[0], (unsigned long long)tbest << 48 | tfirst);
+            p.partial[2 * blockIdx.x] = tbest;
+            p.partial[2 * blockIdx.x + 1] = tcnt;
+        }
+    }
+}
+
+// n_ends: the ends the CTAs counted at the global minimum, and the end position 0 if that minimum is m.  One CTA.
+__global__ void k_nearest_count(uint64_t *result, const uint64_t *partial, uint32_t nparts, uint32_t m) {
+    const uint64_t best = result[0] >> 48;
+    uint64_t sum = threadIdx.x == 0 && best == m ? 1 : 0;
+    for (uint32_t i = threadIdx.x; i < nparts; i += blockDim.x)
+        if (partial[2 * i] == best) sum += partial[2 * i + 1];
+    if (sum) atomicAdd((unsigned long long *)&result[1], (unsigned long long)sum);
+}
+
+}  // namespace fzb

@@ -29,7 +29,7 @@ def _text(seq):
 
 
 __all__ = ["DeviceSequence", "ExactSearch", "SubstitutionsOnlySearch", "LevenshteinSearch",
-           "GenericSearch", "RawMatches", "search_exact"]
+           "GenericSearch", "RawMatches", "search_exact", "nearest_distance", "find_nearest_matches"]
 
 
 class DeviceSequence(object):
@@ -427,3 +427,37 @@ class GenericSearch(FuzzySearchBase):
     @classmethod
     def extra_items_for_chunked_search(cls, subsequence, search_params):
         return max(x for x in [search_params.max_l_dist, search_params.max_insertions] if x is not None)
+
+
+def nearest_distance(subsequence, sequence):
+    """The smallest Levenshtein distance of `subsequence` to any substring of `sequence` (at most
+    ``len(subsequence)``: the empty substring) -- the smallest ``max_l_dist`` at which ``find_near_matches`` finds
+    anything.  One scan of the sequence, whatever the answer (fzb_nearest_distance, DESIGN.md section 5.14).
+    `sequence` is anything find_near_matches takes."""
+    if len(subsequence) == 0:
+        raise ValueError("Given subsequence is empty!")
+    with _lock_for(sequence):
+        pat, hay, _, _ = _prepare(subsequence, sequence)
+        return hay.nearest_distance(pat)[0]
+
+
+def find_nearest_matches(subsequence, sequence, max_l_dist=None):
+    """Where does `subsequence` fit best?  -> exactly ``find_near_matches(subsequence, sequence, max_l_dist=d)`` with
+    d = ``nearest_distance(subsequence, sequence)``, without guessing d: one scan finds it, then the ordinary search
+    runs once, at d, on the same upload.  With `max_l_dist` given the list is empty when d is larger (the cap bounds
+    the cost of the search; the search itself still runs at d, not at the cap)."""
+    if len(subsequence) == 0:
+        raise ValueError("Given subsequence is empty!")
+    if max_l_dist is not None and (not isinstance(max_l_dist, int) or max_l_dist < 0):
+        raise ValueError("max_l_dist must be a non-negative integer or None")
+    with _lock_for(sequence):
+        pat, hay, slicer, _ = _prepare(subsequence, sequence)
+        d = hay.nearest_distance(pat)[0]
+        if max_l_dist is not None and d > max_l_dist:
+            return []
+        # max_l_dist == 0 is the exact search, whose list is its raw stream (ExactSearch does not consolidate)
+        res = hay.search_exact(pat) if d == 0 else hay.search_levenshtein(pat, d)
+        try:
+            return _to_matches(res, _native.RAW if d == 0 else _native.FINAL, slicer)
+        finally:
+            res.close()

@@ -12,8 +12,8 @@ from . import _native
 from .common import LevenshteinSearchParams, Match
 from .search import DeviceSequence, ExactSearch, GenericSearch, LevenshteinSearch, _kind, _text
 
-__all__ = ["BestMatches", "DeviceSequenceSet", "best_match_in_each", "find_near_matches_in_each",
-           "find_near_matches_batch_in_each"]
+__all__ = ["BestMatches", "DeviceSequenceSet", "NearestDistances", "best_match_in_each", "find_near_matches_in_each",
+           "find_near_matches_batch_in_each", "nearest_distance_in_each"]
 
 
 def _set_kind(sequences):
@@ -275,3 +275,47 @@ def _best_on_host(subsequences, seqset, limits):
             elif pat2[r] < 0 or m.dist < dist2[r]:
                 pat2[r], dist2[r] = i, m.dist
     return columns
+
+
+class NearestDistances(object):
+    """What nearest_distance_in_each returns: ``dist`` (int32) and ``end`` (int64), one entry per sequence -- the
+    smallest Levenshtein distance of the pattern to any substring of the sequence and the first end position (in the
+    sequence's own coordinates) of a substring at that distance.  ``nearest[r]`` is ``(dist, end)``."""
+
+    def __init__(self, dist, end):
+        self.dist, self.end = dist, end
+
+    def __len__(self):
+        return len(self.dist)
+
+    def __getitem__(self, r):
+        return int(self.dist[r]), int(self.end[r])
+
+
+def nearest_distance_in_each(subsequence, sequences):
+    """One pattern over many sequences, without a distance limit: -> NearestDistances with, for every sequence,
+    ``nearest_distance(subsequence, sequences[r])`` and where the nearest match first ends; an empty sequence gives
+    ``(len(subsequence), 0)``.  All sequences are scanned in one device pass (fzb_nearest_per_record, DESIGN.md
+    section 5.14).  `sequences` is a list / tuple (uploaded for this call) or a DeviceSequenceSet (resident)."""
+    if len(subsequence) == 0:
+        raise ValueError("Given subsequence is empty!")
+    if isinstance(sequences, DeviceSequenceSet):
+        return _nearest_in_set(subsequence, sequences)
+    if not isinstance(sequences, (list, tuple)):
+        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
+    if not sequences:
+        return NearestDistances(np.zeros(0, np.int32), np.zeros(0, np.int64))
+    seqset = DeviceSequenceSet(sequences)
+    try:
+        return _nearest_in_set(subsequence, seqset)
+    finally:
+        seqset.close()
+
+
+def _nearest_in_set(subsequence, seqset):
+    if len(seqset) == 0:
+        return NearestDistances(np.zeros(0, np.int32), np.zeros(0, np.int64))
+    with seqset._lock:
+        pat = seqset._bind(subsequence)
+        dist, end, _ = seqset._seq.haystack.nearest_per_record(pat)
+    return NearestDistances(dist, end)

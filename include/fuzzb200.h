@@ -293,6 +293,36 @@ int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, const uint32_t
                         int32_t *second_pattern, int32_t *second_dist, /* each: one entry per record */
                         struct fzb_stats_s *total);
 
+/*
+ * The nearest match without a distance limit (DESIGN.md section 5.14).  For the pattern P (m symbols) and the
+ * sequence S (n symbols), E(e) = min over 0 <= s <= e of lev(P, S[s:e]) for every end position e in 0..n (E(0) = m,
+ * E(e) <= m: the empty substring).  One scan of the resident sequence, the bit-vector form of Sellers' recurrence,
+ * computes them all and returns
+ *   dist        d* = the smallest E(e): fzb_search_levenshtein finds a match at max_l_dist == d* and none below;
+ *   n_ends      the number of e with E(e) == d*;
+ *   first_end   the smallest such e.
+ * Nothing is copied back per position.  `stats` (optional) reports the scan as the searches do, as route 11.
+ * Whole-sequence handles only: a shard or a handle in a world is refused with FZB_E_UNSUPPORTED, and so is a handle
+ * with a record set (as by fzb_has_near_match) and any non-zero flag.  The pattern as for the single searches
+ * (1 <= m <= FZB_MAX_PATTERN; only m <= 64 is tuned).  Every refusal and every error leaves the handle as it was; the
+ * call uses neither the handle's counters nor its output area, so the result of an earlier search stays valid and a
+ * following search behaves as if the call had not happened.
+ */
+int fzb_nearest_distance(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
+                         uint32_t *dist, uint64_t *n_ends, uint64_t *first_end, struct fzb_stats_s *stats);
+
+/*
+ * The same for every record of a record set, in one scan: dist[r] = d* of record r alone and end[r] its first_end,
+ * relative to the start of the record; an empty record gives (m, 0).  The column of the recurrence is reset at every
+ * record start, so a separator is never read into an alignment, whatever its value.  The only read-back is 8 bytes
+ * per record.  Needs a handle with a record set (FZB_E_INVALID otherwise).  FZB_E_UNSUPPORTED: a record of 2^32
+ * bytes or more, any non-zero flag.  Every refusal and every error leaves the handle as it was; the arrays then hold
+ * nothing meaningful.
+ */
+int fzb_nearest_per_record(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
+                           int32_t *dist, int64_t *end, /* each: one entry per record */
+                           struct fzb_stats_s *stats);
+
 /* ExactSearch.search (search_exact.py:80-85): all (overlapping) occurrences. FINAL == RAW. */
 int fzb_search_exact(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
                      fzb_result **out);
@@ -349,7 +379,7 @@ typedef struct fzb_stats_s {
     uint32_t route;         /* 0 exact, 1 n-grams (sampled filter), 2 n-grams (dense filter), 3 LP,
                                4 hamming, 5 generic n-grams, 6 generic LP, 7 batch (summed statistics),
                                8 hamming batch scan, 9 generic n-grams batch scan, 10 generic LP batch
-                               scan */
+                               scan, 11 nearest/bit-vector-scan */
 } fzb_stats;
 int fzb_result_stats(const fzb_result *r, fzb_stats *out);
 void fzb_result_destroy(fzb_result *r);
