@@ -1923,6 +1923,9 @@ static int finish_global(fzb_haystack *h, fzb_result *res) {
         if (res->fused_status == MS_TIMEOUT)
             return fail(FZB_E_CUDA, "multi-GPU reduction timed out waiting for a peer (rank %d of %d)", h->rank, h->world);
     }
+    if (h->local_world && res->fused_issued && res->fused_status == MS_OVERFLOW)
+        return fail(FZB_E_UNSUPPORTED, "NCCL-free world: more than %u groups continue across shard seams; the staged "
+                    "fallback needs an NCCL communicator (fzb_haystack_comm_init)", kMaxNonHeads);
     if (h->local_world)
         return fail(FZB_E_UNSUPPORTED, "NCCL-free world: a shard produced more than %u groups (or more than %d raw "
                     "matches); the staged fallback needs an NCCL communicator (fzb_haystack_comm_init)", h->p2p_cap, kPostMax);

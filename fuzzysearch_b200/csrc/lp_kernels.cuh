@@ -206,8 +206,10 @@ k_lev_lp(const ScanParams p, uint32_t *scratch, int cap, RawRec *out, uint32_t o
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     uint32_t *A = scratch + tid * 2 * (int64_t)cap, *B = A + cap;
     if (p.k >= p.m) {  // levenshtein.py:62-65: an empty match (i,i,m) at every index 0..N
-        // (with records: 0..n_r of every record, i.e. every buffer position, separators included, but not N)
-        const int64_t hi = (p.own_hi == p.N) ? p.N + (REC ? 0 : 1) : p.own_hi;
+        // (with records: 0..n_r of every record, i.e. every buffer position, separators included, but not N).
+        // N itself belongs to the one shard whose non-empty range ends there, not to empty ranges [N, N) behind it.
+        const bool owns_end = p.own_hi == p.N && (p.own_lo < p.N || p.N == 0);
+        const int64_t hi = owns_end ? p.N + (REC ? 0 : 1) : p.own_hi;
         for (int64_t i = p.own_lo + tid; i < hi; i += stride) emit(out, ocap, counters, i, i, i, p.m, 1);
         return;
     }
