@@ -24,7 +24,8 @@ F_PER_RECORD = 128  # batches on a handle with a record set: per-record results 
 
 ROUTE_NAMES = {7: "batch", 0: "exact", 1: "ngrams/sampled-filter", 2: "ngrams/dense-filter", 3: "lp",
                4: "hamming", 5: "generic-ngrams", 6: "generic-lp", 8: "hamming/batch-scan",
-               9: "generic-ngrams/batch-scan", 10: "generic-lp/batch-scan", 11: "nearest/bit-vector-scan"}
+               9: "generic-ngrams/batch-scan", 10: "generic-lp/batch-scan", 11: "nearest/bit-vector-scan",
+               12: "nearest/batch-bit-vector-scan"}
 
 
 class NativeLibraryMissing(ImportError):
@@ -90,6 +91,9 @@ SYMBOLS = {
                                    ctypes.POINTER(Stats)]),
     "fzb_nearest_distance": (_i32, [_vp, _u8p, _u32, _u32, _vp, _vp, _vp, ctypes.POINTER(Stats)]),
     "fzb_nearest_per_record": (_i32, [_vp, _u8p, _u32, _u32, _vp, _vp, ctypes.POINTER(Stats)]),
+    "fzb_nearest_distance_batch": (_i32, [_vp, _u8p, _vp, _u32, _u32, _vp, _vp, ctypes.POINTER(Stats)]),
+    "fzb_nearest_best_per_record": (_i32, [_vp, _u8p, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp,
+                                           ctypes.POINTER(Stats)]),
     "fzb_find_near_matches": (_i32, [_u8p, _u32, _u8p, _u64, _u32, _u32, _u32, _u32, _i32, _vpp]),
     "fzb_has_near_match": (_i32, [_vp, _u8p, _u32, _u32, _u32, _u32, _u32, ctypes.POINTER(ctypes.c_int)]),
     "fzb_release_workspace": (None, []),
@@ -437,6 +441,34 @@ class Haystack(object):
         check(lib().fzb_nearest_per_record(self._h, pp, m, flags, ctypes.c_void_p(dist.ctypes.data),
                                            ctypes.c_void_p(end.ctypes.data), ctypes.byref(st)))
         return dist, end, _scan_stats(st)
+
+    @staticmethod
+    def _blob(patterns):
+        pats = [as_u8(p) for p in patterns]
+        blob = np.concatenate(pats) if pats else np.zeros(1, np.uint8)
+        offsets = np.zeros(len(pats) + 1, dtype=np.uint32)
+        offsets[1:] = np.cumsum([p.size for p in pats])
+        return blob, offsets, len(pats)
+
+    def nearest_distance_batch(self, patterns, flags=0):
+        """fzb_nearest_distance_batch: fzb_nearest_distance's (dist, first_end) for every pattern, in shared scans ->
+        (dist int32, first_end int64: one entry per pattern; stats dict)."""
+        blob, offsets, n = self._blob(patterns)
+        dist, first_end, st = np.empty(n, dtype=np.uint32), np.empty(n, dtype=np.uint64), Stats()
+        check(lib().fzb_nearest_distance_batch(self._h, ptr(blob), ptr(offsets), n, flags,
+                                               ctypes.c_void_p(dist.ctypes.data),
+                                               ctypes.c_void_p(first_end.ctypes.data), ctypes.byref(st)))
+        return dist.astype(np.int32), first_end.astype(np.int64), _scan_stats(st)
+
+    def nearest_best_per_record(self, patterns, flags=0):
+        """fzb_nearest_best_per_record on a handle with a record set -> ((pattern int32, dist int32, end int64,
+        second_pattern int32, second_dist int32): one entry per record; stats dict)."""
+        blob, offsets, n = self._blob(patterns)
+        cols = [np.empty(self.record_count, dtype=t) for t in (np.int32, np.int32, np.int64, np.int32, np.int32)]
+        st = Stats()
+        check(lib().fzb_nearest_best_per_record(self._h, ptr(blob), ptr(offsets), n, flags,
+                                                *[ctypes.c_void_p(c.ctypes.data) for c in cols], ctypes.byref(st)))
+        return tuple(cols), _scan_stats(st)
 
     def has_near_match(self, pattern, max_subs, max_ins, max_dels, max_l):
         """True iff the search would return at least one match; stops at the first chunk that holds one."""

@@ -164,6 +164,12 @@ struct NearBufs {  // fzb_nearest_distance / fzb_nearest_per_record (nearest_ker
     DevBuf<uint64_t> d_head;   // the whole-sequence result (2 words), then the partials of kNearMaxGrid CTAs
     DevBuf<uint64_t> d_words;  // one word per record
 };
+struct NearBatchBufs {  // fzb_nearest_distance_batch / fzb_nearest_best_per_record (nearest_kernels.cuh)
+    DevBuf<uint32_t> d_lanes;  // m | ordinal << 16 per lane of every group
+    DevBuf<uint8_t> d_pats;    // kNearBatchMaxM bytes per lane
+    DevBuf<uint64_t> d_words;  // whole sequence: one word per pattern; record set: best[records], then top2[records]
+    DevBuf<uint64_t> d_aux;    // a long pattern's k_nearest_scan: the partials of kNearMaxGrid CTAs, its record words
+};
 struct GatherBufs {  // the staged NCCL all-gather
     uint32_t cap = 0;  // rows per rank
     DevBuf<int64_t> d_send, d_recv;
@@ -302,6 +308,7 @@ struct fzb_haystack {
     std::unique_ptr<BestBufs> bestb;
     BestState *best = nullptr;      // set for the duration of fzb_best_per_record (BestScope)
     std::unique_ptr<NearBufs> nearb;
+    std::unique_ptr<NearBatchBufs> nearbatch;
 };
 
 struct fzb_result {
@@ -3478,6 +3485,16 @@ static int launch_nearest(fzb_haystack *h, int grid, const NearParams &p, const 
     return FZB_OK;
 }
 
+// k_nearest_scan's segment (bytes per thread) and grid for the handle's buffer: segments long against the 2m warm-up
+// on a long sequence, short enough to fill the SMs on a short one
+static int near_geometry(const fzb_haystack *h, int bits, int32_t *seg) {
+    *seg = (int32_t)std::min<uint64_t>(kNearMaxSeg, std::max<uint64_t>(kNearMinSeg,
+                                       round_up(h->buf_len / ((uint64_t)h->sm_count * 1024) + 1, 16)));
+    const uint64_t tile = (uint64_t)kNearThreads * *seg, ntiles = (h->buf_len + tile - 1) / tile;
+    const int per_sm = bits == 32 ? 4 : bits == 64 ? 3 : 2;
+    return (int)std::min<uint64_t>(ntiles, std::min<uint64_t>((uint64_t)h->sm_count * per_sm, kNearMaxGrid));
+}
+
 // The scan over the whole buffer, per record if `rec`.  It keeps to its own buffer group: the counters, the output
 // area and a pending result of the handle are not touched.  On FZB_OK the answer is in nearb->d_head[0..1] or
 // nearb->d_words, and the stream has drained.
@@ -3496,17 +3513,12 @@ static int nearest_scan(fzb_haystack *h, const uint8_t *pattern, uint32_t m, boo
     p.H = h->d;
     p.N = (int64_t)h->buf_len;
     p.m = (int)m;
-    // segments long against the 2m warm-up on a long sequence, short enough to fill the SMs on a short one
-    p.seg = (int)std::min<uint64_t>(kNearMaxSeg, std::max<uint64_t>(kNearMinSeg,
-                                    round_up(h->buf_len / ((uint64_t)h->sm_count * 1024) + 1, 16)));
     p.result = h->nearb->d_head.get();
     p.partial = p.result + 2;
     p.words = h->nearb->d_words.get();
     memcpy(p.P, pattern, m);
     const int bits = m <= 32 ? 32 : (int)round_up(m, 64);
-    const uint64_t tile = (uint64_t)kNearThreads * p.seg, ntiles = (h->buf_len + tile - 1) / tile;
-    const int per_sm = bits == 32 ? 4 : bits == 64 ? 3 : 2;
-    const int grid = (int)std::min<uint64_t>(ntiles, std::min<uint64_t>((uint64_t)h->sm_count * per_sm, kNearMaxGrid));
+    const int grid = near_geometry(h, bits, &p.seg);
     fzb_stats st{};
     st.route = 11;
     st.bytes_scanned = h->buf_len;
@@ -3588,6 +3600,241 @@ extern "C" int fzb_nearest_per_record(fzb_haystack *h, const uint8_t *pattern, u
     for (uint64_t r = 0; r < nrec; r++) {
         dist[r] = (int32_t)(words[r] >> 32);
         end[r] = (int64_t)(words[r] & 0xFFFFFFFFull);
+    }
+    return FZB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// fzb_nearest_distance_batch / fzb_nearest_best_per_record (DESIGN.md section 5.15): many patterns in shared scans
+// ------------------------------------------------------------------------------------------------
+constexpr int64_t kNearBatchMinSeg = 1024;  // bytes per warp: the warm-up (at most 128 bytes) stays <= 1/8 of it
+
+template <int BITS, bool REC>
+static int launch_nearest_batch(fzb_haystack *h, dim3 grid, const NearBatchParams &p, const RecSet &rs) {
+    CK(cudaFuncSetAttribute(k_nearest_batch_scan<BITS, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)near_smem(BITS)));
+    k_nearest_batch_scan<BITS, REC><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
+    CK(cudaGetLastError());
+    return FZB_OK;
+}
+
+// Every pattern checked as its single search would take it (the caller checked the rest): FZB_OK or the refusal
+static int check_nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count,
+                               uint32_t flags, const char *what) {
+    if (flags) return fail(FZB_E_UNSUPPORTED, "%s takes no flags", what);
+    if (count > kBestMaxPatterns) return fail(FZB_E_UNSUPPORTED, "more than %u patterns in one %s call", kBestMaxPatterns, what);
+    if (h->comm || h->local_world || h->peer) return fail(FZB_E_UNSUPPORTED, "%s: a handle in a world", what);
+    for (uint32_t i = 0; i < count; i++) {
+        if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
+        TRY(check_pattern(h, patterns + offsets[i], offsets[i + 1] - offsets[i], 0));
+    }
+    return FZB_OK;
+}
+
+// The scans of all `count` patterns over the whole buffer, per record if `rec`: the patterns of up to 64 symbols in
+// groups of 32 lanes (k_nearest_batch_scan, one launch per word class), longer ones one by one (k_nearest_scan, folded
+// by k_nearest_fold per record).  Its own buffer group only, as nearest_scan.  On FZB_OK the answer is in
+// nearbatch->d_words and the stream has drained.
+static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count, bool rec,
+                         fzb_stats *stats) {
+    auto len = [&](uint32_t i) { return offsets[i + 1] - offsets[i]; };
+    // by (class, m): the lanes of a group share the warm-up of its longest pattern
+    std::vector<uint32_t> order, longs;
+    for (uint32_t i = 0; i < count; i++) (len(i) <= kNearBatchMaxM ? order : longs).push_back(i);
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) {
+        return std::make_pair(len(x) > 32, len(x)) < std::make_pair(len(y) > 32, len(y));
+    });
+    std::vector<uint32_t> lanes;
+    std::vector<uint8_t> pats;
+    uint32_t groups[2] = {0, 0};
+    for (uint32_t i : order) {
+        const int cls = len(i) > 32;
+        if (cls == 1 && groups[1] == 0) lanes.resize(round_up(lanes.size(), kNearBatchLanes), 0);
+        if (lanes.size() % kNearBatchLanes == 0) groups[cls]++;
+        lanes.push_back(len(i) | i << 16);
+    }
+    lanes.resize(round_up(lanes.size(), kNearBatchLanes), 0);
+    pats.assign(lanes.size() * kNearBatchMaxM, 0);
+    for (size_t l = 0; l < lanes.size(); l++)
+        if (lanes[l]) memcpy(&pats[l * kNearBatchMaxM], patterns + offsets[lanes[l] >> 16], lanes[l] & 0xFFFFu);
+
+    CK(cudaSetDevice(h->device));
+    const uint64_t nrec = rec ? h->recs->d_off.size() - 1 : 0;
+    const uint64_t need_lanes = std::max<uint64_t>(lanes.size(), 1), need_words = std::max<uint64_t>(rec ? 2 * nrec : count, 1);
+    const uint64_t need_aux = 2 * (uint64_t)kNearMaxGrid + (rec && !longs.empty() ? nrec : 0);
+    NearBatchBufs *g = h->nearbatch.get();
+    if (!g || g->d_lanes.size() < need_lanes || g->d_words.size() < need_words || g->d_aux.size() < need_aux) {
+        std::unique_ptr<NearBatchBufs> grown;  // built whole, beside the one it replaces
+        TRY(ensure_group(grown, [&](NearBatchBufs &b) -> int {
+            const uint64_t nl = std::max<uint64_t>(need_lanes, g ? g->d_lanes.size() : 0);
+            TRY(b.d_lanes.alloc(nl));
+            TRY(b.d_pats.alloc(nl * kNearBatchMaxM));
+            TRY(b.d_words.alloc(std::max<uint64_t>(need_words, g ? g->d_words.size() : 0)));
+            return b.d_aux.alloc(std::max<uint64_t>(need_aux, g ? g->d_aux.size() : 0));
+        }));
+        h->nearbatch = std::move(grown);
+        g = h->nearbatch.get();
+    }
+    uint64_t *best = g->d_words.get(), *top2 = best + nrec;
+    fzb_stats st{};
+    st.route = 12;
+    CK(cudaEventRecord(h->ev[0], h->stream));
+    if (!lanes.empty()) {
+        CK(cudaMemcpyAsync(g->d_lanes.get(), lanes.data(), lanes.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(g->d_pats.get(), pats.data(), pats.size(), cudaMemcpyHostToDevice, h->stream));
+    }
+    if (rec) {  // the constants of nearest_kernels.cuh: (min m, its ordinal, end 0) and the two smallest (m_i, i)
+        uint64_t key = kBestEmpty, pair2 = kBestEmpty;
+        for (uint32_t i = 0; i < count; i++) {
+            key = std::min<uint64_t>(key, (uint64_t)len(i) << 48 | (uint64_t)i << 32);
+            pair2 = best_top2_merge(pair2, len(i) << 16 | i);
+        }
+        const int fill_grid = (int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8);
+        k_nearest_fill<<<fill_grid, 256, 0, h->stream>>>(best, nrec, key);
+        k_nearest_fill<<<fill_grid, 256, 0, h->stream>>>(top2, nrec, pair2);
+        st.n_launches += 2;
+    } else {  // every pattern's end position 0
+        std::vector<uint64_t> init(count);
+        for (uint32_t i = 0; i < count; i++) init[i] = (uint64_t)len(i) << 48;
+        CK(cudaMemcpyAsync(best, init.data(), count * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+        CK(cudaStreamSynchronize(h->stream));  // (`init` is a pageable local)
+    }
+    CK(cudaGetLastError());
+    const RecSet rs = rec_set(h);
+    uint32_t lane0 = 0;
+    for (int cls = 0; cls < 2; cls++) {
+        if (!groups[cls]) continue;
+        const int per_sm = cls ? 3 : 4;
+        // one wave of CTAs over all groups, one segment per warp: long segments (a small warm-up share) on a long
+        // sequence, at least kNearBatchMinSeg on a short one
+        uint64_t gx = std::max<uint64_t>(1, (uint64_t)h->sm_count * per_sm / groups[cls]);
+        const uint64_t warps = gx * (kNearThreads / 32);
+        NearBatchParams p{};
+        p.H = h->d;
+        p.N = (int64_t)h->buf_len;
+        p.seg = (int64_t)std::max<uint64_t>(kNearBatchMinSeg, round_up((h->buf_len + warps - 1) / warps, 16));
+        gx = std::min<uint64_t>(gx, (h->buf_len + (kNearThreads / 32) * p.seg - 1) / ((kNearThreads / 32) * p.seg));
+        p.lanes = g->d_lanes.get() + lane0;
+        p.pats = g->d_pats.get() + (uint64_t)lane0 * kNearBatchMaxM;
+        p.whole = best;
+        p.best = best;
+        p.top2 = top2;
+        lane0 += groups[cls] * kNearBatchLanes;
+        if (gx == 0) continue;  // (an empty buffer)
+        const dim3 grid((unsigned)gx, groups[cls]);
+        int rc = FZB_OK;
+        with_recs(h, [&](auto r) {
+            constexpr bool R = decltype(r)::value;
+            rc = cls ? launch_nearest_batch<64, R>(h, grid, p, rs) : launch_nearest_batch<32, R>(h, grid, p, rs);
+        });
+        TRY(rc);
+        st.n_launches++;
+        st.bytes_scanned += h->buf_len;
+    }
+    for (uint32_t i : longs) {  // 65-255 symbols: the single scan, pattern by pattern
+        const uint32_t m = len(i);
+        NearParams q{};
+        q.H = h->d;
+        q.N = (int64_t)h->buf_len;
+        q.m = (int)m;
+        q.result = best + i;  // (whole sequence: the pattern's word, prefilled)
+        q.partial = g->d_aux.get();
+        q.words = g->d_aux.get() + 2 * (uint64_t)kNearMaxGrid;
+        memcpy(q.P, patterns + offsets[i], m);
+        const int bits = (int)round_up(m, 64);
+        const int grid = near_geometry(h, bits, &q.seg);
+        if (rec) {
+            k_nearest_fill<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
+                q.words, nrec, (uint64_t)m << 32);
+            CK(cudaGetLastError());
+            st.n_launches++;
+        }
+        if (grid > 0) {
+            int rc = FZB_OK;
+            with_recs(h, [&](auto r) {
+                constexpr bool R = decltype(r)::value;
+                rc = bits == 128   ? launch_nearest<128, R>(h, grid, q, rs)
+                     : bits == 192 ? launch_nearest<192, R>(h, grid, q, rs)
+                                   : launch_nearest<256, R>(h, grid, q, rs);
+            });
+            TRY(rc);
+            st.n_launches++;
+            st.bytes_scanned += h->buf_len;
+        }
+        if (rec) {
+            k_nearest_fold<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
+                q.words, nrec, m, i, best, top2);
+            CK(cudaGetLastError());
+            st.n_launches++;
+        }
+    }
+    CK(cudaEventRecord(h->ev[1], h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
+    st.gpu_ms = st.filter_ms = ms;
+    if (stats) *stats = st;
+    return FZB_OK;
+}
+
+extern "C" int fzb_nearest_distance_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
+                                          uint32_t count, uint32_t flags, uint32_t *dist, uint64_t *first_end,
+                                          fzb_stats *stats) {
+    HandleLock handle_lock(h);
+    if (!h || (count && (!patterns || !offsets || !dist || !first_end))) return fail(FZB_E_INVALID, "NULL argument");
+    if (!is_whole_sequence(h))
+        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_distance_batch needs a whole (unsharded) sequence outside a world");
+    TRY(check_nearest_batch(h, patterns, offsets, count, flags, "fzb_nearest_distance_batch"));
+    TRY(refuse_records(h, "fzb_nearest_distance_batch"));
+    if (stats) *stats = fzb_stats{};
+    if (count == 0) return FZB_OK;
+    TRY(nearest_batch(h, patterns, offsets, count, false, stats));
+    // one read-back of 8 bytes per pattern
+    std::vector<uint64_t> words(count);
+    CK(cudaMemcpyAsync(words.data(), h->nearbatch->d_words.get(), count * sizeof(uint64_t), cudaMemcpyDeviceToHost,
+                       h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    for (uint32_t i = 0; i < count; i++) {
+        dist[i] = (uint32_t)(words[i] >> 48);
+        first_end[i] = words[i] & kNearNoEnd;
+    }
+    return FZB_OK;
+}
+
+extern "C" int fzb_nearest_best_per_record(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
+                                           uint32_t count, uint32_t flags, int32_t *pattern, int32_t *dist,
+                                           int64_t *end, int32_t *second_pattern, int32_t *second_dist,
+                                           fzb_stats *stats) {
+    HandleLock handle_lock(h);
+    if (!h || !pattern || !dist || !end || !second_pattern || !second_dist || (count && (!patterns || !offsets)))
+        return fail(FZB_E_INVALID, "NULL argument");
+    if (!h->recs) return fail(FZB_E_INVALID, "fzb_nearest_best_per_record needs a handle with a record set");
+    TRY(check_nearest_batch(h, patterns, offsets, count, flags, "fzb_nearest_best_per_record"));
+    if (h->recs->longest > (1ull << 32))
+        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_best_per_record needs records shorter than 2^32");
+    const uint64_t nrec = h->recs->d_off.size() - 1;
+    if (stats) *stats = fzb_stats{};
+    if (count == 0) {
+        for (uint64_t r = 0; r < nrec; r++) {
+            pattern[r] = dist[r] = second_pattern[r] = second_dist[r] = -1;
+            end[r] = -1;
+        }
+        return FZB_OK;
+    }
+    TRY(nearest_batch(h, patterns, offsets, count, true, stats));
+    // one read-back of 16 bytes per record
+    std::vector<uint64_t> words(2 * nrec);
+    CK(cudaMemcpyAsync(words.data(), h->nearbatch->d_words.get(), 2 * nrec * sizeof(uint64_t), cudaMemcpyDeviceToHost,
+                       h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    for (uint64_t r = 0; r < nrec; r++) {
+        const uint64_t b = words[r];
+        const uint32_t second = (uint32_t)words[nrec + r] & kBestPairNone;
+        dist[r] = (int32_t)(b >> 48);
+        pattern[r] = (int32_t)((b >> 32) & 0xFFFFu);
+        end[r] = (int64_t)(b & 0xFFFFFFFFull);
+        second_dist[r] = second == kBestPairNone ? -1 : (int32_t)(second >> 16);
+        second_pattern[r] = second == kBestPairNone ? -1 : (int32_t)(second & 0xFFFFu);
     }
     return FZB_OK;
 }

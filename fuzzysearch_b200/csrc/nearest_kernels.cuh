@@ -28,6 +28,7 @@
 // k_nearest_fill set to the empty record's (m, 0).  The end position 0 (score m) is that initial value in both forms.
 #pragma once
 #include "common.cuh"
+#include "best_kernels.cuh"
 
 namespace fzb {
 
@@ -241,6 +242,189 @@ __global__ void k_nearest_count(uint64_t *result, const uint64_t *partial, uint3
     for (uint32_t i = threadIdx.x; i < nparts; i += blockDim.x)
         if (partial[2 * i] == best) sum += partial[2 * i + 1];
     if (sum) atomicAdd((unsigned long long *)&result[1], (unsigned long long)sum);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// fzb_nearest_distance_batch / fzb_nearest_best_per_record (DESIGN.md section 5.15): many patterns at once.
+//
+// k_nearest_batch_scan is the transpose of k_nearest_scan: one lane per pattern, one segment per warp.  The host sorts
+// the patterns of one word class (m <= 32 or m <= 64) by length and packs them into groups of 32 lanes; gridDim.y is
+// the group.  Every CTA builds its group's table PM[c][lane] (thread c writes byte c's masks of all 32 lanes), so the
+// lookup of one text byte by all lanes hits 32 different banks, as in the replicated table of the single scan.  The
+// warp walks its segment in lockstep: its text loads and byte extractions are the same for all lanes.  It warms up
+// from max(a - 2 max m of its group, record start); a warm-up longer than a lane's own 2 m_i is exact as well (the
+// argument at the top of this file: a column started earlier only adds starts that cannot win for e >= w + 2 m_i).
+// A lane carries the ORIGINAL ordinal of its pattern (16 bits), so ties are broken by index whatever the grouping;
+// idle lanes of a last group (m = 0) run along but never report.
+//
+// Whole sequence: a lane keeps its minimum and first end over its warp's segments, the CTA combines them per lane in
+// shared memory and sends one atomicMin of dist << 48 | first_end per (CTA, pattern) into that pattern's word, which
+// the host prefilled with m_i << 48 (the end position 0).
+//
+// Record sets: at every record end (or segment end) each lane with best < m_i offers key = dist << 48 | ordinal << 32
+// | end.  The warp takes the minimum key and, over the lanes whose ordinal differs from the winner's, the minimum pair
+// dist << 16 | ordinal; lane 0 sends one atomicMin into best[r] and merges both pairs into top2[r] (best_top2_merge's
+// word of best_kernels.cuh).  Both words start as constants: best[r] = (min m_i, its smallest ordinal, end 0) and
+// top2[r] = the two smallest pairs (m_i, i).  That is exact although lanes only report scores below their m_i:
+// d*_i <= m_i for every pattern, so a pattern left out of the prefill sits behind two patterns j, k whose
+// (d*_j, j) <= (m_j, j) < (m_i, i) <= (d*_i, i) -- it can be neither first nor second, and a pattern that is never
+// reported has d*_i = m_i with its first end at 0, which is what the prefill says for it.  All updates are minima, so
+// the words depend neither on thread, warp or CTA order nor on how records are split over segments.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int kNearBatchLanes = 32;
+constexpr int kNearBatchMaxM = 64;  // bytes per lane of the pattern buffer
+
+struct NearBatchParams {
+    const uint8_t *H;
+    int64_t N, seg;         // seg: bytes per warp (a multiple of 16)
+    const uint32_t *lanes;  // per lane of every group of this launch: m | ordinal << 16; 0 = idle
+    const uint8_t *pats;    // kNearBatchMaxM bytes per lane
+    uint64_t *whole;        // per ordinal: dist << 48 | first_end
+    uint64_t *best, *top2;  // REC: per record
+};
+
+// `pair` (dist << 16 | ordinal) and `pair2` merged into the top2 word of a record (kBestPairNone: nothing)
+__device__ __forceinline__ void near_top2_add(uint64_t *top2, uint32_t pair, uint32_t pair2) {
+    unsigned long long seen = kBestEmpty;  // (a guess: the first CAS returns the word as it is)
+    for (;;) {
+        unsigned long long want = best_top2_merge(seen, pair);
+        if (pair2 != kBestPairNone) want = best_top2_merge(want, pair2);
+        if (want == seen) break;
+        const unsigned long long was = atomicCAS((unsigned long long *)top2, seen, want);
+        if (was == seen) break;
+        seen = was;
+    }
+}
+
+// The warp's report of one record (all 32 lanes call it with the same record): key as above, ~0 = none
+__device__ __forceinline__ void near_batch_report(uint64_t key, uint64_t *best, uint64_t *top2) {
+    uint64_t kmin = key;
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        const uint64_t o = __shfl_xor_sync(0xFFFFFFFFu, kmin, d);
+        kmin = o < kmin ? o : kmin;
+    }
+    if (kmin == ~0ull) return;  // (the same for every lane)
+    const uint32_t win = (uint32_t)(kmin >> 32);
+    uint32_t second = key != ~0ull && ((uint32_t)(key >> 32) & 0xFFFFu) != (win & 0xFFFFu) ? (uint32_t)(key >> 32)
+                                                                                          : kBestPairNone;
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        const uint32_t o = __shfl_xor_sync(0xFFFFFFFFu, second, d);
+        second = o < second ? o : second;
+    }
+    if ((threadIdx.x & 31u) == 0) {
+        atomicMin((unsigned long long *)best, (unsigned long long)kmin);
+        near_top2_add(top2, win, second);
+    }
+}
+
+template <int BITS, bool REC>
+__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : 3)
+k_nearest_batch_scan(NearBatchParams p, RecSet rs) {
+    static_assert(BITS == 32 || BITS == 64, "one word per lane");
+    typedef typename NearWord<BITS>::type word;
+    extern __shared__ __align__(16) uint64_t near_smem_raw[];
+    __shared__ __align__(16) uint8_t s_pat[kNearBatchLanes * kNearBatchMaxM];
+    __shared__ uint32_t s_m[kNearBatchLanes];
+    __shared__ uint64_t s_key[kNearThreads / 32][kNearBatchLanes];
+    word *pm = reinterpret_cast<word *>(near_smem_raw);
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    const uint32_t *lanes = p.lanes + (size_t)blockIdx.y * kNearBatchLanes;
+    const uint8_t *pats = p.pats + (size_t)blockIdx.y * kNearBatchLanes * kNearBatchMaxM;
+
+    for (uint32_t i = threadIdx.x; i < kNearBatchLanes * kNearBatchMaxM; i += kNearThreads) s_pat[i] = pats[i];
+    if (threadIdx.x < kNearBatchLanes) s_m[threadIdx.x] = lanes[threadIdx.x] & 0xFFFFu;
+    __syncthreads();
+    {  // thread c builds the masks of byte c for every lane
+        const uint32_t c = threadIdx.x;
+        for (int l = 0; l < kNearBatchLanes; l++) {
+            word mask = 0;
+            for (uint32_t i = 0; i < s_m[l]; i++)
+                if (s_pat[l * kNearBatchMaxM + i] == c) mask |= (word)1 << i;
+            pm[c * kNearBatchLanes + l] = mask;
+        }
+    }
+    __syncthreads();
+
+    const uint32_t info = lanes[lane], ord = info >> 16;
+    const bool idle = (info & 0xFFFFu) == 0;
+    const uint32_t m = idle ? 1u : info & 0xFFFFu;
+    uint32_t gm = m;  // the longest pattern of the group: the warm-up of every lane
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        const uint32_t o = __shfl_xor_sync(0xFFFFFFFFu, gm, d);
+        gm = o > gm ? o : gm;
+    }
+    NearCol<BITS> col;
+    col.pm = pm + lane;
+    col.top = m - 1;
+    uint32_t tbest = m;  // whole sequence: over all segments of this warp
+    uint64_t tfirst = kNearNoEnd;
+
+    const int64_t tile = (int64_t)(kNearThreads / 32) * p.seg;
+    for (int64_t base = (int64_t)blockIdx.x * tile; base < p.N; base += (int64_t)gridDim.x * tile) {
+        const int64_t a = base + (int64_t)warp * p.seg;
+        if (a >= p.N) continue;
+        const int64_t b = a + p.seg < p.N ? a + p.seg : p.N;
+        int64_t lo = 0, hi = p.N;  // the record around the column: [lo, hi), its separator at hi
+        uint32_t r = 0;
+        if (REC) {
+            r = rs.first[a >> kGranuleShift];
+            while ((int64_t)rs.off[r + 1] <= a) r++;
+            lo = (int64_t)rs.off[r];
+            hi = (int64_t)rs.off[r + 1] - 1;
+        }
+        col.reset(m);
+        const int64_t w = a - 2 * (int64_t)gm > lo ? a - 2 * (int64_t)gm : lo;
+        col.template run<false>(p.H, w, a, 0);
+        if (!REC) {
+            col.template run<true>(p.H, a, b, 1);
+            if (col.best < tbest) {  // (segments come in increasing order: an equal minimum keeps the earlier end)
+                tbest = col.best;
+                tfirst = (uint64_t)a + col.first;
+            }
+        } else {
+            int64_t x = a;
+            for (;;) {
+                const int64_t stop = b < hi ? b : hi;
+                if (x < stop) col.template run<true>(p.H, x, stop, (uint32_t)(x + 1 - lo));
+                const uint64_t key = !idle && col.best < m
+                                         ? (uint64_t)col.best << 48 | (uint64_t)ord << 32 | col.first
+                                         : ~0ull;
+                near_batch_report(key, p.best + r, p.top2 + r);
+                if (hi + 1 >= b) break;  // (the record behind the separator starts in another segment, or nowhere)
+                r++;
+                lo = hi + 1;
+                hi = (int64_t)rs.off[r + 1] - 1;
+                x = lo;
+                col.reset(m);
+            }
+        }
+    }
+    if (!REC) {  // per lane over the warps of the CTA, then one atomicMin per (CTA, pattern)
+        s_key[warp][lane] = !idle && tbest < m ? (uint64_t)tbest << 48 | tfirst : ~0ull;
+        __syncthreads();
+        if (warp == 0) {
+            uint64_t key = s_key[0][lane];
+            for (int i = 1; i < kNearThreads / 32; i++) key = s_key[i][lane] < key ? s_key[i][lane] : key;
+            if (key != ~0ull) atomicMin((unsigned long long *)&p.whole[ord], (unsigned long long)key);
+        }
+    }
+}
+
+// A pattern of 65-255 symbols scanned alone by k_nearest_scan<BITS, true>: its per-record words (dist << 32 | end)
+// folded into best / top2 as the lanes of k_nearest_batch_scan report.  One thread per record.
+__global__ void k_nearest_fold(const uint64_t *words, uint64_t nrec, uint32_t m, uint32_t ord, uint64_t *best,
+                               uint64_t *top2) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nrec; r += stride) {
+        const uint64_t w = words[r];
+        const uint32_t d = (uint32_t)(w >> 32);
+        if (d >= m) continue;
+        atomicMin((unsigned long long *)&best[r], (unsigned long long)d << 48 | (uint64_t)ord << 32 | (w & 0xFFFFFFFFull));
+        near_top2_add(&top2[r], d << 16 | ord, kBestPairNone);
+    }
 }
 
 }  // namespace fzb

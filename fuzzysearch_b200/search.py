@@ -29,7 +29,8 @@ def _text(seq):
 
 
 __all__ = ["DeviceSequence", "ExactSearch", "SubstitutionsOnlySearch", "LevenshteinSearch",
-           "GenericSearch", "RawMatches", "search_exact", "nearest_distance", "find_nearest_matches"]
+           "GenericSearch", "RawMatches", "search_exact", "nearest_distance", "find_nearest_matches",
+           "nearest_distance_batch", "find_nearest_matches_batch"]
 
 
 class DeviceSequence(object):
@@ -461,3 +462,67 @@ def find_nearest_matches(subsequence, sequence, max_l_dist=None):
             return _to_matches(res, _native.RAW if d == 0 else _native.FINAL, slicer)
         finally:
             res.close()
+
+
+def _nearest_batch(subsequences, sequence):
+    """-> (dist int32, first end int64) arrays, one entry per pattern.  The caller holds the sequence's lock."""
+    try:
+        pats, hay, _ = _prepare_many(subsequences, sequence)
+    except AlphabetTooLarge:
+        # wide symbols and more than 255 distinct ones over all the patterns: no common byte alphabet, so the
+        # patterns go one by one (each reduces the sequence to its own alphabet)
+        rows = []
+        for p in subsequences:
+            pat, hay, _, _ = _prepare(p, sequence)
+            rows.append(hay.nearest_distance(pat)[::2])  # (dist, first_end)
+        return np.array([d for d, _ in rows], dtype=np.int32), np.array([e for _, e in rows], dtype=np.int64)
+    dist, end, _ = hay.nearest_distance_batch(pats)
+    return dist, end
+
+
+def nearest_distance_batch(subsequences, sequence):
+    """Many patterns over one sequence, without a distance limit: -> NearestDistances with one entry per pattern,
+    ``dist[i] == nearest_distance(subsequences[i], sequence)`` and ``end[i]`` the first end position of a substring at
+    that distance.  The patterns of up to 64 symbols share scans of the sequence, 32 at a time
+    (fzb_nearest_distance_batch, DESIGN.md section 5.15).  `sequence` is anything find_near_matches takes."""
+    from .sequence_set import NearestDistances
+    subsequences = list(subsequences)
+    if any(len(p) == 0 for p in subsequences):
+        raise ValueError("Given subsequence is empty!")
+    if not subsequences:
+        return NearestDistances(np.zeros(0, np.int32), np.zeros(0, np.int64))
+    with _lock_for(sequence):
+        return NearestDistances(*_nearest_batch(subsequences, sequence))
+
+
+def find_nearest_matches_batch(subsequences, sequence, max_l_dist=None):
+    """Where does each pattern fit best?  -> exactly ``find_near_matches_batch(subsequences, sequence,
+    max_l_dist=[d_0, d_1, ...])`` with d_i = ``nearest_distance(subsequences[i], sequence)``, found by one batch of
+    shared scans and searched on the same upload.  `max_l_dist` (None, one int, or one value per pattern) caps d_i:
+    a pattern whose d_i is larger gets ``[]`` and is not searched."""
+    from . import _search_batch, choose_search_class, find_nearest_matches
+    from .common import LevenshteinSearchParams
+    subsequences = list(subsequences)
+    n = len(subsequences)
+    caps = max_l_dist if isinstance(max_l_dist, (list, tuple)) else [max_l_dist] * n
+    if len(caps) != n:
+        raise ValueError("one max_l_dist per subsequence expected")
+    if any(c is not None and (not isinstance(c, int) or c < 0) for c in caps):
+        raise ValueError("max_l_dist must be a non-negative integer or None")
+    if any(len(p) == 0 for p in subsequences):
+        raise ValueError("Given subsequence is empty!")
+    if not subsequences:
+        return []
+    with _lock_for(sequence):
+        try:
+            pats, hay, slicer = _prepare_many(subsequences, sequence)
+        except AlphabetTooLarge:
+            return [find_nearest_matches(p, sequence, c) for p, c in zip(subsequences, caps)]
+        dist, _, _ = hay.nearest_distance_batch(pats)
+        todo = [i for i in range(n) if caps[i] is None or dist[i] <= caps[i]]
+        params = [LevenshteinSearchParams(None, None, None, int(dist[i])) for i in todo]
+        lists = _search_batch(hay, [pats[i] for i in todo], params, [choose_search_class(p) for p in params], 0)
+    out = [[] for _ in range(n)]
+    for i, (s, e, d) in zip(todo, lists):
+        out[i] = [Match(a, b, c, matched=slicer(a, b)) for a, b, c in zip(s.tolist(), e.tolist(), d.tolist())]
+    return out

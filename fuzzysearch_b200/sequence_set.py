@@ -12,8 +12,9 @@ from . import _native
 from .common import LevenshteinSearchParams, Match
 from .search import DeviceSequence, ExactSearch, GenericSearch, LevenshteinSearch, _kind, _text
 
-__all__ = ["BestMatches", "DeviceSequenceSet", "NearestDistances", "best_match_in_each", "find_near_matches_in_each",
-           "find_near_matches_batch_in_each", "nearest_distance_in_each"]
+__all__ = ["BestMatches", "DeviceSequenceSet", "NearestDistances", "NearestPatterns", "best_match_in_each",
+           "find_near_matches_in_each", "find_near_matches_batch_in_each", "nearest_distance_in_each",
+           "nearest_pattern_in_each"]
 
 
 def _set_kind(sequences):
@@ -278,9 +279,10 @@ def _best_on_host(subsequences, seqset, limits):
 
 
 class NearestDistances(object):
-    """What nearest_distance_in_each returns: ``dist`` (int32) and ``end`` (int64), one entry per sequence -- the
-    smallest Levenshtein distance of the pattern to any substring of the sequence and the first end position (in the
-    sequence's own coordinates) of a substring at that distance.  ``nearest[r]`` is ``(dist, end)``."""
+    """What nearest_distance_in_each and nearest_distance_batch return: ``dist`` (int32) and ``end`` (int64), one
+    entry per sequence (nearest_distance_in_each) or per pattern (nearest_distance_batch) -- the smallest Levenshtein
+    distance of the pattern to any substring of the sequence and the first end position (in the sequence's own
+    coordinates) of a substring at that distance.  ``nearest[i]`` is ``(dist, end)``."""
 
     def __init__(self, dist, end):
         self.dist, self.end = dist, end
@@ -319,3 +321,78 @@ def _nearest_in_set(subsequence, seqset):
         pat = seqset._bind(subsequence)
         dist, end, _ = seqset._seq.haystack.nearest_per_record(pat)
     return NearestDistances(dist, end)
+
+
+class NearestPatterns(object):
+    """What nearest_pattern_in_each returns: five numpy arrays with one entry per sequence.  ``dist`` (int32): the
+    smallest nearest_distance of any pattern to the sequence; ``pattern`` (int32): the smallest index of a pattern at
+    that distance; ``end`` (int64): where its nearest match first ends, in the sequence's own coordinates (the end
+    nearest_distance_in_each gives for it); ``second_pattern``, ``second_dist`` (int32): the same over the OTHER
+    patterns, for rejecting ambiguous calls by ``second_dist - dist``.  Every pattern has a distance (at most its
+    length), so -1 appears only in the ``second_*`` arrays with a single pattern and everywhere with none.
+    ``nearest[r]`` is ``(pattern, dist, end)``."""
+
+    def __init__(self, columns):
+        self.pattern, self.dist, self.end, self.second_pattern, self.second_dist = columns
+
+    def __len__(self):
+        return len(self.pattern)
+
+    def __getitem__(self, r):
+        return int(self.pattern[r]), int(self.dist[r]), int(self.end[r])
+
+
+def _no_patterns(n):
+    return tuple(np.full(n, -1, dtype=t) for t in (np.int32, np.int32, np.int64, np.int32, np.int32))
+
+
+def nearest_pattern_in_each(subsequences, sequences):
+    """Many patterns over many sequences, without a distance limit: -> NearestPatterns, for every sequence the
+    pattern nearest to it, its distance and first end, and the runner-up among the other patterns -- what reducing
+    ``nearest_distance_in_each(p, sequences)`` over the patterns gives (ties to the smallest index), in shared scans
+    of all sequences with the reduction on the device (fzb_nearest_best_per_record, DESIGN.md section 5.15).  An
+    empty sequence gives the shortest pattern (the smallest index among equals), its length and the end 0.
+    `sequences` is a list / tuple (uploaded for this call) or a DeviceSequenceSet (resident)."""
+    subsequences = list(subsequences)
+    if any(len(p) == 0 for p in subsequences):
+        raise ValueError("Given subsequence is empty!")
+    if isinstance(sequences, DeviceSequenceSet):
+        return _nearest_patterns_in_set(subsequences, sequences)
+    if not isinstance(sequences, (list, tuple)):
+        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
+    if not sequences or not subsequences:
+        return NearestPatterns(_no_patterns(len(sequences)))
+    seqset = DeviceSequenceSet(sequences)
+    try:
+        return _nearest_patterns_in_set(subsequences, seqset)
+    finally:
+        seqset.close()
+
+
+def _nearest_patterns_in_set(subsequences, seqset):
+    n = len(seqset)
+    if n == 0 or not subsequences:
+        return NearestPatterns(_no_patterns(n))
+    from .search import AlphabetTooLarge
+    with seqset._lock:
+        try:
+            pats = seqset._bind_many(subsequences)
+        except AlphabetTooLarge:
+            pats = None  # no common byte alphabet: pattern by pattern, below
+        if pats is not None:
+            columns, _ = seqset._seq.haystack.nearest_best_per_record(pats)
+            return NearestPatterns(columns)
+    return NearestPatterns(_nearest_patterns_on_host(subsequences, seqset))
+
+
+def _nearest_patterns_on_host(subsequences, seqset):
+    """The same rows from nearest_distance_in_each, pattern by pattern (each reduces the set to its own alphabet)."""
+    pattern, dist, end, pat2, dist2 = columns = _no_patterns(len(seqset))
+    for i, p in enumerate(subsequences):
+        got = nearest_distance_in_each(p, seqset)
+        first = (pattern < 0) | (got.dist < dist)  # (an equal distance leaves the earlier pattern in place)
+        second = ~first & ((pat2 < 0) | (got.dist < dist2))
+        pat2[first], dist2[first] = pattern[first], dist[first]
+        pattern[first], dist[first], end[first] = i, got.dist[first], got.end[first]
+        pat2[second], dist2[second] = i, got.dist[second]
+    return columns

@@ -323,6 +323,38 @@ int fzb_nearest_per_record(fzb_haystack *h, const uint8_t *pattern, uint32_t m, 
                            int32_t *dist, int64_t *end, /* each: one entry per record */
                            struct fzb_stats_s *stats);
 
+/*
+ * Many patterns at once, without a distance limit (DESIGN.md section 5.15).  The patterns as for fzb_best_per_record:
+ * pattern i is patterns[offsets[i] .. offsets[i + 1]), count + 1 offsets, each pattern as its single search takes it.
+ * Patterns of up to 64 symbols share scans, 32 per warp (one lane per pattern); longer ones are scanned one by one.
+ *
+ * fzb_nearest_distance_batch: dist[i] and first_end[i] are what fzb_nearest_distance returns for pattern i (no n_ends).
+ * Whole (unsharded) sequences outside a world without a record set only.  The read-back is 8 bytes per pattern.
+ */
+int fzb_nearest_distance_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count,
+                               uint32_t flags, uint32_t *dist, uint64_t *first_end, /* each: one entry per pattern */
+                               struct fzb_stats_s *stats);
+
+/*
+ * fzb_nearest_best_per_record: for every record r of a record set, with d*_i(r) the dist fzb_nearest_per_record gives
+ * pattern i there,
+ *   dist[r]            min over i of d*_i(r);
+ *   pattern[r]         the smallest i that reaches it;
+ *   end[r]             the end fzb_nearest_per_record gives that pattern in r (relative to the record's start);
+ *   second_pattern[r], second_dist[r]   the smallest (d*_i(r), i) over the other patterns, -1 with a single pattern.
+ * Every pattern has a value (d*_i <= m_i), so an empty record gives (the smallest (m_i, i), 0); with no patterns every
+ * array is -1.  The read-back is 16 bytes per record.  Needs a handle with a record set (FZB_E_INVALID otherwise) whose
+ * records are shorter than 2^32.
+ *
+ * Both: FZB_E_UNSUPPORTED for any non-zero flag, more than 65 535 patterns, a shard or a handle in a world.  Every
+ * refusal and every error leaves the handle as it was; the calls use neither the handle's counters, its output area
+ * nor a pending result.  `stats` (optional) reports route 12.
+ */
+int fzb_nearest_best_per_record(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count,
+                                uint32_t flags, int32_t *pattern, int32_t *dist, int64_t *end, int32_t *second_pattern,
+                                int32_t *second_dist, /* each: one entry per record */
+                                struct fzb_stats_s *stats);
+
 /* ExactSearch.search (search_exact.py:80-85): all (overlapping) occurrences. FINAL == RAW. */
 int fzb_search_exact(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
                      fzb_result **out);
@@ -379,7 +411,8 @@ typedef struct fzb_stats_s {
     uint32_t route;         /* 0 exact, 1 n-grams (sampled filter), 2 n-grams (dense filter), 3 LP,
                                4 hamming, 5 generic n-grams, 6 generic LP, 7 batch (summed statistics),
                                8 hamming batch scan, 9 generic n-grams batch scan, 10 generic LP batch
-                               scan, 11 nearest/bit-vector-scan */
+                               scan, 11 nearest/bit-vector-scan,
+                               12 nearest/batch-bit-vector-scan */
 } fzb_stats;
 int fzb_result_stats(const fzb_result *r, fzb_stats *out);
 void fzb_result_destroy(fzb_result *r);
