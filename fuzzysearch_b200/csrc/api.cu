@@ -3478,9 +3478,16 @@ extern "C" int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, con
 // fzb_nearest_distance / fzb_nearest_per_record (DESIGN.md section 5.14): the nearest match without a distance limit
 // ------------------------------------------------------------------------------------------------
 template <int BITS, bool REC>
-static int launch_nearest(fzb_haystack *h, int grid, const NearParams &p, const RecSet &rs) {
-    CK(cudaFuncSetAttribute(k_nearest_scan<BITS, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)near_smem(BITS)));
-    k_nearest_scan<BITS, REC><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
+static int launch_nearest(fzb_haystack *h, int grid, const NearParams &p, const RecSet &rs, bool ham) {
+    if (ham) {
+        CK(cudaFuncSetAttribute(k_nearest_hamming_scan<BITS, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)near_smem(BITS)));
+        k_nearest_hamming_scan<BITS, REC><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
+    } else {
+        CK(cudaFuncSetAttribute(k_nearest_scan<BITS, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)near_smem(BITS)));
+        k_nearest_scan<BITS, REC><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
+    }
     CK(cudaGetLastError());
     return FZB_OK;
 }
@@ -3495,10 +3502,11 @@ static int near_geometry(const fzb_haystack *h, int bits, int32_t *seg) {
     return (int)std::min<uint64_t>(ntiles, std::min<uint64_t>((uint64_t)h->sm_count * per_sm, kNearMaxGrid));
 }
 
-// The scan over the whole buffer, per record if `rec`.  It keeps to its own buffer group: the counters, the output
-// area and a pending result of the handle are not touched.  On FZB_OK the answer is in nearb->d_head[0..1] or
-// nearb->d_words, and the stream has drained.
-static int nearest_scan(fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool rec, fzb_stats *stats) {
+// The scan over the whole buffer, per record if `rec`, under substitutions only if `ham` (DESIGN.md section 5.16).
+// It keeps to its own buffer group: the counters, the output area and a pending result of the handle are not
+// touched.  On FZB_OK the answer is in nearb->d_head[0..1] or nearb->d_words, and the stream has drained.  Without a
+// value (substitutions only: no window) the words keep their prefill, all ones.
+static int nearest_scan(fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool rec, bool ham, fzb_stats *stats) {
     CK(cudaSetDevice(h->device));
     const uint64_t nrec = rec ? h->recs->d_off.size() - 1 : 0;
     if (!h->nearb || h->nearb->d_words.size() < nrec) {  // built whole, beside the one it replaces
@@ -3520,14 +3528,14 @@ static int nearest_scan(fzb_haystack *h, const uint8_t *pattern, uint32_t m, boo
     const int bits = m <= 32 ? 32 : (int)round_up(m, 64);
     const int grid = near_geometry(h, bits, &p.seg);
     fzb_stats st{};
-    st.route = 11;
+    st.route = ham ? 13 : 11;
     st.bytes_scanned = h->buf_len;
     CK(cudaEventRecord(h->ev[0], h->stream));
     if (rec) {
         k_nearest_fill<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
-            p.words, nrec, (uint64_t)m << 32);
+            p.words, nrec, ham ? kBestEmpty : (uint64_t)m << 32);
     } else {
-        k_nearest_fill<<<1, 32, 0, h->stream>>>(p.result, 1, (uint64_t)m << 48);
+        k_nearest_fill<<<1, 32, 0, h->stream>>>(p.result, 1, ham ? kBestEmpty : (uint64_t)m << 48);
         CK(cudaMemsetAsync(p.result + 1, 0, sizeof(uint64_t), h->stream));
     }
     CK(cudaGetLastError());
@@ -3537,18 +3545,18 @@ static int nearest_scan(fzb_haystack *h, const uint8_t *pattern, uint32_t m, boo
         int rc = FZB_OK;
         with_recs(h, [&](auto r) {
             constexpr bool R = decltype(r)::value;
-            rc = bits == 32    ? launch_nearest<32, R>(h, grid, p, rs)
-                 : bits == 64  ? launch_nearest<64, R>(h, grid, p, rs)
-                 : bits == 128 ? launch_nearest<128, R>(h, grid, p, rs)
-                 : bits == 192 ? launch_nearest<192, R>(h, grid, p, rs)
-                               : launch_nearest<256, R>(h, grid, p, rs);
+            rc = bits == 32    ? launch_nearest<32, R>(h, grid, p, rs, ham)
+                 : bits == 64  ? launch_nearest<64, R>(h, grid, p, rs, ham)
+                 : bits == 128 ? launch_nearest<128, R>(h, grid, p, rs, ham)
+                 : bits == 192 ? launch_nearest<192, R>(h, grid, p, rs, ham)
+                               : launch_nearest<256, R>(h, grid, p, rs, ham);
         });
         TRY(rc);
         st.n_launches++;
     }
     CK(cudaEventRecord(h->ev[1], h->stream));
     if (!rec) {
-        k_nearest_count<<<1, 256, 0, h->stream>>>(p.result, p.partial, (uint32_t)grid, m);
+        k_nearest_count<<<1, 256, 0, h->stream>>>(p.result, p.partial, (uint32_t)grid, ham ? ~0u : m);
         CK(cudaGetLastError());
         st.n_launches++;
     }
@@ -3567,17 +3575,19 @@ extern "C" int fzb_nearest_distance(fzb_haystack *h, const uint8_t *pattern, uin
                                     uint32_t *dist, uint64_t *n_ends, uint64_t *first_end, fzb_stats *stats) {
     HandleLock handle_lock(h);
     if (!h || !dist || !n_ends || !first_end) return fail(FZB_E_INVALID, "NULL argument");
-    if (flags) return fail(FZB_E_UNSUPPORTED, "fzb_nearest_distance takes no flags");
+    if (flags & ~FZB_F_SUBSTITUTIONS_ONLY)
+        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_distance takes no flag other than FZB_F_SUBSTITUTIONS_ONLY");
     if (!is_whole_sequence(h) || h->comm || h->local_world || h->peer)
         return fail(FZB_E_UNSUPPORTED, "fzb_nearest_distance needs a whole (unsharded) sequence outside a world");
     TRY(refuse_records(h, "fzb_nearest_distance"));
     TRY(check_pattern(h, pattern, m, 0));
-    TRY(nearest_scan(h, pattern, m, false, stats));
+    TRY(nearest_scan(h, pattern, m, false, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0, stats));
     uint64_t out[2];
     CK(cudaMemcpyAsync(out, h->nearb->d_head.get(), sizeof out, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    *dist = (uint32_t)(out[0] >> 48);
-    *first_end = out[0] & kNearNoEnd;
+    const bool none = out[0] == kBestEmpty;  // (substitutions only: the sequence is shorter than the pattern)
+    *dist = none ? UINT32_MAX : (uint32_t)(out[0] >> 48);
+    *first_end = none ? UINT64_MAX : out[0] & kNearNoEnd;
     *n_ends = out[1];
     return FZB_OK;
 }
@@ -3587,19 +3597,21 @@ extern "C" int fzb_nearest_per_record(fzb_haystack *h, const uint8_t *pattern, u
     HandleLock handle_lock(h);
     if (!h || !dist || !end) return fail(FZB_E_INVALID, "NULL argument");
     if (!h->recs) return fail(FZB_E_INVALID, "fzb_nearest_per_record needs a handle with a record set");
-    if (flags) return fail(FZB_E_UNSUPPORTED, "fzb_nearest_per_record takes no flags");
+    if (flags & ~FZB_F_SUBSTITUTIONS_ONLY)
+        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_per_record takes no flag other than FZB_F_SUBSTITUTIONS_ONLY");
     if (h->recs->longest > (1ull << 32))
         return fail(FZB_E_UNSUPPORTED, "fzb_nearest_per_record needs records shorter than 2^32");
     TRY(check_pattern(h, pattern, m, 0));
-    TRY(nearest_scan(h, pattern, m, true, stats));
+    TRY(nearest_scan(h, pattern, m, true, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0, stats));
     // one read-back of 8 bytes per record
     const uint64_t nrec = h->recs->d_off.size() - 1;
     std::vector<uint64_t> words(nrec);
     CK(cudaMemcpyAsync(words.data(), h->nearb->d_words.get(), nrec * sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     for (uint64_t r = 0; r < nrec; r++) {
-        dist[r] = (int32_t)(words[r] >> 32);
-        end[r] = (int64_t)(words[r] & 0xFFFFFFFFull);
+        const bool none = words[r] == kBestEmpty;  // (substitutions only: a record shorter than the pattern)
+        dist[r] = none ? -1 : (int32_t)(words[r] >> 32);
+        end[r] = none ? -1 : (int64_t)(words[r] & 0xFFFFFFFFull);
     }
     return FZB_OK;
 }
@@ -3610,10 +3622,16 @@ extern "C" int fzb_nearest_per_record(fzb_haystack *h, const uint8_t *pattern, u
 constexpr int64_t kNearBatchMinSeg = 1024;  // bytes per warp: the warm-up (at most 128 bytes) stays <= 1/8 of it
 
 template <int BITS, bool REC>
-static int launch_nearest_batch(fzb_haystack *h, dim3 grid, const NearBatchParams &p, const RecSet &rs) {
-    CK(cudaFuncSetAttribute(k_nearest_batch_scan<BITS, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                            (int)near_smem(BITS)));
-    k_nearest_batch_scan<BITS, REC><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
+static int launch_nearest_batch(fzb_haystack *h, dim3 grid, const NearBatchParams &p, const RecSet &rs, bool ham) {
+    if (ham) {
+        CK(cudaFuncSetAttribute(k_nearest_hamming_batch_scan<BITS, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)near_smem(BITS)));
+        k_nearest_hamming_batch_scan<BITS, REC><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
+    } else {
+        CK(cudaFuncSetAttribute(k_nearest_batch_scan<BITS, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)near_smem(BITS)));
+        k_nearest_batch_scan<BITS, REC><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
+    }
     CK(cudaGetLastError());
     return FZB_OK;
 }
@@ -3621,7 +3639,8 @@ static int launch_nearest_batch(fzb_haystack *h, dim3 grid, const NearBatchParam
 // Every pattern checked as its single search would take it (the caller checked the rest): FZB_OK or the refusal
 static int check_nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count,
                                uint32_t flags, const char *what) {
-    if (flags) return fail(FZB_E_UNSUPPORTED, "%s takes no flags", what);
+    if (flags & ~FZB_F_SUBSTITUTIONS_ONLY)
+        return fail(FZB_E_UNSUPPORTED, "%s takes no flag other than FZB_F_SUBSTITUTIONS_ONLY", what);
     if (count > kBestMaxPatterns) return fail(FZB_E_UNSUPPORTED, "more than %u patterns in one %s call", kBestMaxPatterns, what);
     if (h->comm || h->local_world || h->peer) return fail(FZB_E_UNSUPPORTED, "%s: a handle in a world", what);
     for (uint32_t i = 0; i < count; i++) {
@@ -3633,10 +3652,10 @@ static int check_nearest_batch(fzb_haystack *h, const uint8_t *patterns, const u
 
 // The scans of all `count` patterns over the whole buffer, per record if `rec`: the patterns of up to 64 symbols in
 // groups of 32 lanes (k_nearest_batch_scan, one launch per word class), longer ones one by one (k_nearest_scan, folded
-// by k_nearest_fold per record).  Its own buffer group only, as nearest_scan.  On FZB_OK the answer is in
-// nearbatch->d_words and the stream has drained.
+// by k_nearest_fold per record), under substitutions only if `ham`.  Its own buffer group only, as nearest_scan.  On
+// FZB_OK the answer is in nearbatch->d_words and the stream has drained.
 static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count, bool rec,
-                         fzb_stats *stats) {
+                         bool ham, fzb_stats *stats) {
     auto len = [&](uint32_t i) { return offsets[i + 1] - offsets[i]; };
     // by (class, m): the lanes of a group share the warm-up of its longest pattern
     std::vector<uint32_t> order, longs;
@@ -3677,15 +3696,16 @@ static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_
     }
     uint64_t *best = g->d_words.get(), *top2 = best + nrec;
     fzb_stats st{};
-    st.route = 12;
+    st.route = ham ? 14 : 12;
     CK(cudaEventRecord(h->ev[0], h->stream));
     if (!lanes.empty()) {
         CK(cudaMemcpyAsync(g->d_lanes.get(), lanes.data(), lanes.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
         CK(cudaMemcpyAsync(g->d_pats.get(), pats.data(), pats.size(), cudaMemcpyHostToDevice, h->stream));
     }
-    if (rec) {  // the constants of nearest_kernels.cuh: (min m, its ordinal, end 0) and the two smallest (m_i, i)
+    if (rec) {  // the constants of nearest_kernels.cuh: (min m, its ordinal, end 0) and the two smallest (m_i, i);
+                // nothing under substitutions only, where no pattern has a value before its first window
         uint64_t key = kBestEmpty, pair2 = kBestEmpty;
-        for (uint32_t i = 0; i < count; i++) {
+        for (uint32_t i = 0; i < count && !ham; i++) {
             key = std::min<uint64_t>(key, (uint64_t)len(i) << 48 | (uint64_t)i << 32);
             pair2 = best_top2_merge(pair2, len(i) << 16 | i);
         }
@@ -3693,9 +3713,9 @@ static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_
         k_nearest_fill<<<fill_grid, 256, 0, h->stream>>>(best, nrec, key);
         k_nearest_fill<<<fill_grid, 256, 0, h->stream>>>(top2, nrec, pair2);
         st.n_launches += 2;
-    } else {  // every pattern's end position 0
+    } else {  // every pattern's end position 0 (substitutions only: no value)
         std::vector<uint64_t> init(count);
-        for (uint32_t i = 0; i < count; i++) init[i] = (uint64_t)len(i) << 48;
+        for (uint32_t i = 0; i < count; i++) init[i] = ham ? kBestEmpty : (uint64_t)len(i) << 48;
         CK(cudaMemcpyAsync(best, init.data(), count * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
         CK(cudaStreamSynchronize(h->stream));  // (`init` is a pageable local)
     }
@@ -3725,7 +3745,7 @@ static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_
         int rc = FZB_OK;
         with_recs(h, [&](auto r) {
             constexpr bool R = decltype(r)::value;
-            rc = cls ? launch_nearest_batch<64, R>(h, grid, p, rs) : launch_nearest_batch<32, R>(h, grid, p, rs);
+            rc = cls ? launch_nearest_batch<64, R>(h, grid, p, rs, ham) : launch_nearest_batch<32, R>(h, grid, p, rs, ham);
         });
         TRY(rc);
         st.n_launches++;
@@ -3745,7 +3765,7 @@ static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_
         const int grid = near_geometry(h, bits, &q.seg);
         if (rec) {
             k_nearest_fill<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
-                q.words, nrec, (uint64_t)m << 32);
+                q.words, nrec, ham ? kBestEmpty : (uint64_t)m << 32);
             CK(cudaGetLastError());
             st.n_launches++;
         }
@@ -3753,9 +3773,9 @@ static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_
             int rc = FZB_OK;
             with_recs(h, [&](auto r) {
                 constexpr bool R = decltype(r)::value;
-                rc = bits == 128   ? launch_nearest<128, R>(h, grid, q, rs)
-                     : bits == 192 ? launch_nearest<192, R>(h, grid, q, rs)
-                                   : launch_nearest<256, R>(h, grid, q, rs);
+                rc = bits == 128   ? launch_nearest<128, R>(h, grid, q, rs, ham)
+                     : bits == 192 ? launch_nearest<192, R>(h, grid, q, rs, ham)
+                                   : launch_nearest<256, R>(h, grid, q, rs, ham);
             });
             TRY(rc);
             st.n_launches++;
@@ -3763,7 +3783,7 @@ static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_
         }
         if (rec) {
             k_nearest_fold<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
-                q.words, nrec, m, i, best, top2);
+                q.words, nrec, ham ? m + 1 : m, i, best, top2);
             CK(cudaGetLastError());
             st.n_launches++;
         }
@@ -3788,15 +3808,16 @@ extern "C" int fzb_nearest_distance_batch(fzb_haystack *h, const uint8_t *patter
     TRY(refuse_records(h, "fzb_nearest_distance_batch"));
     if (stats) *stats = fzb_stats{};
     if (count == 0) return FZB_OK;
-    TRY(nearest_batch(h, patterns, offsets, count, false, stats));
+    TRY(nearest_batch(h, patterns, offsets, count, false, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0, stats));
     // one read-back of 8 bytes per pattern
     std::vector<uint64_t> words(count);
     CK(cudaMemcpyAsync(words.data(), h->nearbatch->d_words.get(), count * sizeof(uint64_t), cudaMemcpyDeviceToHost,
                        h->stream));
     CK(cudaStreamSynchronize(h->stream));
     for (uint32_t i = 0; i < count; i++) {
-        dist[i] = (uint32_t)(words[i] >> 48);
-        first_end[i] = words[i] & kNearNoEnd;
+        const bool none = words[i] == kBestEmpty;  // (substitutions only: a pattern longer than the sequence)
+        dist[i] = none ? UINT32_MAX : (uint32_t)(words[i] >> 48);
+        first_end[i] = none ? UINT64_MAX : words[i] & kNearNoEnd;
     }
     return FZB_OK;
 }
@@ -3821,7 +3842,7 @@ extern "C" int fzb_nearest_best_per_record(fzb_haystack *h, const uint8_t *patte
         }
         return FZB_OK;
     }
-    TRY(nearest_batch(h, patterns, offsets, count, true, stats));
+    TRY(nearest_batch(h, patterns, offsets, count, true, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0, stats));
     // one read-back of 16 bytes per record
     std::vector<uint64_t> words(2 * nrec);
     CK(cudaMemcpyAsync(words.data(), h->nearbatch->d_words.get(), 2 * nrec * sizeof(uint64_t), cudaMemcpyDeviceToHost,
@@ -3830,9 +3851,10 @@ extern "C" int fzb_nearest_best_per_record(fzb_haystack *h, const uint8_t *patte
     for (uint64_t r = 0; r < nrec; r++) {
         const uint64_t b = words[r];
         const uint32_t second = (uint32_t)words[nrec + r] & kBestPairNone;
-        dist[r] = (int32_t)(b >> 48);
-        pattern[r] = (int32_t)((b >> 32) & 0xFFFFu);
-        end[r] = (int64_t)(b & 0xFFFFFFFFull);
+        const bool none = b == kBestEmpty;  // (substitutions only: no pattern fits in the record)
+        dist[r] = none ? -1 : (int32_t)(b >> 48);
+        pattern[r] = none ? -1 : (int32_t)((b >> 32) & 0xFFFFu);
+        end[r] = none ? -1 : (int64_t)(b & 0xFFFFFFFFull);
         second_dist[r] = second == kBestPairNone ? -1 : (int32_t)(second >> 16);
         second_pattern[r] = second == kBestPairNone ? -1 : (int32_t)(second & 0xFFFFu);
     }

@@ -80,6 +80,12 @@ struct NearCol {  // one column of the table and what the thread has seen of its
     uint32_t best, cnt, first;    // tracked ends: the minimum below m (else m), its count, the first (as `rel`)
     const word *pm;               // this lane's view of the table
 
+    // what the shared scans ask of a column: the best before any end (the end position 0 scores m), whether a
+    // best is worth reporting (the end position 0 is the prefill's), and how many bytes before a segment make it exact
+    static __device__ __forceinline__ uint32_t none(uint32_t m) { return m; }
+    static __device__ __forceinline__ bool has(uint32_t best, uint32_t m) { return best < m; }
+    static __device__ __forceinline__ int64_t warm(uint32_t m) { return 2 * (int64_t)m; }
+
     __device__ __forceinline__ void reset(uint32_t m) {
 #pragma unroll
         for (int w = 0; w < NW; w++) {
@@ -142,11 +148,98 @@ struct NearCol {  // one column of the table and what the thread has seen of its
     }
 };
 
-template <int BITS, bool REC>
-__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : BITS == 64 ? 3 : 2)
-k_nearest_scan(NearParams p, RecSet rs) {
+// ------------------------------------------------------------------------------------------------------------------
+// Substitutions only (DESIGN.md section 5.16): H(e) = the mismatches of P against the window S[e-m:e], defined for
+// e >= m + the record start.  HamCol keeps one mismatch counter per alignment in flight, bit-sliced: bit j of slice s
+// is bit s of the count of the alignment that has met P[0..j].  Per text byte every slice shifts up one bit (a new
+// alignment enters at bit 0 with count 0, the one at bit m - 1 leaves), then X = ~PM[c] is added by a ripple carry
+// through the slices; the score is bit m - 1 of the slices.  Bits above m - 1 hold partial sums of alignments that
+// are already done: they only move up and are never read, so their wrap-around is harmless.  S slices count to BITS
+// (6 for one 32-bit word, 7 for one 64-bit word, 8 for the 2-4 word forms, m <= 255).
+//
+// H(e) depends on S[e-m:e] only, so m - 1 bytes of warm-up before a segment are exact; `fill` counts the bytes a
+// column still needs after its reset (at a record start, or at the sequence start) before bit m - 1 holds a whole
+// window, and no end is tracked until then.  A column that never tracked an end keeps best = none (~0u), so "has a
+// value" is best <= m: unlike Levenshtein there is no end position 0 with score m.
+// ------------------------------------------------------------------------------------------------------------------
+template <int BITS>
+struct HamCol {
     typedef typename NearWord<BITS>::type word;
-    constexpr int NW = near_words(BITS);
+    static constexpr int NW = near_words(BITS);
+    static constexpr int S = BITS == 32 ? 6 : BITS == 64 ? 7 : 8;
+    static constexpr uint32_t WB = sizeof(word) * 8;
+    word sl[S][NW];
+    uint32_t top, fill;
+    uint32_t best, cnt, first;
+    const word *pm;
+
+    static __device__ __forceinline__ uint32_t none(uint32_t) { return ~0u; }
+    static __device__ __forceinline__ bool has(uint32_t best, uint32_t m) { return best <= m; }
+    static __device__ __forceinline__ int64_t warm(uint32_t m) { return (int64_t)m - 1; }
+
+    __device__ __forceinline__ void reset(uint32_t m) {
+#pragma unroll
+        for (int s = 0; s < S; s++)
+#pragma unroll
+            for (int w = 0; w < NW; w++) sl[s][w] = 0;
+        fill = m - 1;
+        best = ~0u;
+        cnt = 0;
+        first = 0;
+    }
+
+    template <bool TRACK>
+    __device__ __forceinline__ void step(uint32_t c, uint32_t rel) {
+#pragma unroll
+        for (int s = 0; s < S; s++) {
+#pragma unroll
+            for (int w = NW - 1; w > 0; w--) sl[s][w] = sl[s][w] << 1 | sl[s][w - 1] >> (WB - 1);
+            sl[s][0] <<= 1;
+        }
+#pragma unroll
+        for (int w = 0; w < NW; w++) {
+            word carry = ~(NW == 1 ? pm[c * 32] : pm[c * NW + w]);
+#pragma unroll
+            for (int s = 0; s < S; s++) {
+                const word t = sl[s][w] & carry;
+                sl[s][w] ^= carry;
+                carry = t;
+            }
+        }
+        uint32_t score = 0;
+#pragma unroll
+        for (int s = 0; s < S; s++) score |= (uint32_t)((sl[s][NW - 1] >> top) & 1) << s;
+        if (fill) {
+            fill--;
+        } else if (TRACK) {
+            if (score < best) {
+                best = score;
+                cnt = 1;
+                first = rel;
+            } else if (score == best) {
+                cnt++;
+            }
+        }
+    }
+
+    // text bytes [x, end); rel: the end position behind H[x], relative to the caller's base
+    template <bool TRACK>
+    __device__ __forceinline__ void run(const uint8_t *H, int64_t x, int64_t end, uint32_t rel) {
+        for (; x < end && (x & 15); x++) step<TRACK>(H[x], rel++);
+        for (; x + 16 <= end; x += 16) {
+            const uint4 v = __ldg(reinterpret_cast<const uint4 *>(H + x));
+            const uint32_t q[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int j = 0; j < 16; j++) step<TRACK>((q[j >> 2] >> (8 * (j & 3))) & 0xFFu, rel++);
+        }
+        for (; x < end; x++) step<TRACK>(H[x], rel++);
+    }
+};
+
+template <class Col, bool REC>
+__device__ __forceinline__ void near_scan(NearParams p, RecSet rs) {
+    typedef typename Col::word word;
+    constexpr int NW = Col::NW;
     extern __shared__ __align__(16) uint64_t near_smem_raw[];
     __shared__ uint32_t s_best[kNearThreads / 32];
     __shared__ uint64_t s_cnt[kNearThreads / 32], s_first[kNearThreads / 32];
@@ -173,10 +266,10 @@ k_nearest_scan(NearParams p, RecSet rs) {
     }
     __syncthreads();
 
-    NearCol<BITS> col;
+    Col col;
     col.pm = NW == 1 ? pm + lane : pm;
     col.top = (m - 1) % (uint32_t)(sizeof(word) * 8);
-    uint32_t tbest = m;  // whole sequence: over all tiles of this thread
+    uint32_t tbest = Col::none(m);  // whole sequence: over all tiles of this thread
     uint64_t tcnt = 0, tfirst = kNearNoEnd;
 
     const int64_t tile = (int64_t)kNearThreads * p.seg;
@@ -193,17 +286,18 @@ k_nearest_scan(NearParams p, RecSet rs) {
             hi = (int64_t)rs.off[r + 1] - 1;
         }
         col.reset(m);
-        const int64_t w = a - 2 * (int64_t)m > lo ? a - 2 * (int64_t)m : lo;
+        const int64_t w = a - Col::warm(m) > lo ? a - Col::warm(m) : lo;
         col.template run<false>(p.H, w, a, 0);
         if (!REC) {
             col.template run<true>(p.H, a, b, 1);
-            near_merge(tbest, tcnt, tfirst, col.best, col.cnt, col.best < m ? (uint64_t)a + col.first : kNearNoEnd);
+            near_merge(tbest, tcnt, tfirst, col.best, col.cnt,
+                       Col::has(col.best, m) ? (uint64_t)a + col.first : kNearNoEnd);
         } else {
             int64_t x = a;
             for (;;) {
                 const int64_t stop = b < hi ? b : hi;
                 if (x < stop) col.template run<true>(p.H, x, stop, (uint32_t)(x + 1 - lo));
-                if (col.best < m)
+                if (Col::has(col.best, m))
                     atomicMin((unsigned long long *)&p.words[r], (unsigned long long)col.best << 32 | col.first);
                 if (hi + 1 >= b) break;  // (the record behind the separator starts in another segment, or nowhere)
                 r++;
@@ -228,17 +322,31 @@ k_nearest_scan(NearParams p, RecSet rs) {
         __syncthreads();
         if (threadIdx.x == 0) {
             for (int i = 1; i < kNearThreads / 32; i++) near_merge(tbest, tcnt, tfirst, s_best[i], s_cnt[i], s_first[i]);
-            if (tbest < m) atomicMin((unsigned long long *)&p.result[0], (unsigned long long)tbest << 48 | tfirst);
+            if (Col::has(tbest, m))
+                atomicMin((unsigned long long *)&p.result[0], (unsigned long long)tbest << 48 | tfirst);
             p.partial[2 * blockIdx.x] = tbest;
             p.partial[2 * blockIdx.x + 1] = tcnt;
         }
     }
 }
 
-// n_ends: the ends the CTAs counted at the global minimum, and the end position 0 if that minimum is m.  One CTA.
-__global__ void k_nearest_count(uint64_t *result, const uint64_t *partial, uint32_t nparts, uint32_t m) {
+template <int BITS, bool REC>
+__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : BITS == 64 ? 3 : 2)
+k_nearest_scan(NearParams p, RecSet rs) {
+    near_scan<NearCol<BITS>, REC>(p, rs);
+}
+
+template <int BITS, bool REC>
+__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : BITS == 64 ? 3 : 2)
+k_nearest_hamming_scan(NearParams p, RecSet rs) {
+    near_scan<HamCol<BITS>, REC>(p, rs);
+}
+
+// n_ends: the ends the CTAs counted at the global minimum, and the end position 0 if that minimum is m_end0 (the
+// pattern's length; ~0u under substitutions only, where the end position 0 has no window).  One CTA.
+__global__ void k_nearest_count(uint64_t *result, const uint64_t *partial, uint32_t nparts, uint32_t m_end0) {
     const uint64_t best = result[0] >> 48;
-    uint64_t sum = threadIdx.x == 0 && best == m ? 1 : 0;
+    uint64_t sum = threadIdx.x == 0 && best == m_end0 ? 1 : 0;
     for (uint32_t i = threadIdx.x; i < nparts; i += blockDim.x)
         if (partial[2 * i] == best) sum += partial[2 * i + 1];
     if (sum) atomicAdd((unsigned long long *)&result[1], (unsigned long long)sum);
@@ -269,7 +377,9 @@ __global__ void k_nearest_count(uint64_t *result, const uint64_t *partial, uint3
 // d*_i <= m_i for every pattern, so a pattern left out of the prefill sits behind two patterns j, k whose
 // (d*_j, j) <= (m_j, j) < (m_i, i) <= (d*_i, i) -- it can be neither first nor second, and a pattern that is never
 // reported has d*_i = m_i with its first end at 0, which is what the prefill says for it.  All updates are minima, so
-// the words depend neither on thread, warp or CTA order nor on how records are split over segments.
+// the words depend neither on thread, warp or CTA order nor on how records are split over segments.  Under substitutions
+// only (k_nearest_hamming_batch_scan, HamCol) nothing has a value before its first window, so both words start empty
+// (kBestEmpty) and lanes report every tracked minimum, m_i included.
 // ------------------------------------------------------------------------------------------------------------------
 constexpr int kNearBatchLanes = 32;
 constexpr int kNearBatchMaxM = 64;  // bytes per lane of the pattern buffer
@@ -319,11 +429,10 @@ __device__ __forceinline__ void near_batch_report(uint64_t key, uint64_t *best, 
     }
 }
 
-template <int BITS, bool REC>
-__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : 3)
-k_nearest_batch_scan(NearBatchParams p, RecSet rs) {
-    static_assert(BITS == 32 || BITS == 64, "one word per lane");
-    typedef typename NearWord<BITS>::type word;
+template <class Col, bool REC>
+__device__ __forceinline__ void near_batch_scan(NearBatchParams p, RecSet rs) {
+    static_assert(Col::NW == 1, "one word per lane");
+    typedef typename Col::word word;
     extern __shared__ __align__(16) uint64_t near_smem_raw[];
     __shared__ __align__(16) uint8_t s_pat[kNearBatchLanes * kNearBatchMaxM];
     __shared__ uint32_t s_m[kNearBatchLanes];
@@ -356,10 +465,10 @@ k_nearest_batch_scan(NearBatchParams p, RecSet rs) {
         const uint32_t o = __shfl_xor_sync(0xFFFFFFFFu, gm, d);
         gm = o > gm ? o : gm;
     }
-    NearCol<BITS> col;
+    Col col;
     col.pm = pm + lane;
     col.top = m - 1;
-    uint32_t tbest = m;  // whole sequence: over all segments of this warp
+    uint32_t tbest = Col::none(m);  // whole sequence: over all segments of this warp
     uint64_t tfirst = kNearNoEnd;
 
     const int64_t tile = (int64_t)(kNearThreads / 32) * p.seg;
@@ -376,7 +485,7 @@ k_nearest_batch_scan(NearBatchParams p, RecSet rs) {
             hi = (int64_t)rs.off[r + 1] - 1;
         }
         col.reset(m);
-        const int64_t w = a - 2 * (int64_t)gm > lo ? a - 2 * (int64_t)gm : lo;
+        const int64_t w = a - Col::warm(gm) > lo ? a - Col::warm(gm) : lo;
         col.template run<false>(p.H, w, a, 0);
         if (!REC) {
             col.template run<true>(p.H, a, b, 1);
@@ -389,7 +498,7 @@ k_nearest_batch_scan(NearBatchParams p, RecSet rs) {
             for (;;) {
                 const int64_t stop = b < hi ? b : hi;
                 if (x < stop) col.template run<true>(p.H, x, stop, (uint32_t)(x + 1 - lo));
-                const uint64_t key = !idle && col.best < m
+                const uint64_t key = !idle && Col::has(col.best, m)
                                          ? (uint64_t)col.best << 48 | (uint64_t)ord << 32 | col.first
                                          : ~0ull;
                 near_batch_report(key, p.best + r, p.top2 + r);
@@ -403,7 +512,7 @@ k_nearest_batch_scan(NearBatchParams p, RecSet rs) {
         }
     }
     if (!REC) {  // per lane over the warps of the CTA, then one atomicMin per (CTA, pattern)
-        s_key[warp][lane] = !idle && tbest < m ? (uint64_t)tbest << 48 | tfirst : ~0ull;
+        s_key[warp][lane] = !idle && Col::has(tbest, m) ? (uint64_t)tbest << 48 | tfirst : ~0ull;
         __syncthreads();
         if (warp == 0) {
             uint64_t key = s_key[0][lane];
@@ -413,15 +522,29 @@ k_nearest_batch_scan(NearBatchParams p, RecSet rs) {
     }
 }
 
-// A pattern of 65-255 symbols scanned alone by k_nearest_scan<BITS, true>: its per-record words (dist << 32 | end)
-// folded into best / top2 as the lanes of k_nearest_batch_scan report.  One thread per record.
-__global__ void k_nearest_fold(const uint64_t *words, uint64_t nrec, uint32_t m, uint32_t ord, uint64_t *best,
+template <int BITS, bool REC>
+__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : 3)
+k_nearest_batch_scan(NearBatchParams p, RecSet rs) {
+    near_batch_scan<NearCol<BITS>, REC>(p, rs);
+}
+
+template <int BITS, bool REC>
+__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : 3)
+k_nearest_hamming_batch_scan(NearBatchParams p, RecSet rs) {
+    near_batch_scan<HamCol<BITS>, REC>(p, rs);
+}
+
+// A pattern of 65-255 symbols scanned alone by k_nearest_scan<BITS, true> (k_nearest_hamming_scan): its per-record
+// words (dist << 32 | end) below `lim` folded into best / top2 as the lanes of the batch scan report.  lim is m for
+// Levenshtein (the prefill stands for d = m) and m + 1 under substitutions only (d = m is reported, and the empty
+// word, dist 0xFFFFFFFF, is not).  One thread per record.
+__global__ void k_nearest_fold(const uint64_t *words, uint64_t nrec, uint32_t lim, uint32_t ord, uint64_t *best,
                                uint64_t *top2) {
     const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
     for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nrec; r += stride) {
         const uint64_t w = words[r];
         const uint32_t d = (uint32_t)(w >> 32);
-        if (d >= m) continue;
+        if (d >= lim) continue;
         atomicMin((unsigned long long *)&best[r], (unsigned long long)d << 48 | (uint64_t)ord << 32 | (w & 0xFFFFFFFFull));
         near_top2_add(&top2[r], d << 16 | ord, kBestPairNone);
     }

@@ -430,42 +430,60 @@ class GenericSearch(FuzzySearchBase):
         return max(x for x in [search_params.max_l_dist, search_params.max_insertions] if x is not None)
 
 
-def nearest_distance(subsequence, sequence):
+def _nearest_flags(substitutions_only):
+    return _native.F_SUBSTITUTIONS_ONLY if substitutions_only else 0
+
+
+def nearest_distance(subsequence, sequence, *, substitutions_only=False):
     """The smallest Levenshtein distance of `subsequence` to any substring of `sequence` (at most
     ``len(subsequence)``: the empty substring) -- the smallest ``max_l_dist`` at which ``find_near_matches`` finds
     anything.  One scan of the sequence, whatever the answer (fzb_nearest_distance, DESIGN.md section 5.14).
-    `sequence` is anything find_near_matches takes."""
+    `sequence` is anything find_near_matches takes.
+
+    With ``substitutions_only=True``: the smallest number of substitutions of any window of ``len(subsequence)``
+    symbols -- the smallest k at which ``find_near_matches(..., max_substitutions=k, max_insertions=0,
+    max_deletions=0)`` finds anything -- or None when the sequence is shorter than the pattern (DESIGN.md section
+    5.16)."""
     if len(subsequence) == 0:
         raise ValueError("Given subsequence is empty!")
     with _lock_for(sequence):
         pat, hay, _, _ = _prepare(subsequence, sequence)
-        return hay.nearest_distance(pat)[0]
+        d = hay.nearest_distance(pat, _nearest_flags(substitutions_only))[0]
+        return None if d == _native.NO_DIST else d
 
 
-def find_nearest_matches(subsequence, sequence, max_l_dist=None):
+def find_nearest_matches(subsequence, sequence, max_l_dist=None, *, substitutions_only=False):
     """Where does `subsequence` fit best?  -> exactly ``find_near_matches(subsequence, sequence, max_l_dist=d)`` with
     d = ``nearest_distance(subsequence, sequence)``, without guessing d: one scan finds it, then the ordinary search
     runs once, at d, on the same upload.  With `max_l_dist` given the list is empty when d is larger (the cap bounds
-    the cost of the search; the search itself still runs at d, not at the cap)."""
+    the cost of the search; the search itself still runs at d, not at the cap).
+
+    With ``substitutions_only=True``: exactly ``find_near_matches(subsequence, sequence, max_substitutions=d,
+    max_insertions=0, max_deletions=0)`` with d = ``nearest_distance(..., substitutions_only=True)``, and [] when
+    the sequence is shorter than the pattern.  Every window at d is listed, so a d close to ``len(subsequence)``
+    lists almost every window; the cap avoids that."""
     if len(subsequence) == 0:
         raise ValueError("Given subsequence is empty!")
     if max_l_dist is not None and (not isinstance(max_l_dist, int) or max_l_dist < 0):
         raise ValueError("max_l_dist must be a non-negative integer or None")
     with _lock_for(sequence):
         pat, hay, slicer, _ = _prepare(subsequence, sequence)
-        d = hay.nearest_distance(pat)[0]
-        if max_l_dist is not None and d > max_l_dist:
+        d = hay.nearest_distance(pat, _nearest_flags(substitutions_only))[0]
+        if d == _native.NO_DIST or (max_l_dist is not None and d > max_l_dist):
             return []
-        # max_l_dist == 0 is the exact search, whose list is its raw stream (ExactSearch does not consolidate)
-        res = hay.search_exact(pat) if d == 0 else hay.search_levenshtein(pat, d)
+        # max_l_dist == 0 is the exact search, whose list is its raw stream (ExactSearch does not consolidate);
+        # the substitutions-only search does not consolidate either (FINAL == RAW)
+        res = (hay.search_exact(pat) if d == 0 else
+               hay.search_hamming(pat, d) if substitutions_only else hay.search_levenshtein(pat, d))
         try:
             return _to_matches(res, _native.RAW if d == 0 else _native.FINAL, slicer)
         finally:
             res.close()
 
 
-def _nearest_batch(subsequences, sequence):
-    """-> (dist int32, first end int64) arrays, one entry per pattern.  The caller holds the sequence's lock."""
+def _nearest_batch(subsequences, sequence, flags):
+    """-> (dist int32, first end int64) arrays, one entry per pattern, -1 / -1 without a value.  The caller holds
+    the sequence's lock."""
     try:
         pats, hay, _ = _prepare_many(subsequences, sequence)
     except AlphabetTooLarge:
@@ -474,17 +492,20 @@ def _nearest_batch(subsequences, sequence):
         rows = []
         for p in subsequences:
             pat, hay, _, _ = _prepare(p, sequence)
-            rows.append(hay.nearest_distance(pat)[::2])  # (dist, first_end)
+            d, _, e, _ = hay.nearest_distance(pat, flags)
+            rows.append((-1, -1) if d == _native.NO_DIST else (d, e))
         return np.array([d for d, _ in rows], dtype=np.int32), np.array([e for _, e in rows], dtype=np.int64)
-    dist, end, _ = hay.nearest_distance_batch(pats)
+    dist, end, _ = hay.nearest_distance_batch(pats, flags)
     return dist, end
 
 
-def nearest_distance_batch(subsequences, sequence):
+def nearest_distance_batch(subsequences, sequence, *, substitutions_only=False):
     """Many patterns over one sequence, without a distance limit: -> NearestDistances with one entry per pattern,
     ``dist[i] == nearest_distance(subsequences[i], sequence)`` and ``end[i]`` the first end position of a substring at
     that distance.  The patterns of up to 64 symbols share scans of the sequence, 32 at a time
-    (fzb_nearest_distance_batch, DESIGN.md section 5.15).  `sequence` is anything find_near_matches takes."""
+    (fzb_nearest_distance_batch, DESIGN.md section 5.15).  `sequence` is anything find_near_matches takes.  With
+    ``substitutions_only=True`` the distances are ``nearest_distance(..., substitutions_only=True)``, and a pattern
+    longer than the sequence gets -1 / -1."""
     from .sequence_set import NearestDistances
     subsequences = list(subsequences)
     if any(len(p) == 0 for p in subsequences):
@@ -492,14 +513,16 @@ def nearest_distance_batch(subsequences, sequence):
     if not subsequences:
         return NearestDistances(np.zeros(0, np.int32), np.zeros(0, np.int64))
     with _lock_for(sequence):
-        return NearestDistances(*_nearest_batch(subsequences, sequence))
+        return NearestDistances(*_nearest_batch(subsequences, sequence, _nearest_flags(substitutions_only)))
 
 
-def find_nearest_matches_batch(subsequences, sequence, max_l_dist=None):
+def find_nearest_matches_batch(subsequences, sequence, max_l_dist=None, *, substitutions_only=False):
     """Where does each pattern fit best?  -> exactly ``find_near_matches_batch(subsequences, sequence,
     max_l_dist=[d_0, d_1, ...])`` with d_i = ``nearest_distance(subsequences[i], sequence)``, found by one batch of
     shared scans and searched on the same upload.  `max_l_dist` (None, one int, or one value per pattern) caps d_i:
-    a pattern whose d_i is larger gets ``[]`` and is not searched."""
+    a pattern whose d_i is larger gets ``[]`` and is not searched.  With ``substitutions_only=True``: exactly
+    ``find_near_matches_batch(..., max_substitutions=[d_0, d_1, ...], max_insertions=0, max_deletions=0)`` with the
+    substitutions-only d_i, and ``[]`` for a pattern longer than the sequence."""
     from . import _search_batch, choose_search_class, find_nearest_matches
     from .common import LevenshteinSearchParams
     subsequences = list(subsequences)
@@ -517,10 +540,12 @@ def find_nearest_matches_batch(subsequences, sequence, max_l_dist=None):
         try:
             pats, hay, slicer = _prepare_many(subsequences, sequence)
         except AlphabetTooLarge:
-            return [find_nearest_matches(p, sequence, c) for p, c in zip(subsequences, caps)]
-        dist, _, _ = hay.nearest_distance_batch(pats)
-        todo = [i for i in range(n) if caps[i] is None or dist[i] <= caps[i]]
-        params = [LevenshteinSearchParams(None, None, None, int(dist[i])) for i in todo]
+            return [find_nearest_matches(p, sequence, c, substitutions_only=substitutions_only)
+                    for p, c in zip(subsequences, caps)]
+        dist, _, _ = hay.nearest_distance_batch(pats, _nearest_flags(substitutions_only))
+        todo = [i for i in range(n) if dist[i] >= 0 and (caps[i] is None or dist[i] <= caps[i])]
+        params = [LevenshteinSearchParams(int(dist[i]), 0, 0, None) if substitutions_only else
+                  LevenshteinSearchParams(None, None, None, int(dist[i])) for i in todo]
         lists = _search_batch(hay, [pats[i] for i in todo], params, [choose_search_class(p) for p in params], 0)
     out = [[] for _ in range(n)]
     for i, (s, e, d) in zip(todo, lists):

@@ -282,7 +282,10 @@ class NearestDistances(object):
     """What nearest_distance_in_each and nearest_distance_batch return: ``dist`` (int32) and ``end`` (int64), one
     entry per sequence (nearest_distance_in_each) or per pattern (nearest_distance_batch) -- the smallest Levenshtein
     distance of the pattern to any substring of the sequence and the first end position (in the sequence's own
-    coordinates) of a substring at that distance.  ``nearest[i]`` is ``(dist, end)``."""
+    coordinates) of a substring at that distance.  ``nearest[i]`` is ``(dist, end)``.  With
+    ``substitutions_only=True`` ``dist`` is the smallest number of substitutions of a window of the pattern's length,
+    the match starts at ``end - len(pattern)``, and a sequence shorter than the pattern (or a pattern longer than the
+    sequence) gives ``(-1, -1)``."""
 
     def __init__(self, dist, end):
         self.dist, self.end = dist, end
@@ -294,32 +297,35 @@ class NearestDistances(object):
         return int(self.dist[r]), int(self.end[r])
 
 
-def nearest_distance_in_each(subsequence, sequences):
+def nearest_distance_in_each(subsequence, sequences, *, substitutions_only=False):
     """One pattern over many sequences, without a distance limit: -> NearestDistances with, for every sequence,
     ``nearest_distance(subsequence, sequences[r])`` and where the nearest match first ends; an empty sequence gives
     ``(len(subsequence), 0)``.  All sequences are scanned in one device pass (fzb_nearest_per_record, DESIGN.md
-    section 5.14).  `sequences` is a list / tuple (uploaded for this call) or a DeviceSequenceSet (resident)."""
+    section 5.14).  `sequences` is a list / tuple (uploaded for this call) or a DeviceSequenceSet (resident).  With
+    ``substitutions_only=True`` the distances are ``nearest_distance(..., substitutions_only=True)``, and a sequence
+    shorter than the pattern gives ``(-1, -1)`` (DESIGN.md section 5.16)."""
     if len(subsequence) == 0:
         raise ValueError("Given subsequence is empty!")
+    flags = _native.F_SUBSTITUTIONS_ONLY if substitutions_only else 0
     if isinstance(sequences, DeviceSequenceSet):
-        return _nearest_in_set(subsequence, sequences)
+        return _nearest_in_set(subsequence, sequences, flags)
     if not isinstance(sequences, (list, tuple)):
         raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
     if not sequences:
         return NearestDistances(np.zeros(0, np.int32), np.zeros(0, np.int64))
     seqset = DeviceSequenceSet(sequences)
     try:
-        return _nearest_in_set(subsequence, seqset)
+        return _nearest_in_set(subsequence, seqset, flags)
     finally:
         seqset.close()
 
 
-def _nearest_in_set(subsequence, seqset):
+def _nearest_in_set(subsequence, seqset, flags):
     if len(seqset) == 0:
         return NearestDistances(np.zeros(0, np.int32), np.zeros(0, np.int64))
     with seqset._lock:
         pat = seqset._bind(subsequence)
-        dist, end, _ = seqset._seq.haystack.nearest_per_record(pat)
+        dist, end, _ = seqset._seq.haystack.nearest_per_record(pat, flags)
     return NearestDistances(dist, end)
 
 
@@ -330,7 +336,11 @@ class NearestPatterns(object):
     nearest_distance_in_each gives for it); ``second_pattern``, ``second_dist`` (int32): the same over the OTHER
     patterns, for rejecting ambiguous calls by ``second_dist - dist``.  Every pattern has a distance (at most its
     length), so -1 appears only in the ``second_*`` arrays with a single pattern and everywhere with none.
-    ``nearest[r]`` is ``(pattern, dist, end)``."""
+    ``nearest[r]`` is ``(pattern, dist, end)``.
+
+    With ``substitutions_only=True`` only the patterns that fit in the sequence (``len(pattern) <= len(sequence)``)
+    have a distance and take part: a row where none fits is -1 everywhere, one where a single pattern fits has -1 in
+    the ``second_*`` arrays.  The winner's match starts at ``end - len(subsequences[pattern])``."""
 
     def __init__(self, columns):
         self.pattern, self.dist, self.end, self.second_pattern, self.second_dist = columns
@@ -346,30 +356,33 @@ def _no_patterns(n):
     return tuple(np.full(n, -1, dtype=t) for t in (np.int32, np.int32, np.int64, np.int32, np.int32))
 
 
-def nearest_pattern_in_each(subsequences, sequences):
+def nearest_pattern_in_each(subsequences, sequences, *, substitutions_only=False):
     """Many patterns over many sequences, without a distance limit: -> NearestPatterns, for every sequence the
     pattern nearest to it, its distance and first end, and the runner-up among the other patterns -- what reducing
     ``nearest_distance_in_each(p, sequences)`` over the patterns gives (ties to the smallest index), in shared scans
     of all sequences with the reduction on the device (fzb_nearest_best_per_record, DESIGN.md section 5.15).  An
     empty sequence gives the shortest pattern (the smallest index among equals), its length and the end 0.
-    `sequences` is a list / tuple (uploaded for this call) or a DeviceSequenceSet (resident)."""
+    `sequences` is a list / tuple (uploaded for this call) or a DeviceSequenceSet (resident).  With
+    ``substitutions_only=True`` the same over ``nearest_distance_in_each(p, sequences, substitutions_only=True)``,
+    where a pattern longer than a sequence has no distance there (DESIGN.md section 5.16)."""
     subsequences = list(subsequences)
     if any(len(p) == 0 for p in subsequences):
         raise ValueError("Given subsequence is empty!")
+    flags = _native.F_SUBSTITUTIONS_ONLY if substitutions_only else 0
     if isinstance(sequences, DeviceSequenceSet):
-        return _nearest_patterns_in_set(subsequences, sequences)
+        return _nearest_patterns_in_set(subsequences, sequences, flags)
     if not isinstance(sequences, (list, tuple)):
         raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
     if not sequences or not subsequences:
         return NearestPatterns(_no_patterns(len(sequences)))
     seqset = DeviceSequenceSet(sequences)
     try:
-        return _nearest_patterns_in_set(subsequences, seqset)
+        return _nearest_patterns_in_set(subsequences, seqset, flags)
     finally:
         seqset.close()
 
 
-def _nearest_patterns_in_set(subsequences, seqset):
+def _nearest_patterns_in_set(subsequences, seqset, flags):
     n = len(seqset)
     if n == 0 or not subsequences:
         return NearestPatterns(_no_patterns(n))
@@ -380,18 +393,20 @@ def _nearest_patterns_in_set(subsequences, seqset):
         except AlphabetTooLarge:
             pats = None  # no common byte alphabet: pattern by pattern, below
         if pats is not None:
-            columns, _ = seqset._seq.haystack.nearest_best_per_record(pats)
+            columns, _ = seqset._seq.haystack.nearest_best_per_record(pats, flags)
             return NearestPatterns(columns)
-    return NearestPatterns(_nearest_patterns_on_host(subsequences, seqset))
+    return NearestPatterns(_nearest_patterns_on_host(subsequences, seqset, flags))
 
 
-def _nearest_patterns_on_host(subsequences, seqset):
-    """The same rows from nearest_distance_in_each, pattern by pattern (each reduces the set to its own alphabet)."""
+def _nearest_patterns_on_host(subsequences, seqset, flags):
+    """The same rows from nearest_distance_in_each, pattern by pattern (each reduces the set to its own alphabet).
+    A pattern without a distance in a sequence (-1: substitutions only, longer than the sequence) is left out."""
     pattern, dist, end, pat2, dist2 = columns = _no_patterns(len(seqset))
     for i, p in enumerate(subsequences):
-        got = nearest_distance_in_each(p, seqset)
-        first = (pattern < 0) | (got.dist < dist)  # (an equal distance leaves the earlier pattern in place)
-        second = ~first & ((pat2 < 0) | (got.dist < dist2))
+        got = nearest_distance_in_each(p, seqset, substitutions_only=bool(flags & _native.F_SUBSTITUTIONS_ONLY))
+        has = got.dist >= 0
+        first = has & ((pattern < 0) | (got.dist < dist))  # (an equal distance leaves the earlier pattern in place)
+        second = has & ~first & ((pat2 < 0) | (got.dist < dist2))
         pat2[first], dist2[first] = pattern[first], dist[first]
         pattern[first], dist[first], end[first] = i, got.dist[first], got.end[first]
         pat2[second], dist2[second] = i, got.dist[second]

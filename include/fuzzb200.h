@@ -70,6 +70,9 @@ extern "C" {
 #define FZB_F_PER_RECORD 128u /* batches: accept a handle that holds a record set (fzb_haystack_set_records) and
                                  search every record of it; each out[i] is then what the single search of
                                  pattern i returns on that handle.  Refused on a handle without a record set */
+#define FZB_F_SUBSTITUTIONS_ONLY 256u /* the four fzb_nearest_* calls: the nearest match under substitutions only
+                                 (Hamming distance of the pattern to a window of its own length) instead of
+                                 Levenshtein distance; the only flag they take (DESIGN.md section 5.16) */
 
 struct fzb_stats_s;
 typedef struct fzb_haystack fzb_haystack; /* a device-resident sequence (or one shard of it) */
@@ -307,6 +310,11 @@ int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, const uint32_t
  * (1 <= m <= FZB_MAX_PATTERN; only m <= 64 is tuned).  Every refusal and every error leaves the handle as it was; the
  * call uses neither the handle's counters nor its output area, so the result of an earlier search stays valid and a
  * following search behaves as if the call had not happened.
+ *
+ * With FZB_F_SUBSTITUTIONS_ONLY (DESIGN.md section 5.16) E(e) is H(e), the number of positions where the window
+ * S[e-m:e] differs from P, for m <= e <= n only: d* is the smallest H(e), fzb_search_hamming lists exactly the n_ends
+ * windows at max_substitutions == d* (the first ends at first_end, starts at first_end - m) and none below.  With
+ * n < m there is no window: dist = UINT32_MAX, n_ends = 0, first_end = UINT64_MAX.  `stats` reports route 13.
  */
 int fzb_nearest_distance(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
                          uint32_t *dist, uint64_t *n_ends, uint64_t *first_end, struct fzb_stats_s *stats);
@@ -315,9 +323,11 @@ int fzb_nearest_distance(fzb_haystack *h, const uint8_t *pattern, uint32_t m, ui
  * The same for every record of a record set, in one scan: dist[r] = d* of record r alone and end[r] its first_end,
  * relative to the start of the record; an empty record gives (m, 0).  The column of the recurrence is reset at every
  * record start, so a separator is never read into an alignment, whatever its value.  The only read-back is 8 bytes
- * per record.  Needs a handle with a record set (FZB_E_INVALID otherwise).  FZB_E_UNSUPPORTED: a record of 2^32
- * bytes or more, any non-zero flag.  Every refusal and every error leaves the handle as it was; the arrays then hold
- * nothing meaningful.
+ * per record; `stats` reports route 11 (13 with FZB_F_SUBSTITUTIONS_ONLY).  Needs a handle with a record set
+ * (FZB_E_INVALID otherwise).  FZB_E_UNSUPPORTED: a record of 2^32
+ * bytes or more, any flag other than FZB_F_SUBSTITUTIONS_ONLY.  Every refusal and every error leaves the handle as it
+ * was; the arrays then hold nothing meaningful.  With FZB_F_SUBSTITUTIONS_ONLY windows never cross a record's edges,
+ * and a record shorter than m (an empty one included) gives (-1, -1).
  */
 int fzb_nearest_per_record(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
                            int32_t *dist, int64_t *end, /* each: one entry per record */
@@ -330,6 +340,8 @@ int fzb_nearest_per_record(fzb_haystack *h, const uint8_t *pattern, uint32_t m, 
  *
  * fzb_nearest_distance_batch: dist[i] and first_end[i] are what fzb_nearest_distance returns for pattern i (no n_ends).
  * Whole (unsharded) sequences outside a world without a record set only.  The read-back is 8 bytes per pattern.
+ * With FZB_F_SUBSTITUTIONS_ONLY a pattern longer than the sequence gives dist[i] = UINT32_MAX, first_end[i] =
+ * UINT64_MAX.
  */
 int fzb_nearest_distance_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count,
                                uint32_t flags, uint32_t *dist, uint64_t *first_end, /* each: one entry per pattern */
@@ -344,11 +356,14 @@ int fzb_nearest_distance_batch(fzb_haystack *h, const uint8_t *patterns, const u
  *   second_pattern[r], second_dist[r]   the smallest (d*_i(r), i) over the other patterns, -1 with a single pattern.
  * Every pattern has a value (d*_i <= m_i), so an empty record gives (the smallest (m_i, i), 0); with no patterns every
  * array is -1.  The read-back is 16 bytes per record.  Needs a handle with a record set (FZB_E_INVALID otherwise) whose
- * records are shorter than 2^32.
+ * records are shorter than 2^32.  With FZB_F_SUBSTITUTIONS_ONLY only the patterns that fit in record r (m_i <= its
+ * length) have a value and take part: a record where none fits gives -1 in every array, one where a single pattern
+ * fits gives -1 in second_pattern and second_dist.
  *
- * Both: FZB_E_UNSUPPORTED for any non-zero flag, more than 65 535 patterns, a shard or a handle in a world.  Every
- * refusal and every error leaves the handle as it was; the calls use neither the handle's counters, its output area
- * nor a pending result.  `stats` (optional) reports route 12.
+ * Both: FZB_E_UNSUPPORTED for any flag other than FZB_F_SUBSTITUTIONS_ONLY, more than 65 535 patterns, a shard or a
+ * handle in a world.  Every refusal and every error leaves the handle as it was; the calls use neither the handle's
+ * counters, its output area nor a pending result.  `stats` (optional) reports route 12 (14 with
+ * FZB_F_SUBSTITUTIONS_ONLY).
  */
 int fzb_nearest_best_per_record(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count,
                                 uint32_t flags, int32_t *pattern, int32_t *dist, int64_t *end, int32_t *second_pattern,
@@ -412,7 +427,8 @@ typedef struct fzb_stats_s {
                                4 hamming, 5 generic n-grams, 6 generic LP, 7 batch (summed statistics),
                                8 hamming batch scan, 9 generic n-grams batch scan, 10 generic LP batch
                                scan, 11 nearest/bit-vector-scan,
-                               12 nearest/batch-bit-vector-scan */
+                               12 nearest/batch-bit-vector-scan, 13 nearest/substitutions-scan,
+                               14 nearest/substitutions-batch-scan */
 } fzb_stats;
 int fzb_result_stats(const fzb_result *r, fzb_stats *out);
 void fzb_result_destroy(fzb_result *r);
