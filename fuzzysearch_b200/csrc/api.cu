@@ -154,8 +154,8 @@ struct BestBufs {  // fzb_best_per_record (best_kernels.cuh)
     DevBuf<uint64_t> d_words;  // best[records], then top2[records]
     DevBuf<uint32_t> d_ids;    // the pattern ordinals of the pass being reduced
 };
-// fzb_best_per_record in progress on a handle (DESIGN.md section 5.13): the batches it runs reduce the raw records of
-// every pass and of every one-by-one search into these words instead of returning lists.
+// The sink of the batches fzb_best_per_record runs (DESIGN.md section 5.13): they reduce the raw records of every pass
+// and of every one-by-one search into these words instead of returning lists.
 struct BestState {
     uint64_t *best, *top2;    // one word per record each
     const uint32_t *ordinal;  // pattern i of the batch being run is pattern ordinal[i] of the call
@@ -306,7 +306,6 @@ struct fzb_haystack {
     std::unique_ptr<GenericBatchBufs> gbatch;
     std::unique_ptr<RecBufs> recs;  // the record set, if any (cleared by every upload)
     std::unique_ptr<BestBufs> bestb;
-    BestState *best = nullptr;      // set for the duration of fzb_best_per_record (BestScope)
     std::unique_ptr<NearBufs> nearb;
     std::unique_ptr<NearBatchBufs> nearbatch;
 };
@@ -2058,47 +2057,6 @@ static void add_stats(fzb_stats *sum, const fzb_stats &s) {
     sum->n_launches += s.n_launches;
 }
 
-// The attempt loop of a batch pass.  `enqueue()` puts the kernels of one attempt on h->stream (behind h->ev[0]) and
-// returns FZB_OK, an error, or +1 when a device structure of the pass overflowed.  Returns the same, +1 also when a
-// kernel raised CNT_OVERFLOW or the pass emitted more than kMaxRawRecs records; an attempt whose raw records did not
-// fit the output buffer is redone with a larger one.  On FZB_OK `raw` holds the records (under fzb_best_per_record they stay
-// in h->d_out and `raw` stays empty), `cnts` the counters, and `pass` the time and the bytes scanned.
-template <class F>
-static int run_batch_pass(fzb_haystack *h, F enqueue, std::vector<RawRec> &raw, uint32_t cnts[CNT_COUNT],
-                          fzb_stats &pass) {
-    detach_pending(h);  // the kernels are about to overwrite the output buffer an earlier result may still point at
-    for (int attempt = 0; attempt < 8; attempt++) {
-        h->counters_clean = false;  // (a batch pass leaves its counters behind)
-        CK(cudaMemsetAsync(h->d_counters.get(), 0, CNT_COUNT * sizeof(uint32_t), h->stream));
-        CK(cudaEventRecord(h->ev[0], h->stream));
-        int rc = enqueue();
-        if (rc) return rc;
-        CK(cudaEventRecord(h->ev[2], h->stream));
-        rc = read_counters(h, cnts);
-        if (rc) return rc;
-        if (cnts[CNT_OVERFLOW]) return 1;
-        const uint32_t n = cnts[CNT_OUT];
-        // more records than one search may return, over all the patterns of the pass: they go one by one, where
-        // each pattern only has to stay within the limit on its own
-        if (n > kMaxRawRecs) return 1;
-        if (n > h->d_out.size()) {
-            TRY(ensure_out_cap(h, n));
-            continue;
-        }
-        if (!h->best) raw.resize(n);  // (fzb_best_per_record reduces the records where they are: finish_pass)
-        if (!raw.empty()) {
-            CK(cudaMemcpyAsync(raw.data(), h->d_out.get(), (size_t)n * sizeof(RawRec), cudaMemcpyDeviceToHost, h->stream));
-            CK(cudaStreamSynchronize(h->stream));
-        }
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, h->ev[0], h->ev[2]);
-        pass.gpu_ms = ms;
-        pass.bytes_scanned = h->buf_len;
-        return FZB_OK;
-    }
-    return fail(FZB_E_CUDA, "output buffer kept overflowing");
-}
-
 // Splits the raw records of a pass over the patterns ids[] (`ngram` = pattern ordinal << 8 | n-gram) into the results
 // out[ids[i]], consolidates each list (unconsolidated: FINAL is the raw list in canonical order, as the Hamming
 // search returns it), and adds the pass to `sum`.  Every result carries the pass's route, the first one its other
@@ -2145,67 +2103,200 @@ static int split_batch(const std::vector<RawRec> &raw, const std::vector<uint32_
     return FZB_OK;
 }
 
-// The n raw records in h->d_out reduced into the words of the fzb_best_per_record in progress: those of a shared pass
-// whose pattern j is pattern d_ids[j] of the call, or (d_ids == nullptr) those of a single search of pattern `id`.
-static int best_accumulate(fzb_haystack *h, uint32_t n, const uint32_t *d_ids, uint32_t id) {
+// The n raw records in h->d_out reduced into the words of `best`: those of a shared pass whose pattern j is pattern
+// d_ids[j] of the fzb_best_per_record call, or (d_ids == nullptr) those of a single search of pattern `id`.
+static int best_accumulate(fzb_haystack *h, const BestState &best, uint32_t n, const uint32_t *d_ids, uint32_t id) {
     if (n == 0) return FZB_OK;
     const int grid = (int)std::min<uint32_t>((n + kBestThreads - 1) / kBestThreads, (uint32_t)h->sm_count * 8);
     if (d_ids)
         k_best_accumulate<true><<<grid, kBestThreads, 0, h->stream>>>(h->d_out.get(), n, rec_set(h), d_ids, id,
-                                                                     h->best->best, h->best->top2);
+                                                                     best.best, best.top2);
     else
         k_best_accumulate<false><<<grid, kBestThreads, 0, h->stream>>>(h->d_out.get(), n, rec_set(h), d_ids, id,
-                                                                      h->best->best, h->best->top2);
+                                                                      best.best, best.top2);
     CK(cudaGetLastError());
     return FZB_OK;
 }
 
-// What a pass over the patterns ids[] ends with: the per-pattern results of split_batch or, under
-// fzb_best_per_record, its n raw records reduced where they are, each out[ids[i]] then an empty result that marks the
-// pattern as searched and carries the pass's stats.  Every way a pass can still overflow (+1) lies before this point
-// (for the chunked passes: behind the last chunk), so a pass that is redone pattern by pattern has contributed nothing.
-static int finish_pass(fzb_haystack *h, const std::vector<RawRec> &raw, uint32_t n, const std::vector<uint32_t> &ids,
-                       fzb_stats pass, int raw_order, bool unconsolidated, fzb_result **out, fzb_stats *sum) {
-    if (!h->best) return split_batch(raw, ids, pass, raw_order, unconsolidated, out, sum);
-    if (n) {
-        std::vector<uint32_t> ordinals(ids.size());
-        for (size_t j = 0; j < ids.size(); j++) ordinals[j] = h->best->ordinal[ids[j]];
-        // (a pageable source: the copy has left the vector when it returns)
-        CK(cudaMemcpyAsync(h->bestb->d_ids.get(), ordinals.data(), ordinals.size() * sizeof(uint32_t),
-                           cudaMemcpyHostToDevice, h->stream));
-        TRY(best_accumulate(h, n, h->bestb->d_ids.get(), 0));
-        pass.n_launches++;
+// One batch call: a batch entry point's, or one class of fzb_best_per_record's.  It holds the patterns, what the flags
+// let the passes do, the running sum of the stats and the sink the passes and the one-by-one searches end in: the
+// per-pattern results out[count], or (best != nullptr) the words of fzb_best_per_record, into which every record is
+// reduced (DESIGN.md section 5.13).
+struct BatchCall {
+    fzb_haystack *h;
+    const uint8_t *patterns;
+    const uint32_t *offsets;
+    uint32_t count, flags;
+    fzb_result **out;        // list sink: out[i] is pattern i's result once a pass or its own search settled it
+    const BestState *best;   // reduction sink
+    std::vector<uint8_t> done;  // reduction sink: pattern i is settled
+    // FZB_F_TINY_LIST (testing) shrinks the capacities of the shared passes; the passes take no other flag than that
+    // and FZB_F_PER_RECORD (forced routes, raw-only, the multi-GPU reduction: one by one)
+    bool tiny, share;
+    fzb_stats sum{};
+
+    BatchCall(fzb_haystack *h_, const uint8_t *p, const uint32_t *o, uint32_t n, uint32_t f, fzb_result **out_,
+              const BestState *best_)
+        : h(h_), patterns(p), offsets(o), count(n), flags(f), out(out_), best(best_), done(best_ ? n : 0, 0),
+          tiny((f & FZB_F_TINY_LIST) != 0), share((f & ~(FZB_F_TINY_LIST | FZB_F_PER_RECORD)) == 0 && h_->buf_len > 0) {}
+
+    uint32_t len(uint32_t i) const { return offsets[i + 1] - offsets[i]; }
+    bool settled(uint32_t i) const { return best ? done[i] != 0 : out[i] != nullptr; }
+
+    // The refusals of the batch entry points, behind every result cleared.
+    int begin() {
+        for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
+        TRY(check_batch_records(h, flags));
+        for (uint32_t i = 0; i < count; i++)
+            if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
+        return FZB_OK;
     }
-    for (size_t j = 0; j < ids.size(); j++) {
-        fzb_result *res = new (std::nothrow) fzb_result();
-        if (!res) return fail(FZB_E_CUDA, "out of host memory");
-        if (j == 0) res->stats = pass;
-        res->stats.route = pass.route;
-        out[ids[j]] = res;
+
+    // The outcome `rc` of a shared pass over the patterns ids[]: an error drops every result; an overflow (+1) drops
+    // the pass's results, leaving its patterns to the one-by-one searches.
+    int settle(int rc, const std::vector<uint32_t> &ids) {
+        auto drop = [&](uint32_t j) {
+            if (!out) return;  // (the reduction sink keeps no results)
+            fzb_result_destroy(out[j]);
+            out[j] = nullptr;
+        };
+        if (rc < 0)
+            for (uint32_t j = 0; j < count; j++) drop(j);
+        if (rc > 0)
+            for (uint32_t id : ids) drop(id);
+        return rc < 0 ? rc : FZB_OK;
     }
-    add_stats(sum, pass);
+
+    // What a pass over the patterns ids[] ends with: the per-pattern results of split_batch or its n raw records
+    // reduced where they are, and its stats in the sum.  Every way a pass can still overflow (+1) lies before this
+    // point (for the chunked passes: behind the last chunk), so a pass that is redone pattern by pattern has
+    // contributed nothing.
+    int finish_pass(const std::vector<RawRec> &raw, uint32_t n, const std::vector<uint32_t> &ids, fzb_stats pass,
+                    int raw_order, bool unconsolidated) {
+        if (!best) return split_batch(raw, ids, pass, raw_order, unconsolidated, out, &sum);
+        if (n) {
+            std::vector<uint32_t> ordinals(ids.size());
+            for (size_t j = 0; j < ids.size(); j++) ordinals[j] = best->ordinal[ids[j]];
+            // (a pageable source: the copy has left the vector when it returns)
+            CK(cudaMemcpyAsync(h->bestb->d_ids.get(), ordinals.data(), ordinals.size() * sizeof(uint32_t),
+                               cudaMemcpyHostToDevice, h->stream));
+            TRY(best_accumulate(h, *best, n, h->bestb->d_ids.get(), 0));
+            pass.n_launches++;
+        }
+        for (uint32_t id : ids) done[id] = 1;
+        add_stats(&sum, pass);
+        return FZB_OK;
+    }
+
+    // The patterns no pass settled, each searched on its own by `single(i, flags, &res)`, the class's single search
+    // (which honours a record set by itself); then the call's stats in *total.  Under the reduction sink the search
+    // returns the raw stream only, which is reduced while still in h->d_out and dropped, so that nothing reads it back.
+    template <class F>
+    int finish(fzb_stats *total, F single) {
+        const uint32_t f = (flags & ~FZB_F_PER_RECORD) | (best ? FZB_F_NO_FINAL : 0u);
+        for (uint32_t i = 0; i < count; i++) {
+            if (settled(i)) continue;
+            fzb_result *res = nullptr;
+            TRY(settle(single(i, f, &res), {}));
+            if (!best) {
+                add_stats(&sum, res->stats);
+                out[i] = res;
+                continue;
+            }
+            // (destroying the result unlinks it from the handle: nothing fetches the records it leaves in h->d_out)
+            const int rc = best_accumulate(h, *best, res->raw_n, nullptr, best->ordinal[i]);
+            if (res->raw_n) res->stats.n_launches++;
+            add_stats(&sum, res->stats);
+            fzb_result_destroy(res);
+            TRY(rc);
+        }
+        sum.route = 7;  // batch
+        if (total) *total = sum;
+        return FZB_OK;
+    }
+};
+
+// The attempt loop of a batch pass.  `enqueue()` puts the kernels of one attempt on h->stream (behind h->ev[0]) and
+// returns FZB_OK, an error, or +1 when a device structure of the pass overflowed.  Returns the same, +1 also when a
+// kernel raised CNT_OVERFLOW or the pass emitted more than kMaxRawRecs records; an attempt whose raw records did not
+// fit the output buffer is redone with a larger one.  On FZB_OK `raw` holds the records (under the reduction sink they
+// stay in h->d_out and `raw` stays empty), `cnts` the counters, and `pass` the time and the bytes scanned.
+template <class F>
+static int run_batch_pass(const BatchCall &c, F enqueue, std::vector<RawRec> &raw, uint32_t cnts[CNT_COUNT],
+                          fzb_stats &pass) {
+    fzb_haystack *h = c.h;
+    detach_pending(h);  // the kernels are about to overwrite the output buffer an earlier result may still point at
+    for (int attempt = 0; attempt < 8; attempt++) {
+        h->counters_clean = false;  // (a batch pass leaves its counters behind)
+        CK(cudaMemsetAsync(h->d_counters.get(), 0, CNT_COUNT * sizeof(uint32_t), h->stream));
+        CK(cudaEventRecord(h->ev[0], h->stream));
+        int rc = enqueue();
+        if (rc) return rc;
+        CK(cudaEventRecord(h->ev[2], h->stream));
+        rc = read_counters(h, cnts);
+        if (rc) return rc;
+        if (cnts[CNT_OVERFLOW]) return 1;
+        const uint32_t n = cnts[CNT_OUT];
+        // more records than one search may return, over all the patterns of the pass: they go one by one, where
+        // each pattern only has to stay within the limit on its own
+        if (n > kMaxRawRecs) return 1;
+        if (n > h->d_out.size()) {
+            TRY(ensure_out_cap(h, n));
+            continue;
+        }
+        if (!c.best) raw.resize(n);  // (the reduction sink reduces the records where they are: finish_pass)
+        if (!raw.empty()) {
+            CK(cudaMemcpyAsync(raw.data(), h->d_out.get(), (size_t)n * sizeof(RawRec), cudaMemcpyDeviceToHost, h->stream));
+            CK(cudaStreamSynchronize(h->stream));
+        }
+        float ms = 0.f;
+        cudaEventElapsedTime(&ms, h->ev[0], h->ev[2]);
+        pass.gpu_ms = ms;
+        pass.bytes_scanned = h->buf_len;
+        return FZB_OK;
+    }
+    return fail(FZB_E_CUDA, "output buffer kept overflowing");
+}
+
+// The scan times, list lengths and chunks of one attempt of a chunked pass (run_chunks).
+struct ChunkSums {
+    float scan_ms = 0.f;
+    uint64_t listed = 0;  // (over all chunks: more than 2^32 on a large haystack)
+    uint32_t chunks = 0;
+};
+
+// One attempt of a chunked pass (LP, 2-bit) over the own range in chunks of `chunk` positions: per chunk the counters
+// cnts[list] (the scan's list) and the one after it cleared, `scan(lo, hi)` between h->ev[1] and h->ev[2], `verify()`,
+// and the counters read back into cnts.  Returns FZB_OK, an error, or +1 at the first chunk whose kernels raised
+// CNT_OVERFLOW or the counter `full` (a list too small for the chunk).
+template <class S, class V>
+static int run_chunks(fzb_haystack *h, uint64_t chunk, int list, int full, uint32_t cnts[CNT_COUNT], ChunkSums &s,
+                      S scan, V verify) {
+    s = ChunkSums{};
+    for (uint64_t lo = h->own_lo; lo < h->own_hi; lo += chunk) {
+        CK(cudaMemsetAsync(h->d_counters.get() + list, 0, 2 * sizeof(uint32_t), h->stream));
+        CK(cudaEventRecord(h->ev[1], h->stream));
+        scan(lo, std::min<uint64_t>(h->own_hi, lo + chunk));
+        CK(cudaEventRecord(h->ev[2], h->stream));
+        TRY(verify());
+        CK(cudaGetLastError());
+        s.chunks++;
+        TRY(read_counters(h, cnts));
+        float ms = 0.f;
+        cudaEventElapsedTime(&ms, h->ev[1], h->ev[2]);
+        s.scan_ms += ms;
+        s.listed += cnts[list];
+        if (cnts[CNT_OVERFLOW] || cnts[full]) return 1;
+    }
     return FZB_OK;
 }
 
-// The flags of a batch's one-by-one searches.  Under fzb_best_per_record they return the raw stream only
-// (best_single reduces it).
-static uint32_t single_flags(const fzb_haystack *h, uint32_t flags) {
-    return (flags & ~FZB_F_PER_RECORD) | (h->best ? FZB_F_NO_FINAL : 0u);
-}
-
-// Under fzb_best_per_record, behind the one-by-one search of pattern i of a batch: its raw records, still in h->d_out,
-// are reduced there and dropped, so that nothing reads them back.
-static int best_single(fzb_haystack *h, fzb_result *res, uint32_t i) {
-    if (!h->best) return FZB_OK;
-    TRY(best_accumulate(h, res->raw_n, nullptr, h->best->ordinal[i]));
-    if (res->raw_n) res->stats.n_launches++;
-    std::lock_guard<std::mutex> lock(g_pending_mutex);
-    if (res->owner) res->owner->pending = nullptr;
-    res->owner = nullptr;
-    res->raw_in_stage = false;
-    res->raw.clear();
-    res->raw_n = 0;
-    return FZB_OK;
+// The slot of pattern `id` in a pass, limit k; the pass sets its L and n_ngrams.
+static void fill_pat(BatchPat &bp, const BatchCall &c, uint32_t id, uint32_t k) {
+    memset(&bp, 0, sizeof bp);
+    memcpy(bp.P, c.patterns + c.offsets[id], c.len(id));
+    bp.m = (int)c.len(id);
+    bp.k = (int)k;
 }
 
 // Builds the posting table of a pass -- open addressing on the key (key * kGramMul), each slot the key and its first
@@ -2306,28 +2397,24 @@ static void two_bit_key(std::unordered_map<uint32_t, std::vector<uint32_t>> &key
     for (uint32_t x = 0; x < (1u << (2 * (kHbKeySyms - n))); x++) keys[key | (x << (2 * n))].push_back(post);
 }
 
-// One pass over the haystack for the patterns ids[0..cnt): fills out[ids[i]].  Returns FZB_OK, an error, or +1 if
-// the pass overflowed a device structure (the caller then searches these patterns one by one).
+// One pass over the haystack for the patterns ids[0..cnt): settles them in the call's sink.  Returns FZB_OK, an
+// error, or +1 if the pass overflowed a device structure (the caller then searches these patterns one by one).
 // dense = false: the q-sample scan (k_filter_multi / k_verify_multi) over the 4-grams of the patterns;
 // dense = true: the n-gram-prefix scan at every position (k_filter_mdense / k_verify_mhits).
-// tiny: the capacities of FZB_F_TINY_LIST.
 // glim: nullptr for Levenshtein patterns (ks = max_l_dist); for generic patterns (ks = max_l_dist) their limits as
 // prepare_generic_pass takes them, and the generic verify kernels (k_verify_multi_generic / k_verify_mhits_generic).
-static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, const uint32_t *ks,
-                      const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, bool dense, bool tiny,
+static int batch_pass(BatchCall &c, const uint32_t *ks, const std::vector<uint32_t> &ids, bool dense,
                       const uint32_t *glim = nullptr) {
+    fzb_haystack *h = c.h;
     const uint32_t cnt = (uint32_t)ids.size();
     std::vector<BatchPat> pats(cnt);
     std::vector<uint32_t> pinfo(cnt);
     std::unordered_map<uint32_t, std::vector<uint32_t>> grams;
     grams.reserve(cnt * 48);
     for (uint32_t i = 0; i < cnt; i++) {
-        const uint32_t id = ids[i], m = offsets[id + 1] - offsets[id], k = ks[id];
+        const uint32_t id = ids[i], m = c.len(id), k = ks[id];
         BatchPat &bp = pats[i];
-        memset(&bp, 0, sizeof bp);
-        memcpy(bp.P, patterns + offsets[id], m);
-        bp.m = (int)m;
-        bp.k = (int)k;
+        fill_pat(bp, c, id, k);
         bp.L = (int)(m / (k + 1));
         bp.n_ngrams = (int)m / bp.L;
         // The k of pinfo only sets the anchors k_filter_multi marks around a word hit, [g-o-k, g-o+k+m-L].  A generic
@@ -2369,15 +2456,15 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
     mp.set = b.d_mset.get();
     mp.set_mask = (uint32_t)b.d_mset.size() - 1;
     mp.work = b.d_mwork.get();
-    mp.work_cap = tiny ? std::min<uint32_t>(b.d_mwork.size(), kTinyBatchCap) : (uint32_t)b.d_mwork.size();
-    const uint32_t hits_cap = tiny ? std::min<uint32_t>(h->d_mhits.size(), kTinyBatchCap) : (uint32_t)h->d_mhits.size();
+    mp.work_cap = c.tiny ? std::min<uint32_t>(b.d_mwork.size(), kTinyBatchCap) : (uint32_t)b.d_mwork.size();
+    const uint32_t hits_cap = c.tiny ? std::min<uint32_t>(h->d_mhits.size(), kTinyBatchCap) : (uint32_t)h->d_mhits.size();
     const int64_t nvec = (int64_t)(round_up(h->buf_len, 16) / 16);
     const int64_t ntiles = (nvec + kMultiTileVecs - 1) / kMultiTileVecs;
     std::vector<RawRec> raw;
     uint32_t cnts[CNT_COUNT];
     fzb_stats pass{};
     const RecSet rs = rec_set(h);  // (the filters only look at content: only the verify kernels take it)
-    rc = run_batch_pass(h, [&]() -> int {
+    rc = run_batch_pass(c, [&]() -> int {
         MdenseParams dp{mp, b.d_bpats.get(), h->d_mhits.get(), hits_cap};
         if (ntiles > 0) {
             const int grid = (int)std::min<int64_t>(ntiles, h->sm_count);
@@ -2419,16 +2506,16 @@ static int batch_pass(fzb_haystack *h, const uint8_t *patterns, const uint32_t *
     pass.n_candidates = cnts[CNT_CAND];
     pass.n_launches = 2;
     // (the generic n-gram route's raw order: n-gram, hit index, then the window's matches in canonical order)
-    return finish_pass(h, raw, cnts[CNT_OUT], ids, pass, glim ? 2 : 0, false, out, sum);
+    return c.finish_pass(raw, cnts[CNT_OUT], ids, pass, glim ? 2 : 0, false);
 }
 
 // One shared scan for up to 64 LP-route patterns (k_lp_scan_multi / k_lp_verify_multi).  Same return convention
 // as batch_pass.  glim: as for batch_pass (ks = the lowered max_l_dist of the LP route, search_generic); a generic
 // NFA opens a candidate at every start (generic_search.py:81), so the scan applies the counting condition only, and
 // k_lp_verify_multi_generic verifies.
-static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, const uint32_t *ks,
-                         const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, bool tiny,
+static int batch_pass_lp(BatchCall &c, const uint32_t *ks, const std::vector<uint32_t> &ids,
                          const uint32_t *glim = nullptr) {
+    fzb_haystack *h = c.h;
     const uint32_t cnt = (uint32_t)ids.size();
     std::vector<BatchPat> pats(cnt);
     std::vector<ulonglong2> lut(256, make_ulonglong2(0ull, 0ull));
@@ -2437,14 +2524,9 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
     int wmax = 0;
     uint32_t kmax = 0;
     for (uint32_t i = 0; i < cnt; i++) {
-        const uint32_t id = ids[i], m = offsets[id + 1] - offsets[id], k = ks[id];
+        const uint32_t id = ids[i], m = c.len(id), k = ks[id];
         BatchPat &bp = pats[i];
-        memset(&bp, 0, sizeof bp);
-        memcpy(bp.P, patterns + offsets[id], m);
-        bp.m = (int)m;
-        bp.k = (int)k;
-        bp.L = 0;
-        bp.n_ngrams = 0;
+        fill_pat(bp, c, id, k);  // (L = n_ngrams = 0: no n-grams)
         for (uint32_t j = 0; j < m; j++) {
             lut[bp.P[j]].x |= 1ull << i;
             pm32[(size_t)i * 256 + bp.P[j]] |= 1u << j;
@@ -2483,7 +2565,7 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
     lp.pats = h->batch->d_bpats.get();
     lp.pm32 = d_pm32;
     lp.list = lb.d_lmlist.get();
-    lp.list_cap = tiny ? std::min<uint32_t>(lb.d_lmlist.size(), kTinyLpListCap) : (uint32_t)lb.d_lmlist.size();
+    lp.list_cap = c.tiny ? std::min<uint32_t>(lb.d_lmlist.size(), kTinyLpListCap) : (uint32_t)lb.d_lmlist.size();
     lp.counters = h->d_counters.get();
     int per_sm = 2;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lp_scan_multi, kLmThreads, kLmSmem));
@@ -2493,24 +2575,20 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
         TRY(prepare_generic_pass(h, glim, ids, vgrid));
     else
         TRY(ensure_scratch(h, (uint64_t)vgrid * kLpThreads * 2 * sim_cap));
-    const uint64_t chunk = tiny ? kTinyLpChunk : 256ull << 20;  // starts per scan: bounds the survivor list
+    const uint64_t chunk = c.tiny ? kTinyLpChunk : 256ull << 20;  // starts per scan: bounds the survivor list
     std::vector<RawRec> raw;
     uint32_t cnts[CNT_COUNT];
     fzb_stats pass{};
     const RecSet rs = rec_set(h);  // (verify kernels only)
-    float scan_ms = 0.f;
-    uint64_t n_work = 0;
-    int rc = run_batch_pass(h, [&]() -> int {
-        scan_ms = 0.f;
-        n_work = 0;
-        for (uint64_t lo = h->own_lo; lo < h->own_hi; lo += chunk) {
+    ChunkSums cs;
+    int rc = run_batch_pass(c, [&]() -> int {
+        // CNT_LMWORK: the scan's list overflowed
+        return run_chunks(h, chunk, CNT_LMLIST, CNT_LMWORK, cnts, cs, [&](uint64_t lo, uint64_t hi) {
             lp.own_lo = (int64_t)lo;
-            lp.own_hi = (int64_t)std::min<uint64_t>(h->own_hi, lo + chunk);
-            CK(cudaMemsetAsync(h->d_counters.get() + CNT_LMLIST, 0, 2 * sizeof(uint32_t), h->stream));  // list length + flag
-            CK(cudaMemsetAsync(h->d_counters.get() + CNT_LMNEXT, 0, sizeof(uint32_t), h->stream));       // verify work counter
-            CK(cudaEventRecord(h->ev[1], h->stream));
+            lp.own_hi = (int64_t)hi;
             k_lp_scan_multi<<<h->sm_count * per_sm, kLmThreads, kLmSmem, h->stream>>>(lp);
-            CK(cudaEventRecord(h->ev[2], h->stream));
+        }, [&]() -> int {
+            CK(cudaMemsetAsync(h->d_counters.get() + CNT_LMNEXT, 0, sizeof(uint32_t), h->stream));  // verify work counter
             // exact per-pattern windows, then a counting sort by pattern: the scan's list becomes the sorted output
             CK(cudaMemsetAsync(lb.d_lmhist.get(), 0, 256 * sizeof(uint32_t), h->stream));
             k_lm_refine<<<h->sm_count * 8, kLmSortThreads, 0, h->stream>>>(lp, lb.d_lmkept.get(), lb.d_lmhist.get());
@@ -2531,23 +2609,15 @@ static int batch_pass_lp(fzb_haystack *h, const uint8_t *patterns, const uint32_
                         lp, lb.d_lmlist.get(), lb.d_lmhist.get(), h->d_scratch.get(), sim_cap, h->d_out.get(),
                         h->d_out.size(), h->d_counters.get(), rs);
             });
-            CK(cudaGetLastError());
-            const int r2 = read_counters(h, cnts);
-            if (r2) return r2;
-            float ms = 0.f;
-            cudaEventElapsedTime(&ms, h->ev[1], h->ev[2]);
-            scan_ms += ms;
-            n_work += cnts[CNT_LMLIST];
-            sum->n_launches += 4;
-            if (cnts[CNT_LMWORK] || cnts[CNT_OVERFLOW]) return 1;  // survivor list / candidate lists too small
-        }
-        return FZB_OK;
+            return FZB_OK;
+        });
     }, raw, cnts, pass);
     if (rc) return rc;
     pass.route = glim ? 10 : 3;
-    pass.filter_ms = scan_ms;
-    pass.n_candidates = n_work;
-    return finish_pass(h, raw, cnts[CNT_OUT], ids, pass, 1, false, out, sum);
+    pass.filter_ms = cs.scan_ms;
+    pass.n_candidates = cs.listed;
+    pass.n_launches = 4 * cs.chunks;
+    return c.finish_pass(raw, cnts[CNT_OUT], ids, pass, 1, false);
 }
 
 // Admission of n-gram-route Levenshtein patterns to the 2-bit pass (k_filter_mdense2 / k_verify_mhits) on
@@ -2593,23 +2663,19 @@ static double dna_lev_hits(const fzb_haystack *h, uint32_t m, uint32_t k, double
 // as batch_pass.  The own range is scanned and verified in chunks whose expected hits (hits_per_pos per position)
 // fill at most half the hit list; an overflowing chunk sends the pass's patterns one by one.  tiny
 // (FZB_F_TINY_LIST): kTinyBatchCap hits and chunks of kTinyLpChunk positions.
-static int batch_pass_dna(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, const uint32_t *ks,
-                          const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, double hits_per_pos,
-                          bool tiny) {
+static int batch_pass_dna(BatchCall &c, const uint32_t *ks, const std::vector<uint32_t> &ids, double hits_per_pos) {
+    fzb_haystack *h = c.h;
     const uint32_t cnt = (uint32_t)ids.size();
     std::vector<BatchPat> pats(cnt);
     std::vector<uint32_t> pinfo(cnt);
     Mdense2Params p{};
-    two_bit_code(patterns, offsets, ids, p.code);
+    two_bit_code(c.patterns, c.offsets, ids, p.code);
     std::unordered_map<uint32_t, std::vector<uint32_t>> keys;  // key -> postings pattern << 8 | n-gram
     keys.reserve(cnt * 64);
     for (uint32_t i = 0; i < cnt; i++) {
-        const uint32_t id = ids[i], m = offsets[id + 1] - offsets[id], k = ks[id];
+        const uint32_t id = ids[i], m = c.len(id), k = ks[id];
         BatchPat &bp = pats[i];
-        memset(&bp, 0, sizeof bp);
-        memcpy(bp.P, patterns + offsets[id], m);
-        bp.m = (int)m;
-        bp.k = (int)k;
+        fill_pat(bp, c, id, k);
         bp.L = (int)(m / (k + 1));
         bp.n_ngrams = (int)m / bp.L;
         pinfo[i] = m | (k << 8) | ((uint32_t)bp.L << 16);
@@ -2619,149 +2685,149 @@ static int batch_pass_dna(fzb_haystack *h, const uint8_t *patterns, const uint32
     int rc = upload_pass_tables(h, keys, bits, pinfo, pats, [&](uint32_t w) { bits[w >> 5] |= 1u << (w & 31u); });
     if (rc) return rc;
     TRY(ensure_mhits(h));
-    const uint32_t hits_cap = tiny ? std::min<uint32_t>(h->d_mhits.size(), kTinyBatchCap) : (uint32_t)h->d_mhits.size();
+    const uint32_t hits_cap = c.tiny ? std::min<uint32_t>(h->d_mhits.size(), kTinyBatchCap) : (uint32_t)h->d_mhits.size();
     p.dp = MdenseParams{pass_params(h), h->batch->d_bpats.get(), h->d_mhits.get(), hits_cap};
     const uint64_t tile = (uint64_t)kMultiTileVecs * 16;
-    const uint64_t chunk = tiny ? kTinyLpChunk
-                                : std::max(tile, (uint64_t)(hits_cap / 2 / std::max(hits_per_pos, 1e-9)) / tile * tile);
+    const uint64_t chunk = c.tiny ? kTinyLpChunk
+                                  : std::max(tile, (uint64_t)(hits_cap / 2 / std::max(hits_per_pos, 1e-9)) / tile * tile);
     const int64_t nvec = (int64_t)(round_up(h->buf_len, 16) / 16);
     std::vector<RawRec> raw;
     uint32_t cnts[CNT_COUNT];
     fzb_stats pass{};
     const RecSet rs = rec_set(h);  // (verify kernel only)
-    float scan_ms = 0.f;
-    uint32_t nchunks = 0;
-    uint64_t n_hits = 0;  // (over all chunks: more than 2^32 on a large haystack)
-    rc = run_batch_pass(h, [&]() -> int {
-        scan_ms = 0.f;
-        nchunks = 0;
-        n_hits = 0;
-        for (uint64_t lo = h->own_lo; lo < h->own_hi; lo += chunk) {
+    ChunkSums cs;
+    rc = run_batch_pass(c, [&]() -> int {
+        // CNT_OVERFLOW: the chunk's hits did not fit the list
+        return run_chunks(h, chunk, CNT_MHITS, CNT_OVERFLOW, cnts, cs, [&](uint64_t lo, uint64_t hi) {
             p.scan_lo = (int64_t)lo;
-            p.scan_hi = (int64_t)std::min<uint64_t>(h->own_hi, lo + chunk);
+            p.scan_hi = (int64_t)hi;
             const int64_t v0 = (p.scan_lo - (int64_t)h->buf_lo) / 16;
             const int64_t v1 = (p.scan_hi - (int64_t)h->buf_lo + 15) / 16;
             const int64_t ntiles = (v1 - v0 + kMultiTileVecs - 1) / kMultiTileVecs;
             p.dp.mp.counters = h->d_counters.get();
-            CK(cudaMemsetAsync(h->d_counters.get() + CNT_MHITS, 0, 2 * sizeof(uint32_t), h->stream));  // list + work
-            CK(cudaEventRecord(h->ev[1], h->stream));
             k_filter_mdense2<<<(int)std::min<int64_t>(ntiles, h->sm_count), kMultiThreads, kMdense2Smem, h->stream>>>(
                 p, nvec, v0, ntiles);
-            CK(cudaEventRecord(h->ev[2], h->stream));
+        }, [&]() -> int {
             with_recs(h, [&](auto rec) {
                 constexpr bool R = decltype(rec)::value;
                 k_verify_mhits<R><<<h->sm_count * 8, kMhThreads, 0, h->stream>>>(p.dp, h->d_out.get(), h->d_out.size(),
                                                                                     h->d_counters.get(), rs);
             });
-            CK(cudaGetLastError());
-            nchunks++;
-            const int r2 = read_counters(h, cnts);
-            if (r2) return r2;
-            float ms = 0.f;
-            cudaEventElapsedTime(&ms, h->ev[1], h->ev[2]);
-            scan_ms += ms;
-            n_hits += cnts[CNT_MHITS];
-            if (cnts[CNT_OVERFLOW]) return 1;  // the chunk's hits did not fit the list
-        }
-        return FZB_OK;
+            return FZB_OK;
+        });
     }, raw, cnts, pass);
     if (rc) return rc;
     pass.route = 2;
-    pass.filter_ms = scan_ms;
-    pass.n_candidates = n_hits;
-    pass.n_launches = 2 * nchunks;
-    return finish_pass(h, raw, cnts[CNT_OUT], ids, pass, 0, false, out, sum);
+    pass.filter_ms = cs.scan_ms;
+    pass.n_candidates = cs.listed;
+    pass.n_launches = 2 * cs.chunks;
+    return c.finish_pass(raw, cnts[CNT_OUT], ids, pass, 0, false);
 }
 
-// The outcome `rc` of a shared pass over the patterns ids[] of a batch of `count` results: an error drops every
-// result; an overflow (+1) drops the pass's results, leaving its patterns to the one-by-one path.
-static int settle_pass(int rc, const std::vector<uint32_t> &ids, fzb_result **out, uint32_t count) {
-    auto drop = [&](uint32_t j) {
-        if (out[j]) fzb_result_destroy(out[j]);
-        out[j] = nullptr;
-    };
-    if (rc < 0)
-        for (uint32_t j = 0; j < count; j++) drop(j);
-    if (rc > 0)
-        for (uint32_t id : ids) drop(id);
-    return rc < 0 ? rc : FZB_OK;
-}
-
-extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
-                                            const uint32_t *max_l_dist, uint32_t count, uint32_t flags,
-                                            fzb_result **out, fzb_stats *total) {
-    HandleLock handle_lock(h);
-    if (!h || !out || (count && (!patterns || !offsets || !max_l_dist))) return fail(FZB_E_INVALID, "NULL argument");
-    for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
-    TRY(check_batch_records(h, flags));
-    for (uint32_t i = 0; i < count; i++)
-        if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
-    fzb_stats sum{};
-    auto settle = [&](int rc, const std::vector<uint32_t> &ids) { return settle_pass(rc, ids, out, count); };
-    // patterns the shared scan can take: n-gram route, q-sample lemma holds, 4-grams selective on this haystack,
-    // short enough for the 64-bit match table; no special flags (forced routes, raw-only, multi-GPU reduction) other
-    // than FZB_F_TINY_LIST, which shrinks the capacities of the shared passes, and FZB_F_PER_RECORD
-    const bool tiny = (flags & FZB_F_TINY_LIST) != 0;
-    const bool share = (flags & ~(FZB_F_TINY_LIST | FZB_F_PER_RECORD)) == 0 && h->buf_len > 0;
+// The q-sample passes over the patterns `admit(i)` takes, in order, each as many as a pass's pattern slots and gram
+// table hold; ks: the limits the patterns are searched with, glim: as for batch_pass.  A pass of one pattern is not
+// worth it.
+template <class F>
+static int qsample_passes(BatchCall &c, const uint32_t *ks, const uint32_t *glim, F admit) {
     std::vector<uint32_t> shared;
-    if (share) {
-        for (uint32_t i = 0; i < count; i++) {
-            const uint32_t m = offsets[i + 1] - offsets[i], k = max_l_dist[i];
-            if (m == 0 || m > (uint32_t)kBatchMaxM || k == 0 || k >= m) continue;
-            const uint32_t L = m / (k + 1);
-            if (L < 3 || !sampled_filter_applies(m, k, 0)) continue;
-            if (check_halo(h, (uint64_t)m + k) != FZB_OK) continue;
-            if (!sampled_is_selective(h, m, k, (int)L, (int)(m / L))) continue;
-            shared.push_back(i);
-        }
-    }
+    for (uint32_t i = 0; i < c.count; i++)
+        if (admit(i)) shared.push_back(i);
     size_t done = 0;
-    while (done < shared.size()) {  // passes of bounded size (gram table / posting capacity)
+    while (done < shared.size()) {
         std::vector<uint32_t> ids;
         uint64_t ngr = 0;
         while (done < shared.size() && ids.size() < kMaxBatchPats) {
-            const uint32_t m = offsets[shared[done] + 1] - offsets[shared[done]];
+            const uint32_t m = c.len(shared[done]);
             if (ngr + (m - 3) > kMaxBatchGrams) break;
             ngr += m - 3;
             ids.push_back(shared[done++]);
         }
-        if (ids.size() < 2) {  // not worth a shared pass
-            done -= ids.size();
-            break;
-        }
-        const int rc = settle(batch_pass(h, patterns, offsets, max_l_dist, ids, out, &sum, false, tiny), ids);
-        if (rc) return rc;
+        if (ids.size() < 2) break;
+        TRY(c.settle(batch_pass(c, ks, ids, false, glim), ids));
     }
+    return FZB_OK;
+}
+
+// The n-gram-prefix pass over the unsettled n-gram-route patterns `admit(i)` takes (the class's window-slot rule
+// among its conditions), in order, while the expected prefix hits per haystack position stay within 0.02 and the
+// prefix table has room; ks and glim as for qsample_passes.
+template <class F>
+static int dense_pass(BatchCall &c, const uint32_t *ks, const uint32_t *glim, F admit) {
+    std::vector<uint32_t> ids;
+    if (c.share && sample_collision_prob(c.h) == FZB_OK) {
+        double expect = 0.0;
+        uint32_t grams = 0;
+        const double c3 = c.h->coll_prob * c.h->coll_prob * c.h->coll_prob;
+        for (uint32_t i = 0; i < c.count && ids.size() < kMaxBatchPats; i++) {
+            if (c.settled(i) || !admit(i)) continue;
+            const uint32_t n = c.len(i) / (c.len(i) / (ks[i] + 1));  // n-grams
+            if (expect + n * c3 > 0.02) continue;  // (low-entropy text: prefixes hit everywhere -> one by one)
+            if (grams + n > kMaxBatchGrams) continue;  // prefix table capacity
+            expect += n * c3;
+            grams += n;
+            ids.push_back(i);
+        }
+    }
+    return ids.size() >= 2 ? c.settle(batch_pass(c, ks, ids, true, glim), ids) : FZB_OK;
+}
+
+// A candidate of a pass bounded by an expected cost and by postings (greedy_passes).
+struct PassItem {
+    uint32_t i;
+    double cost;
+    uint32_t postings;
+};
+
+// The items in order, each joining the open pass unless that would cross kMaxBatchPats patterns, `max_cost` or
+// kMaxBatchGrams postings (so at most that many distinct keys), which first closes the pass: `run(ids, cost)` runs a
+// closed pass of at least two patterns (a pass of one is not worth it).
+template <class F>
+static int greedy_passes(const std::vector<PassItem> &items, double max_cost, F run) {
+    std::vector<uint32_t> ids;
+    double cost = 0.0;
+    uint64_t npost = 0;
+    auto close = [&]() -> int {
+        const int rc = ids.size() >= 2 ? run(ids, cost) : FZB_OK;
+        ids.clear();
+        cost = 0.0;
+        npost = 0;
+        return rc;
+    };
+    for (const PassItem &it : items) {
+        if (ids.size() == kMaxBatchPats || cost + it.cost > max_cost || npost + it.postings > kMaxBatchGrams)
+            TRY(close());
+        ids.push_back(it.i);
+        cost += it.cost;
+        npost += it.postings;
+    }
+    return close();
+}
+
+static int levenshtein_batch(BatchCall &c, const uint32_t *max_l_dist, fzb_stats *total) {
+    fzb_haystack *h = c.h;
+    // patterns the shared scan can take: n-gram route, q-sample lemma holds, 4-grams selective on this haystack,
+    // short enough for the 64-bit match table
+    TRY(qsample_passes(c, max_l_dist, nullptr, [&](uint32_t i) {
+        const uint32_t m = c.len(i), k = max_l_dist[i];
+        if (!c.share || m == 0 || m > (uint32_t)kBatchMaxM || k == 0 || k >= m) return false;
+        const uint32_t L = m / (k + 1);
+        return L >= 3 && sampled_filter_applies(m, k, 0) && check_halo(h, (uint64_t)m + k) == FZB_OK &&
+               sampled_is_selective(h, m, k, (int)L, (int)(m / L));
+    }));
     // the n-gram-route patterns the lemma does not cover share a scan of their own (n-gram prefixes at every position)
-    std::vector<uint32_t> dense_ids;
-    if (share && sample_collision_prob(h) == FZB_OK) {
-        double expect = 0.0;  // expected prefix hits per haystack position
-        uint32_t dense_grams = 0;
-        const double c3 = h->coll_prob * h->coll_prob * h->coll_prob;
-        for (uint32_t i = 0; i < count && dense_ids.size() < kMaxBatchPats; i++) {
-            if (out[i]) continue;
-            const uint32_t m = offsets[i + 1] - offsets[i], k = max_l_dist[i];
-            if (m == 0 || m > (uint32_t)kBatchMaxM || k == 0 || k >= m) continue;
-            const uint32_t L = m / (k + 1);
-            if (L < 3 || m - L > 32 || m + 2 * k + 12 > (uint32_t)kMhSlotBytes) continue;
-            if (check_halo(h, (uint64_t)m + k) != FZB_OK) continue;
-            if (expect + (m / L) * c3 > 0.02) continue;  // (low-entropy text: prefixes hit everywhere -> one by one)
-            if (dense_grams + m / L > kMaxBatchGrams) continue;  // prefix table capacity
-            expect += (m / L) * c3;
-            dense_grams += m / L;
-            dense_ids.push_back(i);
-        }
-    }
-    if (dense_ids.size() >= 2) {
-        const int rc = settle(batch_pass(h, patterns, offsets, max_l_dist, dense_ids, out, &sum, true, tiny), dense_ids);
-        if (rc) return rc;
-    }
+    TRY(dense_pass(c, max_l_dist, nullptr, [&](uint32_t i) {
+        const uint32_t m = c.len(i), k = max_l_dist[i];
+        if (m == 0 || m > (uint32_t)kBatchMaxM || k == 0 || k >= m) return false;
+        const uint32_t L = m / (k + 1);
+        return L >= 3 && m - L <= 32 && m + 2 * k + 12 <= (uint32_t)kMhSlotBytes &&
+               check_halo(h, (uint64_t)m + k) == FZB_OK;
+    }));
     // LP-route patterns (m // (k+1) < 3) share scans of 64 patterns each (bit-sliced window counters)
     std::vector<uint32_t> lp_ids;
-    if (share) {
-        for (uint32_t i = 0; i < count; i++) {
-            if (out[i]) continue;
-            const uint32_t m = offsets[i + 1] - offsets[i], k = max_l_dist[i];
+    if (c.share) {
+        for (uint32_t i = 0; i < c.count; i++) {
+            if (c.settled(i)) continue;
+            const uint32_t m = c.len(i), k = max_l_dist[i];
             if (m == 0 || k == 0 || k >= m || m / (k + 1) >= 3) continue;
             if (m > 31 || k > 8 || m + k > 31) continue;  // automaton masks / 6-bit window counters
             if (check_halo(h, (uint64_t)m + k) != FZB_OK) continue;
@@ -2771,28 +2837,16 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
     for (size_t first = 0; first + 2 <= lp_ids.size(); first += 64) {
         std::vector<uint32_t> ids(lp_ids.begin() + first, lp_ids.begin() + std::min(lp_ids.size(), first + 64));
         if (ids.size() < 2) break;
-        const int rc = settle(batch_pass_lp(h, patterns, offsets, max_l_dist, ids, out, &sum, tiny), ids);
-        if (rc) return rc;
+        TRY(c.settle(batch_pass_lp(c, max_l_dist, ids), ids));
     }
     // on low-entropy haystacks (at the 0.15 boundary of k_filter_dense2) the n-gram-route patterns left over that cost
     // less in a pass than alone share 2-bit n-gram scans (k_filter_mdense2), in passes bounded by hits and capacity
-    if (share && h->coll_prob >= 0.15) {
-        std::vector<uint32_t> ids;
+    if (c.share && h->coll_prob >= 0.15) {
         const double positions = (double)(h->own_hi - h->own_lo);
-        double hits = 0.0;
-        uint64_t npost = 0;
-        auto run_pass = [&]() -> int {
-            const int rc = ids.size() >= 2 ? settle(batch_pass_dna(h, patterns, offsets, max_l_dist, ids, out, &sum, hits,
-                                                                   tiny), ids)
-                                           : FZB_OK;  // (a pass of one pattern is not worth it)
-            ids.clear();
-            hits = 0.0;
-            npost = 0;
-            return rc;
-        };
-        for (uint32_t i = 0; i < count; i++) {
-            if (out[i]) continue;
-            const uint32_t m = offsets[i + 1] - offsets[i], k = max_l_dist[i];
+        std::vector<PassItem> items;
+        for (uint32_t i = 0; i < c.count; i++) {
+            if (c.settled(i)) continue;
+            const uint32_t m = c.len(i), k = max_l_dist[i];
             if (m == 0 || m > (uint32_t)kBatchMaxM || k == 0 || k >= m) continue;
             const uint32_t L = m / (k + 1);
             if (L < kDnaLevMinL || m - L > 32 || m + 2 * k + 12 > (uint32_t)kMhSlotBytes) continue;
@@ -2802,30 +2856,25 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
             bool rides = false;
             const double phits = dna_lev_hits(h, m, k, positions, &rides);
             if (!rides || phits > kDnaLevPassHits) continue;
-            const uint32_t np = dna_lev_postings(m, k);
-            if (ids.size() == kMaxBatchPats || hits + phits > kDnaLevPassHits || npost + np > kMaxBatchGrams) {
-                const int rc = run_pass();
-                if (rc) return rc;
-            }
-            ids.push_back(i);
-            hits += phits;
-            npost += np;
+            items.push_back({i, phits, dna_lev_postings(m, k)});
         }
-        const int rc = run_pass();
-        if (rc) return rc;
+        TRY(greedy_passes(items, kDnaLevPassHits, [&](const std::vector<uint32_t> &ids, double hits) {
+            return c.settle(batch_pass_dna(c, max_l_dist, ids, hits), ids);
+        }));
     }
-    for (uint32_t i = 0; i < count; i++) {
-        if (out[i]) continue;
-        // (the single search honours a record set by itself)
-        int rc = settle(fzb_search_levenshtein(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_l_dist[i],
-                                               single_flags(h, flags), &out[i]), {});
-        if (rc == FZB_OK) rc = settle(best_single(h, out[i], i), {});
-        if (rc) return rc;
-        add_stats(&sum, out[i]->stats);
-    }
-    sum.route = 7;  // batch
-    if (total) *total = sum;
-    return FZB_OK;
+    return c.finish(total, [&](uint32_t i, uint32_t f, fzb_result **res) {
+        return fzb_search_levenshtein(h, c.patterns + c.offsets[i], c.len(i), max_l_dist[i], f, res);
+    });
+}
+
+extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
+                                            const uint32_t *max_l_dist, uint32_t count, uint32_t flags,
+                                            fzb_result **out, fzb_stats *total) {
+    HandleLock handle_lock(h);
+    if (!h || !out || (count && (!patterns || !offsets || !max_l_dist))) return fail(FZB_E_INVALID, "NULL argument");
+    BatchCall c(h, patterns, offsets, count, flags, out, nullptr);
+    TRY(c.begin());
+    return levenshtein_batch(c, max_l_dist, total);
 }
 
 extern "C" int fzb_search_exact(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
@@ -3026,7 +3075,6 @@ extern "C" int fzb_search_hamming(fzb_haystack *h, const uint8_t *pattern, uint3
 // 4 GiB; the three measured passes averaged 28 ms).
 constexpr double kHamBatchPatExpect = 0.01;
 constexpr double kHamBatchExpect = 0.25;
-constexpr uint32_t kMaxHamBatchPostings = kMaxBatchGrams;  // postings of one pass (so <= that many distinct keys)
 
 // Key width of pattern (m, k) in a pass, in symbols: 2-bit keys are always 8 symbols wide (a piece of 5..7 symbols
 // is entered under every completion); text keys are the first min(L, 4) bytes of a piece, one width per pass.  0 when
@@ -3054,24 +3102,21 @@ static double ham_batch_cost(const fzb_haystack *h, uint32_t m, uint32_t k, uint
 
 // One k_ham_batch_scan pass for the patterns ids[]; same return convention as batch_pass.  two_bit: the 2-bit keys of
 // low-entropy haystacks, else text keys of key_bytes (4 or 3) bytes.
-static int batch_pass_ham(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, const uint32_t *ks,
-                          const std::vector<uint32_t> &ids, fzb_result **out, fzb_stats *sum, bool two_bit,
-                          uint32_t key_bytes, bool tiny) {
+static int batch_pass_ham(BatchCall &c, const uint32_t *ks, const std::vector<uint32_t> &ids, bool two_bit,
+                          uint32_t key_bytes) {
+    fzb_haystack *h = c.h;
     const uint32_t cnt = (uint32_t)ids.size();
     std::vector<BatchPat> pats(cnt);
     std::vector<uint32_t> pinfo(cnt);
     HamBatchParams hp{};
     hp.key_mask = key_bytes == 4 ? 0xFFFFFFFFu : 0x00FFFFFFu;
-    if (two_bit) two_bit_code(patterns, offsets, ids, hp.code);
+    if (two_bit) two_bit_code(c.patterns, c.offsets, ids, hp.code);
     std::unordered_map<uint32_t, std::vector<uint32_t>> keys;  // key -> postings pattern << 8 | piece
     keys.reserve(cnt * 8);
     for (uint32_t i = 0; i < cnt; i++) {
-        const uint32_t id = ids[i], m = offsets[id + 1] - offsets[id], k = ks[id], L = m / (k + 1);
+        const uint32_t id = ids[i], m = c.len(id), k = ks[id], L = m / (k + 1);
         BatchPat &bp = pats[i];
-        memset(&bp, 0, sizeof bp);
-        memcpy(bp.P, patterns + offsets[id], m);
-        bp.m = (int)m;
-        bp.k = (int)k;
+        fill_pat(bp, c, id, k);
         bp.L = (int)L;
         bp.n_ngrams = (int)k + 1;
         pinfo[i] = m | (k << 8) | (L << 16);
@@ -3115,7 +3160,7 @@ static int batch_pass_ham(fzb_haystack *h, const uint8_t *patterns, const uint32
     std::vector<RawRec> raw;
     uint32_t cnts[CNT_COUNT];
     fzb_stats pass{};
-    rc = run_batch_pass(h, [&]() -> int {
+    rc = run_batch_pass(c, [&]() -> int {
         hp.out = h->d_out.get();  // (the output buffer may have grown since the last attempt)
         hp.cap = h->d_out.size();
         if (ntiles > 0) {
@@ -3132,12 +3177,42 @@ static int batch_pass_ham(fzb_haystack *h, const uint8_t *patterns, const uint32
         return FZB_OK;
     }, raw, cnts, pass);
     if (rc) return rc;
-    if (tiny && cnts[CNT_OUT] > kTinyBatchCap) return 1;  // FZB_F_TINY_LIST: the pass's record list holds kTinyBatchCap
+    if (c.tiny && cnts[CNT_OUT] > kTinyBatchCap) return 1;  // FZB_F_TINY_LIST: the pass's record list holds kTinyBatchCap
     pass.route = 8;
     pass.filter_ms = pass.gpu_ms;
     pass.n_candidates = cnts[CNT_CAND];
     pass.n_launches = 1;
-    return finish_pass(h, raw, cnts[CNT_OUT], ids, pass, 1, true, out, sum);
+    return c.finish_pass(raw, cnts[CNT_OUT], ids, pass, 1, true);
+}
+
+static int hamming_batch(BatchCall &c, const uint32_t *max_subs, fzb_stats *total) {
+    fzb_haystack *h = c.h;
+    // a pattern the single search refuses fails the whole call, with the single search's error, before any work
+    for (uint32_t i = 0; i < c.count; i++) {
+        int rc = check_pattern(h, c.patterns + c.offsets[i], c.len(i), c.flags);
+        if (rc == FZB_OK) rc = check_halo(h, c.len(i));
+        if (rc) return rc;
+    }
+    if (c.share && c.count >= 2 && sample_collision_prob(h) == FZB_OK) {
+        const bool two_bit = h->coll_prob >= 0.15;  // the boundary of k_filter_dense2
+        // one group of passes per key width: 8 symbols (2-bit); 4 bytes, then 3 bytes (text)
+        for (uint32_t key = two_bit ? (uint32_t)kHbKeySyms : 4u; key >= (two_bit ? (uint32_t)kHbKeySyms : 3u); key--) {
+            std::vector<PassItem> items;
+            for (uint32_t i = 0; i < c.count; i++) {
+                const uint32_t m = c.len(i), k = max_subs[i];
+                if (ham_batch_key(m, k, two_bit) != key) continue;
+                const double cost = ham_batch_cost(h, m, k, key, two_bit);
+                if (cost > kHamBatchPatExpect) continue;
+                items.push_back({i, cost, ham_batch_postings(m, k, two_bit)});
+            }
+            TRY(greedy_passes(items, kHamBatchExpect, [&](const std::vector<uint32_t> &ids, double) {
+                return c.settle(batch_pass_ham(c, max_subs, ids, two_bit, key), ids);
+            }));
+        }
+    }
+    return c.finish(total, [&](uint32_t i, uint32_t f, fzb_result **res) {
+        return fzb_search_hamming(h, c.patterns + c.offsets[i], c.len(i), max_subs[i], f, res);
+    });
 }
 
 extern "C" int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
@@ -3145,69 +3220,9 @@ extern "C" int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns
                                         fzb_stats *total) {
     HandleLock handle_lock(h);
     if (!h || !out || (count && (!patterns || !offsets || !max_subs))) return fail(FZB_E_INVALID, "NULL argument");
-    for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
-    TRY(check_batch_records(h, flags));
-    for (uint32_t i = 0; i < count; i++)
-        if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
-    // a pattern the single search refuses fails the whole call, with the single search's error, before any work
-    for (uint32_t i = 0; i < count; i++) {
-        const uint32_t m = offsets[i + 1] - offsets[i];
-        int rc = check_pattern(h, patterns + offsets[i], m, flags);
-        if (rc == FZB_OK) rc = check_halo(h, m);
-        if (rc) return rc;
-    }
-    fzb_stats sum{};
-    auto settle = [&](int rc, const std::vector<uint32_t> &ids) { return settle_pass(rc, ids, out, count); };
-    // the shared scan takes no flags other than FZB_F_TINY_LIST and FZB_F_PER_RECORD (forced routes, multi-GPU
-    // reduction: one by one)
-    const bool tiny = (flags & FZB_F_TINY_LIST) != 0;
-    if ((flags & ~(FZB_F_TINY_LIST | FZB_F_PER_RECORD)) == 0 && h->buf_len > 0 && count >= 2 &&
-        sample_collision_prob(h) == FZB_OK) {
-        const bool two_bit = h->coll_prob >= 0.15;  // the boundary of k_filter_dense2
-        std::vector<uint32_t> ids;
-        uint32_t key = 0;
-        double expect = 0.0;
-        uint64_t npost = 0;
-        auto run_pass = [&]() -> int {
-            const int rc = ids.size() >= 2 ? settle(batch_pass_ham(h, patterns, offsets, max_subs, ids, out, &sum, two_bit,
-                                                                   key, tiny), ids)
-                                           : FZB_OK;  // (a pass of one pattern is not worth it)
-            ids.clear();
-            expect = 0.0;
-            npost = 0;
-            return rc;
-        };
-        // one group of passes per key width: 8 symbols (2-bit); 4 bytes, then 3 bytes (text)
-        for (key = two_bit ? (uint32_t)kHbKeySyms : 4u; key >= (two_bit ? (uint32_t)kHbKeySyms : 3u); key--) {
-            for (uint32_t i = 0; i < count; i++) {
-                const uint32_t m = offsets[i + 1] - offsets[i], k = max_subs[i];
-                if (ham_batch_key(m, k, two_bit) != key) continue;
-                const double cost = ham_batch_cost(h, m, k, key, two_bit);
-                if (cost > kHamBatchPatExpect) continue;
-                const uint32_t np = ham_batch_postings(m, k, two_bit);
-                if (ids.size() == kMaxBatchPats || expect + cost > kHamBatchExpect || npost + np > kMaxHamBatchPostings) {
-                    const int rc = run_pass();
-                    if (rc) return rc;
-                }
-                ids.push_back(i);
-                expect += cost;
-                npost += np;
-            }
-            const int rc = run_pass();
-            if (rc) return rc;
-        }
-    }
-    for (uint32_t i = 0; i < count; i++) {
-        if (out[i]) continue;
-        int rc = settle(fzb_search_hamming(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_subs[i],
-                                           single_flags(h, flags), &out[i]), {});
-        if (rc == FZB_OK) rc = settle(best_single(h, out[i], i), {});
-        if (rc) return rc;
-        add_stats(&sum, out[i]->stats);
-    }
-    sum.route = 7;  // batch
-    if (total) *total = sum;
-    return FZB_OK;
+    BatchCall c(h, patterns, offsets, count, flags, out, nullptr);
+    TRY(c.begin());
+    return hamming_batch(c, max_subs, total);
 }
 
 extern "C" int fzb_search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t max_subs,
@@ -3225,31 +3240,23 @@ extern "C" int fzb_search_generic(fzb_haystack *h, const uint8_t *pattern, uint3
     });
 }
 
-extern "C" int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
-                                        const uint32_t *max_subs, const uint32_t *max_ins, const uint32_t *max_dels,
-                                        const uint32_t *max_l_dist, uint32_t count, uint32_t flags, fzb_result **out,
-                                        fzb_stats *total) {
-    HandleLock handle_lock(h);
-    if (!h || !out || (count && (!patterns || !offsets || !max_subs || !max_ins || !max_dels || !max_l_dist)))
-        return fail(FZB_E_INVALID, "NULL argument");
-    for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
-    TRY(check_batch_records(h, flags));
-    for (uint32_t i = 0; i < count; i++)
-        if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
+static int generic_batch(BatchCall &c, const uint32_t *max_subs, const uint32_t *max_ins, const uint32_t *max_dels,
+                         const uint32_t *max_l_dist, fzb_stats *total) {
+    fzb_haystack *h = c.h;
     // Per pattern, as fzb_search_generic would search it: the route, the total limit it works with (the LP route
     // lowers it, search_generic) and the per-operation limits clamped to that total.  A pattern the single search
     // refuses (check_pattern, max_l_dist > 63, the halo, an n-gram length of 0) fails the whole call, with the single
     // search's error, before any work.
-    std::vector<uint32_t> kl(count, 0), glim(count, 0);
-    std::vector<uint8_t> ngram_route(count, 0);
-    for (uint32_t i = 0; i < count; i++) {
-        const uint32_t m = offsets[i + 1] - offsets[i], l = max_l_dist[i];
-        int rc = check_pattern(h, patterns + offsets[i], m, flags);
+    std::vector<uint32_t> kl(c.count, 0), glim(c.count, 0);
+    std::vector<uint8_t> ngram_route(c.count, 0);
+    for (uint32_t i = 0; i < c.count; i++) {
+        const uint32_t m = c.len(i), l = max_l_dist[i];
+        int rc = check_pattern(h, c.patterns + c.offsets[i], m, c.flags);
         if (rc) return rc;
         bool ngrams = m / ((uint64_t)l + 1) >= 3;
-        if (flags & FZB_F_FORCE_NGRAMS) ngrams = true;
-        if (flags & FZB_F_FORCE_LP) ngrams = false;
-        if (l == 0 && !(flags & (FZB_F_FORCE_LP | FZB_F_FORCE_NGRAMS))) {
+        if (c.flags & FZB_F_FORCE_NGRAMS) ngrams = true;
+        if (c.flags & FZB_F_FORCE_LP) ngrams = false;
+        if (l == 0 && !(c.flags & (FZB_F_FORCE_LP | FZB_F_FORCE_NGRAMS))) {
             rc = check_halo(h, m);  // (the exact route)
         } else {
             const uint32_t lk = ngrams ? l : lp_generic_limit(m, max_ins[i], l);
@@ -3263,69 +3270,27 @@ extern "C" int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns
         if (rc) return rc;
         ngram_route[i] = ngrams;
     }
-    fzb_stats sum{};
-    auto settle = [&](int rc, const std::vector<uint32_t> &ids) { return settle_pass(rc, ids, out, count); };
-    // the shared scans take no flags other than FZB_F_TINY_LIST and FZB_F_PER_RECORD (forced routes, raw-only,
-    // multi-GPU reduction: one by one), no exact-route pattern (max_l_dist == 0) and no pattern longer than a BatchPat
-    // holds
-    const bool tiny = (flags & FZB_F_TINY_LIST) != 0;
-    const bool share = (flags & ~(FZB_F_TINY_LIST | FZB_F_PER_RECORD)) == 0 && h->buf_len > 0;
+    // the shared scans take no exact-route pattern (max_l_dist == 0) and no pattern longer than a BatchPat holds
     auto shareable = [&](uint32_t i) {
-        const uint32_t m = offsets[i + 1] - offsets[i];
-        return share && !out[i] && max_l_dist[i] > 0 && m <= (uint32_t)kBatchMaxM;
+        return c.share && !c.settled(i) && max_l_dist[i] > 0 && c.len(i) <= (uint32_t)kBatchMaxM;
     };
     // n-gram route, q-sample lemma holds and its 4-grams are selective on this haystack: q-sample passes, bounded as
-    // in the Levenshtein batch (gram table / posting capacity)
-    std::vector<uint32_t> shared;
-    for (uint32_t i = 0; i < count; i++) {
-        if (!shareable(i) || !ngram_route[i]) continue;
-        const uint32_t m = offsets[i + 1] - offsets[i], k = kl[i], L = m / (k + 1);
-        if (!sampled_filter_applies(m, k, 0) || !sampled_is_selective(h, m, k, (int)L, (int)(m / L))) continue;
-        shared.push_back(i);
-    }
-    size_t done = 0;
-    while (done < shared.size()) {
-        std::vector<uint32_t> ids;
-        uint64_t ngr = 0;
-        while (done < shared.size() && ids.size() < kMaxBatchPats) {
-            const uint32_t m = offsets[shared[done] + 1] - offsets[shared[done]];
-            if (ngr + (m - 3) > kMaxBatchGrams) break;
-            ngr += m - 3;
-            ids.push_back(shared[done++]);
-        }
-        if (ids.size() < 2) break;  // (a pass of one pattern is not worth it)
-        const int rc = settle(batch_pass(h, patterns, offsets, kl.data(), ids, out, &sum, false, tiny, glim.data()), ids);
-        if (rc) return rc;
-    }
-    // the other n-gram-route patterns: one n-gram-prefix pass, under the Levenshtein batch's bound on the expected
-    // prefix hits per position and the prefix table's capacity; a hit's window must fit a warp's slot in
-    // k_verify_mhits_generic
-    std::vector<uint32_t> dense_ids;
-    if (share && sample_collision_prob(h) == FZB_OK) {
-        double expect = 0.0;
-        uint32_t dense_grams = 0;
-        const double c3 = h->coll_prob * h->coll_prob * h->coll_prob;
-        for (uint32_t i = 0; i < count && dense_ids.size() < kMaxBatchPats; i++) {
-            if (!shareable(i) || !ngram_route[i]) continue;
-            const uint32_t m = offsets[i + 1] - offsets[i], k = kl[i], L = m / (k + 1);
-            if (m + 2 * k + 8 > (uint32_t)kMhgSlotBytes) continue;
-            if (expect + (m / L) * c3 > 0.02) continue;  // (low-entropy text: prefixes hit everywhere -> one by one)
-            if (dense_grams + m / L > kMaxBatchGrams) continue;
-            expect += (m / L) * c3;
-            dense_grams += m / L;
-            dense_ids.push_back(i);
-        }
-    }
-    if (dense_ids.size() >= 2) {
-        const int rc = settle(batch_pass(h, patterns, offsets, kl.data(), dense_ids, out, &sum, true, tiny, glim.data()),
-                              dense_ids);
-        if (rc) return rc;
-    }
+    // in the Levenshtein batch
+    TRY(qsample_passes(c, kl.data(), glim.data(), [&](uint32_t i) {
+        if (!shareable(i) || !ngram_route[i]) return false;
+        const uint32_t m = c.len(i), k = kl[i], L = m / (k + 1);
+        return sampled_filter_applies(m, k, 0) && sampled_is_selective(h, m, k, (int)L, (int)(m / L));
+    }));
+    // the other n-gram-route patterns: one n-gram-prefix pass, under the Levenshtein batch's bounds; a hit's window
+    // must fit a warp's slot in k_verify_mhits_generic
+    TRY(dense_pass(c, kl.data(), glim.data(), [&](uint32_t i) {
+        return shareable(i) && ngram_route[i] && c.len(i) + 2 * kl[i] + 8 <= (uint32_t)kMhgSlotBytes;
+    }));
     // LP route (after the lowering of search_generic): passes of at most 64 patterns (6-bit window counters, 32-bit masks)
     std::vector<uint32_t> lp_ids;
-    for (uint32_t i = 0; i < count; i++) {
+    for (uint32_t i = 0; i < c.count; i++) {
         if (!shareable(i) || ngram_route[i]) continue;
-        const uint32_t m = offsets[i + 1] - offsets[i], k = kl[i];
+        const uint32_t m = c.len(i), k = kl[i];
         if (m > 31 || m + k > 31 || k >= m) continue;
         lp_ids.push_back(i);
     }
@@ -3333,20 +3298,24 @@ extern "C" int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns
     const size_t nlp = (lp_ids.size() + 63) / 64;
     for (size_t q = 0; q < nlp && lp_ids.size() >= 2; q++) {
         std::vector<uint32_t> ids(lp_ids.begin() + lp_ids.size() * q / nlp, lp_ids.begin() + lp_ids.size() * (q + 1) / nlp);
-        const int rc = settle(batch_pass_lp(h, patterns, offsets, kl.data(), ids, out, &sum, tiny, glim.data()), ids);
-        if (rc) return rc;
+        TRY(c.settle(batch_pass_lp(c, kl.data(), ids, glim.data()), ids));
     }
-    for (uint32_t i = 0; i < count; i++) {
-        if (out[i]) continue;
-        int rc = settle(fzb_search_generic(h, patterns + offsets[i], offsets[i + 1] - offsets[i], max_subs[i],
-                                           max_ins[i], max_dels[i], max_l_dist[i], single_flags(h, flags), &out[i]), {});
-        if (rc == FZB_OK) rc = settle(best_single(h, out[i], i), {});
-        if (rc) return rc;
-        add_stats(&sum, out[i]->stats);
-    }
-    sum.route = 7;  // batch
-    if (total) *total = sum;
-    return FZB_OK;
+    return c.finish(total, [&](uint32_t i, uint32_t f, fzb_result **res) {
+        return fzb_search_generic(h, c.patterns + c.offsets[i], c.len(i), max_subs[i], max_ins[i], max_dels[i],
+                                  max_l_dist[i], f, res);
+    });
+}
+
+extern "C" int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
+                                        const uint32_t *max_subs, const uint32_t *max_ins, const uint32_t *max_dels,
+                                        const uint32_t *max_l_dist, uint32_t count, uint32_t flags, fzb_result **out,
+                                        fzb_stats *total) {
+    HandleLock handle_lock(h);
+    if (!h || !out || (count && (!patterns || !offsets || !max_subs || !max_ins || !max_dels || !max_l_dist)))
+        return fail(FZB_E_INVALID, "NULL argument");
+    BatchCall c(h, patterns, offsets, count, flags, out, nullptr);
+    TRY(c.begin());
+    return generic_batch(c, max_subs, max_ins, max_dels, max_l_dist, total);
 }
 
 // choose_search_class (__init__.py:60-83) on normalised limits
@@ -3362,14 +3331,6 @@ static int search_by_class(fzb_haystack *h, const uint8_t *pattern, uint32_t m, 
 // ------------------------------------------------------------------------------------------------
 // fzb_best_per_record (DESIGN.md section 5.13): every record of a set assigned its best-matching pattern
 // ------------------------------------------------------------------------------------------------
-struct BestScope {  // h->best for the duration of a call, cleared on every way out
-    fzb_haystack *h;
-    BestScope(fzb_haystack *h_, BestState *s) : h(h_) { h->best = s; }
-    ~BestScope() { h->best = nullptr; }
-    BestScope(const BestScope &) = delete;
-    BestScope &operator=(const BestScope &) = delete;
-};
-
 extern "C" int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
                                    const uint32_t *max_subs, const uint32_t *max_ins, const uint32_t *max_dels,
                                    const uint32_t *max_l_dist, uint32_t count, uint32_t flags, int32_t *pattern,
@@ -3389,7 +3350,7 @@ extern "C" int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, con
     // a batch of its own over its subset of the patterns
     struct Subset {
         std::vector<uint8_t> blob;
-        std::vector<uint32_t> offsets{0}, ordinal, lim[4];  // lim: the limit arrays of the class's batch entry point
+        std::vector<uint32_t> offsets{0}, ordinal, lim[4];  // lim: the limit arrays of the class's batch
     } lev, ham, gen;
     for (uint32_t i = 0; i < count; i++) {
         if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
@@ -3427,7 +3388,6 @@ extern "C" int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, con
         h->bestb = std::move(grown);
     }
     BestState state{h->bestb->d_words.get(), h->bestb->d_words.get() + nrec, nullptr};
-    BestScope scope(h, &state);
     fzb_stats sum{};
     k_best_fill<<<(int)std::min<uint64_t>((2 * nrec + kBestThreads - 1) / kBestThreads, (uint64_t)h->sm_count * 8),
                   kBestThreads, 0, h->stream>>>(state.best, 2 * nrec);
@@ -3437,21 +3397,12 @@ extern "C" int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, con
         const uint32_t n = (uint32_t)sub->ordinal.size();
         if (n == 0) continue;
         state.ordinal = sub->ordinal.data();
-        std::vector<fzb_result *> out(n, nullptr);
-        fzb_stats part{};
-        const uint32_t f = flags | FZB_F_PER_RECORD;
-        if (sub->blob.empty()) sub->blob.push_back(0);
-        const int rc = sub == &lev   ? fzb_search_levenshtein_batch(h, sub->blob.data(), sub->offsets.data(),
-                                                                    sub->lim[0].data(), n, f, out.data(), &part)
-                       : sub == &ham ? fzb_search_hamming_batch(h, sub->blob.data(), sub->offsets.data(),
-                                                                sub->lim[0].data(), n, f, out.data(), &part)
-                                     : fzb_search_generic_batch(h, sub->blob.data(), sub->offsets.data(),
-                                                                sub->lim[0].data(), sub->lim[1].data(), sub->lim[2].data(),
-                                                                sub->lim[3].data(), n, f, out.data(), &part);
-        for (fzb_result *r : out)
-            if (r) fzb_result_destroy(r);
-        if (rc) return rc;
-        add_stats(&sum, part);
+        BatchCall c(h, sub->blob.data(), sub->offsets.data(), n, flags, nullptr, &state);
+        const uint32_t *lim[4] = {sub->lim[0].data(), sub->lim[1].data(), sub->lim[2].data(), sub->lim[3].data()};
+        TRY(sub == &lev   ? levenshtein_batch(c, lim[0], nullptr)
+            : sub == &ham ? hamming_batch(c, lim[0], nullptr)
+                          : generic_batch(c, lim[0], lim[1], lim[2], lim[3], nullptr));
+        add_stats(&sum, c.sum);
     }
     // one read-back of 16 bytes per record, whatever the number of matches
     std::vector<uint64_t> words(2 * nrec);

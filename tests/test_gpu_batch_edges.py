@@ -355,8 +355,11 @@ def test_batch_lp_chunk_seams(cuda_device):
     hs = F.Haystack.from_host(hay)
     res = run_twice(hs, pats, ks, F.F_TINY_LIST)
     assert scans(res) == {LP: [len(pats), 1]}
-    _, st = hs.search_levenshtein_batch(pats, ks, F.F_TINY_LIST)
-    assert st["n_launches"] == 4 * ((n + TINY_LP_CHUNK - 1) // TINY_LP_CHUNK)  # four launches per chunk
+    again, st = hs.search_levenshtein_batch(pats, ks, F.F_TINY_LIST)
+    chunks = (n + TINY_LP_CHUNK - 1) // TINY_LP_CHUNK
+    assert st["n_launches"] == 4 * chunks  # four launches per chunk
+    assert again[0].stats()["n_launches"] == 4 * chunks  # reported by the pass, on its first result
+    close_all(again)
     starts = {s for r in res for s, _, _ in r.triples(F.RAW)}
     for c in range(1, 7):
         assert c * TINY_LP_CHUNK - (1 if c % 2 else 0) in starts and c * TINY_LP_CHUNK - 100 in starts

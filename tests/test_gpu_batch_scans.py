@@ -620,7 +620,7 @@ def test_record_sets(cuda_device, small=False):
 def test_tiny_chunks(cuda_device, small=False):
     """FZB_F_TINY_LIST: the 2-bit and LP passes scan chunks of 3 000 positions (seams inside a vector, a 128-byte run
     and a tile) with small lists; on sparse contents that stay under those caps the count is the same with and
-    without the flag, and the 2-bit pass reports two launches per chunk."""
+    without the flag, and the 2-bit pass reports two launches per chunk, the LP pass four."""
     rng = np.random.default_rng(613)
     n = 7 * TINY_CHUNK + 123 if small else 25 * TINY_CHUNK + 123
     # 2-bit: n-grams of 10 symbols and more, at most 6 hits per chunk, straddling every seam
@@ -644,7 +644,7 @@ def test_tiny_chunks(cuda_device, small=False):
         put(hay, c * TINY_CHUNK - 4 + int(rng.integers(0, 3)), pats[c % 2])
     put(hay, n - 5, pats[1])
     hs = F.Haystack.from_host(hay)
-    a, _, _ = run_pass(hs, LPP, pats, ks, hay=hay, flags=F.F_TINY_LIST, geom=(hay,))
-    b, _, _ = run_pass(hs, LPP, pats, ks, hay=hay, geom=(hay,))
+    a, _, _ = run_pass(hs, LPP, pats, ks, hay=hay, flags=F.F_TINY_LIST, geom=(hay,), want_launches=4 * chunks)
+    b, _, _ = run_pass(hs, LPP, pats, ks, hay=hay, geom=(hay,), want_launches=4)
     assert a == b > 0
     hs.close()
