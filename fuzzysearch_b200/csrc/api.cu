@@ -1333,6 +1333,110 @@ static int check_halo(const fzb_haystack *h, uint64_t halo) {
     return FZB_OK;
 }
 
+static int check_pattern(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags) {
+    if (!h) return fail(FZB_E_INVALID, "haystack handle is NULL");
+    if (flags & FZB_F_GLOBAL) TRY(refuse_records(h, "FZB_F_GLOBAL"));
+    if ((flags & FZB_F_GLOBAL) && !h->comm && !h->local_world)
+        return fail(FZB_E_INVALID, "FZB_F_GLOBAL needs fzb_haystack_comm_init / fzb_comm_init_local on this handle");
+    if (!pattern || m == 0) return fail(FZB_E_INVALID, "Given subsequence is empty!");
+    if (m > FZB_MAX_PATTERN) return fail(FZB_E_UNSUPPORTED, "pattern longer than %d bytes", FZB_MAX_PATTERN);
+    return FZB_OK;
+}
+
+// How one pattern is searched: the route that runs, the total limit k it runs with (after every clamp and lowering)
+// and, on the generic routes, the per-operation limits clamped to k.  The plan_* functions are the one statement of
+// the route rules and of the refusals of the single searches; the single searches, the batches and
+// fzb_best_per_record all run from plans.  Routes: Exact is search_lev_ngrams at k = 0 with the sorted raw list for
+// final list, LevNgrams search_lev_ngrams (also the generic search's k = 0 route), LevLp search_lev_lp, Hamming
+// search_hamming, GenericNgrams and GenericLp the two routes of search_generic.
+enum class Route : uint8_t { Exact, LevNgrams, LevLp, Hamming, GenericNgrams, GenericLp };
+
+struct Plan {
+    Route route;
+    uint32_t m, k, subs, ins, dels;
+    uint32_t L() const { return m / (k + 1); }  // the n-gram length of the n-gram routes
+    bool generic() const { return route == Route::GenericNgrams || route == Route::GenericLp; }
+};
+
+// The n-gram routes take n-grams of at least 3 symbols (levenshtein.py:9-38, generic_search.py:25-54), or k == 0;
+// FZB_F_FORCE_LP, then FZB_F_FORCE_NGRAMS, override.
+static bool ngram_route(uint32_t m, uint32_t k, uint32_t flags) {
+    if (flags & FZB_F_FORCE_LP) return false;
+    return (flags & FZB_F_FORCE_NGRAMS) || k == 0 || m / ((uint64_t)k + 1) >= 3;
+}
+
+static int check_ngram_length(const Plan &pl) {
+    return pl.L() == 0 ? fail(FZB_E_NGRAM_ZERO, "the subsequence length must be greater than max_l_dist") : FZB_OK;
+}
+
+static int plan_exact(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags, Plan &pl) {
+    // check_pattern in the words of the exact search (search_exact.py), which has only this one complaint
+    const int rc = check_pattern(h, pattern, m, flags);
+    if (rc) return rc == FZB_E_INVALID && h ? fail(FZB_E_INVALID, "subsequence must not be empty") : rc;
+    pl = Plan{Route::Exact, m, 0, 0, 0, 0};
+    return check_halo(h, m);
+}
+
+static int plan_levenshtein(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t k, uint32_t flags,
+                            Plan &pl) {
+    TRY(check_pattern(h, pattern, m, flags));
+    // every k >= len(pattern) takes the same branch (levenshtein.py:62-65): (i, i, m) for all i
+    pl = Plan{Route::LevLp, m, std::min(k, m), 0, 0, 0};
+    if (ngram_route(m, pl.k, flags)) {
+        pl.route = Route::LevNgrams;
+        TRY(check_ngram_length(pl));
+    }
+    return check_halo(h, (uint64_t)m + pl.k);
+}
+
+static int plan_hamming(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t k, uint32_t flags,
+                        Plan &pl) {
+    TRY(check_pattern(h, pattern, m, flags));
+    pl = Plan{Route::Hamming, m, std::min(k, m), 0, 0, 0};
+    return check_halo(h, m);
+}
+
+static int plan_generic(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t max_subs,
+                        uint32_t max_ins, uint32_t max_dels, uint32_t max_l, uint32_t flags, Plan &pl) {
+    TRY(check_pattern(h, pattern, m, flags));
+    // find_near_matches_generic (generic_search.py:25-54)
+    if (max_l == 0 && !(flags & (FZB_F_FORCE_LP | FZB_F_FORCE_NGRAMS))) {
+        pl = Plan{Route::LevNgrams, m, 0, 0, 0, 0};
+        return check_halo(h, m);
+    }
+    pl = Plan{Route::GenericNgrams, m, max_l, 0, 0, 0};
+    if (!ngram_route(m, max_l, flags)) {
+        // LP route: every substitution and every deletion consumes a pattern character (so does the "insertion +
+        // deletion" pair the reference books when the substitutions are used up, generic_search.py:111-128), hence a
+        // live candidate at pattern index j has spent l <= j + n_ins < m + max_ins: a total limit above m + max_ins
+        // never binds -- not in `l_dist < max_l_dist` (:101-102), not in the deletion loop's bound (:141), not in the
+        // final loop (:172-177) -- and can be lowered to it without changing the raw stream.  (Not so on the n-gram
+        // route, where max_l_dist also sets the n-gram length and the windows.)  E.g. max_substitutions=100,
+        // max_insertions=1, max_deletions=1 on 20 symbols: 102 -> 21.
+        pl.route = Route::GenericLp;
+        pl.k = (uint32_t)std::min<uint64_t>(max_l, (uint64_t)m + std::min(max_ins, max_l));
+    }
+    // the packed candidate of sim_generic keeps 6 bits per counter
+    if (pl.k > 63) return fail(FZB_E_UNSUPPORTED, "max_l_dist > 63 is not supported by the generic search");
+    // no counter can exceed k (every operation that increments one costs >= 1), so clamping the per-operation limits
+    // to k changes nothing (LevenshteinSearchParams does the same, common.py:108-116)
+    pl.subs = std::min(max_subs, pl.k);
+    pl.ins = std::min(max_ins, pl.k);
+    pl.dels = std::min(max_dels, pl.k);
+    TRY(check_halo(h, (uint64_t)m + pl.k));
+    return pl.route == Route::GenericNgrams ? check_ngram_length(pl) : FZB_OK;
+}
+
+// choose_search_class (__init__.py:60-83) on normalised limits
+static int plan_by_class(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t max_subs,
+                         uint32_t max_ins, uint32_t max_dels, uint32_t max_l, uint32_t flags, Plan &pl) {
+    if (max_l == 0) return plan_exact(h, pattern, m, flags, pl);
+    if (max_ins == 0 && max_dels == 0) return plan_hamming(h, pattern, m, std::min(max_l, max_subs), flags, pl);
+    if (max_l <= std::min(max_subs, std::min(max_ins, max_dels)))
+        return plan_levenshtein(h, pattern, m, max_l, flags, pl);
+    return plan_generic(h, pattern, m, max_subs, max_ins, max_dels, max_l, flags, pl);
+}
+
 constexpr uint64_t kMaxRawRecs = 1ull << 27;  // raw records of one search (or one shared batch pass)
 
 // Grows d_out to hold `need` records.  The new buffer is allocated before the old one is released, so a failure leaves
@@ -1604,6 +1708,12 @@ static bool sampled_is_selective(fzb_haystack *h, uint32_t m, uint32_t k, int L,
     return sampled <= 0.02 || sampled <= dense;
 }
 
+// The filter of an n-gram-route search of plan `pl`: the sampled one, or (false) the dense one.
+static bool sampled_filter(fzb_haystack *h, const Plan &pl, uint32_t flags) {
+    return sampled_filter_applies(pl.m, pl.k, flags) &&
+           ((flags & FZB_F_FORCE_SAMPLED) || sampled_is_selective(h, pl.m, pl.k, (int)pl.L(), (int)(pl.m / pl.L())));
+}
+
 // Enqueue the one pass over the haystack that marks candidate granules; records ev[1] behind it.
 static int enqueue_filter(fzb_haystack *h, const ScanParams &p, bool sampled, fzb_result *res) {
     const int64_t nvec = (int64_t)(round_up(h->buf_len, 16) / 16);
@@ -1653,19 +1763,17 @@ static int enqueue_filter(fzb_haystack *h, const ScanParams &p, bool sampled, fz
 }
 
 // n-gram Levenshtein search (also serves exact search as k == 0, L == m)
-static int search_lev_ngrams(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t k, uint32_t flags,
+static int search_lev_ngrams(fzb_haystack *h, const uint8_t *pattern, const Plan &pl, uint32_t flags,
                              fzb_result *res, int post_mode) {
+    const uint32_t m = pl.m, k = pl.k;
     ScanParams p;
     fill_params(h, pattern, m, p);
     p.k = (int)k;
-    p.L = (int)(m / (k + 1));
-    if (p.L == 0) return fail(FZB_E_NGRAM_ZERO, "the subsequence length must be greater than max_l_dist");
+    p.L = (int)pl.L();
     p.n_ngrams = (int)m / p.L;  // range(0, m-L+1, L)
-    int rc = check_halo(h, (uint64_t)m + k);
-    if (rc) return rc;
+    int rc;
     CK(cudaSetDevice(h->device));
-    const bool sampled = sampled_filter_applies(m, k, flags) &&
-                         ((flags & FZB_F_FORCE_SAMPLED) || sampled_is_selective(h, m, k, p.L, p.n_ngrams));
+    const bool sampled = sampled_filter(h, pl, flags);
     p.q = sampled ? 4 : std::min(p.L, 8);
     res->stats.route = k == 0 ? 0 : (sampled ? 1 : 2);
     res->stats.bytes_scanned = h->buf_len;
@@ -1785,14 +1893,13 @@ static int run_lp(fzb_haystack *h, fzb_result *res, F enqueue, PostPlan post = P
     return fail(FZB_E_UNSUPPORTED, "candidate explosion: more than 16384 live candidates for one start");
 }
 
-static int search_lev_lp(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t k, uint32_t flags,
-                         fzb_result *res, int post_mode) {
-    if (k > 0xFFFF) return fail(FZB_E_UNSUPPORTED, "max_l_dist too large");
+static int search_lev_lp(fzb_haystack *h, const uint8_t *pattern, const Plan &pl, uint32_t flags, fzb_result *res,
+                         int post_mode) {
+    const uint32_t m = pl.m, k = pl.k;
     ScanParams p;
     fill_params(h, pattern, m, p);
     p.k = (int)k;
-    int rc = check_halo(h, (uint64_t)m + k);
-    if (rc) return rc;
+    int rc;
     CK(cudaSetDevice(h->device));
     res->stats.route = 3;
     res->stats.bytes_scanned = h->buf_len;
@@ -1839,41 +1946,19 @@ static int search_lev_lp(fzb_haystack *h, const uint8_t *pattern, uint32_t m, ui
     return FZB_OK;
 }
 
-// The total limit the LP route of the generic search works with (see search_generic).
-static uint32_t lp_generic_limit(uint32_t m, uint32_t max_ins, uint32_t max_l) {
-    return (uint32_t)std::min<uint64_t>(max_l, (uint64_t)m + std::min(max_ins, max_l));
-}
-
-static int search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t max_subs, uint32_t max_ins,
-                          uint32_t max_dels, uint32_t max_l, bool ngrams, uint32_t flags, fzb_result *res,
+static int search_generic(fzb_haystack *h, const uint8_t *pattern, const Plan &pl, uint32_t flags, fzb_result *res,
                           int post_mode) {
-    // LP route: every substitution and every deletion consumes a pattern character (so does the "insertion +
-    // deletion" pair the reference books when the substitutions are used up, generic_search.py:111-128), hence a
-    // live candidate at pattern index j has spent l <= j + n_ins < m + max_ins: a total limit above m + max_ins
-    // never binds -- not in `l_dist < max_l_dist` (:101-102), not in the deletion loop's bound (:141), not in the
-    // final loop (:172-177) -- and can be lowered to it without changing the raw stream.  (Not so on the n-gram
-    // route, where max_l_dist also sets the n-gram length and the windows.)  E.g. max_substitutions=100,
-    // max_insertions=1, max_deletions=1 on 20 symbols: 102 -> 21.
-    if (!ngrams) max_l = lp_generic_limit(m, max_ins, max_l);
-    // the packed candidate of sim_generic keeps 6 bits per counter
-    if (max_l > 63) return fail(FZB_E_UNSUPPORTED, "max_l_dist > 63 is not supported by the generic search");
-    // no counter can exceed max_l (every operation that increments one costs >= 1), so clamping the
-    // per-operation limits to max_l changes nothing (LevenshteinSearchParams does the same, common.py:108-116)
-    max_subs = std::min(max_subs, max_l);
-    max_ins = std::min(max_ins, max_l);
-    max_dels = std::min(max_dels, max_l);
     ScanParams p;
-    fill_params(h, pattern, m, p);
-    p.k = (int)max_l;
-    p.max_subs = (int)max_subs;
-    p.max_ins = (int)max_ins;
-    p.max_dels = (int)max_dels;
-    int rc = check_halo(h, (uint64_t)m + max_l);
-    if (rc) return rc;
+    fill_params(h, pattern, pl.m, p);
+    p.k = (int)pl.k;
+    p.max_subs = (int)pl.subs;
+    p.max_ins = (int)pl.ins;
+    p.max_dels = (int)pl.dels;
+    int rc;
     CK(cudaSetDevice(h->device));
     res->stats.bytes_scanned = h->buf_len;
     const RecSet rs = rec_set(h);
-    if (!ngrams) {
+    if (pl.route == Route::GenericLp) {
         res->stats.route = 6;
         rc = run_lp(h, res, [&](int grid, int cap) -> int {
             with_recs(h, [&](auto rec) {
@@ -1888,11 +1973,9 @@ static int search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, u
         res->raw_order = 1;
         return FZB_OK;
     }
-    p.L = (int)(m / (max_l + 1));
-    if (p.L == 0) return fail(FZB_E_NGRAM_ZERO, "the subsequence length must be greater than max_l_dist");
-    p.n_ngrams = (int)m / p.L;
-    const bool sampled = sampled_filter_applies(m, max_l, flags) &&
-                         ((flags & FZB_F_FORCE_SAMPLED) || sampled_is_selective(h, m, max_l, p.L, p.n_ngrams));
+    p.L = (int)pl.L();
+    p.n_ngrams = (int)pl.m / p.L;
+    const bool sampled = sampled_filter(h, pl, flags);
     p.q = sampled ? 4 : std::min(p.L, 8);
     res->stats.route = 5;
     rc = set_filter_attrs(kScanSmem);
@@ -1962,34 +2045,33 @@ static int make_result(fzb_result **out, fzb_result **res) {
     return FZB_OK;
 }
 
-static int check_pattern(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags) {
-    if (!h) return fail(FZB_E_INVALID, "haystack handle is NULL");
-    if (flags & FZB_F_GLOBAL) TRY(refuse_records(h, "FZB_F_GLOBAL"));
-    if ((flags & FZB_F_GLOBAL) && !h->comm && !h->local_world)
-        return fail(FZB_E_INVALID, "FZB_F_GLOBAL needs fzb_haystack_comm_init / fzb_comm_init_local on this handle");
-    if (!pattern || m == 0) return fail(FZB_E_INVALID, "Given subsequence is empty!");
-    if (m > FZB_MAX_PATTERN) return fail(FZB_E_UNSUPPORTED, "pattern longer than %d bytes", FZB_MAX_PATTERN);
-    return FZB_OK;
+static int search_hamming(fzb_haystack *h, const uint8_t *pattern, const Plan &pl, uint32_t flags, fzb_result *res);
+
+// The route of plan `pl`, then the reduction to the global list under FZB_F_GLOBAL.  The final list of the exact and
+// the Hamming search is their sorted raw list whatever the flags (ExactSearch.consolidate_matches is the base no-op,
+// common.py:198-205); the others honour FZB_F_NO_FINAL (LevenshteinSearch.consolidate_matches,
+// levenshtein.py:158-160, also applies when k == 0).
+static int run_route(fzb_haystack *h, const uint8_t *pattern, const Plan &pl, uint32_t flags, fzb_result *res) {
+    res->unconsolidated = pl.route == Route::Exact || pl.route == Route::Hamming;
+    const int post_mode = res->unconsolidated ? 2 : (flags & FZB_F_NO_FINAL) ? 0 : 1;
+    int rc = pl.route == Route::Hamming ? search_hamming(h, pattern, pl, flags, res)
+             : pl.route == Route::LevLp ? search_lev_lp(h, pattern, pl, flags, res, post_mode)
+             : pl.generic()             ? search_generic(h, pattern, pl, flags, res, post_mode)
+                                        : search_lev_ngrams(h, pattern, pl, flags, res, post_mode);
+    if (rc == FZB_OK && post_mode && (flags & FZB_F_GLOBAL)) rc = finish_global(h, res);
+    return rc;
 }
 
-// check_pattern in the words of the exact search (search_exact.py), which has only this one complaint
-static int check_exact_pattern(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags) {
-    const int rc = check_pattern(h, pattern, m, flags);
-    return rc == FZB_E_INVALID && h ? fail(FZB_E_INVALID, "subsequence must not be empty") : rc;
-}
-
-// The frame of the single-pattern entry points: handle lock, result, `check`, the route's `body(res)`, the
-// reduction to the global list if `global`, and the result destroyed on any error.
-template <class F>
-static int run_search(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags, bool global,
-                      fzb_result **out, F body, decltype(&check_pattern) check = check_pattern) {
+// The frame of the single searches: handle lock, result, `plan(pl)`, its route, and the result destroyed on any error.
+template <class P>
+static int run_search(fzb_haystack *h, const uint8_t *pattern, uint32_t flags, fzb_result **out, P plan) {
     HandleLock handle_lock(h);
     fzb_result *res;
     int rc = make_result(out, &res);
     if (rc) return rc;
-    rc = check(h, pattern, m, flags);
-    if (rc == FZB_OK) rc = body(res);
-    if (rc == FZB_OK && global) rc = finish_global(h, res);
+    Plan pl;
+    rc = plan(pl);
+    if (rc == FZB_OK) rc = run_route(h, pattern, pl, flags, res);
     if (rc) {
         fzb_result_destroy(res);
         return rc;
@@ -2000,17 +2082,7 @@ static int run_search(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint3
 
 extern "C" int fzb_search_levenshtein(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t k,
                                       uint32_t flags, fzb_result **out) {
-    // LevenshteinSearch.consolidate_matches (levenshtein.py:158-160) also applies when k == 0
-    const int post_mode = (flags & FZB_F_NO_FINAL) ? 0 : 1;
-    return run_search(h, pattern, m, flags, post_mode && (flags & FZB_F_GLOBAL), out, [&](fzb_result *res) {
-        // find_near_matches_levenshtein (levenshtein.py:9-38)
-        if (k >= m) k = m;  // every k >= len(pattern) takes the same branch (levenshtein.py:62-65): (i, i, m) for all i
-        bool ngrams = (k == 0) || (m / (k + 1) >= 3);
-        if (flags & FZB_F_FORCE_NGRAMS) ngrams = true;
-        if (flags & FZB_F_FORCE_LP) ngrams = false;
-        return ngrams ? search_lev_ngrams(h, pattern, m, k, flags, res, post_mode)
-                      : search_lev_lp(h, pattern, m, k, flags, res, post_mode);
-    });
+    return run_search(h, pattern, flags, out, [&](Plan &pl) { return plan_levenshtein(h, pattern, m, k, flags, pl); });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2118,15 +2190,16 @@ static int best_accumulate(fzb_haystack *h, const BestState &best, uint32_t n, c
     return FZB_OK;
 }
 
-// One batch call: a batch entry point's, or one class of fzb_best_per_record's.  It holds the patterns, what the flags
-// let the passes do, the running sum of the stats and the sink the passes and the one-by-one searches end in: the
-// per-pattern results out[count], or (best != nullptr) the words of fzb_best_per_record, into which every record is
-// reduced (DESIGN.md section 5.13).
+// One batch call: a batch entry point's, or one class of fzb_best_per_record's.  It holds the patterns and their
+// plans, what the flags let the passes do, the running sum of the stats and the sink the passes and the one-by-one
+// searches end in: the per-pattern results out[count], or (best != nullptr) the words of fzb_best_per_record, into
+// which every record is reduced (DESIGN.md section 5.13).
 struct BatchCall {
     fzb_haystack *h;
     const uint8_t *patterns;
     const uint32_t *offsets;
     uint32_t count, flags;
+    std::vector<Plan> plans;  // plans[i]: how pattern i is searched, in a pass or on its own
     fzb_result **out;        // list sink: out[i] is pattern i's result once a pass or its own search settled it
     const BestState *best;   // reduction sink
     std::vector<uint8_t> done;  // reduction sink: pattern i is settled
@@ -2143,12 +2216,16 @@ struct BatchCall {
     uint32_t len(uint32_t i) const { return offsets[i + 1] - offsets[i]; }
     bool settled(uint32_t i) const { return best ? done[i] != 0 : out[i] != nullptr; }
 
-    // The refusals of the batch entry points, behind every result cleared.
-    int begin() {
+    // The refusals of the batch entry points, behind every result cleared; then every pattern planned by
+    // `plan(i, pattern, m, pl)`, the class's plan function, whose first refusal fails the call before any work.
+    template <class P>
+    int begin(P plan) {
         for (uint32_t i = 0; i < count; i++) out[i] = nullptr;
         TRY(check_batch_records(h, flags));
         for (uint32_t i = 0; i < count; i++)
             if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
+        plans.resize(count);
+        for (uint32_t i = 0; i < count; i++) TRY(plan(i, patterns + offsets[i], len(i), plans[i]));
         return FZB_OK;
     }
 
@@ -2188,16 +2265,16 @@ struct BatchCall {
         return FZB_OK;
     }
 
-    // The patterns no pass settled, each searched on its own by `single(i, flags, &res)`, the class's single search
-    // (which honours a record set by itself); then the call's stats in *total.  Under the reduction sink the search
-    // returns the raw stream only, which is reduced while still in h->d_out and dropped, so that nothing reads it back.
-    template <class F>
-    int finish(fzb_stats *total, F single) {
+    // The patterns no pass settled, each searched on its own by its plan's route (which honours a record set by
+    // itself); then the call's stats in *total.  Under the reduction sink the search returns the raw stream only, which
+    // is reduced while still in h->d_out and dropped, so that nothing reads it back.
+    int finish(fzb_stats *total) {
         const uint32_t f = (flags & ~FZB_F_PER_RECORD) | (best ? FZB_F_NO_FINAL : 0u);
         for (uint32_t i = 0; i < count; i++) {
             if (settled(i)) continue;
             fzb_result *res = nullptr;
-            TRY(settle(single(i, f, &res), {}));
+            auto planned = [&](Plan &pl) { pl = plans[i]; return FZB_OK; };
+            TRY(settle(run_search(h, patterns + offsets[i], f, &res, planned), {}));
             if (!best) {
                 add_stats(&sum, res->stats);
                 out[i] = res;
@@ -2291,12 +2368,12 @@ static int run_chunks(fzb_haystack *h, uint64_t chunk, int list, int full, uint3
     return FZB_OK;
 }
 
-// The slot of pattern `id` in a pass, limit k; the pass sets its L and n_ngrams.
-static void fill_pat(BatchPat &bp, const BatchCall &c, uint32_t id, uint32_t k) {
+// The slot of pattern `id` in a pass, with its plan's limit; the pass sets its L and n_ngrams.
+static void fill_pat(BatchPat &bp, const BatchCall &c, uint32_t id) {
     memset(&bp, 0, sizeof bp);
     memcpy(bp.P, c.patterns + c.offsets[id], c.len(id));
     bp.m = (int)c.len(id);
-    bp.k = (int)k;
+    bp.k = (int)c.plans[id].k;
 }
 
 // Builds the posting table of a pass -- open addressing on the key (key * kGramMul), each slot the key and its first
@@ -2352,12 +2429,13 @@ static MultiParams pass_params(const fzb_haystack *h) {
 // candidates sends the pass's patterns one by one, where the single search grows its lists
 constexpr int kGenericBatchCap = 256;
 
-// A generic pass: uploads the limits glim[id] of the patterns ids[] (max_subs | max_ins << 8 | max_dels << 16) and
-// sizes the candidate lists of `grid` CTAs of the verify kernel.
-static int prepare_generic_pass(fzb_haystack *h, const uint32_t *glim, const std::vector<uint32_t> &ids, int grid) {
+// A generic pass: uploads the per-operation limits of the plans of the patterns ids[] (subs | ins << 8 | dels << 16)
+// and sizes the candidate lists of `grid` CTAs of the verify kernel.
+static int prepare_generic_pass(const BatchCall &c, const std::vector<uint32_t> &ids, int grid) {
+    fzb_haystack *h = c.h;
     TRY(ensure_group(h->gbatch, [](GenericBatchBufs &g) -> int { return g.d_glim.alloc(kMaxBatchPats); }));
-    std::vector<uint32_t> lim(ids.size());
-    for (size_t i = 0; i < ids.size(); i++) lim[i] = glim[ids[i]];
+    std::vector<uint32_t> lim;
+    for (uint32_t id : ids) lim.push_back(c.plans[id].subs | c.plans[id].ins << 8 | c.plans[id].dels << 16);
     CK(cudaMemcpyAsync(h->gbatch->d_glim.get(), lim.data(), lim.size() * 4, cudaMemcpyHostToDevice, h->stream));
     return ensure_scratch(h, (uint64_t)grid * kLpThreads * 2 * kGenericBatchCap);
 }
@@ -2401,27 +2479,27 @@ static void two_bit_key(std::unordered_map<uint32_t, std::vector<uint32_t>> &key
 // error, or +1 if the pass overflowed a device structure (the caller then searches these patterns one by one).
 // dense = false: the q-sample scan (k_filter_multi / k_verify_multi) over the 4-grams of the patterns;
 // dense = true: the n-gram-prefix scan at every position (k_filter_mdense / k_verify_mhits).
-// glim: nullptr for Levenshtein patterns (ks = max_l_dist); for generic patterns (ks = max_l_dist) their limits as
-// prepare_generic_pass takes them, and the generic verify kernels (k_verify_multi_generic / k_verify_mhits_generic).
-static int batch_pass(BatchCall &c, const uint32_t *ks, const std::vector<uint32_t> &ids, bool dense,
-                      const uint32_t *glim = nullptr) {
+// Generic patterns (the generic n-gram route) take the generic verify kernels (k_verify_multi_generic /
+// k_verify_mhits_generic) with their plans' per-operation limits.
+static int batch_pass(BatchCall &c, const std::vector<uint32_t> &ids, bool dense) {
     fzb_haystack *h = c.h;
     const uint32_t cnt = (uint32_t)ids.size();
+    const bool generic = c.plans[ids[0]].generic();
     std::vector<BatchPat> pats(cnt);
     std::vector<uint32_t> pinfo(cnt);
     std::unordered_map<uint32_t, std::vector<uint32_t>> grams;
     grams.reserve(cnt * 48);
     for (uint32_t i = 0; i < cnt; i++) {
-        const uint32_t id = ids[i], m = c.len(id), k = ks[id];
+        const uint32_t id = ids[i], m = c.len(id), k = c.plans[id].k;
         BatchPat &bp = pats[i];
-        fill_pat(bp, c, id, k);
-        bp.L = (int)(m / (k + 1));
+        fill_pat(bp, c, id);
+        bp.L = (int)c.plans[id].L();
         bp.n_ngrams = (int)m / bp.L;
         // The k of pinfo only sets the anchors k_filter_multi marks around a word hit, [g-o-k, g-o+k+m-L].  A generic
         // pattern needs 2k there: its verification runs the NFA from every start of the window [p0-k, p0+m+k) of an
         // n-gram hit, whose end is also the NFA's end of input, so a match that aligns the word with offset o can
         // start anywhere in [g-o-ins, g-o+dels] and its hit p0 anywhere in [g-o-k-dels, g-o+k+dels] (ins + dels <= k).
-        const uint32_t mark_k = glim ? 2 * k : k;  // (n-gram route, m <= 64: k <= 20)
+        const uint32_t mark_k = generic ? 2 * k : k;  // (n-gram route, m <= 64: k <= 20)
         pinfo[i] = m | (mark_k << 8) | ((uint32_t)bp.L << 16);
         if (dense) {  // key: the first 3 bytes of n-gram j; posting: pattern << 8 | j
             for (int j = 0; j < bp.n_ngrams; j++) {
@@ -2449,7 +2527,7 @@ static int batch_pass(BatchCall &c, const uint32_t *ks, const std::vector<uint32
     if (rc) return rc;
     if (dense) TRY(ensure_mhits(h));
     const int ggrid = h->sm_count * 4;  // generic verify kernels: as many lanes (and candidate lists) as run_lp's
-    if (glim) TRY(prepare_generic_pass(h, glim, ids, ggrid));
+    if (generic) TRY(prepare_generic_pass(c, ids, ggrid));
     BatchBufs &b = *h->batch;
     MultiParams mp = pass_params(h);
     mp.bits2 = dense ? nullptr : b.d_mbits.get() + kMultiTblWords;
@@ -2476,11 +2554,11 @@ static int batch_pass(BatchCall &c, const uint32_t *ks, const std::vector<uint32
         CK(cudaEventRecord(h->ev[1], h->stream));
         with_recs(h, [&](auto rec) {
             constexpr bool R = decltype(rec)::value;
-            if (glim && dense)
+            if (generic && dense)
                 k_verify_mhits_generic<R><<<ggrid, kLpThreads, 0, h->stream>>>(
                     dp, h->gbatch->d_glim.get(), h->d_scratch.get(), kGenericBatchCap, h->d_out.get(), h->d_out.size(),
                     h->d_counters.get(), rs);
-            else if (glim)
+            else if (generic)
                 k_verify_multi_generic<R><<<ggrid, kLpThreads, 0, h->stream>>>(
                     mp, b.d_bpats.get(), h->gbatch->d_glim.get(), h->d_scratch.get(), kGenericBatchCap, h->d_out.get(),
                     h->d_out.size(), h->d_counters.get(), rs);
@@ -2501,22 +2579,22 @@ static int batch_pass(BatchCall &c, const uint32_t *ks, const std::vector<uint32
     if (rc) return rc;
     float filter_ms = 0.f;
     cudaEventElapsedTime(&filter_ms, h->ev[0], h->ev[1]);
-    pass.route = glim ? 9 : dense ? 2 : 1;
+    pass.route = generic ? 9 : dense ? 2 : 1;
     pass.filter_ms = filter_ms;
     pass.n_candidates = cnts[CNT_CAND];
     pass.n_launches = 2;
     // (the generic n-gram route's raw order: n-gram, hit index, then the window's matches in canonical order)
-    return c.finish_pass(raw, cnts[CNT_OUT], ids, pass, glim ? 2 : 0, false);
+    return c.finish_pass(raw, cnts[CNT_OUT], ids, pass, generic ? 2 : 0, false);
 }
 
 // One shared scan for up to 64 LP-route patterns (k_lp_scan_multi / k_lp_verify_multi).  Same return convention
-// as batch_pass.  glim: as for batch_pass (ks = the lowered max_l_dist of the LP route, search_generic); a generic
-// NFA opens a candidate at every start (generic_search.py:81), so the scan applies the counting condition only, and
+// as batch_pass.  Generic patterns (the generic LP route, with their plans' lowered limits): a generic NFA opens a
+// candidate at every start (generic_search.py:81), so the scan applies the counting condition only, and
 // k_lp_verify_multi_generic verifies.
-static int batch_pass_lp(BatchCall &c, const uint32_t *ks, const std::vector<uint32_t> &ids,
-                         const uint32_t *glim = nullptr) {
+static int batch_pass_lp(BatchCall &c, const std::vector<uint32_t> &ids) {
     fzb_haystack *h = c.h;
     const uint32_t cnt = (uint32_t)ids.size();
+    const bool generic = c.plans[ids[0]].generic();
     std::vector<BatchPat> pats(cnt);
     std::vector<ulonglong2> lut(256, make_ulonglong2(0ull, 0ull));
     std::vector<uint32_t> pm32((size_t)cnt * 256, 0u);
@@ -2524,14 +2602,14 @@ static int batch_pass_lp(BatchCall &c, const uint32_t *ks, const std::vector<uin
     int wmax = 0;
     uint32_t kmax = 0;
     for (uint32_t i = 0; i < cnt; i++) {
-        const uint32_t id = ids[i], m = c.len(id), k = ks[id];
+        const uint32_t id = ids[i], m = c.len(id), k = c.plans[id].k;
         BatchPat &bp = pats[i];
-        fill_pat(bp, c, id, k);  // (L = n_ngrams = 0: no n-grams)
+        fill_pat(bp, c, id);  // (L = n_ngrams = 0: no n-grams)
         for (uint32_t j = 0; j < m; j++) {
             lut[bp.P[j]].x |= 1ull << i;
             pm32[(size_t)i * 256 + bp.P[j]] |= 1u << j;
         }
-        if (glim)
+        if (generic)
             for (int c = 0; c < 256; c++) lut[c].y |= 1ull << i;
         else
             for (uint32_t j = 0; j <= std::min(k, m - 1); j++) lut[bp.P[j]].y |= 1ull << i;
@@ -2571,8 +2649,8 @@ static int batch_pass_lp(BatchCall &c, const uint32_t *ks, const std::vector<uin
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_lp_scan_multi, kLmThreads, kLmSmem));
     per_sm = std::max(per_sm, 1);
     const int vgrid = h->sm_count * 4, sim_cap = 256;
-    if (glim)
-        TRY(prepare_generic_pass(h, glim, ids, vgrid));
+    if (generic)
+        TRY(prepare_generic_pass(c, ids, vgrid));
     else
         TRY(ensure_scratch(h, (uint64_t)vgrid * kLpThreads * 2 * sim_cap));
     const uint64_t chunk = c.tiny ? kTinyLpChunk : 256ull << 20;  // starts per scan: bounds the survivor list
@@ -2596,7 +2674,7 @@ static int batch_pass_lp(BatchCall &c, const uint32_t *ks, const std::vector<uin
                                                                               lb.d_lmhist.get() + 128, lb.d_lmlist.get());
             with_recs(h, [&](auto rec) {
                 constexpr bool R = decltype(rec)::value;
-                if (glim)
+                if (generic)
                     k_lp_verify_multi_generic<R><<<vgrid, kLpThreads, 0, h->stream>>>(
                         lp, h->gbatch->d_glim.get(), lb.d_lmlist.get(), lb.d_lmhist.get(), h->d_scratch.get(),
                         kGenericBatchCap, h->d_out.get(), h->d_out.size(), h->d_counters.get(), rs);
@@ -2613,7 +2691,7 @@ static int batch_pass_lp(BatchCall &c, const uint32_t *ks, const std::vector<uin
         });
     }, raw, cnts, pass);
     if (rc) return rc;
-    pass.route = glim ? 10 : 3;
+    pass.route = generic ? 10 : 3;
     pass.filter_ms = cs.scan_ms;
     pass.n_candidates = cs.listed;
     pass.n_launches = 4 * cs.chunks;
@@ -2642,14 +2720,13 @@ constexpr double kDnaLevAloneHitNs = 0.29;
 constexpr double kDnaLevPassHits = 4.0;
 constexpr uint32_t kDnaLevMinL = 5;    // n-grams of at least 5 symbols: at most 64 completions of a key
 
-static uint32_t dna_lev_postings(uint32_t m, uint32_t k) {
-    const uint32_t L = m / (k + 1);
-    return (m / L) << (2 * (kHbKeySyms - std::min<uint32_t>(L, kHbKeySyms)));
+static uint32_t dna_lev_postings(const Plan &p) {
+    return (p.m / p.L()) << (2 * (kHbKeySyms - std::min<uint32_t>(p.L(), kHbKeySyms)));
 }
 
-// expected hits per position of pattern (m, k); `rides` whether it costs less in a pass over `positions` than alone
-static double dna_lev_hits(const fzb_haystack *h, uint32_t m, uint32_t k, double positions, bool *rides) {
-    const uint32_t L = m / (k + 1), n = m / L;
+// expected hits per position of pattern `p`; `rides` whether it costs less in a pass over `positions` than alone
+static double dna_lev_hits(const fzb_haystack *h, const Plan &p, double positions, bool *rides) {
+    const uint32_t L = p.L(), n = p.m / L;
     const double c = h->coll_prob;
     const double post = n * std::pow(std::max(c, 0.25), (double)std::min<uint32_t>(L, kHbKeySyms));
     const double hits = n * std::pow(c, (double)L);
@@ -2663,7 +2740,7 @@ static double dna_lev_hits(const fzb_haystack *h, uint32_t m, uint32_t k, double
 // as batch_pass.  The own range is scanned and verified in chunks whose expected hits (hits_per_pos per position)
 // fill at most half the hit list; an overflowing chunk sends the pass's patterns one by one.  tiny
 // (FZB_F_TINY_LIST): kTinyBatchCap hits and chunks of kTinyLpChunk positions.
-static int batch_pass_dna(BatchCall &c, const uint32_t *ks, const std::vector<uint32_t> &ids, double hits_per_pos) {
+static int batch_pass_dna(BatchCall &c, const std::vector<uint32_t> &ids, double hits_per_pos) {
     fzb_haystack *h = c.h;
     const uint32_t cnt = (uint32_t)ids.size();
     std::vector<BatchPat> pats(cnt);
@@ -2673,10 +2750,10 @@ static int batch_pass_dna(BatchCall &c, const uint32_t *ks, const std::vector<ui
     std::unordered_map<uint32_t, std::vector<uint32_t>> keys;  // key -> postings pattern << 8 | n-gram
     keys.reserve(cnt * 64);
     for (uint32_t i = 0; i < cnt; i++) {
-        const uint32_t id = ids[i], m = c.len(id), k = ks[id];
+        const uint32_t id = ids[i], m = c.len(id), k = c.plans[id].k;
         BatchPat &bp = pats[i];
-        fill_pat(bp, c, id, k);
-        bp.L = (int)(m / (k + 1));
+        fill_pat(bp, c, id);
+        bp.L = (int)c.plans[id].L();
         bp.n_ngrams = (int)m / bp.L;
         pinfo[i] = m | (k << 8) | ((uint32_t)bp.L << 16);
         for (int j = 0; j < bp.n_ngrams; j++) two_bit_key(keys, p.code, bp.P + j * bp.L, bp.L, (i << 8) | (uint32_t)j);
@@ -2725,10 +2802,9 @@ static int batch_pass_dna(BatchCall &c, const uint32_t *ks, const std::vector<ui
 }
 
 // The q-sample passes over the patterns `admit(i)` takes, in order, each as many as a pass's pattern slots and gram
-// table hold; ks: the limits the patterns are searched with, glim: as for batch_pass.  A pass of one pattern is not
-// worth it.
+// table hold.  A pass of one pattern is not worth it.
 template <class F>
-static int qsample_passes(BatchCall &c, const uint32_t *ks, const uint32_t *glim, F admit) {
+static int qsample_passes(BatchCall &c, F admit) {
     std::vector<uint32_t> shared;
     for (uint32_t i = 0; i < c.count; i++)
         if (admit(i)) shared.push_back(i);
@@ -2743,16 +2819,16 @@ static int qsample_passes(BatchCall &c, const uint32_t *ks, const uint32_t *glim
             ids.push_back(shared[done++]);
         }
         if (ids.size() < 2) break;
-        TRY(c.settle(batch_pass(c, ks, ids, false, glim), ids));
+        TRY(c.settle(batch_pass(c, ids, false), ids));
     }
     return FZB_OK;
 }
 
 // The n-gram-prefix pass over the unsettled n-gram-route patterns `admit(i)` takes (the class's window-slot rule
 // among its conditions), in order, while the expected prefix hits per haystack position stay within 0.02 and the
-// prefix table has room; ks and glim as for qsample_passes.
+// prefix table has room.
 template <class F>
-static int dense_pass(BatchCall &c, const uint32_t *ks, const uint32_t *glim, F admit) {
+static int dense_pass(BatchCall &c, F admit) {
     std::vector<uint32_t> ids;
     if (c.share && sample_collision_prob(c.h) == FZB_OK) {
         double expect = 0.0;
@@ -2760,7 +2836,7 @@ static int dense_pass(BatchCall &c, const uint32_t *ks, const uint32_t *glim, F 
         const double c3 = c.h->coll_prob * c.h->coll_prob * c.h->coll_prob;
         for (uint32_t i = 0; i < c.count && ids.size() < kMaxBatchPats; i++) {
             if (c.settled(i) || !admit(i)) continue;
-            const uint32_t n = c.len(i) / (c.len(i) / (ks[i] + 1));  // n-grams
+            const uint32_t n = c.len(i) / c.plans[i].L();  // n-grams
             if (expect + n * c3 > 0.02) continue;  // (low-entropy text: prefixes hit everywhere -> one by one)
             if (grams + n > kMaxBatchGrams) continue;  // prefix table capacity
             expect += n * c3;
@@ -2768,7 +2844,7 @@ static int dense_pass(BatchCall &c, const uint32_t *ks, const uint32_t *glim, F 
             ids.push_back(i);
         }
     }
-    return ids.size() >= 2 ? c.settle(batch_pass(c, ks, ids, true, glim), ids) : FZB_OK;
+    return ids.size() >= 2 ? c.settle(batch_pass(c, ids, true), ids) : FZB_OK;
 }
 
 // A candidate of a pass bounded by an expected cost and by postings (greedy_passes).
@@ -2803,41 +2879,31 @@ static int greedy_passes(const std::vector<PassItem> &items, double max_cost, F 
     return close();
 }
 
-static int levenshtein_batch(BatchCall &c, const uint32_t *max_l_dist, fzb_stats *total) {
+static int levenshtein_batch(BatchCall &c, fzb_stats *total) {
     fzb_haystack *h = c.h;
-    // patterns the shared scan can take: n-gram route, q-sample lemma holds, 4-grams selective on this haystack,
-    // short enough for the 64-bit match table
-    TRY(qsample_passes(c, max_l_dist, nullptr, [&](uint32_t i) {
-        const uint32_t m = c.len(i), k = max_l_dist[i];
-        if (!c.share || m == 0 || m > (uint32_t)kBatchMaxM || k == 0 || k >= m) return false;
-        const uint32_t L = m / (k + 1);
-        return L >= 3 && sampled_filter_applies(m, k, 0) && check_halo(h, (uint64_t)m + k) == FZB_OK &&
-               sampled_is_selective(h, m, k, (int)L, (int)(m / L));
-    }));
+    // n-gram-route patterns with k > 0 (the k = 0 route is the exact search's) short enough for the passes' pattern
+    // slots; among them those whose single search takes the sampled filter, and those whose hit windows fit a slot of
+    // k_verify_mhits (the dense and the 2-bit passes)
+    auto ngrams = [&](const Plan &p) { return p.route == Route::LevNgrams && p.k > 0 && p.m <= (uint32_t)kBatchMaxM; };
+    auto mhits = [&](const Plan &p) {
+        return ngrams(p) && p.m - p.L() <= 32 && p.m + 2 * p.k + 12 <= (uint32_t)kMhSlotBytes;
+    };
+    // the patterns the shared scan can take: the q-sample lemma holds and their 4-grams are selective on this haystack
+    TRY(qsample_passes(c, [&](uint32_t i) { return c.share && ngrams(c.plans[i]) && sampled_filter(h, c.plans[i], 0); }));
     // the n-gram-route patterns the lemma does not cover share a scan of their own (n-gram prefixes at every position)
-    TRY(dense_pass(c, max_l_dist, nullptr, [&](uint32_t i) {
-        const uint32_t m = c.len(i), k = max_l_dist[i];
-        if (m == 0 || m > (uint32_t)kBatchMaxM || k == 0 || k >= m) return false;
-        const uint32_t L = m / (k + 1);
-        return L >= 3 && m - L <= 32 && m + 2 * k + 12 <= (uint32_t)kMhSlotBytes &&
-               check_halo(h, (uint64_t)m + k) == FZB_OK;
-    }));
-    // LP-route patterns (m // (k+1) < 3) share scans of 64 patterns each (bit-sliced window counters)
+    TRY(dense_pass(c, [&](uint32_t i) { return mhits(c.plans[i]); }));
+    // LP-route patterns share scans of 64 patterns each (bit-sliced window counters)
     std::vector<uint32_t> lp_ids;
-    if (c.share) {
-        for (uint32_t i = 0; i < c.count; i++) {
-            if (c.settled(i)) continue;
-            const uint32_t m = c.len(i), k = max_l_dist[i];
-            if (m == 0 || k == 0 || k >= m || m / (k + 1) >= 3) continue;
-            if (m > 31 || k > 8 || m + k > 31) continue;  // automaton masks / 6-bit window counters
-            if (check_halo(h, (uint64_t)m + k) != FZB_OK) continue;
-            lp_ids.push_back(i);
-        }
+    for (uint32_t i = 0; c.share && i < c.count; i++) {
+        const Plan &p = c.plans[i];
+        if (c.settled(i) || p.route != Route::LevLp || p.k >= p.m) continue;
+        if (p.m > 31 || p.k > 8 || p.m + p.k > 31) continue;  // automaton masks / 6-bit window counters
+        lp_ids.push_back(i);
     }
     for (size_t first = 0; first + 2 <= lp_ids.size(); first += 64) {
         std::vector<uint32_t> ids(lp_ids.begin() + first, lp_ids.begin() + std::min(lp_ids.size(), first + 64));
         if (ids.size() < 2) break;
-        TRY(c.settle(batch_pass_lp(c, max_l_dist, ids), ids));
+        TRY(c.settle(batch_pass_lp(c, ids), ids));
     }
     // on low-entropy haystacks (at the 0.15 boundary of k_filter_dense2) the n-gram-route patterns left over that cost
     // less in a pass than alone share 2-bit n-gram scans (k_filter_mdense2), in passes bounded by hits and capacity
@@ -2845,26 +2911,19 @@ static int levenshtein_batch(BatchCall &c, const uint32_t *max_l_dist, fzb_stats
         const double positions = (double)(h->own_hi - h->own_lo);
         std::vector<PassItem> items;
         for (uint32_t i = 0; i < c.count; i++) {
-            if (c.settled(i)) continue;
-            const uint32_t m = c.len(i), k = max_l_dist[i];
-            if (m == 0 || m > (uint32_t)kBatchMaxM || k == 0 || k >= m) continue;
-            const uint32_t L = m / (k + 1);
-            if (L < kDnaLevMinL || m - L > 32 || m + 2 * k + 12 > (uint32_t)kMhSlotBytes) continue;
-            if (check_halo(h, (uint64_t)m + k) != FZB_OK) continue;
-            if (sampled_filter_applies(m, k, 0) && sampled_is_selective(h, m, k, (int)L, (int)(m / L)))
-                continue;  // (its single search takes the sampled route: a q-sample pass that overflowed)
+            const Plan &p = c.plans[i];
+            if (c.settled(i) || !mhits(p) || p.L() < kDnaLevMinL) continue;
+            if (sampled_filter(h, p, 0)) continue;  // (a q-sample pass that overflowed)
             bool rides = false;
-            const double phits = dna_lev_hits(h, m, k, positions, &rides);
+            const double phits = dna_lev_hits(h, p, positions, &rides);
             if (!rides || phits > kDnaLevPassHits) continue;
-            items.push_back({i, phits, dna_lev_postings(m, k)});
+            items.push_back({i, phits, dna_lev_postings(p)});
         }
         TRY(greedy_passes(items, kDnaLevPassHits, [&](const std::vector<uint32_t> &ids, double hits) {
-            return c.settle(batch_pass_dna(c, max_l_dist, ids, hits), ids);
+            return c.settle(batch_pass_dna(c, ids, hits), ids);
         }));
     }
-    return c.finish(total, [&](uint32_t i, uint32_t f, fzb_result **res) {
-        return fzb_search_levenshtein(h, c.patterns + c.offsets[i], c.len(i), max_l_dist[i], f, res);
-    });
+    return c.finish(total);
 }
 
 extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
@@ -2873,16 +2932,15 @@ extern "C" int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patt
     HandleLock handle_lock(h);
     if (!h || !out || (count && (!patterns || !offsets || !max_l_dist))) return fail(FZB_E_INVALID, "NULL argument");
     BatchCall c(h, patterns, offsets, count, flags, out, nullptr);
-    TRY(c.begin());
-    return levenshtein_batch(c, max_l_dist, total);
+    TRY(c.begin([&](uint32_t i, const uint8_t *p, uint32_t m, Plan &pl) {
+        return plan_levenshtein(h, p, m, max_l_dist[i], flags, pl);
+    }));
+    return levenshtein_batch(c, total);
 }
 
 extern "C" int fzb_search_exact(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
                                 fzb_result **out) {
-    return run_search(h, pattern, m, flags, (flags & FZB_F_GLOBAL) != 0, out, [&](fzb_result *res) {
-        res->unconsolidated = true;  // ExactSearch.consolidate_matches is the base no-op (common.py:198-205)
-        return search_lev_ngrams(h, pattern, m, 0, flags, res, 2);
-    }, check_exact_pattern);
+    return run_search(h, pattern, flags, out, [&](Plan &pl) { return plan_exact(h, pattern, m, flags, pl); });
 }
 
 // Points a handle at a view of its buffer for its own lifetime; keeps the handle's geometry and restores all of it
@@ -2934,7 +2992,8 @@ extern "C" int fzb_search_exact_window(fzb_haystack *h, const uint8_t *pattern, 
     start = std::min<uint64_t>(start, h->global_len);
     end = std::max<uint64_t>(start, std::min<uint64_t>(end, h->global_len));
     if (end - start < m) {  // no room for an occurrence (also: the empty window): nothing to launch
-        int rc0 = check_exact_pattern(h, pattern, m, flags);
+        Plan pl;
+        int rc0 = plan_exact(h, pattern, m, flags, pl);
         if (rc0) return rc0;
         fzb_result *res;
         rc0 = make_result(out, &res);
@@ -2989,79 +3048,80 @@ static int make_row_maps(fzb_haystack *h, CUtensorMap *map256, CUtensorMap *map8
     return FZB_OK;
 }
 
+static int search_hamming(fzb_haystack *h, const uint8_t *pattern, const Plan &pl, uint32_t flags, fzb_result *res) {
+    const uint32_t m = pl.m;
+    int rc;
+    ScanParams p;
+    fill_params(h, pattern, m, p);
+    p.k = (int)pl.k;
+    if (flags & FZB_F_TINY_LIST) p.glist_cap = std::min(h->glist_cap, 8u);  // (testing) reach the bitmap-mode retry
+    const RecSet rs = rec_set(h);
+    CK(cudaSetDevice(h->device));
+    res->stats.route = 4;
+    res->stats.bytes_scanned = h->buf_len;
+    // counting q-sample filter needs W = floor((m-3)/4) >= k+1 aligned words and 4-bit fields (k <= 7)
+    const bool counting = !(flags & FZB_F_FORCE_DENSE) && (int)m >= 4 * p.k + 7 && p.k <= 7 && h->buf_len > 0;
+    HamCountParams hp{};
+    CUtensorMap map256, map8;
+    int slices = 0;  // of the counters (ham_recur.h)
+    if (counting) {
+        hp.Wc = std::min<int>((int)(m - 3) / 4, 8);
+        // fewer instructions per word: two slices (counting to 4) where the threshold allows, else three
+        slices = hp.Wc - p.k <= 4 ? 2 : 3;
+        hp.bias = (1 << slices) - (hp.Wc - p.k);
+        hp.nrows = (int64_t)(round_up(h->buf_len, kHcRowBytes) / kHcRowBytes);
+        rc = make_row_maps(h, &map256, &map8);
+        if (rc) return rc;
+        CK(cudaFuncSetAttribute(k_hamming_count<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
+        CK(cudaFuncSetAttribute(k_hamming_count<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
+    }
+    bool bitmap_mode = false;
+    PostPlan plan{2, (flags & FZB_F_GLOBAL) != 0};  // FINAL == RAW in (start, end, dist) order, ordered by k_post
+    auto enqueue = [&]() -> int {
+        if (counting) {
+            const int64_t ntiles = (hp.nrows + kHcThreads - 1) / kHcThreads;
+            const int grid = (int)std::min<int64_t>(ntiles, (int64_t)h->sm_count * 2);
+            if (slices == 2)
+                k_hamming_count<2><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
+            else
+                k_hamming_count<3><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
+            CK(cudaEventRecord(h->ev[1], h->stream));
+            h->ev1_recorded = true;
+            // one verify launch: the granule work list -- or, after it overflowed, the whole bitmap
+            with_recs(h, [&](auto rec) {
+                constexpr bool R = decltype(rec)::value;
+                k_verify_ham<R><<<h->sm_count * 4, kVerifyThreads, 0, h->stream>>>(
+                    p, h->d_bitmap.size(), h->d_glist.get(), p.glist_cap, bitmap_mode ? 1 : 0, h->d_out.get(),
+                    h->d_out.size(), h->d_counters.get(), rs);
+            });
+            res->stats.n_launches += 1;
+        } else {
+            with_recs(h, [&](auto rec) {
+                constexpr bool R = decltype(rec)::value;
+                k_hamming_scan<R><<<h->sm_count * 8, kHamThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(),
+                                                                                  h->d_counters.get(), rs);
+            });
+        }
+        res->stats.n_launches++;
+        return FZB_OK;
+    };
+    for (;;) {
+        rc = run_emitting(h, res, enqueue, plan);
+        if (rc) return rc;
+        if (!counting || bitmap_mode || h->h_counters[CNT_GRAN] <= p.glist_cap) break;
+        // the work list overflowed (see search_lev_ngrams)
+        bitmap_mode = true;
+        plan.global = false;
+        p.glist_cap = 0;
+        res->discard_attempt();
+    }
+    res->raw_order = 1;
+    return FZB_OK;
+}
+
 extern "C" int fzb_search_hamming(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t k,
                                   uint32_t flags, fzb_result **out) {
-    return run_search(h, pattern, m, flags, (flags & FZB_F_GLOBAL) != 0, out, [&](fzb_result *res) -> int {
-        int rc = check_halo(h, m);
-        if (rc) return rc;
-        res->unconsolidated = true;
-        ScanParams p;
-        fill_params(h, pattern, m, p);
-        p.k = (int)std::min<uint32_t>(k, m);
-        if (flags & FZB_F_TINY_LIST) p.glist_cap = std::min(h->glist_cap, 8u);  // (testing) reach the bitmap-mode retry
-        const RecSet rs = rec_set(h);
-        CK(cudaSetDevice(h->device));
-        res->stats.route = 4;
-        res->stats.bytes_scanned = h->buf_len;
-        // counting q-sample filter needs W = floor((m-3)/4) >= k+1 aligned words and 4-bit fields (k <= 7)
-        const bool counting = !(flags & FZB_F_FORCE_DENSE) && (int)m >= 4 * p.k + 7 && p.k <= 7 && h->buf_len > 0;
-        HamCountParams hp{};
-        CUtensorMap map256, map8;
-        int slices = 0;  // of the counters (ham_recur.h)
-        if (counting) {
-            hp.Wc = std::min<int>((int)(m - 3) / 4, 8);
-            // fewer instructions per word: two slices (counting to 4) where the threshold allows, else three
-            slices = hp.Wc - p.k <= 4 ? 2 : 3;
-            hp.bias = (1 << slices) - (hp.Wc - p.k);
-            hp.nrows = (int64_t)(round_up(h->buf_len, kHcRowBytes) / kHcRowBytes);
-            rc = make_row_maps(h, &map256, &map8);
-            if (rc) return rc;
-            CK(cudaFuncSetAttribute(k_hamming_count<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
-            CK(cudaFuncSetAttribute(k_hamming_count<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHcSmem));
-        }
-        bool bitmap_mode = false;
-        PostPlan plan{2, (flags & FZB_F_GLOBAL) != 0};  // FINAL == RAW in (start, end, dist) order, ordered by k_post
-        auto enqueue = [&]() -> int {
-            if (counting) {
-                const int64_t ntiles = (hp.nrows + kHcThreads - 1) / kHcThreads;
-                const int grid = (int)std::min<int64_t>(ntiles, (int64_t)h->sm_count * 2);
-                if (slices == 2)
-                    k_hamming_count<2><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
-                else
-                    k_hamming_count<3><<<grid, kHcThreads, kHcSmem, h->stream>>>(p, hp, map256, map8);
-                CK(cudaEventRecord(h->ev[1], h->stream));
-                h->ev1_recorded = true;
-                // one verify launch: the granule work list -- or, after it overflowed, the whole bitmap
-                with_recs(h, [&](auto rec) {
-                    constexpr bool R = decltype(rec)::value;
-                    k_verify_ham<R><<<h->sm_count * 4, kVerifyThreads, 0, h->stream>>>(
-                        p, h->d_bitmap.size(), h->d_glist.get(), p.glist_cap, bitmap_mode ? 1 : 0, h->d_out.get(),
-                        h->d_out.size(), h->d_counters.get(), rs);
-                });
-                res->stats.n_launches += 1;
-            } else {
-                with_recs(h, [&](auto rec) {
-                    constexpr bool R = decltype(rec)::value;
-                    k_hamming_scan<R><<<h->sm_count * 8, kHamThreads, 0, h->stream>>>(p, h->d_out.get(), h->d_out.size(),
-                                                                                      h->d_counters.get(), rs);
-                });
-            }
-            res->stats.n_launches++;
-            return FZB_OK;
-        };
-        for (;;) {
-            rc = run_emitting(h, res, enqueue, plan);
-            if (rc) return rc;
-            if (!counting || bitmap_mode || h->h_counters[CNT_GRAN] <= p.glist_cap) break;
-            // the work list overflowed (see search_lev_ngrams)
-            bitmap_mode = true;
-            plan.global = false;
-            p.glist_cap = 0;
-            res->discard_attempt();
-        }
-        res->raw_order = 1;
-        return FZB_OK;
-    });
+    return run_search(h, pattern, flags, out, [&](Plan &pl) { return plan_hamming(h, pattern, m, k, flags, pl); });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -3076,34 +3136,33 @@ extern "C" int fzb_search_hamming(fzb_haystack *h, const uint8_t *pattern, uint3
 constexpr double kHamBatchPatExpect = 0.01;
 constexpr double kHamBatchExpect = 0.25;
 
-// Key width of pattern (m, k) in a pass, in symbols: 2-bit keys are always 8 symbols wide (a piece of 5..7 symbols
+// Key width of pattern `p` in a pass, in symbols: 2-bit keys are always 8 symbols wide (a piece of 5..7 symbols
 // is entered under every completion); text keys are the first min(L, 4) bytes of a piece, one width per pass.  0 when
 // no pass can take the pattern: too long for the pass's pattern slots, every start matches, or a piece too short for
 // a selective key.
-static uint32_t ham_batch_key(uint32_t m, uint32_t k, bool two_bit) {
-    if (m > (uint32_t)kBatchMaxM || k >= m) return 0;
-    const uint32_t L = m / (k + 1);
+static uint32_t ham_batch_key(const Plan &p, bool two_bit) {
+    if (p.m > (uint32_t)kBatchMaxM || p.k >= p.m) return 0;
+    const uint32_t L = p.L();
     if (two_bit) return L >= 5 ? (uint32_t)kHbKeySyms : 0;
     return L >= 3 ? std::min<uint32_t>(L, 4) : 0;
 }
 
-// Postings of pattern (m, k) in a pass: one per piece, or per completion of a 2-bit key shorter than 8 symbols.
-static uint32_t ham_batch_postings(uint32_t m, uint32_t k, bool two_bit) {
-    const uint32_t L = m / (k + 1);
-    return (k + 1) * (two_bit && L < (uint32_t)kHbKeySyms ? 1u << (2 * (kHbKeySyms - L)) : 1u);
+// Postings of pattern `p` in a pass: one per piece, or per completion of a 2-bit key shorter than 8 symbols.
+static uint32_t ham_batch_postings(const Plan &p, bool two_bit) {
+    const uint32_t L = p.L();
+    return (p.k + 1) * (two_bit && L < (uint32_t)kHbKeySyms ? 1u << (2 * (kHbKeySyms - L)) : 1u);
 }
 
-// Expected postings per haystack position of pattern (m, k) in a pass with keys of `key` symbols.
-static double ham_batch_cost(const fzb_haystack *h, uint32_t m, uint32_t k, uint32_t key, bool two_bit) {
-    const uint32_t L = m / (k + 1);
+// Expected postings per haystack position of pattern `p` in a pass with keys of `key` symbols.
+static double ham_batch_cost(const fzb_haystack *h, const Plan &p, uint32_t key, bool two_bit) {
+    const uint32_t L = p.L();
     const double c = two_bit ? std::max(h->coll_prob, 0.25) : h->coll_prob;  // (2-bit keys see at most 4 codes)
-    return (k + 1) * std::pow(c, (double)std::min(L, key));
+    return (p.k + 1) * std::pow(c, (double)std::min(L, key));
 }
 
 // One k_ham_batch_scan pass for the patterns ids[]; same return convention as batch_pass.  two_bit: the 2-bit keys of
 // low-entropy haystacks, else text keys of key_bytes (4 or 3) bytes.
-static int batch_pass_ham(BatchCall &c, const uint32_t *ks, const std::vector<uint32_t> &ids, bool two_bit,
-                          uint32_t key_bytes) {
+static int batch_pass_ham(BatchCall &c, const std::vector<uint32_t> &ids, bool two_bit, uint32_t key_bytes) {
     fzb_haystack *h = c.h;
     const uint32_t cnt = (uint32_t)ids.size();
     std::vector<BatchPat> pats(cnt);
@@ -3114,9 +3173,9 @@ static int batch_pass_ham(BatchCall &c, const uint32_t *ks, const std::vector<ui
     std::unordered_map<uint32_t, std::vector<uint32_t>> keys;  // key -> postings pattern << 8 | piece
     keys.reserve(cnt * 8);
     for (uint32_t i = 0; i < cnt; i++) {
-        const uint32_t id = ids[i], m = c.len(id), k = ks[id], L = m / (k + 1);
+        const uint32_t id = ids[i], m = c.len(id), k = c.plans[id].k, L = c.plans[id].L();
         BatchPat &bp = pats[i];
-        fill_pat(bp, c, id, k);
+        fill_pat(bp, c, id);
         bp.L = (int)L;
         bp.n_ngrams = (int)k + 1;
         pinfo[i] = m | (k << 8) | (L << 16);
@@ -3185,34 +3244,26 @@ static int batch_pass_ham(BatchCall &c, const uint32_t *ks, const std::vector<ui
     return c.finish_pass(raw, cnts[CNT_OUT], ids, pass, 1, true);
 }
 
-static int hamming_batch(BatchCall &c, const uint32_t *max_subs, fzb_stats *total) {
+static int hamming_batch(BatchCall &c, fzb_stats *total) {
     fzb_haystack *h = c.h;
-    // a pattern the single search refuses fails the whole call, with the single search's error, before any work
-    for (uint32_t i = 0; i < c.count; i++) {
-        int rc = check_pattern(h, c.patterns + c.offsets[i], c.len(i), c.flags);
-        if (rc == FZB_OK) rc = check_halo(h, c.len(i));
-        if (rc) return rc;
-    }
     if (c.share && c.count >= 2 && sample_collision_prob(h) == FZB_OK) {
         const bool two_bit = h->coll_prob >= 0.15;  // the boundary of k_filter_dense2
         // one group of passes per key width: 8 symbols (2-bit); 4 bytes, then 3 bytes (text)
         for (uint32_t key = two_bit ? (uint32_t)kHbKeySyms : 4u; key >= (two_bit ? (uint32_t)kHbKeySyms : 3u); key--) {
             std::vector<PassItem> items;
             for (uint32_t i = 0; i < c.count; i++) {
-                const uint32_t m = c.len(i), k = max_subs[i];
-                if (ham_batch_key(m, k, two_bit) != key) continue;
-                const double cost = ham_batch_cost(h, m, k, key, two_bit);
+                const Plan &p = c.plans[i];
+                if (ham_batch_key(p, two_bit) != key) continue;
+                const double cost = ham_batch_cost(h, p, key, two_bit);
                 if (cost > kHamBatchPatExpect) continue;
-                items.push_back({i, cost, ham_batch_postings(m, k, two_bit)});
+                items.push_back({i, cost, ham_batch_postings(p, two_bit)});
             }
             TRY(greedy_passes(items, kHamBatchExpect, [&](const std::vector<uint32_t> &ids, double) {
-                return c.settle(batch_pass_ham(c, max_subs, ids, two_bit, key), ids);
+                return c.settle(batch_pass_ham(c, ids, two_bit, key), ids);
             }));
         }
     }
-    return c.finish(total, [&](uint32_t i, uint32_t f, fzb_result **res) {
-        return fzb_search_hamming(h, c.patterns + c.offsets[i], c.len(i), max_subs[i], f, res);
-    });
+    return c.finish(total);
 }
 
 extern "C" int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
@@ -3221,76 +3272,39 @@ extern "C" int fzb_search_hamming_batch(fzb_haystack *h, const uint8_t *patterns
     HandleLock handle_lock(h);
     if (!h || !out || (count && (!patterns || !offsets || !max_subs))) return fail(FZB_E_INVALID, "NULL argument");
     BatchCall c(h, patterns, offsets, count, flags, out, nullptr);
-    TRY(c.begin());
-    return hamming_batch(c, max_subs, total);
+    TRY(c.begin([&](uint32_t i, const uint8_t *p, uint32_t m, Plan &pl) {
+        return plan_hamming(h, p, m, max_subs[i], flags, pl);
+    }));
+    return hamming_batch(c, total);
 }
 
 extern "C" int fzb_search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t max_subs,
                                   uint32_t max_ins, uint32_t max_dels, uint32_t max_l, uint32_t flags,
                                   fzb_result **out) {
-    const int post_mode = (flags & FZB_F_NO_FINAL) ? 0 : 1;
-    return run_search(h, pattern, m, flags, post_mode && (flags & FZB_F_GLOBAL), out, [&](fzb_result *res) {
-        // find_near_matches_generic (generic_search.py:25-54)
-        if (max_l == 0 && !(flags & (FZB_F_FORCE_LP | FZB_F_FORCE_NGRAMS)))
-            return search_lev_ngrams(h, pattern, m, 0, flags, res, post_mode);
-        bool ngrams = m / (max_l + 1) >= 3;
-        if (flags & FZB_F_FORCE_NGRAMS) ngrams = true;
-        if (flags & FZB_F_FORCE_LP) ngrams = false;
-        return search_generic(h, pattern, m, max_subs, max_ins, max_dels, max_l, ngrams, flags, res, post_mode);
+    return run_search(h, pattern, flags, out, [&](Plan &pl) {
+        return plan_generic(h, pattern, m, max_subs, max_ins, max_dels, max_l, flags, pl);
     });
 }
 
-static int generic_batch(BatchCall &c, const uint32_t *max_subs, const uint32_t *max_ins, const uint32_t *max_dels,
-                         const uint32_t *max_l_dist, fzb_stats *total) {
+static int generic_batch(BatchCall &c, fzb_stats *total) {
     fzb_haystack *h = c.h;
-    // Per pattern, as fzb_search_generic would search it: the route, the total limit it works with (the LP route
-    // lowers it, search_generic) and the per-operation limits clamped to that total.  A pattern the single search
-    // refuses (check_pattern, max_l_dist > 63, the halo, an n-gram length of 0) fails the whole call, with the single
-    // search's error, before any work.
-    std::vector<uint32_t> kl(c.count, 0), glim(c.count, 0);
-    std::vector<uint8_t> ngram_route(c.count, 0);
-    for (uint32_t i = 0; i < c.count; i++) {
-        const uint32_t m = c.len(i), l = max_l_dist[i];
-        int rc = check_pattern(h, c.patterns + c.offsets[i], m, c.flags);
-        if (rc) return rc;
-        bool ngrams = m / ((uint64_t)l + 1) >= 3;
-        if (c.flags & FZB_F_FORCE_NGRAMS) ngrams = true;
-        if (c.flags & FZB_F_FORCE_LP) ngrams = false;
-        if (l == 0 && !(c.flags & (FZB_F_FORCE_LP | FZB_F_FORCE_NGRAMS))) {
-            rc = check_halo(h, m);  // (the exact route)
-        } else {
-            const uint32_t lk = ngrams ? l : lp_generic_limit(m, max_ins[i], l);
-            if (lk > 63) return fail(FZB_E_UNSUPPORTED, "max_l_dist > 63 is not supported by the generic search");
-            rc = check_halo(h, (uint64_t)m + lk);
-            if (rc == FZB_OK && ngrams && m / (lk + 1) == 0)  // (only under FZB_F_FORCE_NGRAMS)
-                rc = fail(FZB_E_NGRAM_ZERO, "the subsequence length must be greater than max_l_dist");
-            kl[i] = lk;
-            glim[i] = std::min(max_subs[i], lk) | std::min(max_ins[i], lk) << 8 | std::min(max_dels[i], lk) << 16;
-        }
-        if (rc) return rc;
-        ngram_route[i] = ngrams;
-    }
-    // the shared scans take no exact-route pattern (max_l_dist == 0) and no pattern longer than a BatchPat holds
-    auto shareable = [&](uint32_t i) {
-        return c.share && !c.settled(i) && max_l_dist[i] > 0 && c.len(i) <= (uint32_t)kBatchMaxM;
+    // the shared scans take patterns of the two generic routes (not the k = 0 route) no longer than a BatchPat holds
+    auto shareable = [&](uint32_t i, Route r) {
+        return c.share && !c.settled(i) && c.plans[i].route == r && c.len(i) <= (uint32_t)kBatchMaxM;
     };
     // n-gram route, q-sample lemma holds and its 4-grams are selective on this haystack: q-sample passes, bounded as
     // in the Levenshtein batch
-    TRY(qsample_passes(c, kl.data(), glim.data(), [&](uint32_t i) {
-        if (!shareable(i) || !ngram_route[i]) return false;
-        const uint32_t m = c.len(i), k = kl[i], L = m / (k + 1);
-        return sampled_filter_applies(m, k, 0) && sampled_is_selective(h, m, k, (int)L, (int)(m / L));
-    }));
+    TRY(qsample_passes(c, [&](uint32_t i) { return shareable(i, Route::GenericNgrams) && sampled_filter(h, c.plans[i], 0); }));
     // the other n-gram-route patterns: one n-gram-prefix pass, under the Levenshtein batch's bounds; a hit's window
     // must fit a warp's slot in k_verify_mhits_generic
-    TRY(dense_pass(c, kl.data(), glim.data(), [&](uint32_t i) {
-        return shareable(i) && ngram_route[i] && c.len(i) + 2 * kl[i] + 8 <= (uint32_t)kMhgSlotBytes;
+    TRY(dense_pass(c, [&](uint32_t i) {
+        return shareable(i, Route::GenericNgrams) && c.len(i) + 2 * c.plans[i].k + 8 <= (uint32_t)kMhgSlotBytes;
     }));
-    // LP route (after the lowering of search_generic): passes of at most 64 patterns (6-bit window counters, 32-bit masks)
+    // LP route (with the lowered limit): passes of at most 64 patterns (6-bit window counters, 32-bit masks)
     std::vector<uint32_t> lp_ids;
     for (uint32_t i = 0; i < c.count; i++) {
-        if (!shareable(i) || ngram_route[i]) continue;
-        const uint32_t m = c.len(i), k = kl[i];
+        if (!shareable(i, Route::GenericLp)) continue;
+        const uint32_t m = c.len(i), k = c.plans[i].k;
         if (m > 31 || m + k > 31 || k >= m) continue;
         lp_ids.push_back(i);
     }
@@ -3298,12 +3312,9 @@ static int generic_batch(BatchCall &c, const uint32_t *max_subs, const uint32_t 
     const size_t nlp = (lp_ids.size() + 63) / 64;
     for (size_t q = 0; q < nlp && lp_ids.size() >= 2; q++) {
         std::vector<uint32_t> ids(lp_ids.begin() + lp_ids.size() * q / nlp, lp_ids.begin() + lp_ids.size() * (q + 1) / nlp);
-        TRY(c.settle(batch_pass_lp(c, kl.data(), ids, glim.data()), ids));
+        TRY(c.settle(batch_pass_lp(c, ids), ids));
     }
-    return c.finish(total, [&](uint32_t i, uint32_t f, fzb_result **res) {
-        return fzb_search_generic(h, c.patterns + c.offsets[i], c.len(i), max_subs[i], max_ins[i], max_dels[i],
-                                  max_l_dist[i], f, res);
-    });
+    return c.finish(total);
 }
 
 extern "C" int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
@@ -3314,18 +3325,17 @@ extern "C" int fzb_search_generic_batch(fzb_haystack *h, const uint8_t *patterns
     if (!h || !out || (count && (!patterns || !offsets || !max_subs || !max_ins || !max_dels || !max_l_dist)))
         return fail(FZB_E_INVALID, "NULL argument");
     BatchCall c(h, patterns, offsets, count, flags, out, nullptr);
-    TRY(c.begin());
-    return generic_batch(c, max_subs, max_ins, max_dels, max_l_dist, total);
+    TRY(c.begin([&](uint32_t i, const uint8_t *p, uint32_t m, Plan &pl) {
+        return plan_generic(h, p, m, max_subs[i], max_ins[i], max_dels[i], max_l_dist[i], flags, pl);
+    }));
+    return generic_batch(c, total);
 }
 
-// choose_search_class (__init__.py:60-83) on normalised limits
 static int search_by_class(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t max_subs, uint32_t max_ins,
                            uint32_t max_dels, uint32_t max_l, uint32_t flags, fzb_result **out) {
-    if (max_l == 0) return fzb_search_exact(h, pattern, m, flags, out);
-    if (max_ins == 0 && max_dels == 0) return fzb_search_hamming(h, pattern, m, std::min(max_l, max_subs), flags, out);
-    if (max_l <= std::min(max_subs, std::min(max_ins, max_dels)))
-        return fzb_search_levenshtein(h, pattern, m, max_l, flags, out);
-    return fzb_search_generic(h, pattern, m, max_subs, max_ins, max_dels, max_l, flags, out);
+    return run_search(h, pattern, flags, out, [&](Plan &pl) {
+        return plan_by_class(h, pattern, m, max_subs, max_ins, max_dels, max_l, flags, pl);
+    });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -3346,36 +3356,25 @@ extern "C" int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, con
         return fail(FZB_E_UNSUPPORTED, "more than %u patterns in one fzb_best_per_record call", kBestMaxPatterns);
     if (h->recs->longest > (1ull << 31))
         return fail(FZB_E_UNSUPPORTED, "fzb_best_per_record needs records shorter than 2^31");
-    // every pattern as its single search would take it, before any work; then by class (search_by_class), each class
-    // a batch of its own over its subset of the patterns
+    // every pattern planned as its single search would take it (plan_by_class), before any work; then by class, each
+    // class a batch of its own over its subset of the patterns and their plans
     struct Subset {
         std::vector<uint8_t> blob;
-        std::vector<uint32_t> offsets{0}, ordinal, lim[4];  // lim: the limit arrays of the class's batch
+        std::vector<uint32_t> offsets{0}, ordinal;
+        std::vector<Plan> plans;
     } lev, ham, gen;
     for (uint32_t i = 0; i < count; i++) {
         if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
         const uint8_t *p = patterns + offsets[i];
-        const uint32_t m = offsets[i + 1] - offsets[i], l = max_l_dist[i];
-        TRY(l == 0 ? check_exact_pattern(h, p, m, 0) : check_pattern(h, p, m, 0));
-        Subset *sub = &gen;
-        if (l == 0) {  // (the exact search is the Levenshtein batch's k == 0 route)
-            sub = &lev;
-            sub->lim[0].push_back(0);
-        } else if (max_ins[i] == 0 && max_dels[i] == 0) {
-            sub = &ham;
-            sub->lim[0].push_back(std::min(l, max_subs[i]));
-        } else if (l <= std::min(max_subs[i], std::min(max_ins[i], max_dels[i]))) {
-            sub = &lev;
-            sub->lim[0].push_back(l);
-        } else {
-            const uint32_t lk = m / ((uint64_t)l + 1) >= 3 ? l : lp_generic_limit(m, max_ins[i], l);
-            if (lk > 63) return fail(FZB_E_UNSUPPORTED, "max_l_dist > 63 is not supported by the generic search");
-            const uint32_t lims[4] = {max_subs[i], max_ins[i], max_dels[i], l};
-            for (int q = 0; q < 4; q++) sub->lim[q].push_back(lims[q]);
-        }
-        sub->blob.insert(sub->blob.end(), p, p + m);
-        sub->offsets.push_back((uint32_t)sub->blob.size());
-        sub->ordinal.push_back(i);
+        const uint32_t m = offsets[i + 1] - offsets[i];
+        Plan pl;
+        TRY(plan_by_class(h, p, m, max_subs[i], max_ins[i], max_dels[i], max_l_dist[i], flags, pl));
+        if (pl.route == Route::Exact) pl.route = Route::LevNgrams;  // (the Levenshtein batch's k == 0 route)
+        Subset &sub = pl.route == Route::Hamming ? ham : pl.generic() ? gen : lev;
+        sub.blob.insert(sub.blob.end(), p, p + m);
+        sub.offsets.push_back((uint32_t)sub.blob.size());
+        sub.ordinal.push_back(i);
+        sub.plans.push_back(pl);
     }
     CK(cudaSetDevice(h->device));
     const uint64_t nrec = h->recs->d_off.size() - 1;
@@ -3398,10 +3397,8 @@ extern "C" int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, con
         if (n == 0) continue;
         state.ordinal = sub->ordinal.data();
         BatchCall c(h, sub->blob.data(), sub->offsets.data(), n, flags, nullptr, &state);
-        const uint32_t *lim[4] = {sub->lim[0].data(), sub->lim[1].data(), sub->lim[2].data(), sub->lim[3].data()};
-        TRY(sub == &lev   ? levenshtein_batch(c, lim[0], nullptr)
-            : sub == &ham ? hamming_batch(c, lim[0], nullptr)
-                          : generic_batch(c, lim[0], lim[1], lim[2], lim[3], nullptr));
+        c.plans = std::move(sub->plans);
+        TRY(sub == &lev ? levenshtein_batch(c, nullptr) : sub == &ham ? hamming_batch(c, nullptr) : generic_batch(c, nullptr));
         add_stats(&sum, c.sum);
     }
     // one read-back of 16 bytes per record, whatever the number of matches

@@ -230,7 +230,8 @@ int fzb_search_generic(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint
  * The patterns share passes over the haystack (DESIGN.md section 5.5): ONE scan for every pattern the
  * q-sample lemma covers, ONE for the other n-gram-route patterns, ONE per 64 LP-route patterns; patterns
  * longer than 64 bytes are searched one by one.  Each out[i] is exactly what fzb_search_levenshtein would
- * return for pattern i.  `total` (optional) sums the statistics.  On error nothing is returned.
+ * return for pattern i.  `total` (optional) sums the statistics.  A pattern the single search refuses fails
+ * the whole call with its error; on error nothing is returned.
  * On a handle with a record set the three batches need FZB_F_PER_RECORD (DESIGN.md section 5.11).
  */
 int fzb_search_levenshtein_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets,
