@@ -14,16 +14,16 @@ __all__ = ["find_near_matches", "find_near_matches_batch", "find_near_matches_in
            "find_near_matches_batch_in_each", "best_match_in_each", "BestMatches", "find_near_matches_in_file",
            "nearest_distance", "find_nearest_matches", "nearest_distance_in_each", "NearestDistances",
            "nearest_distance_batch", "find_nearest_matches_batch", "nearest_pattern_in_each", "NearestPatterns",
-           "has_near_match", "Match", "LevenshteinSearchParams", "DeviceSequence", "DeviceSequenceSet", "ExactSearch", "SubstitutionsOnlySearch", "LevenshteinSearch",
+           "align_matches", "align_in_each", "Alignments", "has_near_match", "Match", "LevenshteinSearchParams", "DeviceSequence", "DeviceSequenceSet", "ExactSearch", "SubstitutionsOnlySearch", "LevenshteinSearch",
            "GenericSearch", "choose_search_class", "search_exact"]
 
 from .common import LevenshteinSearchParams, Match
 from .search import (DeviceSequence, ExactSearch, GenericSearch, LevenshteinSearch,
                      SubstitutionsOnlySearch, find_nearest_matches, find_nearest_matches_batch,
-                     nearest_distance, nearest_distance_batch, search_exact)
-from .sequence_set import (BestMatches, DeviceSequenceSet, NearestDistances, NearestPatterns, best_match_in_each,
+                     align_matches, nearest_distance, nearest_distance_batch, search_exact)
+from .sequence_set import (Alignments, BestMatches, DeviceSequenceSet, NearestDistances, NearestPatterns, best_match_in_each,
                            find_near_matches_batch_in_each, find_near_matches_in_each, nearest_distance_in_each,
-                           nearest_pattern_in_each)
+                           align_in_each, nearest_pattern_in_each)
 
 
 def find_near_matches(subsequence, sequence, max_substitutions=None, max_insertions=None,

@@ -28,7 +28,7 @@ ROUTE_NAMES = {7: "batch", 0: "exact", 1: "ngrams/sampled-filter", 2: "ngrams/de
                4: "hamming", 5: "generic-ngrams", 6: "generic-lp", 8: "hamming/batch-scan",
                9: "generic-ngrams/batch-scan", 10: "generic-lp/batch-scan", 11: "nearest/bit-vector-scan",
                12: "nearest/batch-bit-vector-scan", 13: "nearest/substitutions-scan",
-               14: "nearest/substitutions-batch-scan"}
+               14: "nearest/substitutions-batch-scan", 15: "alignment"}
 
 
 class NativeLibraryMissing(ImportError):
@@ -97,6 +97,8 @@ SYMBOLS = {
     "fzb_nearest_distance_batch": (_i32, [_vp, _u8p, _vp, _u32, _u32, _vp, _vp, ctypes.POINTER(Stats)]),
     "fzb_nearest_best_per_record": (_i32, [_vp, _u8p, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp,
                                            ctypes.POINTER(Stats)]),
+    "fzb_align": (_i32, [_vp, _u8p, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _u64, _u32, _vp, _vp, _vp, _vp, _vp,
+                         _vp, _vp, ctypes.POINTER(Stats)]),
     "fzb_find_near_matches": (_i32, [_u8p, _u32, _u8p, _u64, _u32, _u32, _u32, _u32, _i32, _vpp]),
     "fzb_has_near_match": (_i32, [_vp, _u8p, _u32, _u32, _u32, _u32, _u32, ctypes.POINTER(ctypes.c_int)]),
     "fzb_release_workspace": (None, []),
@@ -472,6 +474,36 @@ class Haystack(object):
         check(lib().fzb_nearest_best_per_record(self._h, ptr(blob), ptr(offsets), n, flags,
                                                 *[ctypes.c_void_p(c.ctypes.data) for c in cols], ctypes.byref(st)))
         return tuple(cols), _scan_stats(st)
+
+    def align(self, patterns, max_subs, max_ins, max_dels, max_l, item_pattern, item_start, item_end, item_dist,
+              flags=0):
+        """fzb_align: the alignment of every item (pattern item_pattern[i] against [item_start[i], item_end[i]) in
+        buffer coordinates, item_start -1 for a free start, at a cost of at most item_dist[i]); one normalised limit of
+        each kind per pattern -> ((start int64, cost, n_subs, n_ins, n_dels int32: one entry per item, -1 without an
+        alignment), ops uint8 (item i's m_i + n_ins[i] op bytes from op_offsets[i]), op_offsets uint64 (n_items + 1
+        entries), stats dict)."""
+        blob, offsets, n = self._blob(patterns)
+        limits = [np.ascontiguousarray(ks, dtype=np.uint32) for ks in (max_subs, max_ins, max_dels, max_l)]
+        ip = np.ascontiguousarray(item_pattern, dtype=np.uint32)
+        s = np.ascontiguousarray(item_start, dtype=np.int64)
+        e = np.ascontiguousarray(item_end, dtype=np.int64)
+        d = np.ascontiguousarray(item_dist, dtype=np.int32)
+        k = ip.size
+        if not (s.size == e.size == d.size == k):
+            raise ValueError("one start, end and dist per item expected")
+        if k and int(ip.max()) >= n:
+            raise ValueError("unknown pattern index %d" % int(ip.max()))
+        m = np.diff(offsets.astype(np.int64))[ip] if k else np.zeros(0, np.int64)
+        # room: m + w ops, w the window (a free start: at most m + d symbols)
+        w = np.where(s >= 0, e - s, m + np.maximum(d, 0).astype(np.int64))
+        op_offsets = np.zeros(k + 1, dtype=np.uint64)
+        np.cumsum(np.maximum(m + np.maximum(w, 0), 0), out=op_offsets[1:])
+        ops = np.empty(max(int(op_offsets[-1]), 1), dtype=np.uint8)
+        cols = [np.empty(k, dtype=np.int64)] + [np.empty(k, dtype=np.int32) for _ in range(4)]
+        st = Stats()
+        check(lib().fzb_align(self._h, ptr(blob), ptr(offsets), n, *[ptr(x) for x in limits], ptr(ip), ptr(s), ptr(e),
+                              ptr(d), k, flags, *[ptr(c) for c in cols], ptr(op_offsets), ptr(ops), ctypes.byref(st)))
+        return tuple(cols), ops, op_offsets, _scan_stats(st)
 
     def has_near_match(self, pattern, max_subs, max_ins, max_dels, max_l):
         """True iff the search would return at least one match; stops at the first chunk that holds one."""

@@ -33,6 +33,7 @@
 #include "best_kernels.cuh"
 #include "nearest_kernels.cuh"
 #include "sym_kernels.cuh"
+#include "align_kernels.cuh"
 #include <unordered_map>
 #include "debug_kernels.cuh"
 
@@ -3806,6 +3807,207 @@ extern "C" int fzb_nearest_best_per_record(fzb_haystack *h, const uint8_t *patte
         second_dist[r] = second == kBestPairNone ? -1 : (int32_t)(second >> 16);
         second_pattern[r] = second == kBestPairNone ? -1 : (int32_t)(second & 0xFFFFu);
     }
+    return FZB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// fzb_align (DESIGN.md section 5.17): the edit operations of matches, one warp per item
+// ------------------------------------------------------------------------------------------------
+// The class of a pattern by choose_search_class's rule on normalised limits (as plan_by_class decides it)
+static uint8_t align_class(uint32_t max_subs, uint32_t max_ins, uint32_t max_dels, uint32_t max_l) {
+    if (max_l == 0) return kAlignExact;
+    if (max_ins == 0 && max_dels == 0) return kAlignHamming;
+    if (max_l <= std::min(max_subs, std::min(max_ins, max_dels))) return kAlignLevenshtein;
+    return kAlignGeneric;
+}
+
+// Item i checked and turned into an AlignItem with its clamped bounds; *need = its shared-memory bytes, 0 for an item
+// that cannot have an alignment (its outputs stay -1 and it is not launched).
+static int prepare_align_item(const fzb_haystack *h, const std::vector<uint64_t> &off, uint64_t i, const uint32_t *offsets,
+                              uint32_t count, const uint32_t *max_subs, const uint32_t *max_ins,
+                              const uint32_t *max_dels, const uint32_t *max_l_dist, const uint32_t *item_pattern,
+                              const int64_t *item_start, const int64_t *item_end, const int32_t *item_dist,
+                              const uint64_t *op_offsets, AlignItem &it, uint64_t *need) {
+    const unsigned long long ii = i;
+    const uint32_t p = item_pattern[i];
+    if (p >= count) return fail(FZB_E_INVALID, "item %llu: unknown pattern index %u", ii, p);
+    const int64_t s = item_start[i], e = item_end[i];
+    const uint64_t n = h->global_len;
+    if (e < 0 || (uint64_t)e > n || s < -1) return fail(FZB_E_INVALID, "item %llu: outside the buffer", ii);
+    if (s > e) return fail(FZB_E_INVALID, "item %llu: start > end", ii);
+    if (item_dist[i] < 0) return fail(FZB_E_INVALID, "item %llu: negative cost bound", ii);
+    int64_t lo = 0;
+    if (!off.empty()) {  // the record holding end position e: off[r] <= e <= off[r + 1] - 1
+        const uint64_t r = (uint64_t)(std::upper_bound(off.begin(), off.end(), (uint64_t)e) - off.begin()) - 1;
+        if (r + 1 >= off.size()) return fail(FZB_E_INVALID, "item %llu: outside the records", ii);
+        lo = (int64_t)off[r];
+        if (s >= 0 && s < lo) return fail(FZB_E_INVALID, "item %llu: the window crosses a record edge", ii);
+    }
+    const uint32_t m = offsets[p + 1] - offsets[p];
+    const uint8_t cls = align_class(max_subs[p], max_ins[p], max_dels[p], max_l_dist[p]);
+    if (s < 0 && (cls == kAlignExact || cls == kAlignGeneric))
+        return fail(FZB_E_INVALID, "item %llu: a free start needs a Levenshtein or substitutions-only pattern", ii);
+    if (s >= 0 && (cls == kAlignExact || cls == kAlignHamming) && (uint64_t)(e - s) != m)
+        return fail(FZB_E_INVALID, "item %llu: the window of an exact or substitutions-only pattern must have its length", ii);
+    const int64_t d = item_dist[i];
+    if (s < 0 && cls == kAlignLevenshtein && d > (int64_t)m)
+        return fail(FZB_E_UNSUPPORTED, "item %llu: a free start with a cost bound above the pattern's length", ii);
+    const uint64_t w_room = s >= 0 ? (uint64_t)(e - s) : cls == kAlignHamming ? m : (uint64_t)std::min<int64_t>(m + d, e - lo);
+    if (op_offsets[i + 1] < op_offsets[i] || op_offsets[i + 1] - op_offsets[i] < m + w_room)
+        return fail(FZB_E_INVALID, "item %llu: room for fewer than m + w ops", ii);
+
+    it = AlignItem{};
+    it.s = s;
+    it.e = e;
+    it.lo = lo;
+    it.op_off = op_offsets[i];
+    it.idx = i;
+    it.pat_off = offsets[p];
+    it.m = (uint16_t)m;
+    it.cls = cls;
+    *need = 0;
+    const int64_t L = max_l_dist[p];
+    if (cls == kAlignExact || cls == kAlignHamming) {
+        it.d = (int32_t)std::min<int64_t>(std::min<int64_t>(d, m), cls == kAlignExact ? 0 : std::min<int64_t>(max_subs[p], L));
+        *need = 1;
+        return FZB_OK;
+    }
+    // no alignment costs more than max(m, w): a larger bound of an anchored item is lowered to it
+    int64_t de = std::min(d, L);
+    if (s >= 0) de = std::min<int64_t>(de, std::max<int64_t>(m, e - s));
+    if (s < 0 && de < d) return FZB_OK;  // (a free start at d > max_l_dist: no alignment within the limits)
+    if (de >= kAlignInf) return fail(FZB_E_UNSUPPORTED, "item %llu: a cost bound of %d or more", ii, kAlignInf);
+    it.d = (int32_t)de;
+    if (cls == kAlignLevenshtein) {
+        if (s >= 0) {
+            int kmin;
+            const int bw = align_lev_band((int)m, std::min<int64_t>(e - s, 2 * (int64_t)kAlignInf), (int)de, &kmin);
+            if (bw == 0) return FZB_OK;  // |w - m| > d
+            *need = align_vals_bytes(1, bw) + align_table_bytes(1, (int)m, bw);
+        } else {
+            *need = std::max<uint64_t>(align_vals_bytes(1, 2 * (int)de + 1) + 2 * (2 * de + 1),
+                                       align_vals_bytes(1, (int)de + 1) + align_table_bytes(1, (int)m, (int)de + 1));
+        }
+    } else {
+        const int64_t ins = std::min<int64_t>(max_ins[p], de), dels = std::min<int64_t>(max_dels[p], de);
+        const int64_t subs = std::min<int64_t>(std::min<int64_t>(max_subs[p], de), m);
+        it.subs = (uint16_t)subs;
+        it.ins = (uint16_t)std::min<int64_t>(ins, 0xFFFF);
+        it.dels = (uint16_t)std::min<int64_t>(dels, 0xFFFF);
+        it.lim = (uint16_t)std::min<int64_t>(de, subs + ins + dels);
+        *need = align_vals_bytes((int)ins + 1, (int)dels + 1) + align_table_bytes((int)ins + 1, (int)m, (int)dels + 1);
+        if (*need > (uint64_t)kAlignSmemMax)
+            return fail(FZB_E_UNSUPPORTED,
+                        "item %llu: the generic table of %llu bytes exceeds the %d bytes of shared memory of an item",
+                        ii, (unsigned long long)*need, kAlignSmemMax);
+    }
+    if (*need > (uint64_t)kAlignSmemMax)
+        return fail(FZB_E_UNSUPPORTED, "item %llu: a band of %llu bytes exceeds the %d bytes of shared memory of an item",
+                    ii, (unsigned long long)*need, kAlignSmemMax);
+    return FZB_OK;
+}
+
+extern "C" int fzb_align(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count,
+                         const uint32_t *max_subs, const uint32_t *max_ins, const uint32_t *max_dels,
+                         const uint32_t *max_l_dist, const uint32_t *item_pattern, const int64_t *item_start,
+                         const int64_t *item_end, const int32_t *item_dist, uint64_t n_items, uint32_t flags,
+                         int64_t *start, int32_t *cost, int32_t *n_subs, int32_t *n_ins, int32_t *n_dels,
+                         const uint64_t *op_offsets, uint8_t *ops, fzb_stats *stats) {
+    HandleLock handle_lock(h);
+    if (!h || (count && (!patterns || !offsets || !max_subs || !max_ins || !max_dels || !max_l_dist)) ||
+        (n_items && (!item_pattern || !item_start || !item_end || !item_dist || !start || !cost || !n_subs || !n_ins ||
+                     !n_dels || !op_offsets || !ops)))
+        return fail(FZB_E_INVALID, "NULL argument");
+    if (flags) return fail(FZB_E_UNSUPPORTED, "fzb_align takes no flag");
+    if (!is_whole_sequence(h) || h->comm || h->local_world || h->peer)
+        return fail(FZB_E_UNSUPPORTED, "fzb_align needs a whole (unsharded) sequence outside a world");
+    for (uint32_t p = 0; p < count; p++) {
+        if (offsets[p + 1] < offsets[p]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
+        TRY(check_pattern(h, patterns + offsets[p], offsets[p + 1] - offsets[p], 0));
+    }
+    if (stats) *stats = fzb_stats{};
+    if (n_items == 0) return FZB_OK;
+    CK(cudaSetDevice(h->device));
+    std::vector<uint64_t> off;
+    if (h->recs) {
+        off.resize(h->recs->d_off.size());
+        CK(cudaMemcpyAsync(off.data(), h->recs->d_off.get(), off.size() * sizeof(uint64_t), cudaMemcpyDeviceToHost,
+                           h->stream));
+        CK(cudaStreamSynchronize(h->stream));
+    }
+    // every item checked before any work; the launched ones ordered by their shared-memory bucket
+    std::vector<AlignItem> items;
+    std::vector<uint64_t> per_bucket(kAlignBuckets, 0);
+    std::vector<uint8_t> bucket(n_items, 0xFF);
+    for (uint64_t i = 0; i < n_items; i++) {
+        AlignItem it;
+        uint64_t need;
+        TRY(prepare_align_item(h, off, i, offsets, count, max_subs, max_ins, max_dels, max_l_dist, item_pattern,
+                               item_start, item_end, item_dist, op_offsets, it, &need));
+        if (!need) continue;
+        int b = 0;
+        while ((uint64_t)kAlignBucketBytes[b] < need) b++;
+        bucket[i] = (uint8_t)b;
+        per_bucket[b]++;
+    }
+    std::vector<uint64_t> first(kAlignBuckets + 1, 0);
+    for (int b = 0; b < kAlignBuckets; b++) first[b + 1] = first[b] + per_bucket[b];
+    items.resize(first[kAlignBuckets]);
+    {
+        std::vector<uint64_t> at(first.begin(), first.end() - 1);
+        for (uint64_t i = 0; i < n_items; i++) {
+            if (bucket[i] == 0xFF) continue;
+            uint64_t need;
+            TRY(prepare_align_item(h, off, i, offsets, count, max_subs, max_ins, max_dels, max_l_dist, item_pattern,
+                                   item_start, item_end, item_dist, op_offsets, items[at[bucket[i]]++], &need));
+        }
+    }
+    const uint64_t n_ops = op_offsets[n_items], n_pat = count ? offsets[count] : 0;
+    // the call's own buffers, freed when it returns: the handle's counters, output area and pending result stay as
+    // they were
+    DevBuf<AlignItem> d_items;
+    DevBuf<uint8_t> d_pats, d_ops;
+    DevBuf<int64_t> d_start;
+    DevBuf<int32_t> d_ints;
+    TRY(d_items.alloc(std::max<uint64_t>(items.size(), 1)));
+    TRY(d_pats.alloc(std::max<uint64_t>(n_pat, 1)));
+    TRY(d_ops.alloc(std::max<uint64_t>(n_ops, 1)));
+    TRY(d_start.alloc(n_items));
+    TRY(d_ints.alloc(4 * n_items));
+    AlignOut out{d_start.get(), d_ints.get(), d_ints.get() + n_items, d_ints.get() + 2 * n_items,
+                 d_ints.get() + 3 * n_items, d_ops.get()};
+    fzb_stats st{};
+    st.route = 15;
+    st.n_candidates = items.size();
+    CK(cudaEventRecord(h->ev[0], h->stream));
+    CK(cudaMemsetAsync(d_start.get(), 0xFF, n_items * sizeof(int64_t), h->stream));  // -1 everywhere
+    CK(cudaMemsetAsync(d_ints.get(), 0xFF, 4 * n_items * sizeof(int32_t), h->stream));
+    if (!items.empty())
+        CK(cudaMemcpyAsync(d_items.get(), items.data(), items.size() * sizeof(AlignItem), cudaMemcpyHostToDevice,
+                           h->stream));
+    if (n_pat) CK(cudaMemcpyAsync(d_pats.get(), patterns, n_pat, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaFuncSetAttribute(k_align, cudaFuncAttributeMaxDynamicSharedMemorySize, kAlignSmemMax));
+    for (int b = 0; b < kAlignBuckets; b++) {
+        const uint64_t nb = first[b + 1] - first[b];
+        if (!nb) continue;
+        const int per_sm = std::max(1, std::min(32, (int)(200 * 1024 / kAlignBucketBytes[b])));
+        const int grid = (int)std::min<uint64_t>(nb, (uint64_t)h->sm_count * per_sm);
+        k_align<<<grid, 32, kAlignBucketBytes[b], h->stream>>>(h->d, d_pats.get(), d_items.get() + first[b], nb, out);
+        CK(cudaGetLastError());
+        st.n_launches++;
+    }
+    CK(cudaEventRecord(h->ev[1], h->stream));
+    CK(cudaMemcpyAsync(start, d_start.get(), n_items * sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream));
+    int32_t *cols[4] = {cost, n_subs, n_ins, n_dels};
+    for (int c = 0; c < 4; c++)
+        CK(cudaMemcpyAsync(cols[c], d_ints.get() + c * n_items, n_items * sizeof(int32_t), cudaMemcpyDeviceToHost,
+                           h->stream));
+    if (n_ops) CK(cudaMemcpyAsync(ops, d_ops.get(), n_ops, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
+    st.gpu_ms = st.filter_ms = ms;
+    if (stats) *stats = st;
     return FZB_OK;
 }
 

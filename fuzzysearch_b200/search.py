@@ -30,7 +30,7 @@ def _text(seq):
 
 __all__ = ["DeviceSequence", "ExactSearch", "SubstitutionsOnlySearch", "LevenshteinSearch",
            "GenericSearch", "RawMatches", "search_exact", "nearest_distance", "find_nearest_matches",
-           "nearest_distance_batch", "find_nearest_matches_batch"]
+           "nearest_distance_batch", "find_nearest_matches_batch", "align_matches"]
 
 
 class DeviceSequence(object):
@@ -551,3 +551,71 @@ def find_nearest_matches_batch(subsequences, sequence, max_l_dist=None, *, subst
     for i, (s, e, d) in zip(todo, lists):
         out[i] = [Match(a, b, c, matched=slicer(a, b)) for a, b, c in zip(s.tolist(), e.tolist(), d.tolist())]
     return out
+
+
+_BIG = 1 << 29  # an absent limit, as the batches pass it to the library
+
+
+def _normalised_limits(search_params):
+    """-> (max_subs, max_ins, max_dels, max_l) as the library takes them: None becomes a limit that never binds."""
+    return tuple(_BIG if x is None else min(x, _BIG) for x in search_params.unpacked)
+
+
+def _cigars(ops, op_offsets, n_ops, valid):
+    """The op bytes of every item (fzb_align) -> one extended CIGAR string per item, '' where `valid` is false.  The
+    runs are found and counted in numpy: a run starts at each item's first op and wherever the op changes."""
+    out = [""] * len(valid)
+    idx = np.flatnonzero(valid)
+    if idx.size == 0:
+        return out
+    lens = np.asarray(n_ops, dtype=np.int64)[idx]
+    first = np.cumsum(lens) - lens  # each item's first op in the gathered array
+    total = int(lens.sum())
+    item_of = np.repeat(np.arange(idx.size), lens)
+    flat = ops[np.asarray(op_offsets, dtype=np.int64)[idx][item_of] + (np.arange(total) - first[item_of])]
+    brk = np.empty(total, dtype=bool)
+    brk[0] = True
+    brk[1:] = flat[1:] != flat[:-1]
+    brk[first] = True
+    runs = np.flatnonzero(brk)
+    lengths = np.diff(np.append(runs, total))
+    text = np.strings.add(lengths.astype(np.str_), flat[runs].view("S1").astype(np.str_))
+    ends = np.searchsorted(runs, first[1:]) - 1  # the last run of every item but the last one
+    text[ends] = np.strings.add(text[ends], "\n")
+    for i, c in zip(idx.tolist(), "".join(text.tolist()).split("\n")):
+        out[i] = c
+    return out
+
+
+def align_matches(subsequence, sequence, matches, max_substitutions=None, max_insertions=None, max_deletions=None,
+                  max_l_dist=None):
+    """The edit operations of matches: -> one extended CIGAR string per Match, in sequence order ('=' equal, 'X'
+    substituted, 'I' a sequence symbol the pattern lacks, 'D' a pattern symbol the sequence lacks), e.g.
+    ``'5=1X3=1I10='``.  Pass the limits of the search that produced `matches`; they select the cost model as
+    find_near_matches selects its search (fzb_align, DESIGN.md section 5.17).  `sequence` is anything
+    find_near_matches takes.  Each match is aligned on the device, one warp per match; the alignment is the cheapest
+    one of the pattern against ``sequence[start:end]``, the canonical one among equals.  Its cost is at most
+    ``Match.dist``: exactly it for the exact and substitutions-only searches, ``lev(subsequence, matched)`` for
+    Levenshtein, which can be below ``Match.dist``.  A match with no alignment within its dist and the limits (a
+    wrong pattern, sequence or limit) raises ValueError."""
+    from .common import LevenshteinSearchParams
+    search_params = LevenshteinSearchParams(max_substitutions, max_insertions, max_deletions, max_l_dist)
+    if len(subsequence) == 0:
+        raise ValueError("Given subsequence is empty!")
+    matches = list(matches)
+    if not matches:
+        return []
+    s = np.fromiter((x.start for x in matches), dtype=np.int64, count=len(matches))
+    e = np.fromiter((x.end for x in matches), dtype=np.int64, count=len(matches))
+    d = np.fromiter((x.dist for x in matches), dtype=np.int32, count=len(matches))
+    if (s < 0).any() or (d < 0).any():
+        raise ValueError("matches need non-negative starts and dists")
+    lims = _normalised_limits(search_params)
+    with _lock_for(sequence):
+        pat, hay, _, _ = _prepare(subsequence, sequence)
+        (_, cost, _, ins, _), ops, op_offsets, _ = hay.align([pat], *[[x] for x in lims], np.zeros(len(matches)), s,
+                                                             e, d)
+    bad = np.flatnonzero(cost < 0)
+    if bad.size:
+        raise ValueError("no alignment of the subsequence within the dist and limits of %r" % (matches[int(bad[0])],))
+    return _cigars(ops, op_offsets, len(pat) + ins, cost >= 0)

@@ -12,7 +12,8 @@ from . import _native
 from .common import LevenshteinSearchParams, Match
 from .search import DeviceSequence, ExactSearch, GenericSearch, LevenshteinSearch, _kind, _text
 
-__all__ = ["BestMatches", "DeviceSequenceSet", "NearestDistances", "NearestPatterns", "best_match_in_each",
+__all__ = ["Alignments", "BestMatches", "DeviceSequenceSet", "NearestDistances", "NearestPatterns", "align_in_each",
+           "best_match_in_each",
            "find_near_matches_in_each", "find_near_matches_batch_in_each", "nearest_distance_in_each",
            "nearest_pattern_in_each"]
 
@@ -411,3 +412,130 @@ def _nearest_patterns_on_host(subsequences, seqset, flags):
         pattern[first], dist[first], end[first] = i, got.dist[first], got.end[first]
         pat2[second], dist2[second] = i, got.dist[second]
     return columns
+
+
+class Alignments(object):
+    """What align_in_each returns: numpy columns with one entry per sequence, -1 where a row has no match.  ``start``,
+    ``end`` (int64): the aligned window in the sequence's own coordinates; ``dist`` (int32): the alignment's cost,
+    ``substitutions + insertions + deletions``; ``cigar``: a list of extended CIGAR strings ('' for rows without a
+    match).  ``al[r]`` is None or ``(start, end, cigar)``."""
+
+    def __init__(self, columns, cigar):
+        self.start, self.end, self.dist, self.substitutions, self.insertions, self.deletions = columns
+        self.cigar = cigar
+
+    def __len__(self):
+        return len(self.start)
+
+    def __getitem__(self, r):
+        if self.start[r] < 0:
+            return None
+        return int(self.start[r]), int(self.end[r]), self.cigar[r]
+
+
+def align_in_each(subsequences, sequences, rows, max_l_dist=None, *, max_substitutions=None, max_insertions=None,
+                  max_deletions=None, substitutions_only=False):
+    """The edit operations of one result row per sequence, aligned on the device (fzb_align, DESIGN.md section 5.17):
+    -> Alignments.  `rows` is what one of these returned for the same patterns and sequences:
+
+    * best_match_in_each: each row's match is aligned as align_matches aligns it; pass the limits it was computed
+      with (taken as best_match_in_each takes them).
+    * nearest_pattern_in_each / nearest_distance_in_each (one pattern): the rows give only the distance d and the end
+      e; the alignment starts at the smallest s with ``lev(pattern, sequence[s:e]) == d`` -- the longest match at the
+      nearest distance, found on the device from a window of at most ``len(pattern) + d`` symbols -- and its cost is
+      d.  Pass the same ``substitutions_only`` (then s = e - len(pattern)); no limits.
+
+    `sequences` is a list / tuple (uploaded for this call) or a DeviceSequenceSet (resident)."""
+    from .search import _cigars, _normalised_limits
+    if not isinstance(subsequences, (list, tuple)):
+        subsequences = [subsequences]
+    subsequences = list(subsequences)
+    if any(len(p) == 0 for p in subsequences):
+        raise ValueError("Given subsequence is empty!")
+    n = len(rows)
+    if isinstance(rows, BestMatches):
+        from . import _batch_params
+        subsequences, _, params, _ = _batch_params(subsequences, max_substitutions, max_insertions, max_deletions,
+                                                   max_l_dist)
+        lims = [_normalised_limits(p) for p in params]
+        pattern, start, dist = rows.pattern, rows.start, rows.dist
+        nearest = False
+    else:
+        if any(x is not None for x in (max_l_dist, max_substitutions, max_insertions, max_deletions)):
+            raise ValueError("limits are taken only with BestMatches rows")
+        big = 1 << 29
+        lims = [(big, 0, 0, big) if substitutions_only else (big, big, big, big)] * len(subsequences)
+        if isinstance(rows, NearestPatterns):
+            pattern = rows.pattern
+        elif isinstance(rows, NearestDistances):
+            if len(subsequences) != 1:
+                raise ValueError("NearestDistances rows belong to one subsequence")
+            pattern = np.where(rows.dist >= 0, 0, -1).astype(np.int32)
+        else:
+            raise TypeError("rows must be a BestMatches, NearestPatterns or NearestDistances")
+        start, dist = np.full(n, -1, dtype=np.int64), rows.dist
+        nearest = True
+    if isinstance(sequences, DeviceSequenceSet):
+        seqset, own = sequences, False
+    elif isinstance(sequences, (list, tuple)):
+        seqset, own = (DeviceSequenceSet(sequences) if sequences else None), True
+    else:
+        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
+    if len(sequences) != n:
+        raise ValueError("one row per sequence expected")
+    cols = [np.full(n, -1, dtype=t) for t in (np.int64, np.int64, np.int32, np.int32, np.int32, np.int32)]
+    live = np.flatnonzero(np.asarray(pattern) >= 0)
+    if live.size == 0:
+        if own and seqset is not None:
+            seqset.close()
+        return Alignments(cols, [""] * n)
+    pidx = np.asarray(pattern)[live].astype(np.int64)
+    if pidx.max() >= len(subsequences):
+        raise ValueError("a row names pattern %d of %d" % (int(pidx.max()), len(subsequences)))
+    base = seqset.offsets.astype(np.int64)[live]
+    s = np.where(np.asarray(start)[live] >= 0, np.asarray(start)[live] + base, -1)
+    e = np.asarray(rows.end)[live].astype(np.int64) + base
+    d = np.asarray(dist)[live].astype(np.int32)
+    try:
+        got, cigar = _align_set(seqset, subsequences, lims, pidx, s, e, d)
+    finally:
+        if own:
+            seqset.close()
+    g_start, g_cost, g_x, g_ins, g_dels = got
+    if nearest and (g_cost != d).any():
+        r = int(live[np.flatnonzero(g_cost != d)[0]])
+        raise RuntimeError("row %d: an alignment of cost %d at the nearest distance %d" %
+                           (r, int(g_cost[np.flatnonzero(live == r)[0]]), int(dist[r])))
+    ok = g_cost >= 0
+    start_c, end_c, dist_c, x_c, ins_c, dels_c = cols
+    rl = live[ok]
+    start_c[rl] = g_start[ok] - base[ok]
+    end_c[rl] = e[ok] - base[ok]
+    dist_c[rl], x_c[rl], ins_c[rl], dels_c[rl] = g_cost[ok], g_x[ok], g_ins[ok], g_dels[ok]
+    out = [""] * n
+    for r, c in zip(live.tolist(), cigar):
+        out[r] = c
+    return Alignments(cols, out)
+
+
+def _align_set(seqset, subsequences, lims, pidx, s, e, d):
+    """fzb_align over the set's buffer for the items (pattern pidx[i], window [s[i], e[i]) or a free start, bound
+    d[i]) -> ((start, cost, substitutions, insertions, deletions) arrays, CIGAR list)."""
+    from .search import AlphabetTooLarge, _cigars
+    with seqset._lock:
+        try:  # (item selection, bound patterns, their limits, each item's pattern among them)
+            groups = [(np.arange(len(pidx)), seqset._bind_many(subsequences), lims, pidx)]
+        except AlphabetTooLarge:  # no common byte alphabet: pattern by pattern, each reducing the set to its own
+            groups = [(sel, seqset._bind_many([subsequences[p]]), [lims[p]], np.zeros(sel.size, dtype=np.int64))
+                      for p in np.unique(pidx).tolist() for sel in [np.flatnonzero(pidx == p)]]
+        k = len(pidx)
+        cols = [np.full(k, -1, dtype=np.int64)] + [np.full(k, -1, dtype=np.int32) for _ in range(4)]
+        cigar = [""] * k
+        for sel, pats, pl, ip in groups:
+            got, ops, op_offsets, _ = seqset._seq.haystack.align(pats, *zip(*pl), ip, s[sel], e[sel], d[sel])
+            for c, g in zip(cols, got):
+                c[sel] = g
+            m = np.array([len(p) for p in pats], dtype=np.int64)[ip]
+            for i, cg in zip(sel.tolist(), _cigars(ops, op_offsets, m + got[3], got[1] >= 0)):
+                cigar[i] = cg
+    return tuple(cols), cigar

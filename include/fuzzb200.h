@@ -371,6 +371,53 @@ int fzb_nearest_best_per_record(fzb_haystack *h, const uint8_t *patterns, const 
                                 int32_t *second_dist, /* each: one entry per record */
                                 struct fzb_stats_s *stats);
 
+/*
+ * The edit operations of matches (DESIGN.md section 5.17): the alignment of a pattern against a window of the resident
+ * sequence, one warp per item.  The patterns and their limits as for fzb_best_per_record; pattern i's class follows
+ * the same rule (max_l_dist == 0 exact, max_ins == max_dels == 0 substitutions-only, max_l_dist <= every other limit
+ * Levenshtein, else generic) and sets the cost model: exact and substitutions-only windows have no gaps and must be m
+ * long; Levenshtein costs are the unit edit distance; generic ones the smallest X + I + D with X <= max_subs,
+ * I <= max_ins, D <= max_dels and a total <= max_l_dist.  Nothing is searched.
+ *
+ * Item i is pattern item_pattern[i] against the window [item_start[i], item_end[i]) in buffer coordinates, at a cost
+ * of at most item_dist[i] (a larger bound of a window is lowered to max(m, w), which no alignment exceeds):
+ *   anchored (item_start[i] >= 0): the alignment of the smallest cost; none within the bound or the limits gives -1;
+ *   free start (item_start[i] == -1; Levenshtein and substitutions-only patterns only): the smallest s in
+ *     [max(first symbol of e's record, e - m - d), e] with lev(P, S[s:e)) == d (the longest match), then the anchored
+ *     alignment there; substitutions-only: s = e - m.  No such s gives -1.
+ * Among equal costs the alignment is the canonical one: traced back from (m, w), the diagonal step (= or X) before a
+ * deletion before an insertion wherever each stays on an optimal path; a generic item first takes the final state of
+ * the smallest total, then the fewest insertions.  For every match a search returns, the cost is at most its dist,
+ * and exactly its dist for the exact and substitutions-only classes.
+ *
+ * Outputs, one entry per item, all -1 for an item without an alignment: start[i] (the window start, the one found for
+ * a free start), cost[i] = n_subs[i] + n_ins[i] + n_dels[i].  op_offsets has n_items + 1 non-decreasing entries; item
+ * i has room [op_offsets[i], op_offsets[i + 1]) of at least m_i + w_i bytes, w_i the window length (for a free start
+ * min(m_i + d_i, e_i - record start), m_i under substitutions only), and writes exactly m_i + n_ins[i] (==
+ * w_i + n_dels[i]) op bytes from op_offsets[i], in sequence order: '=' an equal pair, 'X' a substitution, 'I' a symbol
+ * of the sequence with no counterpart in the pattern, 'D' a pattern symbol missing from the sequence.  `stats`
+ * (optional) reports route 15.
+ *
+ * FZB_E_INVALID: an item outside the buffer, or outside the records of a record set, or an anchored window that crosses
+ * a record's edge (a free start is clipped at the record's first symbol instead); start > end; a negative item_dist;
+ * an unknown pattern index; a free start on an exact or generic pattern; an anchored exact or substitutions-only
+ * window whose length is not m; room for fewer than m + w ops.  FZB_E_UNSUPPORTED: any flag, a shard or a handle in
+ * a world, a free start with d > m, a cost bound of 16 383 or more, and an item whose table exceeds 65 536 bytes of
+ * shared memory: a Levenshtein item needs V(1, bw) + T(1, bw), bw = |w - m| + 2 floor((d - |w - m|) / 2) + 1 (a
+ * free start the larger of V(1, 2d + 1) + 4d + 2 and V(1, d + 1) + T(1, d + 1)); a generic item V(I' + 1, D' + 1) +
+ * T(I' + 1, D' + 1) with I' = min(max_ins, d'), D' = min(max_dels, d'), d' = min(d, max_l_dist) as lowered; where
+ * V(l, b) = 6 l (floor(b / 2) + 2) rounded up to 16 and T(l, b) = 4 ceil(l (m + 1) b / 16).  Every d <= m Levenshtein
+ * item fits (at most 17 KiB), so does an anchored window of up to 2m symbols at any bound (at most 34 KiB), and so do
+ * generic limits of up to 3 insertions and deletions for every m <= 255.  Every refusal and every error leaves the
+ * handle as it was; the call uses neither the handle's counters, its output area nor a pending result.
+ */
+int fzb_align(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count,
+              const uint32_t *max_subs, const uint32_t *max_ins, const uint32_t *max_dels, const uint32_t *max_l_dist,
+              const uint32_t *item_pattern, const int64_t *item_start /* -1 = free */, const int64_t *item_end,
+              const int32_t *item_dist, uint64_t n_items, uint32_t flags,
+              int64_t *start, int32_t *cost, int32_t *n_subs, int32_t *n_ins, int32_t *n_dels,
+              const uint64_t *op_offsets, uint8_t *ops, struct fzb_stats_s *stats);
+
 /* ExactSearch.search (search_exact.py:80-85): all (overlapping) occurrences. FINAL == RAW. */
 int fzb_search_exact(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
                      fzb_result **out);
@@ -429,7 +476,7 @@ typedef struct fzb_stats_s {
                                8 hamming batch scan, 9 generic n-grams batch scan, 10 generic LP batch
                                scan, 11 nearest/bit-vector-scan,
                                12 nearest/batch-bit-vector-scan, 13 nearest/substitutions-scan,
-                               14 nearest/substitutions-batch-scan */
+                               14 nearest/substitutions-batch-scan, 15 alignment (fzb_align) */
 } fzb_stats;
 int fzb_result_stats(const fzb_result *r, fzb_stats *out);
 void fzb_result_destroy(fzb_result *r);
