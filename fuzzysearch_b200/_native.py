@@ -22,13 +22,14 @@ RAW, FINAL = 0, 1
 F_NO_FINAL, F_FORCE_DENSE, F_FORCE_LP, F_FORCE_NGRAMS, F_TINY_LIST, F_GLOBAL, F_FORCE_SAMPLED = 1, 2, 4, 8, 16, 32, 64
 F_PER_RECORD = 128  # batches on a handle with a record set: per-record results (DESIGN.md section 5.11)
 F_SUBSTITUTIONS_ONLY = 256  # the nearest_* calls: Hamming distance instead of Levenshtein (DESIGN.md section 5.16)
+F_ANCHOR_START, F_ANCHOR_END = 1024, 2048  # nearest_per_record / nearest_best_per_record (DESIGN.md section 5.18)
 NO_DIST = 0xFFFFFFFF  # nearest_distance(..., F_SUBSTITUTIONS_ONLY): the sequence is shorter than the pattern
 
 ROUTE_NAMES = {7: "batch", 0: "exact", 1: "ngrams/sampled-filter", 2: "ngrams/dense-filter", 3: "lp",
                4: "hamming", 5: "generic-ngrams", 6: "generic-lp", 8: "hamming/batch-scan",
                9: "generic-ngrams/batch-scan", 10: "generic-lp/batch-scan", 11: "nearest/bit-vector-scan",
                12: "nearest/batch-bit-vector-scan", 13: "nearest/substitutions-scan",
-               14: "nearest/substitutions-batch-scan", 15: "alignment"}
+               14: "nearest/substitutions-batch-scan", 15: "alignment", 16: "nearest/anchored"}
 
 
 class NativeLibraryMissing(ImportError):

@@ -3455,9 +3455,7 @@ static int near_geometry(const fzb_haystack *h, int bits, int32_t *seg) {
 // It keeps to its own buffer group: the counters, the output area and a pending result of the handle are not
 // touched.  On FZB_OK the answer is in nearb->d_head[0..1] or nearb->d_words, and the stream has drained.  Without a
 // value (substitutions only: no window) the words keep their prefill, all ones.
-static int nearest_scan(fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool rec, bool ham, fzb_stats *stats) {
-    CK(cudaSetDevice(h->device));
-    const uint64_t nrec = rec ? h->recs->d_off.size() - 1 : 0;
+static int ensure_near_bufs(fzb_haystack *h, uint64_t nrec) {
     if (!h->nearb || h->nearb->d_words.size() < nrec) {  // built whole, beside the one it replaces
         std::unique_ptr<NearBufs> grown;
         TRY(ensure_group(grown, [&](NearBufs &b) -> int {
@@ -3466,6 +3464,13 @@ static int nearest_scan(fzb_haystack *h, const uint8_t *pattern, uint32_t m, boo
         }));
         h->nearb = std::move(grown);
     }
+    return FZB_OK;
+}
+
+static int nearest_scan(fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool rec, bool ham, fzb_stats *stats) {
+    CK(cudaSetDevice(h->device));
+    const uint64_t nrec = rec ? h->recs->d_off.size() - 1 : 0;
+    TRY(ensure_near_bufs(h, nrec));
     NearParams p{};
     p.H = h->d;
     p.N = (int64_t)h->buf_len;
@@ -3520,6 +3525,99 @@ static int nearest_scan(fzb_haystack *h, const uint8_t *pattern, uint32_t m, boo
     return FZB_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Anchored nearest matches (DESIGN.md section 5.18): k_nearest_anchored over the records, for fzb_nearest_per_record
+// and fzb_nearest_best_per_record with FZB_F_ANCHOR_START / FZB_F_ANCHOR_END
+// ------------------------------------------------------------------------------------------------
+template <int BITS, bool HAM, bool BATCH>
+static int launch_anchored(fzb_haystack *h, dim3 grid, const NearAnchParams &p, const RecSet &rs) {
+    CK(cudaFuncSetAttribute(k_nearest_anchored<BITS, HAM, BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)near_smem(BITS)));
+    k_nearest_anchored<BITS, HAM, BATCH><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
+    CK(cudaGetLastError());
+    return FZB_OK;
+}
+
+// k_nearest_anchored of `bits` (one lane per record unless BATCH) over all records, `rows` CTA rows (pattern groups)
+template <bool BATCH>
+static int launch_anchored_bits(fzb_haystack *h, int bits, bool ham, uint32_t rows, const NearAnchParams &p) {
+    const uint64_t per = (uint64_t)(kNearThreads / 32) * (32 / p.g);  // records per CTA and round
+    const int per_sm = bits == 32 ? 4 : bits == 64 ? 3 : 2;
+    const uint64_t gx = std::min<uint64_t>((p.nrec + per - 1) / per,
+                                           std::max<uint64_t>(1, (uint64_t)h->sm_count * per_sm / rows));
+    if (gx == 0) return FZB_OK;  // (no records)
+    const dim3 grid((unsigned)gx, rows);
+    const RecSet rs = rec_set(h);
+    if (BATCH)
+        return bits == 32 ? (ham ? launch_anchored<32, true, BATCH>(h, grid, p, rs) : launch_anchored<32, false, BATCH>(h, grid, p, rs))
+                          : (ham ? launch_anchored<64, true, BATCH>(h, grid, p, rs) : launch_anchored<64, false, BATCH>(h, grid, p, rs));
+    switch (bits) {
+    case 32: return ham ? launch_anchored<32, true, false>(h, grid, p, rs) : launch_anchored<32, false, false>(h, grid, p, rs);
+    case 64: return ham ? launch_anchored<64, true, false>(h, grid, p, rs) : launch_anchored<64, false, false>(h, grid, p, rs);
+    case 128: return ham ? launch_anchored<128, true, false>(h, grid, p, rs) : launch_anchored<128, false, false>(h, grid, p, rs);
+    case 192: return ham ? launch_anchored<192, true, false>(h, grid, p, rs) : launch_anchored<192, false, false>(h, grid, p, rs);
+    default: return ham ? launch_anchored<256, true, false>(h, grid, p, rs) : launch_anchored<256, false, false>(h, grid, p, rs);
+    }
+}
+
+// The parameters of one pattern's anchored scan (one lane per record): 'end' walks the records backwards with the
+// reversed pattern, except under substitutions only, whose window is compared forwards
+static NearAnchParams anchored_single(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool ham, bool end,
+                                      uint64_t *words, uint64_t *steps) {
+    NearAnchParams p{};
+    p.H = h->d;
+    p.nrec = h->recs->d_off.size() - 1;
+    p.words = words;
+    p.steps = steps;
+    p.m = (int32_t)m;
+    p.g = 1;
+    p.end = end;
+    for (uint32_t i = 0; i < m; i++) p.P[i] = pattern[end && !ham ? m - 1 - i : i];
+    return p;
+}
+
+static void anchored_flip(fzb_haystack *h, uint64_t *words, uint64_t nrec) {
+    k_nearest_anchored_flip<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
+        words, nrec, rec_set(h));
+}
+
+// fzb_nearest_per_record with an anchor: as nearest_scan (its buffer group only; on FZB_OK the answer is in
+// nearb->d_words and the stream has drained), the symbols read counted in nearb->d_head[0]
+static int nearest_anchored(fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool ham, bool end, fzb_stats *stats) {
+    CK(cudaSetDevice(h->device));
+    const uint64_t nrec = h->recs->d_off.size() - 1;
+    TRY(ensure_near_bufs(h, nrec));
+    uint64_t *steps = h->nearb->d_head.get();
+    const NearAnchParams p = anchored_single(h, pattern, m, ham, end, h->nearb->d_words.get(), steps);
+    fzb_stats st{};
+    st.route = 16;
+    CK(cudaEventRecord(h->ev[0], h->stream));
+    CK(cudaMemsetAsync(steps, 0, sizeof(uint64_t), h->stream));
+    TRY(launch_anchored_bits<false>(h, m <= 32 ? 32 : (int)round_up(m, 64), ham, 1, p));
+    st.n_launches = 1;
+    if (end) {
+        anchored_flip(h, p.words, nrec);
+        CK(cudaGetLastError());
+        st.n_launches++;
+    }
+    CK(cudaEventRecord(h->ev[1], h->stream));
+    CK(cudaMemcpyAsync(&st.bytes_scanned, steps, sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
+    st.gpu_ms = st.filter_ms = ms;
+    if (stats) *stats = st;
+    return FZB_OK;
+}
+
+// The anchor of a flag word: 0, FZB_F_ANCHOR_START or FZB_F_ANCHOR_END; FZB_E_INVALID for both
+static int anchor_of(uint32_t flags, uint32_t *anchor) {
+    *anchor = flags & (FZB_F_ANCHOR_START | FZB_F_ANCHOR_END);
+    if (*anchor == (FZB_F_ANCHOR_START | FZB_F_ANCHOR_END))
+        return fail(FZB_E_INVALID, "FZB_F_ANCHOR_START and FZB_F_ANCHOR_END exclude each other");
+    return FZB_OK;
+}
+
 extern "C" int fzb_nearest_distance(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
                                     uint32_t *dist, uint64_t *n_ends, uint64_t *first_end, fzb_stats *stats) {
     HandleLock handle_lock(h);
@@ -3546,12 +3644,19 @@ extern "C" int fzb_nearest_per_record(fzb_haystack *h, const uint8_t *pattern, u
     HandleLock handle_lock(h);
     if (!h || !dist || !end) return fail(FZB_E_INVALID, "NULL argument");
     if (!h->recs) return fail(FZB_E_INVALID, "fzb_nearest_per_record needs a handle with a record set");
-    if (flags & ~FZB_F_SUBSTITUTIONS_ONLY)
-        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_per_record takes no flag other than FZB_F_SUBSTITUTIONS_ONLY");
+    if (flags & ~(FZB_F_SUBSTITUTIONS_ONLY | FZB_F_ANCHOR_START | FZB_F_ANCHOR_END))
+        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_per_record takes no flag other than FZB_F_SUBSTITUTIONS_ONLY and "
+                                       "one anchor");
+    uint32_t anchor = 0;
+    TRY(anchor_of(flags, &anchor));
     if (h->recs->longest > (1ull << 32))
         return fail(FZB_E_UNSUPPORTED, "fzb_nearest_per_record needs records shorter than 2^32");
     TRY(check_pattern(h, pattern, m, 0));
-    TRY(nearest_scan(h, pattern, m, true, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0, stats));
+    const bool ham = (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0;
+    if (anchor)
+        TRY(nearest_anchored(h, pattern, m, ham, anchor == FZB_F_ANCHOR_END, stats));
+    else
+        TRY(nearest_scan(h, pattern, m, true, ham, stats));
     // one read-back of 8 bytes per record
     const uint64_t nrec = h->recs->d_off.size() - 1;
     std::vector<uint64_t> words(nrec);
@@ -3587,9 +3692,12 @@ static int launch_nearest_batch(fzb_haystack *h, dim3 grid, const NearBatchParam
 
 // Every pattern checked as its single search would take it (the caller checked the rest): FZB_OK or the refusal
 static int check_nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count,
-                               uint32_t flags, const char *what) {
-    if (flags & ~FZB_F_SUBSTITUTIONS_ONLY)
-        return fail(FZB_E_UNSUPPORTED, "%s takes no flag other than FZB_F_SUBSTITUTIONS_ONLY", what);
+                               uint32_t flags, uint32_t anchors, const char *what) {
+    if (flags & ~(FZB_F_SUBSTITUTIONS_ONLY | anchors))
+        return fail(FZB_E_UNSUPPORTED, "%s takes no flag other than FZB_F_SUBSTITUTIONS_ONLY%s", what,
+                    anchors ? " and one anchor" : "");
+    uint32_t anchor = 0;
+    TRY(anchor_of(flags, &anchor));
     if (count > kBestMaxPatterns) return fail(FZB_E_UNSUPPORTED, "more than %u patterns in one %s call", kBestMaxPatterns, what);
     if (h->comm || h->local_world || h->peer) return fail(FZB_E_UNSUPPORTED, "%s: a handle in a world", what);
     for (uint32_t i = 0; i < count; i++) {
@@ -3602,9 +3710,12 @@ static int check_nearest_batch(fzb_haystack *h, const uint8_t *patterns, const u
 // The scans of all `count` patterns over the whole buffer, per record if `rec`: the patterns of up to 64 symbols in
 // groups of 32 lanes (k_nearest_batch_scan, one launch per word class), longer ones one by one (k_nearest_scan, folded
 // by k_nearest_fold per record), under substitutions only if `ham`.  Its own buffer group only, as nearest_scan.  On
-// FZB_OK the answer is in nearbatch->d_words and the stream has drained.
+// FZB_OK the answer is in nearbatch->d_words and the stream has drained.  `anchor` (record sets only): the same
+// groups and folds through k_nearest_anchored (DESIGN.md section 5.18), g lanes per record, the symbols read counted
+// in d_aux[0] (the partials are a whole sequence's).
 static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count, bool rec,
-                         bool ham, fzb_stats *stats) {
+                         bool ham, uint32_t anchor, fzb_stats *stats) {
+    const bool end = anchor == FZB_F_ANCHOR_END, rev = end && !ham;  // rev: 'end' walks back with reversed patterns
     auto len = [&](uint32_t i) { return offsets[i + 1] - offsets[i]; };
     // by (class, m): the lanes of a group share the warm-up of its longest pattern
     std::vector<uint32_t> order, longs;
@@ -3624,7 +3735,8 @@ static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_
     lanes.resize(round_up(lanes.size(), kNearBatchLanes), 0);
     pats.assign(lanes.size() * kNearBatchMaxM, 0);
     for (size_t l = 0; l < lanes.size(); l++)
-        if (lanes[l]) memcpy(&pats[l * kNearBatchMaxM], patterns + offsets[lanes[l] >> 16], lanes[l] & 0xFFFFu);
+        for (uint32_t i = 0, m = lanes[l] & 0xFFFFu; i < m; i++)
+            pats[l * kNearBatchMaxM + i] = patterns[offsets[lanes[l] >> 16] + (rev ? m - 1 - i : i)];
 
     CK(cudaSetDevice(h->device));
     const uint64_t nrec = rec ? h->recs->d_off.size() - 1 : 0;
@@ -3645,8 +3757,10 @@ static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_
     }
     uint64_t *best = g->d_words.get(), *top2 = best + nrec;
     fzb_stats st{};
-    st.route = ham ? 14 : 12;
+    st.route = anchor ? 16 : ham ? 14 : 12;
+    uint64_t *steps = g->d_aux.get();
     CK(cudaEventRecord(h->ev[0], h->stream));
+    if (anchor) CK(cudaMemsetAsync(steps, 0, sizeof(uint64_t), h->stream));
     if (!lanes.empty()) {
         CK(cudaMemcpyAsync(g->d_lanes.get(), lanes.data(), lanes.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
         CK(cudaMemcpyAsync(g->d_pats.get(), pats.data(), pats.size(), cudaMemcpyHostToDevice, h->stream));
@@ -3673,6 +3787,24 @@ static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_
     uint32_t lane0 = 0;
     for (int cls = 0; cls < 2; cls++) {
         if (!groups[cls]) continue;
+        if (anchor) {  // g: the class's pattern count rounded up to a power of two, at most 32
+            const uint32_t n_cls = (uint32_t)std::count_if(order.begin(), order.end(),
+                                                           [&](uint32_t i) { return (len(i) > 32) == (cls == 1); });
+            NearAnchParams p{};
+            p.H = h->d;
+            p.nrec = nrec;
+            p.lanes = g->d_lanes.get() + lane0;
+            p.pats = g->d_pats.get() + (uint64_t)lane0 * kNearBatchMaxM;
+            p.best = best;
+            p.top2 = top2;
+            p.steps = steps;
+            p.end = end;
+            for (p.g = 1; p.g < (int32_t)std::min<uint32_t>(n_cls, kNearBatchLanes); p.g *= 2) {}
+            lane0 += groups[cls] * kNearBatchLanes;
+            TRY(launch_anchored_bits<true>(h, cls ? 64 : 32, ham, groups[cls], p));
+            st.n_launches++;
+            continue;
+        }
         const int per_sm = cls ? 3 : 4;
         // one wave of CTAs over all groups, one segment per warp: long segments (a small warm-up share) on a long
         // sequence, at least kNearBatchMinSeg on a short one
@@ -3711,6 +3843,14 @@ static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_
         q.words = g->d_aux.get() + 2 * (uint64_t)kNearMaxGrid;
         memcpy(q.P, patterns + offsets[i], m);
         const int bits = (int)round_up(m, 64);
+        if (anchor) {  // every record's word written (no prefill), then folded as below
+            TRY(launch_anchored_bits<false>(h, bits, ham, 1, anchored_single(h, patterns + offsets[i], m, ham, end, q.words, steps)));
+            k_nearest_fold<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
+                q.words, nrec, ham ? m + 1 : m, i, best, top2);
+            CK(cudaGetLastError());
+            st.n_launches += 2;
+            continue;
+        }
         const int grid = near_geometry(h, bits, &q.seg);
         if (rec) {
             k_nearest_fill<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
@@ -3737,7 +3877,13 @@ static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_
             st.n_launches++;
         }
     }
+    if (end) {  // the winners' ends in the mirrored records -> their starts
+        anchored_flip(h, best, nrec);
+        CK(cudaGetLastError());
+        st.n_launches++;
+    }
     CK(cudaEventRecord(h->ev[1], h->stream));
+    if (anchor) CK(cudaMemcpyAsync(&st.bytes_scanned, steps, sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     float ms = 0.f;
     CK(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
@@ -3753,11 +3899,11 @@ extern "C" int fzb_nearest_distance_batch(fzb_haystack *h, const uint8_t *patter
     if (!h || (count && (!patterns || !offsets || !dist || !first_end))) return fail(FZB_E_INVALID, "NULL argument");
     if (!is_whole_sequence(h))
         return fail(FZB_E_UNSUPPORTED, "fzb_nearest_distance_batch needs a whole (unsharded) sequence outside a world");
-    TRY(check_nearest_batch(h, patterns, offsets, count, flags, "fzb_nearest_distance_batch"));
+    TRY(check_nearest_batch(h, patterns, offsets, count, flags, 0, "fzb_nearest_distance_batch"));
     TRY(refuse_records(h, "fzb_nearest_distance_batch"));
     if (stats) *stats = fzb_stats{};
     if (count == 0) return FZB_OK;
-    TRY(nearest_batch(h, patterns, offsets, count, false, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0, stats));
+    TRY(nearest_batch(h, patterns, offsets, count, false, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0, 0, stats));
     // one read-back of 8 bytes per pattern
     std::vector<uint64_t> words(count);
     CK(cudaMemcpyAsync(words.data(), h->nearbatch->d_words.get(), count * sizeof(uint64_t), cudaMemcpyDeviceToHost,
@@ -3779,7 +3925,8 @@ extern "C" int fzb_nearest_best_per_record(fzb_haystack *h, const uint8_t *patte
     if (!h || !pattern || !dist || !end || !second_pattern || !second_dist || (count && (!patterns || !offsets)))
         return fail(FZB_E_INVALID, "NULL argument");
     if (!h->recs) return fail(FZB_E_INVALID, "fzb_nearest_best_per_record needs a handle with a record set");
-    TRY(check_nearest_batch(h, patterns, offsets, count, flags, "fzb_nearest_best_per_record"));
+    TRY(check_nearest_batch(h, patterns, offsets, count, flags, FZB_F_ANCHOR_START | FZB_F_ANCHOR_END,
+                            "fzb_nearest_best_per_record"));
     if (h->recs->longest > (1ull << 32))
         return fail(FZB_E_UNSUPPORTED, "fzb_nearest_best_per_record needs records shorter than 2^32");
     const uint64_t nrec = h->recs->d_off.size() - 1;
@@ -3791,7 +3938,8 @@ extern "C" int fzb_nearest_best_per_record(fzb_haystack *h, const uint8_t *patte
         }
         return FZB_OK;
     }
-    TRY(nearest_batch(h, patterns, offsets, count, true, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0, stats));
+    TRY(nearest_batch(h, patterns, offsets, count, true, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0,
+                      flags & (FZB_F_ANCHOR_START | FZB_F_ANCHOR_END), stats));
     // one read-back of 16 bytes per record
     std::vector<uint64_t> words(2 * nrec);
     CK(cudaMemcpyAsync(words.data(), h->nearbatch->d_words.get(), 2 * nrec * sizeof(uint64_t), cudaMemcpyDeviceToHost,

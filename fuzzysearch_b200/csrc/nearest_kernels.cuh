@@ -97,10 +97,11 @@ struct NearCol {  // one column of the table and what the thread has seen of its
         first = 0;
     }
 
-    // the column behind text byte c; rel: the end position it closes, relative to the caller's base
-    template <bool TRACK>
+    // the column behind text byte c; rel: the end position it closes, relative to the caller's base.  HIN: the
+    // horizontal delta of row 0 -- 0 in the search form (D[0][j] = 0), +1 in the prefix-anchored form (D[0][j] = j)
+    template <bool TRACK, int HIN = 0>
     __device__ __forceinline__ void step(uint32_t c, uint32_t rel) {
-        int hin = 0;
+        int hin = HIN;
 #pragma unroll
         for (int w = 0; w < NW; w++) {
             word Eq = NW == 1 ? pm[c * 32] : pm[c * NW + w];
@@ -114,7 +115,7 @@ struct NearCol {  // one column of the table and what the thread has seen of its
             const int hout = (int)((Ph >> bit) & 1) - (int)((Mh >> bit) & 1);
             Ph <<= 1;
             Mh <<= 1;
-            if (NW > 1) {
+            if (NW > 1 || HIN != 0) {
                 Ph |= (word)(hin > 0);
                 Mh |= (word)(hin < 0);
             }
@@ -547,6 +548,186 @@ __global__ void k_nearest_fold(const uint64_t *words, uint64_t nrec, uint32_t li
         if (d >= lim) continue;
         atomicMin((unsigned long long *)&best[r], (unsigned long long)d << 48 | (uint64_t)ord << 32 | (w & 0xFFFFFFFFull));
         near_top2_add(&top2[r], d << 16 | ord, kBestPairNone);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Anchored nearest matches (DESIGN.md section 5.18): fzb_nearest_per_record / fzb_nearest_best_per_record with
+// FZB_F_ANCHOR_START or FZB_F_ANCHOR_END.  For the pattern P (m symbols) and a record R (n symbols):
+//   'start'  A(e) = lev(P, R[0:e]), e in 0..n: dist = min A, pos = the smallest e that reaches it;
+//   'end'    B(s) = lev(P, R[s:n]): the same problem on (P reversed, R reversed), so the kernel walks the record
+//            backwards with the reversed pattern's table (the host reverses it) and pos = n - s, the end in the
+//            mirrored record -- the smallest such pos is the largest s.  k_nearest_anchored_flip turns pos into s.
+// A is the bottom row of the prefix-anchored table (D[0][j] = j: NearCol::step with HIN = +1).  A(0) = m and
+// A(e) >= e - m, so no e >= m + best can win: a lane reads at most min(n, 2m) symbols and stops at e - m >= best.
+// Under substitutions only (HAM) dist = the mismatches of P against R[0:m] ('start', pos = m) or R[n-m:n] ('end',
+// pos = m as well, the mirror's end); a record shorter than m has no value.  Either way a window never leaves its
+// record, so a separator is never read.
+//
+// Layout: one record per lane group of g lanes (g a power of two, 1 to 32), lane l on pattern slot l % g of the
+// CTA row's group (blockIdx.y), records grid-stride.  The table is k_nearest_batch_scan's PM[c][lane], lane l
+// holding the masks of its own slot, so 32 lanes never share a bank.  BATCH: every lane group sends the smallest
+// key dist << 48 | ordinal << 32 | pos and the runner-up pair of near_batch_report into best[r] / top2[r], over the
+// prefills of section 5.15 / 5.16 (a Levenshtein lane reports only dist < m: the prefill (m_i, i, pos 0) is A(0)).
+// Single pattern (!BATCH): g = 1, one lane per record writes words[r] = dist << 32 | pos (all ones: no value),
+// without prefill; with 2-4 words (m <= 255) the table is [c][word], shared by all lanes, as in k_nearest_scan.
+// `steps` counts the symbols read: per lane group, the longest window one of its lanes read.
+// ------------------------------------------------------------------------------------------------------------------
+struct NearAnchParams {
+    const uint8_t *H;
+    uint64_t nrec;
+    const uint32_t *lanes;  // BATCH: m | ordinal << 16 per lane of every group (0 = idle), as NearBatchParams
+    const uint8_t *pats;    // BATCH: kNearBatchMaxM bytes per lane
+    uint64_t *words;        // single: dist << 32 | pos per record
+    uint64_t *best, *top2;  // BATCH: per record
+    uint64_t *steps;        // the symbols read (added to)
+    int32_t m, g, end;      // m: single; g: lanes per record; end: 'end' (walk the records backwards)
+    uint8_t P[256];         // single
+};
+
+template <int BITS, bool HAM, bool BATCH>
+__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : BITS == 64 ? 3 : 2)
+k_nearest_anchored(NearAnchParams p, RecSet rs) {
+    typedef typename NearWord<BITS>::type word;
+    constexpr int NW = near_words(BITS);
+    constexpr uint32_t WB = sizeof(word) * 8;
+    static_assert(!BATCH || NW == 1, "one word per lane");
+    extern __shared__ __align__(16) uint64_t near_smem_raw[];
+    __shared__ __align__(16) uint8_t s_pat[BATCH ? kNearBatchLanes * kNearBatchMaxM : 256];
+    __shared__ uint32_t s_m[kNearBatchLanes];
+    word *pm = reinterpret_cast<word *>(near_smem_raw);
+    const uint32_t lane = threadIdx.x & 31u, g = BATCH ? (uint32_t)p.g : 1u, slot = lane % g;
+
+    if (BATCH) {
+        const uint8_t *pats = p.pats + (size_t)blockIdx.y * kNearBatchLanes * kNearBatchMaxM;
+        for (uint32_t i = threadIdx.x; i < kNearBatchLanes * kNearBatchMaxM; i += kNearThreads) s_pat[i] = pats[i];
+        if (threadIdx.x < kNearBatchLanes) s_m[threadIdx.x] = p.lanes[blockIdx.y * kNearBatchLanes + threadIdx.x] & 0xFFFFu;
+    } else {
+        s_pat[threadIdx.x] = p.P[threadIdx.x];
+    }
+    __syncthreads();
+    {  // thread c builds the masks of byte c: per lane (of its slot) with one word, [c][word] with more
+        const uint32_t c = threadIdx.x;
+        if (NW == 1) {
+            for (uint32_t l = 0; l < 32; l++) {
+                const uint32_t k = BATCH ? l % g : 0, mk = BATCH ? s_m[k] : (uint32_t)p.m;
+                word mask = 0;
+                for (uint32_t i = 0; i < mk; i++)
+                    if (s_pat[(BATCH ? k * kNearBatchMaxM : 0) + i] == c) mask |= (word)1 << i;
+                pm[c * 32 + l] = mask;
+            }
+        } else {
+            word mask[NW];
+#pragma unroll
+            for (int w = 0; w < NW; w++) mask[w] = 0;
+            for (uint32_t i = 0; i < (uint32_t)p.m; i++)
+                if (s_pat[i] == c) {
+#pragma unroll
+                    for (int w = 0; w < NW; w++)
+                        if ((int)(i / WB) == w) mask[w] |= (word)1 << (i % WB);
+                }
+#pragma unroll
+            for (int w = 0; w < NW; w++) pm[c * NW + w] = mask[w];
+        }
+    }
+    __syncthreads();
+
+    const uint32_t info = BATCH ? p.lanes[blockIdx.y * kNearBatchLanes + slot] : (uint32_t)p.m;
+    const uint32_t m = info & 0xFFFFu, ord = info >> 16;  // (m = 0: an idle lane)
+    const word *tab = NW == 1 ? pm + lane : pm;
+    auto mask_of = [&](uint32_t c, int w) -> word { return NW == 1 ? tab[c * 32] : tab[c * NW + w]; };
+    NearCol<BITS> col;
+    col.pm = tab;
+    col.top = (m - 1) % WB;
+    uint64_t nread = 0;  // lane group leaders: the symbols their group read
+
+    const uint64_t per = (uint64_t)(kNearThreads / 32) * (32 / g);  // records per CTA and round
+    // (the trip count is the same for the lanes of a warp: the collectives below take all 32)
+    for (uint64_t base = (uint64_t)blockIdx.x * per + (threadIdx.x >> 5) * (32 / g); base < p.nrec;
+         base += (uint64_t)gridDim.x * per) {
+        const uint64_t r = base + lane / g;
+        uint32_t dist = ~0u, pos = 0, read = 0;
+        if (r < p.nrec && m) {
+            const int64_t lo = (int64_t)rs.off[r], hi = (int64_t)rs.off[r + 1] - 1;
+            const uint32_t n = (uint32_t)(hi - lo);
+            if (HAM) {
+                if (n >= m) {
+                    const int64_t at = p.end ? hi - m : lo;
+                    word hit[NW];
+#pragma unroll
+                    for (int w = 0; w < NW; w++) hit[w] = 0;
+                    for (uint32_t i = 0; i < m; i++) {
+                        const uint32_t c = __ldg(p.H + at + i);
+#pragma unroll
+                        for (int w = 0; w < NW; w++)
+                            if ((int)(i / WB) == w) hit[w] |= mask_of(c, w) & (word)1 << (i % WB);
+                    }
+                    uint32_t same = 0;
+#pragma unroll
+                    for (int w = 0; w < NW; w++) same += WB == 64 ? __popcll((uint64_t)hit[w]) : __popc((uint32_t)hit[w]);
+                    dist = m - same;
+                    pos = read = m;
+                }
+            } else {
+#pragma unroll
+                for (int w = 0; w < NW; w++) {
+                    col.Pv[w] = ~(word)0;
+                    col.Mv[w] = 0;
+                }
+                col.score = dist = m;
+                const uint32_t lim = n < 2 * m ? n : 2 * m;
+                for (uint32_t e = 1; e <= lim && (int)e - (int)m < (int)dist; e++) {
+                    col.template step<false, 1>(__ldg(p.H + (p.end ? hi - e : lo + e - 1)), 0);
+                    read = e;
+                    if (col.score < dist) {
+                        dist = col.score;
+                        pos = e;
+                    }
+                }
+            }
+        }
+        if (!BATCH) {
+            if (r < p.nrec) p.words[r] = dist == ~0u ? kBestEmpty : (uint64_t)dist << 32 | pos;
+            nread += read;
+            continue;
+        }
+        // the lane group's smallest key and, over its other patterns, the smallest pair (near_batch_report per group)
+        const bool has = dist != ~0u && (HAM || dist < m);
+        const uint64_t key = has ? (uint64_t)dist << 48 | (uint64_t)ord << 32 | pos : ~0ull;
+        uint64_t kmin = key;
+        for (uint32_t d = g >> 1; d; d >>= 1) {
+            const uint64_t o = __shfl_xor_sync(0xFFFFFFFFu, kmin, d);
+            kmin = o < kmin ? o : kmin;
+        }
+        const uint32_t win = (uint32_t)(kmin >> 32);
+        uint32_t second = has && ord != (win & 0xFFFFu) ? (uint32_t)(key >> 32) : kBestPairNone;
+        for (uint32_t d = g >> 1; d; d >>= 1) {
+            const uint32_t o = __shfl_xor_sync(0xFFFFFFFFu, second, d);
+            second = o < second ? o : second;
+            const uint32_t oread = __shfl_xor_sync(0xFFFFFFFFu, read, d);
+            read = oread > read ? oread : read;
+        }
+        if (slot == 0 && r < p.nrec) {
+            nread += read;
+            if (kmin != ~0ull) {
+                atomicMin((unsigned long long *)&p.best[r], (unsigned long long)kmin);
+                near_top2_add(&p.top2[r], win, second);
+            }
+        }
+    }
+    for (int d = 16; d > 0; d >>= 1) nread += __shfl_xor_sync(0xFFFFFFFFu, nread, d);
+    if (lane == 0 && nread) atomicAdd((unsigned long long *)p.steps, (unsigned long long)nread);
+}
+
+// 'end': the pos of every word with a value (dist << 32 | pos, or a best key) from the mirrored record's end to the
+// start in the record, n - pos.  One thread per record.
+__global__ void k_nearest_anchored_flip(uint64_t *words, uint64_t nrec, RecSet rs) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nrec; r += stride) {
+        const uint64_t w = words[r];
+        if (w == kBestEmpty) continue;
+        const uint64_t n = rs.off[r + 1] - 1 - rs.off[r];
+        words[r] = (w & ~0xFFFFFFFFull) | (n - (w & 0xFFFFFFFFull));
     }
 }
 

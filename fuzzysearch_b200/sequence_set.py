@@ -286,10 +286,14 @@ class NearestDistances(object):
     coordinates) of a substring at that distance.  ``nearest[i]`` is ``(dist, end)``.  With
     ``substitutions_only=True`` ``dist`` is the smallest number of substitutions of a window of the pattern's length,
     the match starts at ``end - len(pattern)``, and a sequence shorter than the pattern (or a pattern longer than the
-    sequence) gives ``(-1, -1)``."""
+    sequence) gives ``(-1, -1)``.
 
-    def __init__(self, dist, end):
-        self.dist, self.end = dist, end
+    ``start`` (int64) is None, except for anchored results (``anchor='start'`` / ``'end'``), where it holds the
+    match's start on every row with a distance (-1 elsewhere): 0 for ``'start'``, and for ``'end'`` the largest start
+    at that distance, the match then ending at the sequence's end."""
+
+    def __init__(self, dist, end, start=None):
+        self.dist, self.end, self.start = dist, end, start
 
     def __len__(self):
         return len(self.dist)
@@ -298,22 +302,57 @@ class NearestDistances(object):
         return int(self.dist[r]), int(self.end[r])
 
 
-def nearest_distance_in_each(subsequence, sequences, *, substitutions_only=False):
+def _nearest_flags(substitutions_only, anchor):
+    """The flags of the nearest_*_in_each calls; ValueError for an anchor other than None, 'start' or 'end'."""
+    flags = _native.F_SUBSTITUTIONS_ONLY if substitutions_only else 0
+    if anchor is None:
+        return flags
+    if isinstance(anchor, str) and anchor == "start":
+        return flags | _native.F_ANCHOR_START
+    if isinstance(anchor, str) and anchor == "end":
+        return flags | _native.F_ANCHOR_END
+    raise ValueError("anchor must be None, 'start' or 'end', not %r" % (anchor,))
+
+
+def _anchored_span(seqset, flags, has, pos):
+    """The (start, end) columns of anchored rows in the sequences' own coordinates from the call's per-record
+    position (the end under 'start', the start under 'end'); -1 where a row has no distance.  Unanchored: (None,
+    pos)."""
+    if not flags & (_native.F_ANCHOR_START | _native.F_ANCHOR_END):
+        return None, pos
+    if flags & _native.F_ANCHOR_START:
+        return np.where(has, 0, -1).astype(np.int64), pos
+    n = np.diff(seqset.offsets.astype(np.int64)) - 1
+    return pos, np.where(has, n, -1).astype(np.int64)
+
+
+def _no_distances(flags):
+    anchored = flags & (_native.F_ANCHOR_START | _native.F_ANCHOR_END)
+    return NearestDistances(np.zeros(0, np.int32), np.zeros(0, np.int64), np.zeros(0, np.int64) if anchored else None)
+
+
+def nearest_distance_in_each(subsequence, sequences, *, substitutions_only=False, anchor=None):
     """One pattern over many sequences, without a distance limit: -> NearestDistances with, for every sequence,
     ``nearest_distance(subsequence, sequences[r])`` and where the nearest match first ends; an empty sequence gives
     ``(len(subsequence), 0)``.  All sequences are scanned in one device pass (fzb_nearest_per_record, DESIGN.md
     section 5.14).  `sequences` is a list / tuple (uploaded for this call) or a DeviceSequenceSet (resident).  With
     ``substitutions_only=True`` the distances are ``nearest_distance(..., substitutions_only=True)``, and a sequence
-    shorter than the pattern gives ``(-1, -1)`` (DESIGN.md section 5.16)."""
+    shorter than the pattern gives ``(-1, -1)`` (DESIGN.md section 5.16).
+
+    ``anchor='start'`` takes only matches that start at the sequence's first symbol: ``dist`` is the smallest
+    ``lev(subsequence, seq[0:e])``, ``end`` the smallest such e, ``start`` 0.  ``anchor='end'`` takes only matches
+    that end at its last symbol: the smallest ``lev(subsequence, seq[s:])``, ``start`` the largest such s, ``end``
+    ``len(seq)``.  Under ``substitutions_only=True`` the window is the first (last) ``len(subsequence)`` symbols.
+    An anchored scan reads at most ``2 * len(subsequence)`` symbols of a sequence (DESIGN.md section 5.18)."""
     if len(subsequence) == 0:
         raise ValueError("Given subsequence is empty!")
-    flags = _native.F_SUBSTITUTIONS_ONLY if substitutions_only else 0
+    flags = _nearest_flags(substitutions_only, anchor)
     if isinstance(sequences, DeviceSequenceSet):
         return _nearest_in_set(subsequence, sequences, flags)
     if not isinstance(sequences, (list, tuple)):
         raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
     if not sequences:
-        return NearestDistances(np.zeros(0, np.int32), np.zeros(0, np.int64))
+        return _no_distances(flags)
     seqset = DeviceSequenceSet(sequences)
     try:
         return _nearest_in_set(subsequence, seqset, flags)
@@ -323,11 +362,12 @@ def nearest_distance_in_each(subsequence, sequences, *, substitutions_only=False
 
 def _nearest_in_set(subsequence, seqset, flags):
     if len(seqset) == 0:
-        return NearestDistances(np.zeros(0, np.int32), np.zeros(0, np.int64))
+        return _no_distances(flags)
     with seqset._lock:
         pat = seqset._bind(subsequence)
         dist, end, _ = seqset._seq.haystack.nearest_per_record(pat, flags)
-    return NearestDistances(dist, end)
+    start, end = _anchored_span(seqset, flags, dist >= 0, end)
+    return NearestDistances(dist, end, start)
 
 
 class NearestPatterns(object):
@@ -341,10 +381,14 @@ class NearestPatterns(object):
 
     With ``substitutions_only=True`` only the patterns that fit in the sequence (``len(pattern) <= len(sequence)``)
     have a distance and take part: a row where none fits is -1 everywhere, one where a single pattern fits has -1 in
-    the ``second_*`` arrays.  The winner's match starts at ``end - len(subsequences[pattern])``."""
+    the ``second_*`` arrays.  The winner's match starts at ``end - len(subsequences[pattern])``.
 
-    def __init__(self, columns):
+    ``start`` (int64) is None, except for anchored results, where it holds the winner's match start on every row
+    with a pattern (-1 elsewhere), as NearestDistances.start does."""
+
+    def __init__(self, columns, start=None):
         self.pattern, self.dist, self.end, self.second_pattern, self.second_dist = columns
+        self.start = start
 
     def __len__(self):
         return len(self.pattern)
@@ -357,7 +401,12 @@ def _no_patterns(n):
     return tuple(np.full(n, -1, dtype=t) for t in (np.int32, np.int32, np.int64, np.int32, np.int32))
 
 
-def nearest_pattern_in_each(subsequences, sequences, *, substitutions_only=False):
+def _no_patterns_rows(n, flags):
+    anchored = flags & (_native.F_ANCHOR_START | _native.F_ANCHOR_END)
+    return NearestPatterns(_no_patterns(n), np.full(n, -1, dtype=np.int64) if anchored else None)
+
+
+def nearest_pattern_in_each(subsequences, sequences, *, substitutions_only=False, anchor=None):
     """Many patterns over many sequences, without a distance limit: -> NearestPatterns, for every sequence the
     pattern nearest to it, its distance and first end, and the runner-up among the other patterns -- what reducing
     ``nearest_distance_in_each(p, sequences)`` over the patterns gives (ties to the smallest index), in shared scans
@@ -365,17 +414,19 @@ def nearest_pattern_in_each(subsequences, sequences, *, substitutions_only=False
     empty sequence gives the shortest pattern (the smallest index among equals), its length and the end 0.
     `sequences` is a list / tuple (uploaded for this call) or a DeviceSequenceSet (resident).  With
     ``substitutions_only=True`` the same over ``nearest_distance_in_each(p, sequences, substitutions_only=True)``,
-    where a pattern longer than a sequence has no distance there (DESIGN.md section 5.16)."""
+    where a pattern longer than a sequence has no distance there (DESIGN.md section 5.16).  With ``anchor='start'``
+    or ``'end'`` the same over ``nearest_distance_in_each(p, sequences, ..., anchor=anchor)``, the winner's match
+    spanning ``[start, end)`` (DESIGN.md section 5.18): the barcode at a fixed end of a read."""
     subsequences = list(subsequences)
     if any(len(p) == 0 for p in subsequences):
         raise ValueError("Given subsequence is empty!")
-    flags = _native.F_SUBSTITUTIONS_ONLY if substitutions_only else 0
+    flags = _nearest_flags(substitutions_only, anchor)
     if isinstance(sequences, DeviceSequenceSet):
         return _nearest_patterns_in_set(subsequences, sequences, flags)
     if not isinstance(sequences, (list, tuple)):
         raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
     if not sequences or not subsequences:
-        return NearestPatterns(_no_patterns(len(sequences)))
+        return _no_patterns_rows(len(sequences), flags)
     seqset = DeviceSequenceSet(sequences)
     try:
         return _nearest_patterns_in_set(subsequences, seqset, flags)
@@ -386,7 +437,7 @@ def nearest_pattern_in_each(subsequences, sequences, *, substitutions_only=False
 def _nearest_patterns_in_set(subsequences, seqset, flags):
     n = len(seqset)
     if n == 0 or not subsequences:
-        return NearestPatterns(_no_patterns(n))
+        return _no_patterns_rows(n, flags)
     from .search import AlphabetTooLarge
     with seqset._lock:
         try:
@@ -395,23 +446,31 @@ def _nearest_patterns_in_set(subsequences, seqset, flags):
             pats = None  # no common byte alphabet: pattern by pattern, below
         if pats is not None:
             columns, _ = seqset._seq.haystack.nearest_best_per_record(pats, flags)
-            return NearestPatterns(columns)
-    return NearestPatterns(_nearest_patterns_on_host(subsequences, seqset, flags))
+            start, end = _anchored_span(seqset, flags, columns[0] >= 0, columns[2])
+            return NearestPatterns(columns[:2] + (end,) + columns[3:], start)
+    columns, start = _nearest_patterns_on_host(subsequences, seqset, flags)
+    return NearestPatterns(columns, start)
 
 
 def _nearest_patterns_on_host(subsequences, seqset, flags):
-    """The same rows from nearest_distance_in_each, pattern by pattern (each reduces the set to its own alphabet).
-    A pattern without a distance in a sequence (-1: substitutions only, longer than the sequence) is left out."""
+    """The same rows from nearest_distance_in_each, pattern by pattern (each reduces the set to its own alphabet),
+    and the winners' starts (None unanchored).  A pattern without a distance in a sequence (-1: substitutions only,
+    longer than the sequence) is left out."""
     pattern, dist, end, pat2, dist2 = columns = _no_patterns(len(seqset))
+    start = np.full(len(seqset), -1, dtype=np.int64)
+    anchor = "start" if flags & _native.F_ANCHOR_START else "end" if flags & _native.F_ANCHOR_END else None
     for i, p in enumerate(subsequences):
-        got = nearest_distance_in_each(p, seqset, substitutions_only=bool(flags & _native.F_SUBSTITUTIONS_ONLY))
+        got = nearest_distance_in_each(p, seqset, substitutions_only=bool(flags & _native.F_SUBSTITUTIONS_ONLY),
+                                       anchor=anchor)
         has = got.dist >= 0
         first = has & ((pattern < 0) | (got.dist < dist))  # (an equal distance leaves the earlier pattern in place)
         second = has & ~first & ((pat2 < 0) | (got.dist < dist2))
         pat2[first], dist2[first] = pattern[first], dist[first]
         pattern[first], dist[first], end[first] = i, got.dist[first], got.end[first]
+        if anchor is not None:
+            start[first] = got.start[first]
         pat2[second], dist2[second] = i, got.dist[second]
-    return columns
+    return columns, (start if anchor is not None else None)
 
 
 class Alignments(object):
@@ -443,7 +502,8 @@ def align_in_each(subsequences, sequences, rows, max_l_dist=None, *, max_substit
     * nearest_pattern_in_each / nearest_distance_in_each (one pattern): the rows give only the distance d and the end
       e; the alignment starts at the smallest s with ``lev(pattern, sequence[s:e]) == d`` -- the longest match at the
       nearest distance, found on the device from a window of at most ``len(pattern) + d`` symbols -- and its cost is
-      d.  Pass the same ``substitutions_only`` (then s = e - len(pattern)); no limits.
+      d.  Pass the same ``substitutions_only`` (then s = e - len(pattern)); no limits.  Anchored rows (``anchor=``)
+      carry their start: the window ``[start, end)`` is aligned as it is, at cost d.
 
     `sequences` is a list / tuple (uploaded for this call) or a DeviceSequenceSet (resident)."""
     from .search import _cigars, _normalised_limits
@@ -473,7 +533,8 @@ def align_in_each(subsequences, sequences, rows, max_l_dist=None, *, max_substit
             pattern = np.where(rows.dist >= 0, 0, -1).astype(np.int32)
         else:
             raise TypeError("rows must be a BestMatches, NearestPatterns or NearestDistances")
-        start, dist = np.full(n, -1, dtype=np.int64), rows.dist
+        start = np.full(n, -1, dtype=np.int64) if rows.start is None else np.asarray(rows.start, dtype=np.int64)
+        dist = rows.dist
         nearest = True
     if isinstance(sequences, DeviceSequenceSet):
         seqset, own = sequences, False

@@ -72,7 +72,13 @@ extern "C" {
                                  pattern i returns on that handle.  Refused on a handle without a record set */
 #define FZB_F_SUBSTITUTIONS_ONLY 256u /* the four fzb_nearest_* calls: the nearest match under substitutions only
                                  (Hamming distance of the pattern to a window of its own length) instead of
-                                 Levenshtein distance; the only flag they take (DESIGN.md section 5.16) */
+                                 Levenshtein distance (DESIGN.md section 5.16); the only flag they take besides
+                                 the anchors of fzb_nearest_per_record / fzb_nearest_best_per_record */
+#define FZB_F_ANCHOR_START 1024u /* fzb_nearest_per_record / fzb_nearest_best_per_record: only alignments that start
+                                 at the record's first symbol (the prefixes R[0:e]); the end array holds the
+                                 match's end (DESIGN.md section 5.18) */
+#define FZB_F_ANCHOR_END 2048u /* the same for alignments that end at the record's last symbol (the suffixes
+                                 R[s:n]); the end array holds the match's START.  Not with FZB_F_ANCHOR_START */
 
 struct fzb_stats_s;
 typedef struct fzb_haystack fzb_haystack; /* a device-resident sequence (or one shard of it) */
@@ -329,6 +335,18 @@ int fzb_nearest_distance(fzb_haystack *h, const uint8_t *pattern, uint32_t m, ui
  * bytes or more, any flag other than FZB_F_SUBSTITUTIONS_ONLY.  Every refusal and every error leaves the handle as it
  * was; the arrays then hold nothing meaningful.  With FZB_F_SUBSTITUTIONS_ONLY windows never cross a record's edges,
  * and a record shorter than m (an empty one included) gives (-1, -1).
+ *
+ * Anchored (DESIGN.md section 5.18), with one of FZB_F_ANCHOR_START / FZB_F_ANCHOR_END, alone or with
+ * FZB_F_SUBSTITUTIONS_ONLY, for a record R of n symbols:
+ *   FZB_F_ANCHOR_START  dist[r] = min over e of lev(P, R[0:e]), end[r] = the smallest e that reaches it (the match
+ *                       is R[0:end[r]]); an empty record gives (m, 0).  Substitutions only: the mismatches of P
+ *                       against R[0:m], end[r] = m.
+ *   FZB_F_ANCHOR_END    dist[r] = min over s of lev(P, R[s:n]), end[r] holds the START: the largest s that reaches
+ *                       it (the match is R[s:n]); an empty record gives (m, 0).  Substitutions only: against
+ *                       R[n-m:n], end[r] = n - m.
+ * Under substitutions only a record shorter than m gives (-1, -1).  A scan reads at most min(n, 2m) symbols of a
+ * record (m under substitutions only) and `stats` reports route 16 with bytes_scanned = the symbols read.  Both
+ * anchors together: FZB_E_INVALID.  Limits, refusals and handle behaviour as without an anchor.
  */
 int fzb_nearest_per_record(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
                            int32_t *dist, int64_t *end, /* each: one entry per record */
@@ -365,6 +383,11 @@ int fzb_nearest_distance_batch(fzb_haystack *h, const uint8_t *patterns, const u
  * handle in a world.  Every refusal and every error leaves the handle as it was; the calls use neither the handle's
  * counters, its output area nor a pending result.  `stats` (optional) reports route 12 (14 with
  * FZB_F_SUBSTITUTIONS_ONLY).
+ *
+ * fzb_nearest_best_per_record also takes one anchor flag, alone or with FZB_F_SUBSTITUTIONS_ONLY: d*_i(r) is then
+ * the anchored dist of fzb_nearest_per_record, end[r] the winner's end (FZB_F_ANCHOR_START) or start
+ * (FZB_F_ANCHOR_END) there, with the same reduction, ties and -1 rules; route 16.  fzb_nearest_distance_batch, like
+ * fzb_nearest_distance, refuses both anchor flags (FZB_E_UNSUPPORTED).
  */
 int fzb_nearest_best_per_record(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count,
                                 uint32_t flags, int32_t *pattern, int32_t *dist, int64_t *end, int32_t *second_pattern,
@@ -476,7 +499,8 @@ typedef struct fzb_stats_s {
                                8 hamming batch scan, 9 generic n-grams batch scan, 10 generic LP batch
                                scan, 11 nearest/bit-vector-scan,
                                12 nearest/batch-bit-vector-scan, 13 nearest/substitutions-scan,
-                               14 nearest/substitutions-batch-scan, 15 alignment (fzb_align) */
+                               14 nearest/substitutions-batch-scan, 15 alignment (fzb_align),
+                               16 nearest/anchored (FZB_F_ANCHOR_START / _END) */
 } fzb_stats;
 int fzb_result_stats(const fzb_result *r, fzb_stats *out);
 void fzb_result_destroy(fzb_result *r);
