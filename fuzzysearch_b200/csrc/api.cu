@@ -161,15 +161,15 @@ struct BestState {
     uint64_t *best, *top2;    // one word per record each
     const uint32_t *ordinal;  // pattern i of the batch being run is pattern ordinal[i] of the call
 };
-struct NearBufs {  // fzb_nearest_distance / fzb_nearest_per_record (nearest_kernels.cuh)
-    DevBuf<uint64_t> d_head;   // the whole-sequence result (2 words), then the partials of kNearMaxGrid CTAs
-    DevBuf<uint64_t> d_words;  // one word per record
-};
-struct NearBatchBufs {  // fzb_nearest_distance_batch / fzb_nearest_best_per_record (nearest_kernels.cuh)
-    DevBuf<uint32_t> d_lanes;  // m | ordinal << 16 per lane of every group
-    DevBuf<uint8_t> d_pats;    // kNearBatchMaxM bytes per lane
-    DevBuf<uint64_t> d_words;  // whole sequence: one word per pattern; record set: best[records], then top2[records]
-    DevBuf<uint64_t> d_aux;    // a long pattern's k_nearest_scan: the partials of kNearMaxGrid CTAs, its record words
+struct NearBufs {  // the nearest calls, single and batch (nearest_kernels.cuh)
+    DevBuf<uint32_t> d_lanes;  // batches: m | ordinal << 16 per lane of every group
+    DevBuf<uint8_t> d_pats;    // batches: kNearBatchMaxM bytes per lane
+    DevBuf<uint64_t> d_words;  // the answer: the whole-sequence result (2 words), one word per record or per pattern,
+                               // or best[records] then top2[records]
+    DevBuf<uint64_t> d_scan;   // the symbols read, the partials of kNearMaxGrid CTAs, then a long pattern's record words
+    uint64_t *steps() const { return d_scan.get(); }
+    uint64_t *partials() const { return d_scan.get() + 1; }
+    uint64_t *rec_words() const { return d_scan.get() + 1 + 2 * (uint64_t)kNearMaxGrid; }
 };
 struct GatherBufs {  // the staged NCCL all-gather
     uint32_t cap = 0;  // rows per rank
@@ -308,7 +308,6 @@ struct fzb_haystack {
     std::unique_ptr<RecBufs> recs;  // the record set, if any (cleared by every upload)
     std::unique_ptr<BestBufs> bestb;
     std::unique_ptr<NearBufs> nearb;
-    std::unique_ptr<NearBatchBufs> nearbatch;
 };
 
 struct fzb_result {
@@ -830,17 +829,14 @@ extern "C" int fzb_haystack_set_records(fzb_haystack *h, const uint64_t *offsets
 }
 
 // The record set the exact stages of a search on `h` take (null pointers without one) and its compile-time switch:
-// with_recs(h, f) calls f(std::true_type) on a handle with a record set, f(std::false_type) otherwise.
+// with_recs(h, f) returns f(std::true_type) on a handle with a record set, f(std::false_type) otherwise.
 static RecSet rec_set(const fzb_haystack *h) {
     return h->recs ? RecSet{h->recs->d_off.get(), h->recs->d_first.get()} : RecSet{nullptr, nullptr};
 }
 
 template <class F>
-static void with_recs(const fzb_haystack *h, F f) {
-    if (h->recs)
-        f(std::true_type{});
-    else
-        f(std::false_type{});
+static auto with_recs(const fzb_haystack *h, F f) {
+    return h->recs ? f(std::true_type{}) : f(std::false_type{});
 }
 
 // The entry points outside a record set's scope (batches, has_near_match, windows, FZB_F_GLOBAL) refuse to run on one.
@@ -3424,21 +3420,102 @@ extern "C" int fzb_best_per_record(fzb_haystack *h, const uint8_t *patterns, con
 }
 
 // ------------------------------------------------------------------------------------------------
-// fzb_nearest_distance / fzb_nearest_per_record (DESIGN.md section 5.14): the nearest match without a distance limit
+// The nearest match without a distance limit (nearest_kernels.cuh): fzb_nearest_distance / fzb_nearest_per_record
+// (DESIGN.md sections 5.14, 5.16, 5.18) and their batches fzb_nearest_distance_batch / fzb_nearest_best_per_record
+// (sections 5.15, 5.16, 5.18)
 // ------------------------------------------------------------------------------------------------
-template <int BITS, bool REC>
-static int launch_nearest(fzb_haystack *h, int grid, const NearParams &p, const RecSet &rs, bool ham) {
-    if (ham) {
-        CK(cudaFuncSetAttribute(k_nearest_hamming_scan<BITS, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)near_smem(BITS)));
-        k_nearest_hamming_scan<BITS, REC><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
-    } else {
-        CK(cudaFuncSetAttribute(k_nearest_scan<BITS, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)near_smem(BITS)));
-        k_nearest_scan<BITS, REC><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
+constexpr int64_t kNearBatchMinSeg = 1024;  // bytes per warp: the warm-up (at most 128 bytes) stays <= 1/8 of it
+
+// Gives the handle a nearest group of at least `lanes` batch lanes, `words` answer words and `rec_words` record words
+// of a long pattern, built whole beside the one it replaces; a grown group keeps every size of the one before.
+static int ensure_near_bufs(fzb_haystack *h, uint64_t lanes, uint64_t words, uint64_t rec_words) {
+    const NearBufs *g = h->nearb.get();
+    lanes = std::max<uint64_t>(lanes, 1);
+    words = std::max<uint64_t>(words, 2);
+    const uint64_t scan = 1 + 2 * (uint64_t)kNearMaxGrid + rec_words;
+    if (g && g->d_lanes.size() >= lanes && g->d_words.size() >= words && g->d_scan.size() >= scan) return FZB_OK;
+    std::unique_ptr<NearBufs> grown;
+    TRY(ensure_group(grown, [&](NearBufs &b) -> int {
+        const uint64_t nl = std::max<uint64_t>(lanes, g ? g->d_lanes.size() : 0);
+        TRY(b.d_lanes.alloc(nl));
+        TRY(b.d_pats.alloc(nl * kNearBatchMaxM));
+        TRY(b.d_words.alloc(std::max<uint64_t>(words, g ? g->d_words.size() : 0)));
+        return b.d_scan.alloc(std::max<uint64_t>(scan, g ? g->d_scan.size() : 0));
+    }));
+    h->nearb = std::move(grown);
+    return FZB_OK;
+}
+
+// f(std::integral_constant<int, BITS>{}) for a pattern's word width `bits`: 32 or 64, or with WIDE 128, 192 or 256
+template <bool WIDE, class F>
+static int with_bits(int bits, F f) {
+    if (bits == 32) return f(std::integral_constant<int, 32>{});
+    if constexpr (WIDE) {
+        if (bits == 128) return f(std::integral_constant<int, 128>{});
+        if (bits == 192) return f(std::integral_constant<int, 192>{});
+        if (bits == 256) return f(std::integral_constant<int, 256>{});
     }
+    return f(std::integral_constant<int, 64>{});
+}
+
+template <class F>
+static int with_bool(bool b, F f) {
+    return b ? f(std::true_type{}) : f(std::false_type{});
+}
+
+// A nearest kernel of word width `bits` on the handle's stream, its table in dynamic shared memory
+template <auto kernel, class P>
+static int near_launch(fzb_haystack *h, dim3 grid, int bits, const P &p) {
+    CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)near_smem(bits)));
+    kernel<<<grid, kNearThreads, near_smem(bits), h->stream>>>(p, rec_set(h));
     CK(cudaGetLastError());
     return FZB_OK;
+}
+
+// k_nearest_scan, k_nearest_hamming_scan under substitutions only; per record on a handle with a record set
+static int launch_near_scan(fzb_haystack *h, int bits, bool ham, int grid, const NearParams &p) {
+    return with_bits<true>(bits, [&](auto b) {
+        return with_recs(h, [&](auto r) {
+            constexpr int B = decltype(b)::value;
+            constexpr bool R = decltype(r)::value;
+            return ham ? near_launch<k_nearest_hamming_scan<B, R>>(h, grid, B, p)
+                       : near_launch<k_nearest_scan<B, R>>(h, grid, B, p);
+        });
+    });
+}
+
+// k_nearest_batch_scan, k_nearest_hamming_batch_scan under substitutions only; per record on a handle with a record set
+static int launch_near_batch_scan(fzb_haystack *h, int bits, bool ham, dim3 grid, const NearBatchParams &p) {
+    return with_bits<false>(bits, [&](auto b) {
+        return with_recs(h, [&](auto r) {
+            constexpr int B = decltype(b)::value;
+            constexpr bool R = decltype(r)::value;
+            return ham ? near_launch<k_nearest_hamming_batch_scan<B, R>>(h, grid, B, p)
+                       : near_launch<k_nearest_batch_scan<B, R>>(h, grid, B, p);
+        });
+    });
+}
+
+// k_nearest_anchored over all records, p.g lanes per record (a batch: one CTA row per group of `rows`)
+static int launch_near_anchored(fzb_haystack *h, int bits, bool ham, bool batch, uint32_t rows, const NearAnchParams &p) {
+    const uint64_t per = (uint64_t)(kNearThreads / 32) * (32 / p.g);  // records per CTA and round
+    const uint64_t gx = std::min<uint64_t>((p.nrec + per - 1) / per,
+                                           std::max<uint64_t>(1, (uint64_t)h->sm_count * near_ctas_per_sm(bits) / rows));
+    if (gx == 0) return FZB_OK;  // (no records)
+    return with_bool(batch, [&](auto t) {
+        constexpr bool T = decltype(t)::value;
+        return with_bits<!T>(bits, [&](auto b) {
+            return with_bool(ham, [&](auto x) {
+                constexpr int B = decltype(b)::value;
+                return near_launch<k_nearest_anchored<B, decltype(x)::value, T>>(h, dim3((unsigned)gx, rows), B, p);
+            });
+        });
+    });
+}
+
+// The grid of the kernels with one thread per record
+static int near_rec_grid(const fzb_haystack *h, uint64_t nrec) {
+    return (int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8);
 }
 
 // k_nearest_scan's segment (bytes per thread) and grid for the handle's buffer: segments long against the 2m warm-up
@@ -3447,74 +3524,81 @@ static int near_geometry(const fzb_haystack *h, int bits, int32_t *seg) {
     *seg = (int32_t)std::min<uint64_t>(kNearMaxSeg, std::max<uint64_t>(kNearMinSeg,
                                        round_up(h->buf_len / ((uint64_t)h->sm_count * 1024) + 1, 16)));
     const uint64_t tile = (uint64_t)kNearThreads * *seg, ntiles = (h->buf_len + tile - 1) / tile;
-    const int per_sm = bits == 32 ? 4 : bits == 64 ? 3 : 2;
-    return (int)std::min<uint64_t>(ntiles, std::min<uint64_t>((uint64_t)h->sm_count * per_sm, kNearMaxGrid));
+    return (int)std::min<uint64_t>(ntiles, std::min<uint64_t>((uint64_t)h->sm_count * near_ctas_per_sm(bits), kNearMaxGrid));
 }
 
-// The scan over the whole buffer, per record if `rec`, under substitutions only if `ham` (DESIGN.md section 5.16).
-// It keeps to its own buffer group: the counters, the output area and a pending result of the handle are not
-// touched.  On FZB_OK the answer is in nearb->d_head[0..1] or nearb->d_words, and the stream has drained.  Without a
-// value (substitutions only: no window) the words keep their prefill, all ones.
-static int ensure_near_bufs(fzb_haystack *h, uint64_t nrec) {
-    if (!h->nearb || h->nearb->d_words.size() < nrec) {  // built whole, beside the one it replaces
-        std::unique_ptr<NearBufs> grown;
-        TRY(ensure_group(grown, [&](NearBufs &b) -> int {
-            TRY(b.d_head.alloc(2 + 2 * (uint64_t)kNearMaxGrid));
-            return b.d_words.alloc(std::max<uint64_t>(nrec, 1));
-        }));
-        h->nearb = std::move(grown);
-    }
-    return FZB_OK;
-}
-
-static int nearest_scan(fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool rec, bool ham, fzb_stats *stats) {
-    CK(cudaSetDevice(h->device));
-    const uint64_t nrec = rec ? h->recs->d_off.size() - 1 : 0;
-    TRY(ensure_near_bufs(h, nrec));
+// Enqueues one pattern's unanchored scan of the whole buffer, under substitutions only if `ham`.  On a handle with a
+// record set every record's word (dist << 32 | end) lands in `words`, prefilled here; otherwise the minimum
+// (dist << 48 | first_end) in result[0], prefilled by the caller, and the CTAs' (minimum, count) in `partial`, *grid
+// of them.
+static int near_scan_enqueue(fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool ham, uint64_t *result,
+                             uint64_t *partial, uint64_t *words, fzb_stats &st, int *grid) {
     NearParams p{};
     p.H = h->d;
     p.N = (int64_t)h->buf_len;
     p.m = (int)m;
-    p.result = h->nearb->d_head.get();
-    p.partial = p.result + 2;
-    p.words = h->nearb->d_words.get();
+    p.result = result;
+    p.partial = partial;
+    p.words = words;
     memcpy(p.P, pattern, m);
     const int bits = m <= 32 ? 32 : (int)round_up(m, 64);
-    const int grid = near_geometry(h, bits, &p.seg);
-    fzb_stats st{};
-    st.route = ham ? 13 : 11;
-    st.bytes_scanned = h->buf_len;
-    CK(cudaEventRecord(h->ev[0], h->stream));
-    if (rec) {
-        k_nearest_fill<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
-            p.words, nrec, ham ? kBestEmpty : (uint64_t)m << 32);
-    } else {
-        k_nearest_fill<<<1, 32, 0, h->stream>>>(p.result, 1, ham ? kBestEmpty : (uint64_t)m << 48);
-        CK(cudaMemsetAsync(p.result + 1, 0, sizeof(uint64_t), h->stream));
-    }
-    CK(cudaGetLastError());
-    st.n_launches = 1;
-    if (grid > 0) {
-        const RecSet rs = rec_set(h);
-        int rc = FZB_OK;
-        with_recs(h, [&](auto r) {
-            constexpr bool R = decltype(r)::value;
-            rc = bits == 32    ? launch_nearest<32, R>(h, grid, p, rs, ham)
-                 : bits == 64  ? launch_nearest<64, R>(h, grid, p, rs, ham)
-                 : bits == 128 ? launch_nearest<128, R>(h, grid, p, rs, ham)
-                 : bits == 192 ? launch_nearest<192, R>(h, grid, p, rs, ham)
-                               : launch_nearest<256, R>(h, grid, p, rs, ham);
-        });
-        TRY(rc);
-        st.n_launches++;
-    }
-    CK(cudaEventRecord(h->ev[1], h->stream));
-    if (!rec) {
-        k_nearest_count<<<1, 256, 0, h->stream>>>(p.result, p.partial, (uint32_t)grid, ham ? ~0u : m);
+    *grid = near_geometry(h, bits, &p.seg);
+    if (h->recs) {
+        const uint64_t nrec = h->recs->d_off.size() - 1;
+        k_nearest_fill<<<near_rec_grid(h, nrec), 256, 0, h->stream>>>(words, nrec, ham ? kBestEmpty : (uint64_t)m << 32);
         CK(cudaGetLastError());
         st.n_launches++;
     }
+    if (*grid > 0) {
+        TRY(launch_near_scan(h, bits, ham, *grid, p));
+        st.n_launches++;
+        st.bytes_scanned += h->buf_len;
+    }
+    return FZB_OK;
+}
+
+// Enqueues one pattern's anchored scan of the records, one lane per record: every record's word dist << 32 | pos
+// (all ones: no value) is written to `words`, the symbols read are added to the group's step slot.  'end' walks the
+// records backwards with the reversed pattern, except under substitutions only, whose window is compared forwards.
+static int near_anchored_enqueue(fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool ham, bool end,
+                                 uint64_t *words, fzb_stats &st) {
+    NearAnchParams p{};
+    p.H = h->d;
+    p.nrec = h->recs->d_off.size() - 1;
+    p.words = words;
+    p.steps = h->nearb->steps();
+    p.m = (int32_t)m;
+    p.g = 1;
+    p.end = end;
+    for (uint32_t i = 0; i < m; i++) p.P[i] = pattern[end && !ham ? m - 1 - i : i];
+    TRY(launch_near_anchored(h, m <= 32 ? 32 : (int)round_up(m, 64), ham, false, 1, p));
+    st.n_launches++;
+    return FZB_OK;
+}
+
+// 'end': the pos of every record word with a value (a record's own word or a best key) turned into the start
+static int near_flip(fzb_haystack *h, uint64_t *words, fzb_stats &st) {
+    const uint64_t nrec = h->recs->d_off.size() - 1;
+    k_nearest_anchored_flip<<<near_rec_grid(h, nrec), 256, 0, h->stream>>>(words, nrec, rec_set(h));
+    CK(cudaGetLastError());
+    st.n_launches++;
+    return FZB_OK;
+}
+
+// The frame of every nearest call on the handle's stream: `scan` between events 0 and 1 (filter_ms), `tail` up to
+// event 2 (gpu_ms); with `steps` the symbols read, counted from zero in the group's step slot, become bytes_scanned.
+// The calls keep to their own buffer group: the counters, the output area and a pending result of the handle are not
+// touched.  On FZB_OK the stream has drained and *stats holds `st`.
+template <class Scan, class Tail>
+static int near_frame(fzb_haystack *h, bool steps, fzb_stats st, fzb_stats *stats, Scan scan, Tail tail) {
+    uint64_t *d_steps = h->nearb->steps();
+    CK(cudaEventRecord(h->ev[0], h->stream));
+    if (steps) CK(cudaMemsetAsync(d_steps, 0, sizeof(uint64_t), h->stream));
+    TRY(scan(st));
+    CK(cudaEventRecord(h->ev[1], h->stream));
+    TRY(tail(st));
     CK(cudaEventRecord(h->ev[2], h->stream));
+    if (steps) CK(cudaMemcpyAsync(&st.bytes_scanned, d_steps, sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     float ms = 0.f;
     CK(cudaEventElapsedTime(&ms, h->ev[0], h->ev[2]));
@@ -3525,196 +3609,49 @@ static int nearest_scan(fzb_haystack *h, const uint8_t *pattern, uint32_t m, boo
     return FZB_OK;
 }
 
-// ------------------------------------------------------------------------------------------------
-// Anchored nearest matches (DESIGN.md section 5.18): k_nearest_anchored over the records, for fzb_nearest_per_record
-// and fzb_nearest_best_per_record with FZB_F_ANCHOR_START / FZB_F_ANCHOR_END
-// ------------------------------------------------------------------------------------------------
-template <int BITS, bool HAM, bool BATCH>
-static int launch_anchored(fzb_haystack *h, dim3 grid, const NearAnchParams &p, const RecSet &rs) {
-    CK(cudaFuncSetAttribute(k_nearest_anchored<BITS, HAM, BATCH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                            (int)near_smem(BITS)));
-    k_nearest_anchored<BITS, HAM, BATCH><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
-    CK(cudaGetLastError());
-    return FZB_OK;
-}
-
-// k_nearest_anchored of `bits` (one lane per record unless BATCH) over all records, `rows` CTA rows (pattern groups)
-template <bool BATCH>
-static int launch_anchored_bits(fzb_haystack *h, int bits, bool ham, uint32_t rows, const NearAnchParams &p) {
-    const uint64_t per = (uint64_t)(kNearThreads / 32) * (32 / p.g);  // records per CTA and round
-    const int per_sm = bits == 32 ? 4 : bits == 64 ? 3 : 2;
-    const uint64_t gx = std::min<uint64_t>((p.nrec + per - 1) / per,
-                                           std::max<uint64_t>(1, (uint64_t)h->sm_count * per_sm / rows));
-    if (gx == 0) return FZB_OK;  // (no records)
-    const dim3 grid((unsigned)gx, rows);
-    const RecSet rs = rec_set(h);
-    if (BATCH)
-        return bits == 32 ? (ham ? launch_anchored<32, true, BATCH>(h, grid, p, rs) : launch_anchored<32, false, BATCH>(h, grid, p, rs))
-                          : (ham ? launch_anchored<64, true, BATCH>(h, grid, p, rs) : launch_anchored<64, false, BATCH>(h, grid, p, rs));
-    switch (bits) {
-    case 32: return ham ? launch_anchored<32, true, false>(h, grid, p, rs) : launch_anchored<32, false, false>(h, grid, p, rs);
-    case 64: return ham ? launch_anchored<64, true, false>(h, grid, p, rs) : launch_anchored<64, false, false>(h, grid, p, rs);
-    case 128: return ham ? launch_anchored<128, true, false>(h, grid, p, rs) : launch_anchored<128, false, false>(h, grid, p, rs);
-    case 192: return ham ? launch_anchored<192, true, false>(h, grid, p, rs) : launch_anchored<192, false, false>(h, grid, p, rs);
-    default: return ham ? launch_anchored<256, true, false>(h, grid, p, rs) : launch_anchored<256, false, false>(h, grid, p, rs);
-    }
-}
-
-// The parameters of one pattern's anchored scan (one lane per record): 'end' walks the records backwards with the
-// reversed pattern, except under substitutions only, whose window is compared forwards
-static NearAnchParams anchored_single(const fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool ham, bool end,
-                                      uint64_t *words, uint64_t *steps) {
-    NearAnchParams p{};
-    p.H = h->d;
-    p.nrec = h->recs->d_off.size() - 1;
-    p.words = words;
-    p.steps = steps;
-    p.m = (int32_t)m;
-    p.g = 1;
-    p.end = end;
-    for (uint32_t i = 0; i < m; i++) p.P[i] = pattern[end && !ham ? m - 1 - i : i];
-    return p;
-}
-
-static void anchored_flip(fzb_haystack *h, uint64_t *words, uint64_t nrec) {
-    k_nearest_anchored_flip<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
-        words, nrec, rec_set(h));
-}
-
-// fzb_nearest_per_record with an anchor: as nearest_scan (its buffer group only; on FZB_OK the answer is in
-// nearb->d_words and the stream has drained), the symbols read counted in nearb->d_head[0]
-static int nearest_anchored(fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool ham, bool end, fzb_stats *stats) {
+// One pattern over the whole buffer, per record on a handle with a record set, under substitutions only if `ham`
+// (DESIGN.md section 5.16), anchored at `anchor` (section 5.18).  On FZB_OK the group's words hold the answer: the
+// whole sequence's dist << 48 | first_end and n_ends, or one word dist << 32 | end per record (all ones: no value).
+static int nearest_single(fzb_haystack *h, const uint8_t *pattern, uint32_t m, bool ham, uint32_t anchor,
+                          fzb_stats *stats) {
     CK(cudaSetDevice(h->device));
-    const uint64_t nrec = h->recs->d_off.size() - 1;
-    TRY(ensure_near_bufs(h, nrec));
-    uint64_t *steps = h->nearb->d_head.get();
-    const NearAnchParams p = anchored_single(h, pattern, m, ham, end, h->nearb->d_words.get(), steps);
+    TRY(ensure_near_bufs(h, 0, h->recs ? h->recs->d_off.size() - 1 : 0, 0));
+    uint64_t *words = h->nearb->d_words.get(), *partial = h->nearb->partials();
+    const auto none = [](fzb_stats &) { return FZB_OK; };
     fzb_stats st{};
-    st.route = 16;
-    CK(cudaEventRecord(h->ev[0], h->stream));
-    CK(cudaMemsetAsync(steps, 0, sizeof(uint64_t), h->stream));
-    TRY(launch_anchored_bits<false>(h, m <= 32 ? 32 : (int)round_up(m, 64), ham, 1, p));
-    st.n_launches = 1;
-    if (end) {
-        anchored_flip(h, p.words, nrec);
+    if (anchor) {
+        st.route = 16;
+        return near_frame(h, true, st, stats, [&](fzb_stats &s) {
+            TRY(near_anchored_enqueue(h, pattern, m, ham, anchor == FZB_F_ANCHOR_END, words, s));
+            return anchor == FZB_F_ANCHOR_END ? near_flip(h, words, s) : FZB_OK;
+        }, none);
+    }
+    st.route = ham ? 13 : 11;
+    int grid = 0;
+    return near_frame(h, false, st, stats, [&](fzb_stats &s) {
+        if (!h->recs) {  // the end position 0 (substitutions only: no value), no end counted yet
+            k_nearest_fill<<<1, 32, 0, h->stream>>>(words, 1, ham ? kBestEmpty : (uint64_t)m << 48);
+            CK(cudaMemsetAsync(words + 1, 0, sizeof(uint64_t), h->stream));
+            CK(cudaGetLastError());
+            s.n_launches++;
+        }
+        return near_scan_enqueue(h, pattern, m, ham, words, partial, words, s, &grid);
+    }, [&](fzb_stats &s) {
+        if (h->recs) return FZB_OK;
+        k_nearest_count<<<1, 256, 0, h->stream>>>(words, partial, (uint32_t)grid, ham ? ~0u : m);
         CK(cudaGetLastError());
-        st.n_launches++;
-    }
-    CK(cudaEventRecord(h->ev[1], h->stream));
-    CK(cudaMemcpyAsync(&st.bytes_scanned, steps, sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
-    st.gpu_ms = st.filter_ms = ms;
-    if (stats) *stats = st;
-    return FZB_OK;
+        s.n_launches++;
+        return FZB_OK;
+    });
 }
 
-// The anchor of a flag word: 0, FZB_F_ANCHOR_START or FZB_F_ANCHOR_END; FZB_E_INVALID for both
-static int anchor_of(uint32_t flags, uint32_t *anchor) {
-    *anchor = flags & (FZB_F_ANCHOR_START | FZB_F_ANCHOR_END);
-    if (*anchor == (FZB_F_ANCHOR_START | FZB_F_ANCHOR_END))
-        return fail(FZB_E_INVALID, "FZB_F_ANCHOR_START and FZB_F_ANCHOR_END exclude each other");
-    return FZB_OK;
-}
-
-extern "C" int fzb_nearest_distance(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
-                                    uint32_t *dist, uint64_t *n_ends, uint64_t *first_end, fzb_stats *stats) {
-    HandleLock handle_lock(h);
-    if (!h || !dist || !n_ends || !first_end) return fail(FZB_E_INVALID, "NULL argument");
-    if (flags & ~FZB_F_SUBSTITUTIONS_ONLY)
-        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_distance takes no flag other than FZB_F_SUBSTITUTIONS_ONLY");
-    if (!is_whole_sequence(h) || h->comm || h->local_world || h->peer)
-        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_distance needs a whole (unsharded) sequence outside a world");
-    TRY(refuse_records(h, "fzb_nearest_distance"));
-    TRY(check_pattern(h, pattern, m, 0));
-    TRY(nearest_scan(h, pattern, m, false, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0, stats));
-    uint64_t out[2];
-    CK(cudaMemcpyAsync(out, h->nearb->d_head.get(), sizeof out, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    const bool none = out[0] == kBestEmpty;  // (substitutions only: the sequence is shorter than the pattern)
-    *dist = none ? UINT32_MAX : (uint32_t)(out[0] >> 48);
-    *first_end = none ? UINT64_MAX : out[0] & kNearNoEnd;
-    *n_ends = out[1];
-    return FZB_OK;
-}
-
-extern "C" int fzb_nearest_per_record(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
-                                      int32_t *dist, int64_t *end, fzb_stats *stats) {
-    HandleLock handle_lock(h);
-    if (!h || !dist || !end) return fail(FZB_E_INVALID, "NULL argument");
-    if (!h->recs) return fail(FZB_E_INVALID, "fzb_nearest_per_record needs a handle with a record set");
-    if (flags & ~(FZB_F_SUBSTITUTIONS_ONLY | FZB_F_ANCHOR_START | FZB_F_ANCHOR_END))
-        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_per_record takes no flag other than FZB_F_SUBSTITUTIONS_ONLY and "
-                                       "one anchor");
-    uint32_t anchor = 0;
-    TRY(anchor_of(flags, &anchor));
-    if (h->recs->longest > (1ull << 32))
-        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_per_record needs records shorter than 2^32");
-    TRY(check_pattern(h, pattern, m, 0));
-    const bool ham = (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0;
-    if (anchor)
-        TRY(nearest_anchored(h, pattern, m, ham, anchor == FZB_F_ANCHOR_END, stats));
-    else
-        TRY(nearest_scan(h, pattern, m, true, ham, stats));
-    // one read-back of 8 bytes per record
-    const uint64_t nrec = h->recs->d_off.size() - 1;
-    std::vector<uint64_t> words(nrec);
-    CK(cudaMemcpyAsync(words.data(), h->nearb->d_words.get(), nrec * sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    for (uint64_t r = 0; r < nrec; r++) {
-        const bool none = words[r] == kBestEmpty;  // (substitutions only: a record shorter than the pattern)
-        dist[r] = none ? -1 : (int32_t)(words[r] >> 32);
-        end[r] = none ? -1 : (int64_t)(words[r] & 0xFFFFFFFFull);
-    }
-    return FZB_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
-// fzb_nearest_distance_batch / fzb_nearest_best_per_record (DESIGN.md section 5.15): many patterns in shared scans
-// ------------------------------------------------------------------------------------------------
-constexpr int64_t kNearBatchMinSeg = 1024;  // bytes per warp: the warm-up (at most 128 bytes) stays <= 1/8 of it
-
-template <int BITS, bool REC>
-static int launch_nearest_batch(fzb_haystack *h, dim3 grid, const NearBatchParams &p, const RecSet &rs, bool ham) {
-    if (ham) {
-        CK(cudaFuncSetAttribute(k_nearest_hamming_batch_scan<BITS, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)near_smem(BITS)));
-        k_nearest_hamming_batch_scan<BITS, REC><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
-    } else {
-        CK(cudaFuncSetAttribute(k_nearest_batch_scan<BITS, REC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)near_smem(BITS)));
-        k_nearest_batch_scan<BITS, REC><<<grid, kNearThreads, near_smem(BITS), h->stream>>>(p, rs);
-    }
-    CK(cudaGetLastError());
-    return FZB_OK;
-}
-
-// Every pattern checked as its single search would take it (the caller checked the rest): FZB_OK or the refusal
-static int check_nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count,
-                               uint32_t flags, uint32_t anchors, const char *what) {
-    if (flags & ~(FZB_F_SUBSTITUTIONS_ONLY | anchors))
-        return fail(FZB_E_UNSUPPORTED, "%s takes no flag other than FZB_F_SUBSTITUTIONS_ONLY%s", what,
-                    anchors ? " and one anchor" : "");
-    uint32_t anchor = 0;
-    TRY(anchor_of(flags, &anchor));
-    if (count > kBestMaxPatterns) return fail(FZB_E_UNSUPPORTED, "more than %u patterns in one %s call", kBestMaxPatterns, what);
-    if (h->comm || h->local_world || h->peer) return fail(FZB_E_UNSUPPORTED, "%s: a handle in a world", what);
-    for (uint32_t i = 0; i < count; i++) {
-        if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
-        TRY(check_pattern(h, patterns + offsets[i], offsets[i + 1] - offsets[i], 0));
-    }
-    return FZB_OK;
-}
-
-// The scans of all `count` patterns over the whole buffer, per record if `rec`: the patterns of up to 64 symbols in
-// groups of 32 lanes (k_nearest_batch_scan, one launch per word class), longer ones one by one (k_nearest_scan, folded
-// by k_nearest_fold per record), under substitutions only if `ham`.  Its own buffer group only, as nearest_scan.  On
-// FZB_OK the answer is in nearbatch->d_words and the stream has drained.  `anchor` (record sets only): the same
-// groups and folds through k_nearest_anchored (DESIGN.md section 5.18), g lanes per record, the symbols read counted
-// in d_aux[0] (the partials are a whole sequence's).
-static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count, bool rec,
-                         bool ham, uint32_t anchor, fzb_stats *stats) {
+// The scans of all `count` patterns over the whole buffer, per record on a handle with a record set, under
+// substitutions only if `ham`: the patterns of up to 64 symbols in groups of 32 lanes (k_nearest_batch_scan, one launch
+// per word class), longer ones one by one (near_scan_enqueue, folded by k_nearest_fold per record).  `anchor` (record
+// sets only): the same groups and folds through k_nearest_anchored (DESIGN.md section 5.18), g lanes per record.  On
+// FZB_OK the group's words hold the answer: one word per pattern, or best[records] then top2[records].
+static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_t *offsets, uint32_t count, bool ham,
+                         uint32_t anchor, fzb_stats *stats) {
     const bool end = anchor == FZB_F_ANCHOR_END, rev = end && !ham;  // rev: 'end' walks back with reversed patterns
     auto len = [&](uint32_t i) { return offsets[i + 1] - offsets[i]; };
     // by (class, m): the lanes of a group share the warm-up of its longest pattern
@@ -3739,156 +3676,162 @@ static int nearest_batch(fzb_haystack *h, const uint8_t *patterns, const uint32_
             pats[l * kNearBatchMaxM + i] = patterns[offsets[lanes[l] >> 16] + (rev ? m - 1 - i : i)];
 
     CK(cudaSetDevice(h->device));
-    const uint64_t nrec = rec ? h->recs->d_off.size() - 1 : 0;
-    const uint64_t need_lanes = std::max<uint64_t>(lanes.size(), 1), need_words = std::max<uint64_t>(rec ? 2 * nrec : count, 1);
-    const uint64_t need_aux = 2 * (uint64_t)kNearMaxGrid + (rec && !longs.empty() ? nrec : 0);
-    NearBatchBufs *g = h->nearbatch.get();
-    if (!g || g->d_lanes.size() < need_lanes || g->d_words.size() < need_words || g->d_aux.size() < need_aux) {
-        std::unique_ptr<NearBatchBufs> grown;  // built whole, beside the one it replaces
-        TRY(ensure_group(grown, [&](NearBatchBufs &b) -> int {
-            const uint64_t nl = std::max<uint64_t>(need_lanes, g ? g->d_lanes.size() : 0);
-            TRY(b.d_lanes.alloc(nl));
-            TRY(b.d_pats.alloc(nl * kNearBatchMaxM));
-            TRY(b.d_words.alloc(std::max<uint64_t>(need_words, g ? g->d_words.size() : 0)));
-            return b.d_aux.alloc(std::max<uint64_t>(need_aux, g ? g->d_aux.size() : 0));
-        }));
-        h->nearbatch = std::move(grown);
-        g = h->nearbatch.get();
-    }
+    const uint64_t nrec = h->recs ? h->recs->d_off.size() - 1 : 0;
+    TRY(ensure_near_bufs(h, lanes.size(), h->recs ? 2 * nrec : count, longs.empty() ? 0 : nrec));
+    const NearBufs *g = h->nearb.get();
     uint64_t *best = g->d_words.get(), *top2 = best + nrec;
     fzb_stats st{};
     st.route = anchor ? 16 : ham ? 14 : 12;
-    uint64_t *steps = g->d_aux.get();
-    CK(cudaEventRecord(h->ev[0], h->stream));
-    if (anchor) CK(cudaMemsetAsync(steps, 0, sizeof(uint64_t), h->stream));
-    if (!lanes.empty()) {
-        CK(cudaMemcpyAsync(g->d_lanes.get(), lanes.data(), lanes.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(g->d_pats.get(), pats.data(), pats.size(), cudaMemcpyHostToDevice, h->stream));
-    }
-    if (rec) {  // the constants of nearest_kernels.cuh: (min m, its ordinal, end 0) and the two smallest (m_i, i);
-                // nothing under substitutions only, where no pattern has a value before its first window
-        uint64_t key = kBestEmpty, pair2 = kBestEmpty;
-        for (uint32_t i = 0; i < count && !ham; i++) {
-            key = std::min<uint64_t>(key, (uint64_t)len(i) << 48 | (uint64_t)i << 32);
-            pair2 = best_top2_merge(pair2, len(i) << 16 | i);
+    return near_frame(h, anchor != 0, st, stats, [&](fzb_stats &st) {
+        if (!lanes.empty()) {
+            CK(cudaMemcpyAsync(g->d_lanes.get(), lanes.data(), lanes.size() * sizeof(uint32_t), cudaMemcpyHostToDevice,
+                               h->stream));
+            CK(cudaMemcpyAsync(g->d_pats.get(), pats.data(), pats.size(), cudaMemcpyHostToDevice, h->stream));
         }
-        const int fill_grid = (int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8);
-        k_nearest_fill<<<fill_grid, 256, 0, h->stream>>>(best, nrec, key);
-        k_nearest_fill<<<fill_grid, 256, 0, h->stream>>>(top2, nrec, pair2);
-        st.n_launches += 2;
-    } else {  // every pattern's end position 0 (substitutions only: no value)
-        std::vector<uint64_t> init(count);
-        for (uint32_t i = 0; i < count; i++) init[i] = ham ? kBestEmpty : (uint64_t)len(i) << 48;
-        CK(cudaMemcpyAsync(best, init.data(), count * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
-        CK(cudaStreamSynchronize(h->stream));  // (`init` is a pageable local)
-    }
-    CK(cudaGetLastError());
-    const RecSet rs = rec_set(h);
-    uint32_t lane0 = 0;
-    for (int cls = 0; cls < 2; cls++) {
-        if (!groups[cls]) continue;
-        if (anchor) {  // g: the class's pattern count rounded up to a power of two, at most 32
-            const uint32_t n_cls = (uint32_t)std::count_if(order.begin(), order.end(),
-                                                           [&](uint32_t i) { return (len(i) > 32) == (cls == 1); });
-            NearAnchParams p{};
+        if (h->recs) {  // the constants of nearest_kernels.cuh: (min m, its ordinal, end 0) and the two smallest
+                        // (m_i, i); nothing under substitutions only, where no pattern has a value before its first window
+            uint64_t key = kBestEmpty, pair2 = kBestEmpty;
+            for (uint32_t i = 0; i < count && !ham; i++) {
+                key = std::min<uint64_t>(key, (uint64_t)len(i) << 48 | (uint64_t)i << 32);
+                pair2 = best_top2_merge(pair2, len(i) << 16 | i);
+            }
+            k_nearest_fill<<<near_rec_grid(h, nrec), 256, 0, h->stream>>>(best, nrec, key);
+            k_nearest_fill<<<near_rec_grid(h, nrec), 256, 0, h->stream>>>(top2, nrec, pair2);
+            st.n_launches += 2;
+        } else {  // every pattern's end position 0 (substitutions only: no value)
+            std::vector<uint64_t> init(count);
+            for (uint32_t i = 0; i < count; i++) init[i] = ham ? kBestEmpty : (uint64_t)len(i) << 48;
+            CK(cudaMemcpyAsync(best, init.data(), count * sizeof(uint64_t), cudaMemcpyHostToDevice, h->stream));
+            CK(cudaStreamSynchronize(h->stream));  // (`init` is a pageable local)
+        }
+        CK(cudaGetLastError());
+        uint32_t lane0 = 0;
+        for (int cls = 0; cls < 2; cls++) {
+            if (!groups[cls]) continue;
+            const int bits = cls ? 64 : 32;
+            const uint32_t *cls_lanes = g->d_lanes.get() + lane0;
+            const uint8_t *cls_pats = g->d_pats.get() + (uint64_t)lane0 * kNearBatchMaxM;
+            lane0 += groups[cls] * kNearBatchLanes;
+            if (anchor) {  // g: the class's pattern count rounded up to a power of two, at most 32
+                const uint32_t n_cls = (uint32_t)std::count_if(order.begin(), order.end(),
+                                                               [&](uint32_t i) { return (len(i) > 32) == (cls == 1); });
+                NearAnchParams p{};
+                p.H = h->d;
+                p.nrec = nrec;
+                p.lanes = cls_lanes;
+                p.pats = cls_pats;
+                p.best = best;
+                p.top2 = top2;
+                p.steps = g->steps();
+                p.end = end;
+                for (p.g = 1; p.g < (int32_t)std::min<uint32_t>(n_cls, kNearBatchLanes); p.g *= 2) {}
+                TRY(launch_near_anchored(h, bits, ham, true, groups[cls], p));
+                st.n_launches++;
+                continue;
+            }
+            // one wave of CTAs over all groups, one segment per warp: long segments (a small warm-up share) on a long
+            // sequence, at least kNearBatchMinSeg on a short one
+            uint64_t gx = std::max<uint64_t>(1, (uint64_t)h->sm_count * near_ctas_per_sm(bits) / groups[cls]);
+            const uint64_t warps = gx * (kNearThreads / 32);
+            NearBatchParams p{};
             p.H = h->d;
-            p.nrec = nrec;
-            p.lanes = g->d_lanes.get() + lane0;
-            p.pats = g->d_pats.get() + (uint64_t)lane0 * kNearBatchMaxM;
+            p.N = (int64_t)h->buf_len;
+            p.seg = (int64_t)std::max<uint64_t>(kNearBatchMinSeg, round_up((h->buf_len + warps - 1) / warps, 16));
+            gx = std::min<uint64_t>(gx, (h->buf_len + (kNearThreads / 32) * p.seg - 1) / ((kNearThreads / 32) * p.seg));
+            p.lanes = cls_lanes;
+            p.pats = cls_pats;
+            p.whole = best;
             p.best = best;
             p.top2 = top2;
-            p.steps = steps;
-            p.end = end;
-            for (p.g = 1; p.g < (int32_t)std::min<uint32_t>(n_cls, kNearBatchLanes); p.g *= 2) {}
-            lane0 += groups[cls] * kNearBatchLanes;
-            TRY(launch_anchored_bits<true>(h, cls ? 64 : 32, ham, groups[cls], p));
-            st.n_launches++;
-            continue;
-        }
-        const int per_sm = cls ? 3 : 4;
-        // one wave of CTAs over all groups, one segment per warp: long segments (a small warm-up share) on a long
-        // sequence, at least kNearBatchMinSeg on a short one
-        uint64_t gx = std::max<uint64_t>(1, (uint64_t)h->sm_count * per_sm / groups[cls]);
-        const uint64_t warps = gx * (kNearThreads / 32);
-        NearBatchParams p{};
-        p.H = h->d;
-        p.N = (int64_t)h->buf_len;
-        p.seg = (int64_t)std::max<uint64_t>(kNearBatchMinSeg, round_up((h->buf_len + warps - 1) / warps, 16));
-        gx = std::min<uint64_t>(gx, (h->buf_len + (kNearThreads / 32) * p.seg - 1) / ((kNearThreads / 32) * p.seg));
-        p.lanes = g->d_lanes.get() + lane0;
-        p.pats = g->d_pats.get() + (uint64_t)lane0 * kNearBatchMaxM;
-        p.whole = best;
-        p.best = best;
-        p.top2 = top2;
-        lane0 += groups[cls] * kNearBatchLanes;
-        if (gx == 0) continue;  // (an empty buffer)
-        const dim3 grid((unsigned)gx, groups[cls]);
-        int rc = FZB_OK;
-        with_recs(h, [&](auto r) {
-            constexpr bool R = decltype(r)::value;
-            rc = cls ? launch_nearest_batch<64, R>(h, grid, p, rs, ham) : launch_nearest_batch<32, R>(h, grid, p, rs, ham);
-        });
-        TRY(rc);
-        st.n_launches++;
-        st.bytes_scanned += h->buf_len;
-    }
-    for (uint32_t i : longs) {  // 65-255 symbols: the single scan, pattern by pattern
-        const uint32_t m = len(i);
-        NearParams q{};
-        q.H = h->d;
-        q.N = (int64_t)h->buf_len;
-        q.m = (int)m;
-        q.result = best + i;  // (whole sequence: the pattern's word, prefilled)
-        q.partial = g->d_aux.get();
-        q.words = g->d_aux.get() + 2 * (uint64_t)kNearMaxGrid;
-        memcpy(q.P, patterns + offsets[i], m);
-        const int bits = (int)round_up(m, 64);
-        if (anchor) {  // every record's word written (no prefill), then folded as below
-            TRY(launch_anchored_bits<false>(h, bits, ham, 1, anchored_single(h, patterns + offsets[i], m, ham, end, q.words, steps)));
-            k_nearest_fold<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
-                q.words, nrec, ham ? m + 1 : m, i, best, top2);
-            CK(cudaGetLastError());
-            st.n_launches += 2;
-            continue;
-        }
-        const int grid = near_geometry(h, bits, &q.seg);
-        if (rec) {
-            k_nearest_fill<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
-                q.words, nrec, ham ? kBestEmpty : (uint64_t)m << 32);
-            CK(cudaGetLastError());
-            st.n_launches++;
-        }
-        if (grid > 0) {
-            int rc = FZB_OK;
-            with_recs(h, [&](auto r) {
-                constexpr bool R = decltype(r)::value;
-                rc = bits == 128   ? launch_nearest<128, R>(h, grid, q, rs, ham)
-                     : bits == 192 ? launch_nearest<192, R>(h, grid, q, rs, ham)
-                                   : launch_nearest<256, R>(h, grid, q, rs, ham);
-            });
-            TRY(rc);
+            if (gx == 0) continue;  // (an empty buffer)
+            TRY(launch_near_batch_scan(h, bits, ham, dim3((unsigned)gx, groups[cls]), p));
             st.n_launches++;
             st.bytes_scanned += h->buf_len;
         }
-        if (rec) {
-            k_nearest_fold<<<(int)std::min<uint64_t>((nrec + 255) / 256, (uint64_t)h->sm_count * 8), 256, 0, h->stream>>>(
-                q.words, nrec, ham ? m + 1 : m, i, best, top2);
-            CK(cudaGetLastError());
-            st.n_launches++;
+        for (uint32_t i : longs) {  // 65-255 symbols: the single scan, pattern by pattern, folded per record
+            const uint32_t m = len(i);
+            int grid = 0;
+            if (anchor)
+                TRY(near_anchored_enqueue(h, patterns + offsets[i], m, ham, end, g->rec_words(), st));
+            else  // (whole sequence: into the pattern's word, prefilled)
+                TRY(near_scan_enqueue(h, patterns + offsets[i], m, ham, best + i, g->partials(), g->rec_words(), st, &grid));
+            if (h->recs) {
+                k_nearest_fold<<<near_rec_grid(h, nrec), 256, 0, h->stream>>>(g->rec_words(), nrec, ham ? m + 1 : m, i,
+                                                                             best, top2);
+                CK(cudaGetLastError());
+                st.n_launches++;
+            }
         }
+        return end ? near_flip(h, best, st) : FZB_OK;  // (the winners' ends in the mirrored records -> their starts)
+    }, [](fzb_stats &) { return FZB_OK; });
+}
+
+// The refusals of a nearest call, in the order that decides its code: `what` names the call; it takes
+// FZB_F_SUBSTITUTIONS_ONLY and the flags of `anchors`, needs a record set if `per_record` (and refuses one
+// otherwise), and a whole (unsharded) sequence outside a world if `whole`.  A batch's `count` patterns are checked
+// before the record set; a single search checks its one pattern after this call.
+static int check_nearest(const fzb_haystack *h, const char *what, uint32_t flags, uint32_t anchors, bool per_record,
+                         bool whole, const uint8_t *patterns = nullptr, const uint32_t *offsets = nullptr,
+                         uint32_t count = 0) {
+    if (per_record && !h->recs) return fail(FZB_E_INVALID, "%s needs a handle with a record set", what);
+    if (flags & ~(FZB_F_SUBSTITUTIONS_ONLY | anchors))
+        return fail(FZB_E_UNSUPPORTED, "%s takes no flag other than FZB_F_SUBSTITUTIONS_ONLY%s", what,
+                    anchors ? " and one anchor" : "");
+    if ((flags & anchors) == (FZB_F_ANCHOR_START | FZB_F_ANCHOR_END))
+        return fail(FZB_E_INVALID, "FZB_F_ANCHOR_START and FZB_F_ANCHOR_END exclude each other");
+    if (whole && (!is_whole_sequence(h) || h->comm || h->local_world || h->peer))
+        return fail(FZB_E_UNSUPPORTED, "%s needs a whole (unsharded) sequence outside a world", what);
+    if (count > kBestMaxPatterns) return fail(FZB_E_UNSUPPORTED, "more than %u patterns in one %s call", kBestMaxPatterns, what);
+    for (uint32_t i = 0; i < count; i++) {
+        if (offsets[i + 1] < offsets[i]) return fail(FZB_E_INVALID, "offsets must be non-decreasing");
+        TRY(check_pattern(h, patterns + offsets[i], offsets[i + 1] - offsets[i], 0));
     }
-    if (end) {  // the winners' ends in the mirrored records -> their starts
-        anchored_flip(h, best, nrec);
-        CK(cudaGetLastError());
-        st.n_launches++;
-    }
-    CK(cudaEventRecord(h->ev[1], h->stream));
-    if (anchor) CK(cudaMemcpyAsync(&st.bytes_scanned, steps, sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
+    if (!per_record) return refuse_records(h, what);
+    if (h->recs->longest > (1ull << 32)) return fail(FZB_E_UNSUPPORTED, "%s needs records shorter than 2^32", what);
+    return FZB_OK;
+}
+
+// The first n answer words of the call that just ran
+static int near_read(fzb_haystack *h, std::vector<uint64_t> &words, uint64_t n) {
+    words.resize(n);
+    CK(cudaMemcpyAsync(words.data(), h->nearb->d_words.get(), n * sizeof(uint64_t), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, h->ev[0], h->ev[1]));
-    st.gpu_ms = st.filter_ms = ms;
-    if (stats) *stats = st;
+    return FZB_OK;
+}
+
+extern "C" int fzb_nearest_distance(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
+                                    uint32_t *dist, uint64_t *n_ends, uint64_t *first_end, fzb_stats *stats) {
+    HandleLock handle_lock(h);
+    if (!h || !dist || !n_ends || !first_end) return fail(FZB_E_INVALID, "NULL argument");
+    TRY(check_nearest(h, "fzb_nearest_distance", flags, 0, false, true));
+    TRY(check_pattern(h, pattern, m, 0));
+    TRY(nearest_single(h, pattern, m, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0, 0, stats));
+    std::vector<uint64_t> out;
+    TRY(near_read(h, out, 2));
+    const bool none = out[0] == kBestEmpty;  // (substitutions only: the sequence is shorter than the pattern)
+    *dist = none ? UINT32_MAX : (uint32_t)(out[0] >> 48);
+    *first_end = none ? UINT64_MAX : out[0] & kNearNoEnd;
+    *n_ends = out[1];
+    return FZB_OK;
+}
+
+extern "C" int fzb_nearest_per_record(fzb_haystack *h, const uint8_t *pattern, uint32_t m, uint32_t flags,
+                                      int32_t *dist, int64_t *end, fzb_stats *stats) {
+    HandleLock handle_lock(h);
+    if (!h || !dist || !end) return fail(FZB_E_INVALID, "NULL argument");
+    TRY(check_nearest(h, "fzb_nearest_per_record", flags, FZB_F_ANCHOR_START | FZB_F_ANCHOR_END, true, false));
+    TRY(check_pattern(h, pattern, m, 0));
+    TRY(nearest_single(h, pattern, m, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0,
+                       flags & (FZB_F_ANCHOR_START | FZB_F_ANCHOR_END), stats));
+    // one read-back of 8 bytes per record
+    const uint64_t nrec = h->recs->d_off.size() - 1;
+    std::vector<uint64_t> words;
+    TRY(near_read(h, words, nrec));
+    for (uint64_t r = 0; r < nrec; r++) {
+        const bool none = words[r] == kBestEmpty;  // (substitutions only: a record shorter than the pattern)
+        dist[r] = none ? -1 : (int32_t)(words[r] >> 32);
+        end[r] = none ? -1 : (int64_t)(words[r] & 0xFFFFFFFFull);
+    }
     return FZB_OK;
 }
 
@@ -3897,18 +3840,13 @@ extern "C" int fzb_nearest_distance_batch(fzb_haystack *h, const uint8_t *patter
                                           fzb_stats *stats) {
     HandleLock handle_lock(h);
     if (!h || (count && (!patterns || !offsets || !dist || !first_end))) return fail(FZB_E_INVALID, "NULL argument");
-    if (!is_whole_sequence(h))
-        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_distance_batch needs a whole (unsharded) sequence outside a world");
-    TRY(check_nearest_batch(h, patterns, offsets, count, flags, 0, "fzb_nearest_distance_batch"));
-    TRY(refuse_records(h, "fzb_nearest_distance_batch"));
+    TRY(check_nearest(h, "fzb_nearest_distance_batch", flags, 0, false, true, patterns, offsets, count));
     if (stats) *stats = fzb_stats{};
     if (count == 0) return FZB_OK;
-    TRY(nearest_batch(h, patterns, offsets, count, false, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0, 0, stats));
+    TRY(nearest_batch(h, patterns, offsets, count, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0, 0, stats));
     // one read-back of 8 bytes per pattern
-    std::vector<uint64_t> words(count);
-    CK(cudaMemcpyAsync(words.data(), h->nearbatch->d_words.get(), count * sizeof(uint64_t), cudaMemcpyDeviceToHost,
-                       h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    std::vector<uint64_t> words;
+    TRY(near_read(h, words, count));
     for (uint32_t i = 0; i < count; i++) {
         const bool none = words[i] == kBestEmpty;  // (substitutions only: a pattern longer than the sequence)
         dist[i] = none ? UINT32_MAX : (uint32_t)(words[i] >> 48);
@@ -3924,11 +3862,8 @@ extern "C" int fzb_nearest_best_per_record(fzb_haystack *h, const uint8_t *patte
     HandleLock handle_lock(h);
     if (!h || !pattern || !dist || !end || !second_pattern || !second_dist || (count && (!patterns || !offsets)))
         return fail(FZB_E_INVALID, "NULL argument");
-    if (!h->recs) return fail(FZB_E_INVALID, "fzb_nearest_best_per_record needs a handle with a record set");
-    TRY(check_nearest_batch(h, patterns, offsets, count, flags, FZB_F_ANCHOR_START | FZB_F_ANCHOR_END,
-                            "fzb_nearest_best_per_record"));
-    if (h->recs->longest > (1ull << 32))
-        return fail(FZB_E_UNSUPPORTED, "fzb_nearest_best_per_record needs records shorter than 2^32");
+    TRY(check_nearest(h, "fzb_nearest_best_per_record", flags, FZB_F_ANCHOR_START | FZB_F_ANCHOR_END, true, true,
+                      patterns, offsets, count));
     const uint64_t nrec = h->recs->d_off.size() - 1;
     if (stats) *stats = fzb_stats{};
     if (count == 0) {
@@ -3938,13 +3873,11 @@ extern "C" int fzb_nearest_best_per_record(fzb_haystack *h, const uint8_t *patte
         }
         return FZB_OK;
     }
-    TRY(nearest_batch(h, patterns, offsets, count, true, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0,
+    TRY(nearest_batch(h, patterns, offsets, count, (flags & FZB_F_SUBSTITUTIONS_ONLY) != 0,
                       flags & (FZB_F_ANCHOR_START | FZB_F_ANCHOR_END), stats));
     // one read-back of 16 bytes per record
-    std::vector<uint64_t> words(2 * nrec);
-    CK(cudaMemcpyAsync(words.data(), h->nearbatch->d_words.get(), 2 * nrec * sizeof(uint64_t), cudaMemcpyDeviceToHost,
-                       h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    std::vector<uint64_t> words;
+    TRY(near_read(h, words, 2 * nrec));
     for (uint64_t r = 0; r < nrec; r++) {
         const uint64_t b = words[r];
         const uint32_t second = (uint32_t)words[nrec + r] & kBestPairNone;

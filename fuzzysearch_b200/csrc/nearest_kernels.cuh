@@ -51,6 +51,8 @@ template <int BITS> struct NearWord { typedef uint64_t type; };
 template <> struct NearWord<32> { typedef uint32_t type; };
 
 __host__ __device__ constexpr int near_words(int bits) { return bits <= 64 ? 1 : bits / 64; }
+// resident CTAs per SM of a nearest kernel of word width `bits`: its __launch_bounds__ and the host's grids
+__host__ __device__ constexpr int near_ctas_per_sm(int bits) { return bits == 32 ? 4 : bits == 64 ? 3 : 2; }
 __host__ __device__ constexpr size_t near_smem(int bits) { return bits <= 64 ? (size_t)256 * 32 * (bits / 8) : (size_t)256 * (bits / 8); }
 
 __global__ void k_nearest_fill(uint64_t *words, uint64_t n, uint64_t value) {
@@ -134,19 +136,6 @@ struct NearCol {  // one column of the table and what the thread has seen of its
             }
         }
     }
-
-    // text bytes [x, end); rel: the end position behind H[x], relative to the caller's base
-    template <bool TRACK>
-    __device__ __forceinline__ void run(const uint8_t *H, int64_t x, int64_t end, uint32_t rel) {
-        for (; x < end && (x & 15); x++) step<TRACK>(H[x], rel++);
-        for (; x + 16 <= end; x += 16) {
-            const uint4 v = __ldg(reinterpret_cast<const uint4 *>(H + x));
-            const uint32_t q[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int j = 0; j < 16; j++) step<TRACK>((q[j >> 2] >> (8 * (j & 3))) & 0xFFu, rel++);
-        }
-        for (; x < end; x++) step<TRACK>(H[x], rel++);
-    }
 };
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -222,20 +211,21 @@ struct HamCol {
             }
         }
     }
-
-    // text bytes [x, end); rel: the end position behind H[x], relative to the caller's base
-    template <bool TRACK>
-    __device__ __forceinline__ void run(const uint8_t *H, int64_t x, int64_t end, uint32_t rel) {
-        for (; x < end && (x & 15); x++) step<TRACK>(H[x], rel++);
-        for (; x + 16 <= end; x += 16) {
-            const uint4 v = __ldg(reinterpret_cast<const uint4 *>(H + x));
-            const uint32_t q[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int j = 0; j < 16; j++) step<TRACK>((q[j >> 2] >> (8 * (j & 3))) & 0xFFu, rel++);
-        }
-        for (; x < end; x++) step<TRACK>(H[x], rel++);
-    }
 };
+
+// A column (NearCol or HamCol) over the text bytes [x, end); rel: the end position behind H[x], relative to the
+// caller's base
+template <bool TRACK, class Col>
+__device__ __forceinline__ void near_run(Col &col, const uint8_t *H, int64_t x, int64_t end, uint32_t rel) {
+    for (; x < end && (x & 15); x++) col.template step<TRACK>(H[x], rel++);
+    for (; x + 16 <= end; x += 16) {
+        const uint4 v = __ldg(reinterpret_cast<const uint4 *>(H + x));
+        const uint32_t q[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int j = 0; j < 16; j++) col.template step<TRACK>((q[j >> 2] >> (8 * (j & 3))) & 0xFFu, rel++);
+    }
+    for (; x < end; x++) col.template step<TRACK>(H[x], rel++);
+}
 
 template <class Col, bool REC>
 __device__ __forceinline__ void near_scan(NearParams p, RecSet rs) {
@@ -288,16 +278,16 @@ __device__ __forceinline__ void near_scan(NearParams p, RecSet rs) {
         }
         col.reset(m);
         const int64_t w = a - Col::warm(m) > lo ? a - Col::warm(m) : lo;
-        col.template run<false>(p.H, w, a, 0);
+        near_run<false>(col, p.H, w, a, 0);
         if (!REC) {
-            col.template run<true>(p.H, a, b, 1);
+            near_run<true>(col, p.H, a, b, 1);
             near_merge(tbest, tcnt, tfirst, col.best, col.cnt,
                        Col::has(col.best, m) ? (uint64_t)a + col.first : kNearNoEnd);
         } else {
             int64_t x = a;
             for (;;) {
                 const int64_t stop = b < hi ? b : hi;
-                if (x < stop) col.template run<true>(p.H, x, stop, (uint32_t)(x + 1 - lo));
+                if (x < stop) near_run<true>(col, p.H, x, stop, (uint32_t)(x + 1 - lo));
                 if (Col::has(col.best, m))
                     atomicMin((unsigned long long *)&p.words[r], (unsigned long long)col.best << 32 | col.first);
                 if (hi + 1 >= b) break;  // (the record behind the separator starts in another segment, or nowhere)
@@ -332,13 +322,13 @@ __device__ __forceinline__ void near_scan(NearParams p, RecSet rs) {
 }
 
 template <int BITS, bool REC>
-__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : BITS == 64 ? 3 : 2)
+__global__ void __launch_bounds__(kNearThreads, near_ctas_per_sm(BITS))
 k_nearest_scan(NearParams p, RecSet rs) {
     near_scan<NearCol<BITS>, REC>(p, rs);
 }
 
 template <int BITS, bool REC>
-__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : BITS == 64 ? 3 : 2)
+__global__ void __launch_bounds__(kNearThreads, near_ctas_per_sm(BITS))
 k_nearest_hamming_scan(NearParams p, RecSet rs) {
     near_scan<HamCol<BITS>, REC>(p, rs);
 }
@@ -487,9 +477,9 @@ __device__ __forceinline__ void near_batch_scan(NearBatchParams p, RecSet rs) {
         }
         col.reset(m);
         const int64_t w = a - Col::warm(gm) > lo ? a - Col::warm(gm) : lo;
-        col.template run<false>(p.H, w, a, 0);
+        near_run<false>(col, p.H, w, a, 0);
         if (!REC) {
-            col.template run<true>(p.H, a, b, 1);
+            near_run<true>(col, p.H, a, b, 1);
             if (col.best < tbest) {  // (segments come in increasing order: an equal minimum keeps the earlier end)
                 tbest = col.best;
                 tfirst = (uint64_t)a + col.first;
@@ -498,7 +488,7 @@ __device__ __forceinline__ void near_batch_scan(NearBatchParams p, RecSet rs) {
             int64_t x = a;
             for (;;) {
                 const int64_t stop = b < hi ? b : hi;
-                if (x < stop) col.template run<true>(p.H, x, stop, (uint32_t)(x + 1 - lo));
+                if (x < stop) near_run<true>(col, p.H, x, stop, (uint32_t)(x + 1 - lo));
                 const uint64_t key = !idle && Col::has(col.best, m)
                                          ? (uint64_t)col.best << 48 | (uint64_t)ord << 32 | col.first
                                          : ~0ull;
@@ -524,13 +514,13 @@ __device__ __forceinline__ void near_batch_scan(NearBatchParams p, RecSet rs) {
 }
 
 template <int BITS, bool REC>
-__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : 3)
+__global__ void __launch_bounds__(kNearThreads, near_ctas_per_sm(BITS))
 k_nearest_batch_scan(NearBatchParams p, RecSet rs) {
     near_batch_scan<NearCol<BITS>, REC>(p, rs);
 }
 
 template <int BITS, bool REC>
-__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : 3)
+__global__ void __launch_bounds__(kNearThreads, near_ctas_per_sm(BITS))
 k_nearest_hamming_batch_scan(NearBatchParams p, RecSet rs) {
     near_batch_scan<HamCol<BITS>, REC>(p, rs);
 }
@@ -586,7 +576,7 @@ struct NearAnchParams {
 };
 
 template <int BITS, bool HAM, bool BATCH>
-__global__ void __launch_bounds__(kNearThreads, BITS == 32 ? 4 : BITS == 64 ? 3 : 2)
+__global__ void __launch_bounds__(kNearThreads, near_ctas_per_sm(BITS))
 k_nearest_anchored(NearAnchParams p, RecSet rs) {
     typedef typename NearWord<BITS>::type word;
     constexpr int NW = near_words(BITS);
