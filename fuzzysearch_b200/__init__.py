@@ -45,16 +45,13 @@ def has_near_match(subsequence, sequence, max_substitutions=None, max_insertions
     reference's internal has_near_match_* helpers (substitutions_only.py:18-34,139-145,218-233;
     generic_search.py:240-253), with early termination: the sequence is searched in chunks of growing size and
     the call returns after the first chunk that holds a match (fzb_has_near_match)."""
-    from .search import _lock_for, _prepare
+    from .search import _lock_for, _normalised_limits, _prepare
     search_params = LevenshteinSearchParams(max_substitutions, max_insertions, max_deletions, max_l_dist)
     if len(subsequence) == 0:
         raise ValueError("Given subsequence is empty!")
-    subs, ins, dels, l = search_params.unpacked
-    big = 1 << 29
-    subs, ins, dels = (big if subs is None else subs), (big if ins is None else ins), (big if dels is None else dels)
     with _lock_for(sequence):
-        pat, hay, _, _ = _prepare(subsequence, sequence)
-        return hay.has_near_match(pat, min(subs, big), min(ins, big), min(dels, big), l)
+        pat, hay, _ = _prepare(subsequence, sequence)
+        return hay.has_near_match(pat, *_normalised_limits(search_params))
 
 
 def find_near_matches_batch(subsequences, sequence, max_l_dist=None, *, max_substitutions=None,
@@ -70,18 +67,13 @@ def find_near_matches_batch(subsequences, sequence, max_l_dist=None, *, max_subs
                                                           max_deletions, max_l_dist)
     if not subsequences:
         return []
-    from .search import AlphabetTooLarge, _lock_for, _prepare_many
+    from .search import _bind_common, _lock_for, _prepare_many, _to_matches
     with _lock_for(sequence):
-        try:
-            pats, hay, slicer = _prepare_many(subsequences, sequence)
-        except AlphabetTooLarge:
-            # wide symbols and more than 255 distinct ones over all the patterns: no common byte alphabet,
-            # so the patterns go one by one (each reduces the sequence to its own alphabet)
+        bound = _bind_common(_prepare_many, subsequences, sequence)
+        if bound is None:
             return [find_near_matches(p, sequence, *lim) for p, lim in zip(subsequences, limits)]
-        out = []
-        for s, e, d in _search_batch(hay, pats, params, classes, 0):
-            out.append([Match(a, b, c, matched=slicer(a, b)) for a, b, c in zip(s.tolist(), e.tolist(), d.tolist())])
-    return out
+        pats, hay, slicer = bound
+        return [_to_matches(arrays, slicer) for arrays in _search_batch(hay, pats, params, classes, 0)]
 
 
 def _batch_params(subsequences, max_substitutions, max_insertions, max_deletions, max_l_dist):
@@ -104,12 +96,12 @@ def _batch_params(subsequences, max_substitutions, max_insertions, max_deletions
     limits = list(zip(per_pattern("max_substitutions", max_substitutions),
                       per_pattern("max_insertions", max_insertions),
                       per_pattern("max_deletions", max_deletions), per_pattern("max_l_dist", max_l_dist)))
+    from .search import _check_pattern
     params, classes = [], []
     for p, lim in zip(subsequences, limits):
         sp = LevenshteinSearchParams(*lim)  # same validation as find_near_matches
         cls = choose_search_class(sp)
-        if len(p) == 0:
-            raise ValueError("subsequence must not be empty" if cls is ExactSearch else "Given subsequence is empty!")
+        _check_pattern(cls, p)
         params.append(sp)
         classes.append(cls)
     return subsequences, limits, params, classes
@@ -120,7 +112,7 @@ def _search_batch(hay, pats, params, classes, flags):
     Levenshtein batch, substitutions-only ones in one Hamming batch, generic ones in one generic batch (a lone
     generic pattern on its own).  -> per pattern, its (start, end, dist) arrays in the list find_near_matches
     returns.  The caller holds the handle's lock."""
-    from . import _native
+    from .search import _list_of, _max_substitutions, _search_one
     n = len(pats)
     results = [None] * n
     lev = [i for i in range(n) if classes[i] in (ExactSearch, LevenshteinSearch)]
@@ -131,22 +123,19 @@ def _search_batch(hay, pats, params, classes, flags):
             rs, _ = hay.search_levenshtein_batch([pats[i] for i in lev], [params[i].max_l_dist for i in lev], flags)
             for i, r in zip(lev, rs):
                 results[i] = r
-        if ham:  # the limit SubstitutionsOnlySearch.search applies
-            ks = [min(x for x in (params[i].max_l_dist, params[i].max_substitutions) if x is not None) for i in ham]
+        if ham:
+            ks = [_max_substitutions(params[i]) for i in ham]
             rs, _ = hay.search_hamming_batch([pats[i] for i in ham], ks, flags)
             for i, r in zip(ham, rs):
                 results[i] = r
         if len(gen) == 1:  # (nothing to share; the single search needs no flag to honour a record set)
-            results[gen[0]] = hay.search_generic(pats[gen[0]], *params[gen[0]].unpacked)
+            results[gen[0]] = _search_one(GenericSearch, hay, pats[gen[0]], params[gen[0]])[0]
         elif gen:  # the normalised limits GenericSearch.search applies
             rs, _ = hay.search_generic_batch([pats[i] for i in gen], *zip(*[params[i].unpacked for i in gen]),
                                              flags=flags)
             for i, r in zip(gen, rs):
                 results[i] = r
-        # ExactSearch does not consolidate (search_exact.py:80-89): its list is the RAW stream of the k == 0
-        # route; the Hamming results have FINAL == RAW
-        return [res.arrays(_native.RAW if cls is ExactSearch else _native.FINAL)
-                for res, cls in zip(results, classes)]
+        return [res.arrays(_list_of(cls)) for res, cls in zip(results, classes)]
     finally:
         for res in results:
             if res is not None:

@@ -226,15 +226,23 @@ class Result(object):
     def stats(self):
         st = Stats()
         check(lib().fzb_result_stats(self._h, ctypes.byref(st)))
-        return {"gpu_ms": st.gpu_ms, "filter_ms": st.filter_ms, "bytes_scanned": st.bytes_scanned,
-                "n_candidates": st.n_candidates, "n_launches": st.n_launches,
-                "route": ROUTE_NAMES.get(st.route, str(st.route))}
+        return _stats(st)
 
 
-def _scan_stats(st):
+def _stats(st):
     return {"gpu_ms": st.gpu_ms, "filter_ms": st.filter_ms, "bytes_scanned": st.bytes_scanned,
             "n_candidates": st.n_candidates, "n_launches": st.n_launches,
             "route": ROUTE_NAMES.get(st.route, str(st.route))}
+
+
+def _pack(patterns):
+    """-> (the patterns joined into one uint8 blob, their uint32 offsets (count + 1 entries), count).  The blob of no
+    patterns is one spare byte; that of empty patterns only is empty, passed as NULL (ptr) and refused as such."""
+    pats = [as_u8(p) for p in patterns]
+    blob = np.concatenate(pats) if pats else np.zeros(1, np.uint8)
+    offsets = np.zeros(len(pats) + 1, dtype=np.uint32)
+    offsets[1:] = np.cumsum([p.size for p in pats])
+    return blob, offsets, len(pats)
 
 
 class Haystack(object):
@@ -399,35 +407,25 @@ class Haystack(object):
 
     def _batch(self, fn, patterns, limits, flags):
         """limits: the C-ABI's per-pattern limit arrays, in its order (one value per pattern each)."""
-        pats = [as_u8(p) for p in patterns]
-        blob = np.concatenate(pats) if pats else np.zeros(0, np.uint8)
-        offsets = np.zeros(len(pats) + 1, dtype=np.uint32)
-        offsets[1:] = np.cumsum([p.size for p in pats])
+        blob, offsets, n = _pack(patterns)
         limits = [np.ascontiguousarray(ks, dtype=np.uint32) for ks in limits]
-        out = (ctypes.c_void_p * max(len(pats), 1))()
+        out = (ctypes.c_void_p * max(n, 1))()
         st = Stats()
-        check(fn(self._h, ptr(blob), ptr(offsets), *[ptr(ks) for ks in limits], len(pats), flags, out,
-                 ctypes.byref(st)))
-        results = [Result(ctypes.c_void_p(out[i])) for i in range(len(pats))]
-        return results, {"gpu_ms": st.gpu_ms, "filter_ms": st.filter_ms, "bytes_scanned": st.bytes_scanned,
-                         "n_candidates": st.n_candidates, "n_launches": st.n_launches, "route": "batch"}
+        check(fn(self._h, ptr(blob), ptr(offsets), *[ptr(ks) for ks in limits], n, flags, out, ctypes.byref(st)))
+        return [Result(ctypes.c_void_p(out[i])) for i in range(n)], _stats(st)
 
     def best_per_record(self, patterns, max_subs, max_ins, max_dels, max_l, flags=0):
         """fzb_best_per_record on a handle with a record set: one normalised limit of each kind per pattern ->
         ((pattern, start, end, dist, second_pattern, second_dist) arrays with one entry per record, -1 where a record
         holds no match; summed stats dict)."""
-        pats = [as_u8(p) for p in patterns]
-        blob = np.concatenate(pats) if pats else np.zeros(0, np.uint8)
-        offsets = np.zeros(len(pats) + 1, dtype=np.uint32)
-        offsets[1:] = np.cumsum([p.size for p in pats])
+        blob, offsets, n = _pack(patterns)
         limits = [np.ascontiguousarray(ks, dtype=np.uint32) for ks in (max_subs, max_ins, max_dels, max_l)]
-        n = self.record_count
-        cols = [np.empty(n, dtype=t) for t in (np.int32, np.int64, np.int64, np.int32, np.int32, np.int32)]
+        nrec = self.record_count
+        cols = [np.empty(nrec, dtype=t) for t in (np.int32, np.int64, np.int64, np.int32, np.int32, np.int32)]
         st = Stats()
-        check(lib().fzb_best_per_record(self._h, ptr(blob), ptr(offsets), *[ptr(ks) for ks in limits], len(pats), flags,
+        check(lib().fzb_best_per_record(self._h, ptr(blob), ptr(offsets), *[ptr(ks) for ks in limits], n, flags,
                                         *[ctypes.c_void_p(c.ctypes.data) for c in cols], ctypes.byref(st)))
-        return tuple(cols), {"gpu_ms": st.gpu_ms, "filter_ms": st.filter_ms, "bytes_scanned": st.bytes_scanned,
-                             "n_candidates": st.n_candidates, "n_launches": st.n_launches, "route": "batch"}
+        return tuple(cols), _stats(st)
 
     def nearest_distance(self, pattern, flags=0):
         """fzb_nearest_distance: the nearest match of the pattern anywhere in the sequence, without a limit ->
@@ -436,7 +434,7 @@ class Haystack(object):
         dist, n_ends, first_end, st = ctypes.c_uint32(0), ctypes.c_uint64(0), ctypes.c_uint64(0), Stats()
         check(lib().fzb_nearest_distance(self._h, pp, m, flags, ctypes.byref(dist), ctypes.byref(n_ends),
                                          ctypes.byref(first_end), ctypes.byref(st)))
-        return dist.value, n_ends.value, first_end.value, _scan_stats(st)
+        return dist.value, n_ends.value, first_end.value, _stats(st)
 
     def nearest_per_record(self, pattern, flags=0):
         """fzb_nearest_per_record on a handle with a record set -> (dist int32, end int64: one entry per record,
@@ -446,35 +444,27 @@ class Haystack(object):
         st = Stats()
         check(lib().fzb_nearest_per_record(self._h, pp, m, flags, ctypes.c_void_p(dist.ctypes.data),
                                            ctypes.c_void_p(end.ctypes.data), ctypes.byref(st)))
-        return dist, end, _scan_stats(st)
-
-    @staticmethod
-    def _blob(patterns):
-        pats = [as_u8(p) for p in patterns]
-        blob = np.concatenate(pats) if pats else np.zeros(1, np.uint8)
-        offsets = np.zeros(len(pats) + 1, dtype=np.uint32)
-        offsets[1:] = np.cumsum([p.size for p in pats])
-        return blob, offsets, len(pats)
+        return dist, end, _stats(st)
 
     def nearest_distance_batch(self, patterns, flags=0):
         """fzb_nearest_distance_batch: fzb_nearest_distance's (dist, first_end) for every pattern, in shared scans ->
         (dist int32, first_end int64: one entry per pattern; stats dict)."""
-        blob, offsets, n = self._blob(patterns)
+        blob, offsets, n = _pack(patterns)
         dist, first_end, st = np.empty(n, dtype=np.uint32), np.empty(n, dtype=np.uint64), Stats()
         check(lib().fzb_nearest_distance_batch(self._h, ptr(blob), ptr(offsets), n, flags,
                                                ctypes.c_void_p(dist.ctypes.data),
                                                ctypes.c_void_p(first_end.ctypes.data), ctypes.byref(st)))
-        return dist.astype(np.int32), first_end.astype(np.int64), _scan_stats(st)
+        return dist.astype(np.int32), first_end.astype(np.int64), _stats(st)
 
     def nearest_best_per_record(self, patterns, flags=0):
         """fzb_nearest_best_per_record on a handle with a record set -> ((pattern int32, dist int32, end int64,
         second_pattern int32, second_dist int32): one entry per record; stats dict)."""
-        blob, offsets, n = self._blob(patterns)
+        blob, offsets, n = _pack(patterns)
         cols = [np.empty(self.record_count, dtype=t) for t in (np.int32, np.int32, np.int64, np.int32, np.int32)]
         st = Stats()
         check(lib().fzb_nearest_best_per_record(self._h, ptr(blob), ptr(offsets), n, flags,
                                                 *[ctypes.c_void_p(c.ctypes.data) for c in cols], ctypes.byref(st)))
-        return tuple(cols), _scan_stats(st)
+        return tuple(cols), _stats(st)
 
     def align(self, patterns, max_subs, max_ins, max_dels, max_l, item_pattern, item_start, item_end, item_dist,
               flags=0):
@@ -483,7 +473,7 @@ class Haystack(object):
         each kind per pattern -> ((start int64, cost, n_subs, n_ins, n_dels int32: one entry per item, -1 without an
         alignment), ops uint8 (item i's m_i + n_ins[i] op bytes from op_offsets[i]), op_offsets uint64 (n_items + 1
         entries), stats dict)."""
-        blob, offsets, n = self._blob(patterns)
+        blob, offsets, n = _pack(patterns)
         limits = [np.ascontiguousarray(ks, dtype=np.uint32) for ks in (max_subs, max_ins, max_dels, max_l)]
         ip = np.ascontiguousarray(item_pattern, dtype=np.uint32)
         s = np.ascontiguousarray(item_start, dtype=np.int64)
@@ -504,7 +494,7 @@ class Haystack(object):
         st = Stats()
         check(lib().fzb_align(self._h, ptr(blob), ptr(offsets), n, *[ptr(x) for x in limits], ptr(ip), ptr(s), ptr(e),
                               ptr(d), k, flags, *[ptr(c) for c in cols], ptr(op_offsets), ptr(ops), ctypes.byref(st)))
-        return tuple(cols), ops, op_offsets, _scan_stats(st)
+        return tuple(cols), ops, op_offsets, _stats(st)
 
     def has_near_match(self, pattern, max_subs, max_ins, max_dels, max_l):
         """True iff the search would return at least one match; stops at the first chunk that holds one."""

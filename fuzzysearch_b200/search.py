@@ -144,6 +144,16 @@ class AlphabetTooLarge(_native.UnsupportedError):
     pass
 
 
+def _bind_common(bind, *args):
+    """-> bind(*args), or None when the patterns it binds have no common byte alphabet (wide symbols and more than 255
+    distinct ones over all of them): the caller then takes the patterns one by one, each reducing the sequence to its
+    own alphabet."""
+    try:
+        return bind(*args)
+    except AlphabetTooLarge:
+        return None
+
+
 def _make_alphabet(subsequences, kind):
     """The reduction every algorithm on the path is invariant under (they only ever compare a pattern symbol
     with a sequence symbol -- levenshtein_ngram.py:49,113, levenshtein.py:83, generic_search.py:86,
@@ -205,12 +215,12 @@ class RawMatches(Sequence):
         self._slicer = slicer
         self._list = None
         self.stats = result.stats()
-        self.final = _to_matches(result, _native.FINAL, slicer) if consolidated else None
+        self.final = _to_matches(result.arrays(_native.FINAL), slicer) if consolidated else None
         self._n = result.count(_native.RAW)
 
     def materialize(self):
         if self._list is None:
-            self._list = _to_matches(self._result, _native.RAW, self._slicer)
+            self._list = _to_matches(self._result.arrays(_native.RAW), self._slicer)
             self._result.close()
             self._result = None
         return self._list
@@ -243,9 +253,9 @@ class RawMatches(Sequence):
 
 
 def _prepare(subsequence, sequence):
-    """-> (pattern u8, haystack handle, slicer, owns_handle)"""
+    """-> (pattern u8, haystack handle, slicer)"""
     pats, hay, slicer = _prepare_many([subsequence], sequence)
-    return pats[0], hay, slicer, False
+    return pats[0], hay, slicer
 
 
 def _prepare_many(subsequences, sequence):
@@ -267,15 +277,16 @@ def _prepare_many(subsequences, sequence):
         pats = [_rename(p, kind, alphabet) for p in subsequences]
         hay = _workspace(len(sequence))
         _upload_reduced(hay, sequence, kind, alphabet)
-    if kind != "bytes" or isinstance(sequence, (bytes, bytearray)):
-        def slicer(s, e):
-            return original[s:e]
-    else:
-        mv = memoryview(host)
+    return pats, hay, _slicer(original, kind, host)
 
-        def slicer(s, e):
-            return bytes(mv[s:e])
-    return pats, hay, slicer
+
+def _slicer(original, kind, u8=None):
+    """Match.matched as find_near_matches(pattern, original) slices it: a slice of the original object, as bytes for a
+    byte-like object other than bytes / bytearray (u8: its uint8 view, when the caller already has it)."""
+    if kind != "bytes" or isinstance(original, (bytes, bytearray)):
+        return lambda s, e: original[s:e]
+    mv = memoryview(_native.as_u8(original) if u8 is None else u8)
+    return lambda s, e: bytes(mv[s:e])
 
 
 _WORKSPACE = {}
@@ -310,14 +321,56 @@ def release_workspace():
     _native.lib().fzb_release_workspace()
 
 
-def _to_matches(result, which, slicer):
-    s, e, d = result.arrays(which)
-    return [Match(a, b, c, matched=slicer(a, b)) for a, b, c in zip(s.tolist(), e.tolist(), d.tolist())]
+def _matches(starts, ends, dists, slicer):
+    """(start, end, dist) lists of ints -> the Match list, `matched` cut by slicer."""
+    return [Match(a, b, c, matched=slicer(a, b)) for a, b, c in zip(starts, ends, dists)]
+
+
+def _to_matches(arrays, slicer):
+    """The (start, end, dist) arrays of a list -> its Match list."""
+    return _matches(*(x.tolist() for x in arrays), slicer)
+
+
+def _check_pattern(cls, subsequence):
+    """The empty-pattern refusal of cls.search (ExactSearch words it as search_exact does)."""
+    if len(subsequence) == 0:
+        raise ValueError("subsequence must not be empty" if cls is ExactSearch else "Given subsequence is empty!")
+
+
+def _max_substitutions(search_params):
+    """The limit SubstitutionsOnlySearch.search applies (substitutions_only.py:288-301)."""
+    return min(x for x in (search_params.max_l_dist, search_params.max_substitutions) if x is not None)
+
+
+def _list_of(cls):
+    """Which list of a search of class cls find_near_matches returns: ExactSearch does not consolidate
+    (search_exact.py:80-89), its list is the RAW stream of the k == 0 route; the others the FINAL list (the Hamming
+    FINAL list equals RAW)."""
+    return _native.RAW if cls is ExactSearch else _native.FINAL
+
+
+def _search_one(cls, hay, pat, search_params):
+    """One pattern searched on the handle `hay` as cls.search searches it -> (Result, the list to read)."""
+    if cls is ExactSearch:
+        res = hay.search_exact(pat)
+    elif cls is SubstitutionsOnlySearch:
+        res = hay.search_hamming(pat, _max_substitutions(search_params))
+    elif cls is LevenshteinSearch:
+        res = hay.search_levenshtein(pat, search_params.max_l_dist)
+    else:
+        res = hay.search_generic(pat, *search_params.unpacked)
+    return res, _list_of(cls)
+
+
+def _search_class(cls, subsequence, sequence, search_params, consolidated):
+    """cls.search: the pattern checked, then searched as _search_one searches it -> RawMatches."""
+    _check_pattern(cls, subsequence)
+    return _run(subsequence, sequence, lambda h, p: _search_one(cls, h, p, search_params)[0], consolidated)
 
 
 def _run(subsequence, sequence, call, consolidated):
     with _lock_for(sequence):
-        pat, hay, slicer, _ = _prepare(subsequence, sequence)
+        pat, hay, slicer = _prepare(subsequence, sequence)
         res = call(hay, pat)
         try:
             return RawMatches(res, slicer, consolidated)
@@ -355,7 +408,7 @@ def search_exact(subsequence, sequence, start_index=0, end_index=None):
         else:
             window = sequence[start_index:end_index]
         with _WORKSPACE_LOCK:
-            pat, hay, _, _ = _prepare(subsequence, window)
+            pat, hay, _ = _prepare(subsequence, window)
             res = hay.search_exact(pat)
             starts = res.arrays(_native.RAW)[0]
             res.close()
@@ -367,9 +420,7 @@ class ExactSearch(FuzzySearchBase):
 
     @classmethod
     def search(cls, subsequence, sequence, search_params=None):
-        if len(subsequence) == 0:
-            raise ValueError("subsequence must not be empty")
-        return _run(subsequence, sequence, lambda h, p: h.search_exact(p), False)
+        return _search_class(ExactSearch, subsequence, sequence, search_params, False)
 
     @classmethod
     def extra_items_for_chunked_search(cls, subsequence, search_params):
@@ -381,11 +432,7 @@ class SubstitutionsOnlySearch(FuzzySearchBase):
 
     @classmethod
     def search(cls, subsequence, sequence, search_params):
-        if len(subsequence) == 0:
-            raise ValueError("Given subsequence is empty!")
-        actual_max_subs = min(x for x in [search_params.max_l_dist, search_params.max_substitutions]
-                              if x is not None)
-        return _run(subsequence, sequence, lambda h, p: h.search_hamming(p, actual_max_subs), False)
+        return _search_class(SubstitutionsOnlySearch, subsequence, sequence, search_params, False)
 
     @classmethod
     def extra_items_for_chunked_search(cls, subsequence, search_params):
@@ -397,10 +444,7 @@ class LevenshteinSearch(FuzzySearchBase):
 
     @classmethod
     def search(cls, subsequence, sequence, search_params):
-        if len(subsequence) == 0:
-            raise ValueError("Given subsequence is empty!")
-        k = search_params.max_l_dist
-        return _run(subsequence, sequence, lambda h, p: h.search_levenshtein(p, k), True)
+        return _search_class(LevenshteinSearch, subsequence, sequence, search_params, True)
 
     @classmethod
     def consolidate_matches(cls, matches):
@@ -416,10 +460,7 @@ class GenericSearch(FuzzySearchBase):
 
     @classmethod
     def search(cls, subsequence, sequence, search_params):
-        if len(subsequence) == 0:
-            raise ValueError("Given subsequence is empty!")
-        subs, ins, dels, l = search_params.unpacked
-        return _run(subsequence, sequence, lambda h, p: h.search_generic(p, subs, ins, dels, l), True)
+        return _search_class(GenericSearch, subsequence, sequence, search_params, True)
 
     @classmethod
     def consolidate_matches(cls, matches):
@@ -430,8 +471,25 @@ class GenericSearch(FuzzySearchBase):
         return max(x for x in [search_params.max_l_dist, search_params.max_insertions] if x is not None)
 
 
-def _nearest_flags(substitutions_only):
-    return _native.F_SUBSTITUTIONS_ONLY if substitutions_only else 0
+def _nearest_flags(substitutions_only, anchor=None):
+    """The flags of the nearest_* calls; ValueError for an anchor other than None, 'start' or 'end'."""
+    flags = _native.F_SUBSTITUTIONS_ONLY if substitutions_only else 0
+    if anchor is None:
+        return flags
+    if isinstance(anchor, str) and anchor == "start":
+        return flags | _native.F_ANCHOR_START
+    if isinstance(anchor, str) and anchor == "end":
+        return flags | _native.F_ANCHOR_END
+    raise ValueError("anchor must be None, 'start' or 'end', not %r" % (anchor,))
+
+
+def _nearest_params(d, substitutions_only):
+    """The limits at which find_near_matches lists the matches at the nearest distance d -> (params, search class)."""
+    from . import choose_search_class
+    from .common import LevenshteinSearchParams
+    params = (LevenshteinSearchParams(d, 0, 0, None) if substitutions_only else
+              LevenshteinSearchParams(None, None, None, d))
+    return params, choose_search_class(params)
 
 
 def nearest_distance(subsequence, sequence, *, substitutions_only=False):
@@ -447,7 +505,7 @@ def nearest_distance(subsequence, sequence, *, substitutions_only=False):
     if len(subsequence) == 0:
         raise ValueError("Given subsequence is empty!")
     with _lock_for(sequence):
-        pat, hay, _, _ = _prepare(subsequence, sequence)
+        pat, hay, _ = _prepare(subsequence, sequence)
         d = hay.nearest_distance(pat, _nearest_flags(substitutions_only))[0]
         return None if d == _native.NO_DIST else d
 
@@ -467,16 +525,14 @@ def find_nearest_matches(subsequence, sequence, max_l_dist=None, *, substitution
     if max_l_dist is not None and (not isinstance(max_l_dist, int) or max_l_dist < 0):
         raise ValueError("max_l_dist must be a non-negative integer or None")
     with _lock_for(sequence):
-        pat, hay, slicer, _ = _prepare(subsequence, sequence)
+        pat, hay, slicer = _prepare(subsequence, sequence)
         d = hay.nearest_distance(pat, _nearest_flags(substitutions_only))[0]
         if d == _native.NO_DIST or (max_l_dist is not None and d > max_l_dist):
             return []
-        # max_l_dist == 0 is the exact search, whose list is its raw stream (ExactSearch does not consolidate);
-        # the substitutions-only search does not consolidate either (FINAL == RAW)
-        res = (hay.search_exact(pat) if d == 0 else
-               hay.search_hamming(pat, d) if substitutions_only else hay.search_levenshtein(pat, d))
+        params, cls = _nearest_params(d, substitutions_only)
+        res, which = _search_one(cls, hay, pat, params)
         try:
-            return _to_matches(res, _native.RAW if d == 0 else _native.FINAL, slicer)
+            return _to_matches(res.arrays(which), slicer)
         finally:
             res.close()
 
@@ -484,19 +540,16 @@ def find_nearest_matches(subsequence, sequence, max_l_dist=None, *, substitution
 def _nearest_batch(subsequences, sequence, flags):
     """-> (dist int32, first end int64) arrays, one entry per pattern, -1 / -1 without a value.  The caller holds
     the sequence's lock."""
-    try:
-        pats, hay, _ = _prepare_many(subsequences, sequence)
-    except AlphabetTooLarge:
-        # wide symbols and more than 255 distinct ones over all the patterns: no common byte alphabet, so the
-        # patterns go one by one (each reduces the sequence to its own alphabet)
-        rows = []
-        for p in subsequences:
-            pat, hay, _, _ = _prepare(p, sequence)
-            d, _, e, _ = hay.nearest_distance(pat, flags)
-            rows.append((-1, -1) if d == _native.NO_DIST else (d, e))
-        return np.array([d for d, _ in rows], dtype=np.int32), np.array([e for _, e in rows], dtype=np.int64)
-    dist, end, _ = hay.nearest_distance_batch(pats, flags)
-    return dist, end
+    bound = _bind_common(_prepare_many, subsequences, sequence)
+    if bound is not None:
+        dist, end, _ = bound[1].nearest_distance_batch(bound[0], flags)
+        return dist, end
+    rows = []
+    for p in subsequences:
+        pat, hay, _ = _prepare(p, sequence)
+        d, _, e, _ = hay.nearest_distance(pat, flags)
+        rows.append((-1, -1) if d == _native.NO_DIST else (d, e))
+    return np.array([d for d, _ in rows], dtype=np.int32), np.array([e for _, e in rows], dtype=np.int64)
 
 
 def nearest_distance_batch(subsequences, sequence, *, substitutions_only=False):
@@ -523,8 +576,7 @@ def find_nearest_matches_batch(subsequences, sequence, max_l_dist=None, *, subst
     a pattern whose d_i is larger gets ``[]`` and is not searched.  With ``substitutions_only=True``: exactly
     ``find_near_matches_batch(..., max_substitutions=[d_0, d_1, ...], max_insertions=0, max_deletions=0)`` with the
     substitutions-only d_i, and ``[]`` for a pattern longer than the sequence."""
-    from . import _search_batch, choose_search_class, find_nearest_matches
-    from .common import LevenshteinSearchParams
+    from . import _search_batch
     subsequences = list(subsequences)
     n = len(subsequences)
     caps = max_l_dist if isinstance(max_l_dist, (list, tuple)) else [max_l_dist] * n
@@ -537,19 +589,18 @@ def find_nearest_matches_batch(subsequences, sequence, max_l_dist=None, *, subst
     if not subsequences:
         return []
     with _lock_for(sequence):
-        try:
-            pats, hay, slicer = _prepare_many(subsequences, sequence)
-        except AlphabetTooLarge:
+        bound = _bind_common(_prepare_many, subsequences, sequence)
+        if bound is None:
             return [find_nearest_matches(p, sequence, c, substitutions_only=substitutions_only)
                     for p, c in zip(subsequences, caps)]
+        pats, hay, slicer = bound
         dist, _, _ = hay.nearest_distance_batch(pats, _nearest_flags(substitutions_only))
         todo = [i for i in range(n) if dist[i] >= 0 and (caps[i] is None or dist[i] <= caps[i])]
-        params = [LevenshteinSearchParams(int(dist[i]), 0, 0, None) if substitutions_only else
-                  LevenshteinSearchParams(None, None, None, int(dist[i])) for i in todo]
-        lists = _search_batch(hay, [pats[i] for i in todo], params, [choose_search_class(p) for p in params], 0)
+        found = [_nearest_params(int(dist[i]), substitutions_only) for i in todo]
+        lists = _search_batch(hay, [pats[i] for i in todo], [p for p, _ in found], [c for _, c in found], 0)
     out = [[] for _ in range(n)]
-    for i, (s, e, d) in zip(todo, lists):
-        out[i] = [Match(a, b, c, matched=slicer(a, b)) for a, b, c in zip(s.tolist(), e.tolist(), d.tolist())]
+    for i, arrays in zip(todo, lists):
+        out[i] = _to_matches(arrays, slicer)
     return out
 
 
@@ -612,7 +663,7 @@ def align_matches(subsequence, sequence, matches, max_substitutions=None, max_in
         raise ValueError("matches need non-negative starts and dists")
     lims = _normalised_limits(search_params)
     with _lock_for(sequence):
-        pat, hay, _, _ = _prepare(subsequence, sequence)
+        pat, hay, _ = _prepare(subsequence, sequence)
         (_, cost, _, ins, _), ops, op_offsets, _ = hay.align([pat], *[[x] for x in lims], np.zeros(len(matches)), s,
                                                              e, d)
     bad = np.flatnonzero(cost < 0)

@@ -10,7 +10,8 @@ import numpy as np
 
 from . import _native
 from .common import LevenshteinSearchParams, Match
-from .search import DeviceSequence, ExactSearch, GenericSearch, LevenshteinSearch, _kind, _text
+from .search import (_BIG, DeviceSequence, _bind_common, _check_pattern, _kind, _matches, _nearest_flags,
+                     _normalised_limits, _search_one, _slicer, _text)
 
 __all__ = ["Alignments", "BestMatches", "DeviceSequenceSet", "NearestDistances", "NearestPatterns", "align_in_each",
            "best_match_in_each",
@@ -29,14 +30,6 @@ def _set_kind(sequences):
     if len(kinds) > 1:
         raise TypeError("the sequences of a set must all be str or all be byte-like")
     return kinds.pop() if kinds else "bytes"
-
-
-def _slicer(orig, kind):
-    """Match.matched as find_near_matches(pattern, orig) slices it."""
-    if kind == "str" or isinstance(orig, (bytes, bytearray)):
-        return lambda s, e: orig[s:e]
-    mv = memoryview(_native.as_u8(orig))
-    return lambda s, e: bytes(mv[s:e])
 
 
 class DeviceSequenceSet(object):
@@ -81,6 +74,27 @@ class DeviceSequenceSet(object):
         self._seq.close()
 
 
+def _check_sequences(sequences):
+    if not isinstance(sequences, (DeviceSequenceSet, list, tuple)):
+        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
+
+
+def _in_each(sequences, empty, body):
+    """The frame of the *_in_each calls: -> body(seqset) on a resident set -- `sequences` itself, or one uploaded from
+    the list / tuple for this call and closed on every exit -- or empty(sequences), uploading nothing, when there is
+    nothing to do: no sequences, or no body (nothing to search for)."""
+    _check_sequences(sequences)
+    if body is None or len(sequences) == 0:
+        return empty(sequences)
+    if isinstance(sequences, DeviceSequenceSet):
+        return body(sequences)
+    seqset = DeviceSequenceSet(sequences)
+    try:
+        return body(seqset)
+    finally:
+        seqset.close()
+
+
 def find_near_matches_in_each(subsequence, sequences, max_substitutions=None, max_insertions=None,
                               max_deletions=None, max_l_dist=None):
     """One pattern over many sequences: -> a list with, for every sequence, exactly
@@ -90,39 +104,15 @@ def find_near_matches_in_each(subsequence, sequences, max_substitutions=None, ma
     search_params = LevenshteinSearchParams(max_substitutions, max_insertions, max_deletions, max_l_dist)
     from . import choose_search_class
     cls = choose_search_class(search_params)
-    if len(subsequence) == 0:
-        raise ValueError("subsequence must not be empty" if cls is ExactSearch else "Given subsequence is empty!")
-    if isinstance(sequences, DeviceSequenceSet):
-        return _search_set(subsequence, sequences, cls, search_params)
-    if not isinstance(sequences, (list, tuple)):
-        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
-    if not sequences:
-        return []
-    seqset = DeviceSequenceSet(sequences)
-    try:
-        return _search_set(subsequence, seqset, cls, search_params)
-    finally:
-        seqset.close()
+    _check_pattern(cls, subsequence)
+    return _in_each(sequences, lambda _: [], lambda seqset: _search_set(subsequence, seqset, cls, search_params))
 
 
 def _search_set(subsequence, seqset, cls, search_params):
-    if len(seqset) == 0:
-        return []
-    subs, ins, dels, l = search_params.unpacked
     with seqset._lock:
-        pat = seqset._bind(subsequence)
-        hay = seqset._seq.haystack
-        if cls is ExactSearch:
-            res = hay.search_exact(pat)
-        elif cls is LevenshteinSearch:
-            res = hay.search_levenshtein(pat, l)
-        elif cls is GenericSearch:
-            res = hay.search_generic(pat, subs, ins, dels, l)
-        else:  # the limit SubstitutionsOnlySearch.search applies
-            res = hay.search_hamming(pat, min(x for x in (l, subs) if x is not None))
+        res, which = _search_one(cls, seqset._seq.haystack, seqset._bind(subsequence), search_params)
         try:
-            # ExactSearch does not consolidate: its list is the RAW stream; the Hamming FINAL list equals RAW
-            s, e, d = res.arrays(_native.RAW if cls is ExactSearch else _native.FINAL)
+            s, e, d = res.arrays(which)
         finally:
             res.close()
     out = [[] for _ in range(len(seqset))]
@@ -144,8 +134,7 @@ def _split_by_record(seqset, s, e, d):
     hit_recs, firsts = np.unique(rec, return_index=True)
     ends = np.append(firsts[1:], len(s))
     for i, lo, hi in zip(hit_recs.tolist(), firsts.tolist(), ends.tolist()):
-        sl = _slicer(seqset._orig[i], seqset._kind)
-        yield i, [Match(a, b, c, matched=sl(a, b)) for a, b, c in zip(s[lo:hi], e[lo:hi], d[lo:hi])]
+        yield i, _matches(s[lo:hi], e[lo:hi], d[lo:hi], _slicer(seqset._orig[i], seqset._kind))
 
 
 def find_near_matches_batch_in_each(subsequences, sequences, max_l_dist=None, *, max_substitutions=None,
@@ -161,31 +150,14 @@ def find_near_matches_batch_in_each(subsequences, sequences, max_l_dist=None, *,
                                                           max_deletions, max_l_dist)
     if not subsequences:
         return []
-    if isinstance(sequences, DeviceSequenceSet):
-        return _search_set_batch(subsequences, sequences, limits, params, classes)
-    if not isinstance(sequences, (list, tuple)):
-        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
-    if not sequences:
-        return [{} for _ in subsequences]
-    seqset = DeviceSequenceSet(sequences)
-    try:
-        return _search_set_batch(subsequences, seqset, limits, params, classes)
-    finally:
-        seqset.close()
+    return _in_each(sequences, lambda _: [{} for _ in subsequences],
+                    lambda seqset: _search_set_batch(subsequences, seqset, limits, params, classes))
 
 
 def _search_set_batch(subsequences, seqset, limits, params, classes):
-    if len(seqset) == 0:
-        return [{} for _ in subsequences]
     from . import _search_batch
-    from .search import AlphabetTooLarge
     with seqset._lock:
-        try:
-            pats = seqset._bind_many(subsequences)
-        except AlphabetTooLarge:
-            # wide symbols and more than 255 distinct ones over all the patterns: no common byte alphabet, so the
-            # patterns go one by one (each reduces the set to its own alphabet)
-            pats = None
+        pats = _bind_common(seqset._bind_many, subsequences)
         if pats is not None:
             lists = _search_batch(seqset._seq.haystack, pats, params, classes, _native.F_PER_RECORD)
     if pats is None:
@@ -231,32 +203,19 @@ def best_match_in_each(subsequences, sequences, max_l_dist=None, *, max_substitu
     from . import _batch_params
     subsequences, limits, params, classes = _batch_params(subsequences, max_substitutions, max_insertions,
                                                           max_deletions, max_l_dist)
-    if isinstance(sequences, DeviceSequenceSet):
-        return _best_in_set(subsequences, sequences, limits, params)
-    if not isinstance(sequences, (list, tuple)):
-        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
-    if not sequences or not subsequences:
-        return BestMatches(list(sequences), _set_kind(sequences), _no_matches(len(sequences)))
-    seqset = DeviceSequenceSet(sequences)
-    try:
-        return _best_in_set(subsequences, seqset, limits, params)
-    finally:
-        seqset.close()
+
+    def no_rows(seqs):
+        orig = seqs._orig if isinstance(seqs, DeviceSequenceSet) else list(seqs)
+        return BestMatches(orig, _set_kind(orig), _no_matches(len(orig)))
+    return _in_each(sequences, no_rows, (lambda seqset: _best_in_set(subsequences, seqset, limits, params))
+                    if subsequences else None)
 
 
 def _best_in_set(subsequences, seqset, limits, params):
-    n = len(seqset)
-    if n == 0 or not subsequences:
-        return BestMatches(seqset._orig, seqset._kind, _no_matches(n))
-    from .search import AlphabetTooLarge
-    big = 1 << 29
     with seqset._lock:
-        try:
-            pats = seqset._bind_many(subsequences)
-        except AlphabetTooLarge:
-            pats = None  # no common byte alphabet: pattern by pattern, below
+        pats = _bind_common(seqset._bind_many, subsequences)
         if pats is not None:
-            lims = zip(*[[big if x is None else min(x, big) for x in p.unpacked] for p in params])
+            lims = zip(*[_normalised_limits(p) for p in params])
             columns, _ = seqset._seq.haystack.best_per_record(pats, *lims)
     if pats is None:
         columns = _best_on_host(subsequences, seqset, limits)
@@ -267,16 +226,29 @@ def _best_on_host(subsequences, seqset, limits):
     """The same rows from find_near_matches_in_each, pattern by pattern (each reduces the set to its own alphabet)."""
     pat, start, end, dist, pat2, dist2 = columns = _no_matches(len(seqset))
     for i, (p, lim) in enumerate(zip(subsequences, limits)):
+        d, s, e = np.full(len(seqset), -1, dtype=np.int32), np.full(len(seqset), -1), np.full(len(seqset), -1)
         for r, matches in enumerate(find_near_matches_in_each(p, seqset, *lim)):
-            if not matches:
-                continue
-            m = min(matches, key=lambda x: (x.dist, x.start - x.end, x.start))
-            if pat[r] < 0 or m.dist < dist[r]:  # (an equal distance leaves the earlier pattern in place)
-                pat2[r], dist2[r] = pat[r], dist[r]
-                pat[r], start[r], end[r], dist[r] = i, m.start, m.end, m.dist
-            elif pat2[r] < 0 or m.dist < dist2[r]:
-                pat2[r], dist2[r] = i, m.dist
+            if matches:
+                m = min(matches, key=lambda x: (x.dist, x.start - x.end, x.start))
+                d[r], s[r], e[r] = m.dist, m.start, m.end
+        _fold(i, d, (pat, dist, pat2, dist2), ((start, s), (end, e)))
     return columns
+
+
+def _fold(i, dist, columns, carried):
+    """Fold pattern i's distance to every record (-1: none there) into the (pattern, dist, second_pattern,
+    second_dist) columns: a strictly smaller distance replaces the winner, which becomes the runner-up; an equal one
+    leaves the earlier (smaller) index in place.  carried: (column, pattern i's values) pairs that go with the
+    winner."""
+    pattern, best, pat2, dist2 = columns
+    has = dist >= 0
+    first = has & ((pattern < 0) | (dist < best))
+    second = has & ~first & ((pat2 < 0) | (dist < dist2))
+    pat2[first], dist2[first] = pattern[first], best[first]
+    pattern[first], best[first] = i, dist[first]
+    for column, values in carried:
+        column[first] = values[first]
+    pat2[second], dist2[second] = i, dist[second]
 
 
 class NearestDistances(object):
@@ -300,18 +272,6 @@ class NearestDistances(object):
 
     def __getitem__(self, r):
         return int(self.dist[r]), int(self.end[r])
-
-
-def _nearest_flags(substitutions_only, anchor):
-    """The flags of the nearest_*_in_each calls; ValueError for an anchor other than None, 'start' or 'end'."""
-    flags = _native.F_SUBSTITUTIONS_ONLY if substitutions_only else 0
-    if anchor is None:
-        return flags
-    if isinstance(anchor, str) and anchor == "start":
-        return flags | _native.F_ANCHOR_START
-    if isinstance(anchor, str) and anchor == "end":
-        return flags | _native.F_ANCHOR_END
-    raise ValueError("anchor must be None, 'start' or 'end', not %r" % (anchor,))
 
 
 def _anchored_span(seqset, flags, has, pos):
@@ -347,22 +307,11 @@ def nearest_distance_in_each(subsequence, sequences, *, substitutions_only=False
     if len(subsequence) == 0:
         raise ValueError("Given subsequence is empty!")
     flags = _nearest_flags(substitutions_only, anchor)
-    if isinstance(sequences, DeviceSequenceSet):
-        return _nearest_in_set(subsequence, sequences, flags)
-    if not isinstance(sequences, (list, tuple)):
-        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
-    if not sequences:
-        return _no_distances(flags)
-    seqset = DeviceSequenceSet(sequences)
-    try:
-        return _nearest_in_set(subsequence, seqset, flags)
-    finally:
-        seqset.close()
+    return _in_each(sequences, lambda _: _no_distances(flags),
+                    lambda seqset: _nearest_in_set(subsequence, seqset, flags))
 
 
 def _nearest_in_set(subsequence, seqset, flags):
-    if len(seqset) == 0:
-        return _no_distances(flags)
     with seqset._lock:
         pat = seqset._bind(subsequence)
         dist, end, _ = seqset._seq.haystack.nearest_per_record(pat, flags)
@@ -421,29 +370,13 @@ def nearest_pattern_in_each(subsequences, sequences, *, substitutions_only=False
     if any(len(p) == 0 for p in subsequences):
         raise ValueError("Given subsequence is empty!")
     flags = _nearest_flags(substitutions_only, anchor)
-    if isinstance(sequences, DeviceSequenceSet):
-        return _nearest_patterns_in_set(subsequences, sequences, flags)
-    if not isinstance(sequences, (list, tuple)):
-        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
-    if not sequences or not subsequences:
-        return _no_patterns_rows(len(sequences), flags)
-    seqset = DeviceSequenceSet(sequences)
-    try:
-        return _nearest_patterns_in_set(subsequences, seqset, flags)
-    finally:
-        seqset.close()
+    return _in_each(sequences, lambda seqs: _no_patterns_rows(len(seqs), flags),
+                    (lambda seqset: _nearest_patterns_in_set(subsequences, seqset, flags)) if subsequences else None)
 
 
 def _nearest_patterns_in_set(subsequences, seqset, flags):
-    n = len(seqset)
-    if n == 0 or not subsequences:
-        return _no_patterns_rows(n, flags)
-    from .search import AlphabetTooLarge
     with seqset._lock:
-        try:
-            pats = seqset._bind_many(subsequences)
-        except AlphabetTooLarge:
-            pats = None  # no common byte alphabet: pattern by pattern, below
+        pats = _bind_common(seqset._bind_many, subsequences)
         if pats is not None:
             columns, _ = seqset._seq.haystack.nearest_best_per_record(pats, flags)
             start, end = _anchored_span(seqset, flags, columns[0] >= 0, columns[2])
@@ -462,14 +395,7 @@ def _nearest_patterns_on_host(subsequences, seqset, flags):
     for i, p in enumerate(subsequences):
         got = nearest_distance_in_each(p, seqset, substitutions_only=bool(flags & _native.F_SUBSTITUTIONS_ONLY),
                                        anchor=anchor)
-        has = got.dist >= 0
-        first = has & ((pattern < 0) | (got.dist < dist))  # (an equal distance leaves the earlier pattern in place)
-        second = has & ~first & ((pat2 < 0) | (got.dist < dist2))
-        pat2[first], dist2[first] = pattern[first], dist[first]
-        pattern[first], dist[first], end[first] = i, got.dist[first], got.end[first]
-        if anchor is not None:
-            start[first] = got.start[first]
-        pat2[second], dist2[second] = i, got.dist[second]
+        _fold(i, got.dist, (pattern, dist, pat2, dist2), ((end, got.end),) + (((start, got.start),) if anchor else ()))
     return columns, (start if anchor is not None else None)
 
 
@@ -506,7 +432,6 @@ def align_in_each(subsequences, sequences, rows, max_l_dist=None, *, max_substit
       carry their start: the window ``[start, end)`` is aligned as it is, at cost d.
 
     `sequences` is a list / tuple (uploaded for this call) or a DeviceSequenceSet (resident)."""
-    from .search import _cigars, _normalised_limits
     if not isinstance(subsequences, (list, tuple)):
         subsequences = [subsequences]
     subsequences = list(subsequences)
@@ -523,8 +448,7 @@ def align_in_each(subsequences, sequences, rows, max_l_dist=None, *, max_substit
     else:
         if any(x is not None for x in (max_l_dist, max_substitutions, max_insertions, max_deletions)):
             raise ValueError("limits are taken only with BestMatches rows")
-        big = 1 << 29
-        lims = [(big, 0, 0, big) if substitutions_only else (big, big, big, big)] * len(subsequences)
+        lims = [(_BIG, 0, 0, _BIG) if substitutions_only else (_BIG,) * 4] * len(subsequences)  # limits that never bind
         if isinstance(rows, NearestPatterns):
             pattern = rows.pattern
         elif isinstance(rows, NearestDistances):
@@ -536,67 +460,59 @@ def align_in_each(subsequences, sequences, rows, max_l_dist=None, *, max_substit
         start = np.full(n, -1, dtype=np.int64) if rows.start is None else np.asarray(rows.start, dtype=np.int64)
         dist = rows.dist
         nearest = True
-    if isinstance(sequences, DeviceSequenceSet):
-        seqset, own = sequences, False
-    elif isinstance(sequences, (list, tuple)):
-        seqset, own = (DeviceSequenceSet(sequences) if sequences else None), True
-    else:
-        raise TypeError("sequences must be a list, a tuple or a DeviceSequenceSet")
+    _check_sequences(sequences)
     if len(sequences) != n:
         raise ValueError("one row per sequence expected")
-    cols = [np.full(n, -1, dtype=t) for t in (np.int64, np.int64, np.int32, np.int32, np.int32, np.int32)]
     live = np.flatnonzero(np.asarray(pattern) >= 0)
-    if live.size == 0:
-        if own and seqset is not None:
-            seqset.close()
-        return Alignments(cols, [""] * n)
     pidx = np.asarray(pattern)[live].astype(np.int64)
-    if pidx.max() >= len(subsequences):
+    if live.size and pidx.max() >= len(subsequences):
         raise ValueError("a row names pattern %d of %d" % (int(pidx.max()), len(subsequences)))
-    base = seqset.offsets.astype(np.int64)[live]
-    s = np.where(np.asarray(start)[live] >= 0, np.asarray(start)[live] + base, -1)
-    e = np.asarray(rows.end)[live].astype(np.int64) + base
-    d = np.asarray(dist)[live].astype(np.int32)
-    try:
-        got, cigar = _align_set(seqset, subsequences, lims, pidx, s, e, d)
-    finally:
-        if own:
-            seqset.close()
-    g_start, g_cost, g_x, g_ins, g_dels = got
-    if nearest and (g_cost != d).any():
-        r = int(live[np.flatnonzero(g_cost != d)[0]])
-        raise RuntimeError("row %d: an alignment of cost %d at the nearest distance %d" %
-                           (r, int(g_cost[np.flatnonzero(live == r)[0]]), int(dist[r])))
-    ok = g_cost >= 0
-    start_c, end_c, dist_c, x_c, ins_c, dels_c = cols
-    rl = live[ok]
-    start_c[rl] = g_start[ok] - base[ok]
-    end_c[rl] = e[ok] - base[ok]
-    dist_c[rl], x_c[rl], ins_c[rl], dels_c[rl] = g_cost[ok], g_x[ok], g_ins[ok], g_dels[ok]
-    out = [""] * n
-    for r, c in zip(live.tolist(), cigar):
-        out[r] = c
-    return Alignments(cols, out)
+    cols = [np.full(n, -1, dtype=t) for t in (np.int64, np.int64, np.int32, np.int32, np.int32, np.int32)]
+    cigars = [""] * n
+
+    def align(seqset):
+        base = seqset.offsets.astype(np.int64)[live]
+        s = np.where(np.asarray(start)[live] >= 0, np.asarray(start)[live] + base, -1)
+        e = np.asarray(rows.end)[live].astype(np.int64) + base
+        d = np.asarray(dist)[live].astype(np.int32)
+        (g_start, g_cost, g_x, g_ins, g_dels), cigar = _align_set(seqset, subsequences, lims, pidx, s, e, d)
+        if nearest and (g_cost != d).any():
+            r = int(live[np.flatnonzero(g_cost != d)[0]])
+            raise RuntimeError("row %d: an alignment of cost %d at the nearest distance %d" %
+                               (r, int(g_cost[np.flatnonzero(live == r)[0]]), int(dist[r])))
+        ok = g_cost >= 0
+        start_c, end_c, dist_c, x_c, ins_c, dels_c = cols
+        rl = live[ok]
+        start_c[rl] = g_start[ok] - base[ok]
+        end_c[rl] = e[ok] - base[ok]
+        dist_c[rl], x_c[rl], ins_c[rl], dels_c[rl] = g_cost[ok], g_x[ok], g_ins[ok], g_dels[ok]
+        for r, c in zip(live.tolist(), cigar):
+            cigars[r] = c
+    _in_each(sequences, lambda _: None, align if live.size else None)
+    return Alignments(cols, cigars)
 
 
 def _align_set(seqset, subsequences, lims, pidx, s, e, d):
     """fzb_align over the set's buffer for the items (pattern pidx[i], window [s[i], e[i]) or a free start, bound
     d[i]) -> ((start, cost, substitutions, insertions, deletions) arrays, CIGAR list)."""
-    from .search import AlphabetTooLarge, _cigars
+    from .search import _cigars
+    k = len(pidx)
+    cols = [np.full(k, -1, dtype=np.int64)] + [np.full(k, -1, dtype=np.int32) for _ in range(4)]
+    cigar = [""] * k
+
+    def align(sel, pats, pl, ip):  # the items `sel`, item i of pattern pats[ip[i]] with limits pl[ip[i]]
+        got, ops, op_offsets, _ = seqset._seq.haystack.align(pats, *zip(*pl), ip, s[sel], e[sel], d[sel])
+        for c, g in zip(cols, got):
+            c[sel] = g
+        m = np.array([len(p) for p in pats], dtype=np.int64)[ip]
+        for i, cg in zip(sel.tolist(), _cigars(ops, op_offsets, m + got[3], got[1] >= 0)):
+            cigar[i] = cg
     with seqset._lock:
-        try:  # (item selection, bound patterns, their limits, each item's pattern among them)
-            groups = [(np.arange(len(pidx)), seqset._bind_many(subsequences), lims, pidx)]
-        except AlphabetTooLarge:  # no common byte alphabet: pattern by pattern, each reducing the set to its own
-            groups = [(sel, seqset._bind_many([subsequences[p]]), [lims[p]], np.zeros(sel.size, dtype=np.int64))
-                      for p in np.unique(pidx).tolist() for sel in [np.flatnonzero(pidx == p)]]
-        k = len(pidx)
-        cols = [np.full(k, -1, dtype=np.int64)] + [np.full(k, -1, dtype=np.int32) for _ in range(4)]
-        cigar = [""] * k
-        for sel, pats, pl, ip in groups:
-            got, ops, op_offsets, _ = seqset._seq.haystack.align(pats, *zip(*pl), ip, s[sel], e[sel], d[sel])
-            for c, g in zip(cols, got):
-                c[sel] = g
-            m = np.array([len(p) for p in pats], dtype=np.int64)[ip]
-            for i, cg in zip(sel.tolist(), _cigars(ops, op_offsets, m + got[3], got[1] >= 0)):
-                cigar[i] = cg
+        pats = _bind_common(seqset._bind_many, subsequences)
+        if pats is not None:
+            align(np.arange(k), pats, lims, pidx)
+        else:  # pattern by pattern, each bound (reducing the set to its own alphabet) right before its items
+            for p in np.unique(pidx).tolist():
+                sel = np.flatnonzero(pidx == p)
+                align(sel, seqset._bind_many([subsequences[p]]), [lims[p]], np.zeros(sel.size, dtype=np.int64))
     return tuple(cols), cigar
